@@ -52,8 +52,8 @@ def lib():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
-            f"{LIB_PATH} is missing: the B200 kernels are not built. Run `python -m audiocraft_b200.build` "
-            "(nvcc, sm_100a). There is no CPU / PyTorch fallback for this path.")
+            f"{LIB_PATH} is missing: the CUDA kernels are not built. Run `python -m audiocraft_b200.build` "
+            "(nvcc, sm_90a). There is no CPU / PyTorch fallback for this path.")
     L = C.CDLL(LIB_PATH)
     vp, ci, cf, i64 = C.c_void_p, C.c_int, C.c_float, C.c_int64
     L.acb_last_error.restype = C.c_char_p
@@ -126,5 +126,5 @@ def stream() -> int:
 
 def require_cuda(device):
     if not torch.cuda.is_available():
-        raise RuntimeError("audiocraft_b200 runs on CUDA (B200, sm_100a) only; no CPU fallback exists")
+        raise RuntimeError("audiocraft_b200 runs on CUDA (H100, sm_90a) only; no CPU fallback exists")
     return torch.device(device if device is not None else 'cuda')

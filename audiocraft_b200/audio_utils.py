@@ -1,7 +1,7 @@
 """`convert_audio` for the prompt path of `generate_continuation` (audiocraft/data/audio_utils.py:20-59).
 
 Host-side preprocessing, not the hot path: a prompt is resampled once per call.  The reference delegates the
-resampling to a third-party dependency that is NOT in /root/reference and not installed in this image:
+resampling to a third-party dependency that is NOT part of the reference and not a dependency here:
 `julius.resample_frac` (requirements.txt:7, unpinned; algorithm restated here from julius 0.2.x `ResampleFrac`):
 
 * reduce `old_sr/new_sr` by their gcd; cutoff `sr = rolloff * min(old, new)` with `rolloff = 0.945`, `zeros = 24`;

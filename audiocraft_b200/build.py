@@ -1,8 +1,8 @@
-"""Build libaudiocraft_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libaudiocraft_b200.so in-tree with nvcc for the H100 (sm_90a; cross-compiles without a GPU).
 
     python -m audiocraft_b200.build [--force]
 
-The .so is git-ignored but travels to the GPU box with the gpurun snapshot.
+The .so, the objects, the stamp and build.log are build products (git-ignored).
 """
 import hashlib
 import os
@@ -14,12 +14,11 @@ CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libaudiocraft_b200.so')
 STAMP = LIB + '.stamp'
 SOURCES = ['api.cu', 'encodec.cu', 'lm.cu', 'lm_step.cu', 'lm_probe.cu']
-HEADERS = ['common.cuh', 'gridbar.cuh', 'lm_step.cuh', os.path.join('..', '..', 'include', 'audiocraft_b200.h')]
+HEADERS = ['common.cuh', 'gridbar.cuh', 'lm_step.cuh', 'wgmma.cuh', os.path.join('..', '..', 'include', 'audiocraft_b200.h')]
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
-FLAGS = ['-O3', '-std=c++17', '-lineinfo', '-gencode', 'arch=compute_100a,code=sm_100a', '-Xcompiler', '-fPIC',
+ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
+FLAGS = ['-O3', '-std=c++17', '-lineinfo'] + ARCH + ['-Xcompiler', '-fPIC',
          '-Xptxas', '-v']
-if os.environ.get('ACB_STEP_NCW'):   # experiment: compute warps per CTA of the fused decode step (csrc/lm_step.cu)
-    FLAGS.append('-DACB_STEP_NCW=' + os.environ['ACB_STEP_NCW'])
 OBJ_SUFFIX = '.o'
 if os.environ.get('ACB_BUILD_VARIANT'):   # experiment builds: extra -D flags (ACB_BUILD_DEFS) into libaudiocraft_b200_<variant>.so; run with ACB_LIB=<path>
     _v = os.environ['ACB_BUILD_VARIANT']
@@ -60,7 +59,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         logs.append(f'== {f}\n{out}')
         if p.returncode != 0:
             raise RuntimeError(f'nvcc failed on {f}:\n{out}')
-    cmd = [NVCC, '-shared', '-o', LIB] + objs + ['-gencode', 'arch=compute_100a,code=sm_100a', '-lcudart']
+    cmd = [NVCC, '-shared', '-o', LIB] + objs + ARCH + ['-lcudart']
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         raise RuntimeError(f'link failed:\n{r.stdout}')

@@ -134,7 +134,7 @@ class ConditionFuser:
         assert all(k in self.FUSING_METHODS for k in fuse2cond.keys())
         for m in ('sum', 'prepend', 'input_interpolate'):
             if fuse2cond.get(m):
-                raise NotImplementedError(f"fuse method '{m}' is not built on the B200 path (only 'cross')")
+                raise NotImplementedError(f"fuse method '{m}' is not built on this path (only 'cross')")
         if cross_attention_pos_emb:
             raise NotImplementedError("cross_attention_pos_emb is not built (false for MusicGen)")
         self.fuse2cond = fuse2cond

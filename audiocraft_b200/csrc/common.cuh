@@ -1,4 +1,4 @@
-// Shared helpers for the audiocraft_b200 kernels (sm_100a).
+// Shared helpers for the audiocraft_b200 kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -31,9 +31,8 @@ static inline int acb_ceil_div(int a, int b) { return (a + b - 1) / b; }
 
 // ELU(alpha=1) as torch computes it: x > 0 ? x : exp(x) - 1   (ATen elu kernel; not expm1)
 // ELU: exp through ex2.approx (__expf, 2 instructions) instead of libm's expf (~10): absolute error ~1e-7 on (0, 1], the size of an
-// fp32 rounding of the result.  Every golden stays index-exact and every layer test inside its tolerance; the whole codec gets 7 %
-// faster (encode 52.9 -> 47.6 ms: the slab staging of every encoder layer runs ELU per element; profiles/r2_perf_encodec_v9* vs
-// v10*).  -DACB_PRECISE_ELU restores expf.
+// fp32 rounding of the result.  Every golden stays index-exact and every layer test inside its tolerance; the slab staging of every
+// encoder layer runs ELU per element, so the cheaper exp matters.  -DACB_PRECISE_ELU restores expf.
 #ifdef ACB_PRECISE_ELU
 __device__ __forceinline__ float acb_elu(float v) { return v > 0.f ? v : expf(v) - 1.f; }
 #else

@@ -1,13 +1,14 @@
-// EnCodec hot path for B200 (sm_100a): SEANet convolutions, LSTM recurrence, residual VQ.
+// EnCodec hot path for H100 (sm_90a): SEANet convolutions, LSTM recurrence, residual VQ.
 //
 // fp32 CUDA-core arithmetic on purpose: RVQ code indices must match the fp32 reference bit for bit on the
 // same latent, and a TF32/BF16 tensor-core conv would move the latents by ~1e-3 and flip near-tie codes
-// (SURVEY.md section 7 "hard parts").  What is B200-specific here is the data movement: padding, ELU,
+// (SURVEY.md section 7 "hard parts").  What is GPU-specific here is the data movement: padding, ELU,
 // bias, residual add and the transposed-conv trim are folded into the conv kernels (one read + one write
 // of every activation per layer), weight-norm is folded once at load, the [frames x bins] VQ distance
 // matrix never leaves the SM, and the LSTM keeps W_hh resident in the 227 KB shared memory of 128 SMs.
 #include "common.cuh"
 #include "gridbar.cuh"
+#include "wgmma.cuh"
 #include <stdlib.h>
 
 // ------------------------------------------------------------------------------------------------
@@ -44,7 +45,7 @@ extern "C" int acb_weight_norm_fold(const float* v, const float* g, float* w, in
 struct ConvParams {
     const float* x; const float* w; const float* bias; const float* res; float* y;
     int c_in, c_out, t_in, t_virt, t_out, K, stride, dil, pad_left, reflect, elu, ci_chunk, span, PL;
-    int tr_S, tr_trim, tr_tout;   // transposed conv as a GEMM over virtual channels n' = co*S + phase (tcgen05 kernel only)
+    int tr_S, tr_trim, tr_tout;   // transposed conv as a GEMM over virtual channels n' = co*S + phase (conv1d_t5 only)
 };
 
 // One warp stages dst[q] = act(x[g0 + q * gstep]) for q in [0, n) (zero beyond, up to n_store): the global loads of 8 lane-strided
@@ -194,7 +195,7 @@ __device__ __forceinline__ uint32_t to_tf32(float v) {
 __device__ __forceinline__ uint32_t to_tf32(float v) { return (__float_as_uint(v) + 0x1000u) & 0xFFFFE000u; }
 #endif
 // (Handing the low term x - hi to the tensor core unrounded -- it reads only the upper 19 bits of a tf32 operand -- saves two more
-//  instructions per element and measured no faster: 84.63 vs 84.74 ms for the codec, profiles/r2_perf_encodec_v12*.  Not kept.)
+//  instructions per element but was measured no faster.  Not kept.)
 __device__ __forceinline__ void mma_tf32(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
     asm volatile(
         "mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
@@ -325,7 +326,7 @@ static int launch_conv1d_tc(const ConvParams& p, int batch, cudaStream_t s) {
 // SEANetResnetBlock with the identity skip (audiocraft/modules/seanet.py:44-69, true_skip=True) as ONE kernel:
 //     y = x + W2 . elu(b1 + W1 * elu(x)) + b2          W1: k=3 conv C -> C/2,  W2: 1x1 conv C/2 -> C
 // As two layer kernels the block moves x, the hidden tensor (twice) and y through HBM (4 C-equivalents + 1.5 C of hidden traffic)
-// and is bandwidth / latency bound at 64-128 channels (7-8 ms each for 32 x 10 s at 64 channels).  Here a CTA owns 128 time steps
+// and is bandwidth / latency bound at 64-128 channels.  Here a CTA owns 128 time steps
 // of one item: the ELU'd input slab [C][128 + 2 dil] is staged once, GEMM 1 (M = C/2 hidden channels, N = 128 steps, K = 3C; W1
 // streamed in chunks of 16 input channels x 3 taps) leaves the hidden tile in registers, bias + ELU moves it to shared memory (over
 // the slab), GEMM 2 (M = C in chunks of 64 output channels, K = C/2) reads it from there and the epilogue adds bias and the skip.
@@ -955,38 +956,16 @@ extern "C" int acb_resblock(const float* x, const float* w1, const float* b1, co
 }
 
 // ------------------------------------------------------------------------------------------------
-// conv1d on the 5th-generation tensor cores: tcgen05.mma.kind::tf32 with the accumulator in TMEM, 3xTF32 split.
-//   D[128 time steps (TMEM lanes)][N output channels (TMEM columns)] += A[128][8] . B[N][8]^T   per instruction
+// conv1d on the tensor cores: wgmma.mma_async tf32 (m64nNk8) with the accumulator in registers, 3xTF32 split.
+//   D[64 time steps][N output channels] += A[64][8] . B[N][8]^T   per instruction and warpgroup; the two warpgroups of the
+//   CTA own time steps [0, 64) and [64, 128) of the tile
 //   A = im2col rows of the staged input slab, B = weight rows, both K-major in the canonical 128-byte-swizzled layout
 //       offset(row, k16B) = row * 128 B + ((k16B ^ (row % 8)) * 16 B)              (one 32-row reduction chunk = one 128-byte row)
 // Per reduction chunk of 32 rows (r = channel x tap) every thread builds its im2col row (hi and lo tf32 parts) and a
-// share of the weight tile, a proxy fence publishes them to the async proxy, ONE thread issues 4 k-steps x 3 MMAs
-// (lo*hi, hi*lo, hi*hi) and commits to an mbarrier; the epilogue reads the accumulator with tcgen05.ld (lane = time
-// step, so the [B][C][T] stores are coalesced) and fuses bias + residual.
+// share of the weight tile, a proxy fence publishes them to the async proxy, each warpgroup issues 4 k-steps x 3 MMAs
+// (lo*hi, hi*lo, hi*hi) and waits for them; the epilogue fuses bias + residual into the stores.
 // ------------------------------------------------------------------------------------------------
 constexpr int T5_M = 128, T5_RC = 32;
-
-__device__ __forceinline__ uint64_t t5_desc(uint32_t smem_addr, uint32_t lbo_bytes) {
-    // UMMA shared-memory descriptor (cute/arch/mma_sm100_desc.hpp): start [0,14) >>4, LBO [16,30) >>4, SBO [32,46) >>4,
-    // version [46,48) = 1, layout_type [61,64) = 0 (SWIZZLE_NONE)
-    return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(128u >> 4) << 32) |
-           ((uint64_t)1 << 46);
-}
-// The same descriptor for the 128-byte-swizzled K-major layout (layout_type 2, SBO = 1024 B between 8-row groups, LBO unused):
-// a tile row is 32 fp32 = 128 contiguous bytes and its 16-byte chunk c sits at position c ^ (row & 7); tiles are 1024-byte
-// aligned and a K step of 8 tf32 advances the start address by 32 bytes.  conv1d_t5 stages its im2col and weight tiles in this
-// layout (conflict-free 16-byte stores, and what a tensor-map TMA load would produce).  Measured: NO speed difference against the
-// INTERLEAVE layout it used in round 1 (decode 60.3 vs 60.2 ms, profiles/r2_perf_encodec_v1_fp32tc_encoder.log): the kernel
-// is bound by building its tiles, not by the tensor core's operand fetch.  conv1d_t6 keeps INTERLEAVE: its taps are descriptor
-// start-address shifts by whole rows, which a swizzled layout would need base-offset arithmetic for.
-__device__ __forceinline__ uint64_t t5_desc_sw128(uint32_t smem_addr) {
-    return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024u >> 4) << 32) | ((uint64_t)1 << 46) |
-           ((uint64_t)2 << 61);
-}
-__device__ __forceinline__ void t5_mma(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile("{\n .reg .pred p;\n setp.ne.b32 p, %4, 0;\n tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n}"
-                 ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
 
 // TERMS = 2: x ~ hi + lo -> 3 MMAs per product (lo*hi, hi*lo, hi*hi).  (A 3-term / 6-MMA split was measured: identical
 // end-to-end error, 1.43e-4 on the 32 kHz latents -- the residual is the tensor core's accumulate rounding, not the
@@ -1004,30 +983,19 @@ __device__ __forceinline__ void t5_split(float x, float (&out)[TERMS]) {
 }
 
 template <int TERMS, int NW>   // NW = weight elements per thread and chunk = N * 32 / 256
-__global__ void __launch_bounds__(256, 2) conv1d_t5_kernel(ConvParams p, int xsp) {
+__global__ void __launch_bounds__(256, NW >= 8 ? 1 : 2) conv1d_t5_kernel(ConvParams p, int xsp) {
     constexpr int N = NW * 8;
     extern __shared__ __align__(1024) unsigned char t5sm[];   // swizzled operand tiles are 1024-byte aligned
-    // [A terms: TERMS x 16 KB][B terms: TERMS x N*128 B][slab][roff][mbar][tmem slot]
+    // [A terms: TERMS x 16 KB][B terms: TERMS x N*128 B][slab][roff]
     float* a_t = reinterpret_cast<float*>(t5sm);
     float* b_t = a_t + TERMS * T5_M * T5_RC;
     float* xs = b_t + TERMS * N * T5_RC;
     int* roff = reinterpret_cast<int*>(xs + ((p.ci_chunk * xsp + 3) & ~3));   // keep 16-byte alignment behind the slab
-    uint64_t* mbar = reinterpret_cast<uint64_t*>(roff + T5_RC);
-    uint32_t* tslot = reinterpret_cast<uint32_t*>(mbar + 1);
 
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
     const int t0 = blockIdx.x * T5_M, co0 = blockIdx.y * N, b = blockIdx.z;
     const float* xb = p.x + (size_t)b * p.c_in * p.t_in;
-    constexpr uint32_t ncols = N < 32 ? 32u : (uint32_t)N;
 
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32_(tslot)), "r"(ncols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    if (tid == 32) {
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32_(mbar)) : "memory");
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
     // ---- chunk-invariant staging maps: where each of this thread's slab elements comes from (relative to the first
     //      channel of a chunk) and where it goes (phase-de-interleaved slab), computed once
     const int g0 = t0 * p.stride - p.pad_left;
@@ -1052,13 +1020,13 @@ __global__ void __launch_bounds__(256, 2) conv1d_t5_kernel(ConvParams p, int xsp
         const int cl = r / p.K, k = r - cl * p.K, kd = k * p.dil;
         roff[r] = cl < p.ci_chunk ? cl * xsp + (kd % p.stride) * p.PL + kd / p.stride : 0;
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem = *tslot;
 
-    const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(T5_M >> 4) << 24);
-    const uint32_t a_s = smem_u32_(a_t), b_s = smem_u32_(b_t);
+    // this warpgroup's 64 rows of A start 64 x 128 B into each A term
+    const uint32_t a_s = smem_u32_(a_t) + (uint32_t)wg * (64u * 128u), b_s = smem_u32_(b_t);
+    float acc[N / 2];
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
 
     float xr[T5_SLAB_PT], wr[NW];
     auto prefetch = [&](int ci0) {   // raw global values of one chunk into registers (no dependence on smem state)
@@ -1075,7 +1043,6 @@ __global__ void __launch_bounds__(256, 2) conv1d_t5_kernel(ConvParams p, int xsp
     };
     prefetch(0);
 
-    uint32_t phase = 0, first = 1;
     for (int ci0 = 0; ci0 < p.c_in; ci0 += p.ci_chunk) {
         // (the previous chunk's MMAs have completed -- waited at the bottom -- so slab and tiles may be rewritten)
 #pragma unroll
@@ -1108,83 +1075,53 @@ __global__ void __launch_bounds__(256, 2) conv1d_t5_kernel(ConvParams p, int xsp
         }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to the tensor core
         __syncthreads();
-        if (tid == 0) {
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+        wgmma_fence();
+        wgmma_fence_regs(acc);
 #pragma unroll
-            for (int ks = 0; ks < T5_RC / 8; ++ks) {   // one instruction = 8 reduction rows = two 16-byte k-chunks
-                uint64_t ad[TERMS], bd[TERMS];
+        for (int ks = 0; ks < T5_RC / 8; ++ks) {   // one instruction = 8 reduction rows = two 16-byte k-chunks
+            uint64_t ad[TERMS], bd[TERMS];
 #pragma unroll
-                for (int q = 0; q < TERMS; ++q) {
-                    ad[q] = t5_desc_sw128(a_s + q * (T5_M * T5_RC * 4) + ks * 32);
-                    bd[q] = t5_desc_sw128(b_s + q * (N * T5_RC * 4) + ks * 32);
-                }
-                // smallest cross terms first; term index 0 = hi.  Keep products a_i * b_j with i + j < TERMS.
-#pragma unroll
-                for (int sum = TERMS - 1; sum >= 0; --sum)
-#pragma unroll
-                    for (int i = 0; i <= sum; ++i) {
-                        t5_mma(tmem, ad[i], bd[sum - i], idesc, first ? 0u : 1u);
-                        first = 0;
-                    }
+            for (int q = 0; q < TERMS; ++q) {
+                ad[q] = wgmma_desc_sw128(a_s + q * (T5_M * T5_RC * 4) + ks * 32);
+                bd[q] = wgmma_desc_sw128(b_s + q * (N * T5_RC * 4) + ks * 32);
             }
-            asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32_(mbar)) : "memory");
+            // smallest cross terms first; term index 0 = hi.  Keep products a_i * b_j with i + j < TERMS.
+#pragma unroll
+            for (int sum = TERMS - 1; sum >= 0; --sum)
+#pragma unroll
+                for (int i = 0; i <= sum; ++i) wgmma_tf32<N>(acc, ad[i], bd[sum - i], 1u);
         }
-        {   // everyone waits for the tensor core to finish reading this chunk's tiles
-            uint32_t ok = 0;
-            do {
-                asm volatile("{\n .reg .pred q;\n mbarrier.try_wait.parity.shared::cta.b64 q, [%1], %2;\n selp.u32 %0, 1, 0, q;\n}"
-                             : "=r"(ok) : "r"(smem_u32_(mbar)), "r"(phase) : "memory");
-            } while (!ok);
-            phase ^= 1u;
-        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(acc);
+        __syncthreads();   // both warpgroups are done reading this chunk's tiles
     }
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    if (warp < 4) {   // warp w reads TMEM lanes [32w, 32w+32) = time steps; 16 output channels per load
-        const int t = t0 + warp * 32 + lane;
-        for (int c0 = 0; c0 < N; c0 += 16) {
-            uint32_t v[16];
-            const uint32_t taddr = tmem + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0;
-            asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                         : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-                           "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-                         : "r"(taddr));
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+    {   // thread (warp w of the warpgroup, lane l): time steps 64 wg + 16 w + l / 4 (+ 8), channels 8 j + 2 (l % 4) (+ 1)
+        const int tr = t0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+        for (int i = 0; i < N / 2; ++i) {
+            const int t = tr + ((i >> 1) & 1) * 8, c = co0 + (i >> 2) * 8 + (lane & 3) * 2 + (i & 1);
+            if (t >= p.t_out || c >= p.c_out) continue;
             if (p.tr_S == 0) {
-#pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    const int co = co0 + c0 + j;
-                    if (co < p.c_out && t < p.t_out) {
-                        const size_t o = ((size_t)b * p.c_out + co) * p.t_out + t;
-                        float y = __uint_as_float(v[j]) + (p.bias ? p.bias[co] : 0.f);
-                        if (p.res) y += p.res[o];
-                        p.y[o] = y;
-                    }
-                }
+                const size_t o = ((size_t)b * p.c_out + c) * p.t_out + t;
+                float y = acc[i] + (p.bias ? p.bias[c] : 0.f);
+                if (p.res) y += p.res[o];
+                p.y[o] = y;
             } else {   // transposed conv: column n' = co*S + phase, output step = t*S + phase - trim
-                const int cout = p.c_out / p.tr_S;
-#pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    const int n = co0 + c0 + j;
-                    if (n < p.c_out && t < p.t_out) {
-                        const int co = n / p.tr_S, ph = n - co * p.tr_S, o = t * p.tr_S + ph - p.tr_trim;
-                        if (o >= 0 && o < p.tr_tout)
-                            p.y[((size_t)b * cout + co) * p.tr_tout + o] = __uint_as_float(v[j]) + (p.bias ? p.bias[co] : 0.f);
-                    }
-                }
+                const int cout = p.c_out / p.tr_S, co = c / p.tr_S, ph = c - co * p.tr_S, o = t * p.tr_S + ph - p.tr_trim;
+                if (o >= 0 && o < p.tr_tout)
+                    p.y[((size_t)b * cout + co) * p.tr_tout + o] = acc[i] + (p.bias ? p.bias[co] : 0.f);
             }
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(ncols) : "memory");
 }
 
 template <int TERMS, int NW>
 static int launch_t5_one(const ConvParams& q, int xsp, int batch, cudaStream_t s) {
     constexpr int N = NW * 8;
     size_t smem = ((size_t)TERMS * T5_M * T5_RC + (size_t)TERMS * N * T5_RC + (size_t)((q.ci_chunk * xsp + 3) & ~3)) * sizeof(float) +
-                  T5_RC * sizeof(int) + 8 + 8;
-    ACB_REQUIRE(smem <= 200 * 1024, "acb_conv1d: tcgen05 tile needs %zu B of shared memory", smem);
+                  T5_RC * sizeof(int);
+    ACB_REQUIRE(smem <= 200 * 1024, "acb_conv1d: tensor-core tile needs %zu B of shared memory", smem);
     ACB_CHECK_CUDA(cudaFuncSetAttribute(conv1d_t5_kernel<TERMS, NW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     dim3 grid(acb_ceil_div(q.t_out, T5_M), acb_ceil_div(q.c_out, N), batch);
     conv1d_t5_kernel<TERMS, NW><<<grid, 256, smem, s>>>(q, xsp);
@@ -1198,21 +1135,20 @@ static int launch_conv1d_t5(const ConvParams& p, int batch, cudaStream_t s) {
     q.span = (T5_M - 1) * p.stride + (p.K - 1) * p.dil + 1;
     q.PL = acb_ceil_div(q.span, p.stride);
     const int xsp = p.stride * q.PL;
-    ACB_REQUIRE(q.ci_chunk * q.span <= 256 * T5_SLAB_PT, "acb_conv1d: tcgen05 slab too large (%d elements)", q.ci_chunk * q.span);
-    if (p.c_out >= 256) return launch_t5_one<2, 32>(q, xsp, batch, s);
+    ACB_REQUIRE(q.ci_chunk * q.span <= 256 * T5_SLAB_PT, "acb_conv1d: tensor-core slab too large (%d elements)", q.ci_chunk * q.span);
+    // N <= 128: the 64 x N accumulator of each warpgroup lives in registers (64 per thread at N = 128)
     if (p.c_out >= 128) return launch_t5_one<2, 16>(q, xsp, batch, s);
     if (p.c_out >= 64) return launch_t5_one<2, 8>(q, xsp, batch, s);
     return launch_t5_one<2, 4>(q, xsp, batch, s);
 }
 
 // ------------------------------------------------------------------------------------------------
-// Written at the end of round 1 without GPU time; validated on B200 in round 2 (every test green on first contact) and since then the
-// encoder's kernel for k > 1 with >= 128 output channels (EncodecModel encoder_precision='fp32_tc').  Round-2 changes, each from an ncu
-// capture: raw input samples through a cp.async ring instead of one vector at a time, and the CTA persistent over tiles.
+// The encoder's kernel for k > 1 with >= 128 output channels (EncodecModel encoder_precision='fp32_tc'): raw input samples
+// through a cp.async ring, the CTA persistent over tiles.
 //
-// conv1d_t6: implicit-GEMM convolution on tcgen05 WITHOUT an im2col tile, warp-specialised and double-buffered, with
-// the TMEM accumulator flushed into fp32 registers once per 8-channel group.  It answers the two measured problems of
-// conv1d_t5_kernel (profiles/r1_ncu_t5v2_raw.csv, DESIGN.md 3.2):
+// conv1d_t6: implicit-GEMM convolution on wgmma WITHOUT an im2col tile, warp-specialised and double-buffered, with
+// the tensor-core accumulator flushed into fp32 registers once per 8-channel group.  It answers two problems of
+// conv1d_t5_kernel:
 //   (1) t5 is BUILD-bound, not MMA-bound: per 32 reduction rows it writes a 128 x 32 im2col tile (every input sample
 //       is split and stored once per tap).  Here the reduction index of one MMA is 8 consecutive INPUT CHANNELS at a
 //       fixed tap, and the staged input slab is laid out [4-channel chunk][stride phase][time][4 channels], i.e. with
@@ -1220,15 +1156,16 @@ static int launch_conv1d_t5(const ConvParams& p, int batch, cudaStream_t s) {
 //       of the shared-memory descriptor (phase plane (k*D) % S, row offset (k*D) / S).  Each input sample is split and
 //       stored once per 8-channel group instead of once per tap (7-16x less build work).
 //   (2) t5's error is the tensor core's truncating fp32 accumulate over up to 3 072 chained MMAs.  Here the chain is
-//       3*K MMAs (one 8-channel group); the epilogue warps tcgen05.ld that partial sum and add it to register
-//       accumulators with round-to-nearest fp32 adds while the MMA warp fills the other TMEM accumulator.
-// Roles (320 threads): warps 0-3 stage the input slab (ELU, reflect / zero padding, hi/lo tf32 split), warp 4 issues the
-// MMAs, warps 5-8 flush / own the output tile (TMEM lane quarter = warp % 4), warp 9 streams the pre-split, pre-laid-out
-// weight tiles with TMA bulk copies.  Pipelines: slab x2 (a_full / a_empty), weight stage x2 (b_full / b_empty),
-// TMEM accumulator x2 (acc_full / acc_empty); tcgen05.commit releases slab, weight stage and accumulator.
+//       3*K MMAs (one 8-channel group) into a fresh accumulator, which is then added to register accumulators with
+//       round-to-nearest fp32 adds.
+// Roles (384 threads): warpgroup 0 (warps 0-3) stages the input slab (ELU, reflect / zero padding, hi/lo tf32 split);
+// warpgroups 1 and 2 issue the MMAs on time steps [0, 64) and [64, 128) of the tile and own those rows of the output, and
+// thread 0 of warpgroup 1 streams the pre-split, pre-laid-out weight tiles with TMA bulk copies, refilling each weight stage as
+// soon as both warpgroups have released it (a producer-side loader would block the slab staging behind that release).  Pipelines: slab x2 (a_full / a_empty), weight
+// stage x2 (b_full / b_empty); every consumer warp arrives on the empty barriers once its MMAs have completed.
 // Weights are packed by the host as w6[co_tile][cg][k][term(hi,lo)][c(2)][n(N)][4 channels]  (fp32 bits, tf32-exact).
 // ------------------------------------------------------------------------------------------------
-constexpr int T6_M = 128, T6_THREADS = 320, T6_MAXV = 20;
+constexpr int T6_M = 128, T6_THREADS = 384, T6_MAXV = 20;
 
 struct T6Params {
     const float* x; const float* w6; const float* bias; const float* res; float* y;
@@ -1254,9 +1191,6 @@ __device__ __forceinline__ void t6_mbar_wait(uint64_t* b, uint32_t parity) {
                      : "=r"(ok) : "r"(smem_u32_(b)), "r"(parity) : "memory");
     } while (!ok);
 }
-__device__ __forceinline__ void t6_commit(uint64_t* b) {   // arrives on b once every MMA issued so far by this thread is done
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32_(b)) : "memory");
-}
 __device__ __forceinline__ void t6_bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(smem_u32_(dst)), "l"(src), "r"(bytes), "r"(smem_u32_(bar)) : "memory");
@@ -1275,53 +1209,41 @@ __host__ __device__ inline T6Smem t6_smem(int N, int S, int PL, int TB, int raw_
     L.slab = 0;
     L.btile = 2 * L.slab_stage;
     L.bars = L.btile + 2 * L.b_stage;
-    L.raw = L.bars + 12 * 8 + 16;           // [DEPTH][NV][4 channels][128 threads] raw samples (NV <= 12 only)
+    L.raw = L.bars + 8 * 8;                 // [DEPTH][NV][4 channels][128 threads] raw samples (NV <= 12 only)
     L.raw_stage = raw_vec * 4 * 128 * 4;
     L.total = L.raw + raw_depth * L.raw_stage;
     return L;
 }
 
-// NV = slab vectors per staging thread (4 / 12 / 20): the maps and the prefetched raw samples live in registers, and 10 warps are allocated
-// as 12 (warp allocation granularity 4), which caps the kernel at 168 registers per thread.
+// NV = slab vectors per staging thread (4 / 12 / 20): the maps and the prefetched raw samples live in registers; 12 warps cap the
+// kernel at 168 registers per thread.
 template <int N, int NV, int DEPTH>   // DEPTH: cp.async ring depth (0: register prefetch)
 __global__ void __launch_bounds__(T6_THREADS, 1) conv1d_t6_kernel(T6Params p) {
     extern __shared__ __align__(128) unsigned char t6sm[];
     const T6Smem L = t6_smem(N, p.S, p.PL, p.TB, p.raw_vec, DEPTH);
     uint64_t* bars = reinterpret_cast<uint64_t*>(t6sm + L.bars);
     uint64_t* a_full = bars;          // [2] slab staged            (1 arrival: elected producer)
-    uint64_t* a_empty = bars + 2;     // [2] slab consumed          (tcgen05.commit)
+    uint64_t* a_empty = bars + 2;     // [2] slab consumed          (8 arrivals: one per consumer warp)
     uint64_t* b_full = bars + 4;      // [2] weight stage landed    (1 arrival + TMA bytes)
-    uint64_t* b_empty = bars + 6;     // [2] weight stage consumed  (tcgen05.commit)
-    uint64_t* acc_full = bars + 8;    // [2] partial sum complete   (tcgen05.commit)
-    uint64_t* acc_empty = bars + 10;  // [2] partial sum flushed    (4 arrivals: one per epilogue warp)
-    uint32_t* tslot = reinterpret_cast<uint32_t*>(bars + 12);
+    uint64_t* b_empty = bars + 6;     // [2] weight stage consumed  (8 arrivals: one per consumer warp)
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    // PERSISTENT over tiles (one CTA per SM fits: 131 KB of shared memory, 2 N TMEM columns): tile = blockIdx.x, += gridDim.x.  Every
+    const int wgi = __shfl_sync(0xffffffffu, tid >> 7, 0);   // warpgroup index, provably warp-uniform (keeps the MMAs pipelined)
+    // PERSISTENT over tiles (one CTA per SM fits: 131 KB of shared memory): tile = blockIdx.x, += gridDim.x.  Every
     // role walks the same tile sequence with running group / stage counters, so the mbarrier pipelines simply continue across tiles:
-    // the staging warps fill the next tile's first slabs and the MMA warp starts on them while the epilogue warps still store the
-    // previous tile.  (One tile per CTA measured 65-82 us per tile of which the 192 MMAs need ~7: prologue, pipeline fill and the
-    // 128-stores-per-thread epilogue ran with nothing else resident on the SM.)
+    // the staging warps fill the next tile's first slabs while the consumers still work on (and store) the previous tile.
     const int nstage_b = (p.K + p.TB - 1) / p.TB;   // weight stages per channel group
 
-    if (warp == 4) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32_(tslot)), "n"(2 * N) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
     if (tid == 0) {
         for (int i = 0; i < 2; ++i) {
-            t6_mbar_init(a_full + i, 1); t6_mbar_init(a_empty + i, 1);
-            t6_mbar_init(b_full + i, 1); t6_mbar_init(b_empty + i, 1);
-            t6_mbar_init(acc_full + i, 1); t6_mbar_init(acc_empty + i, 4);
+            t6_mbar_init(a_full + i, 1); t6_mbar_init(a_empty + i, 8);
+            t6_mbar_init(b_full + i, 1); t6_mbar_init(b_empty + i, 8);
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem = *tslot;
 
-    if (warp < 4) {
+    if (wgi == 0) {
         // ================= producers: stage the 8-channel slab of every channel group =================
         // chunk-invariant maps: this thread's (time j, 4-channel chunk c) vectors -> source index / destination
         const int nvec = 2 * p.span;
@@ -1339,8 +1261,7 @@ __global__ void __launch_bounds__(T6_THREADS, 1) conv1d_t6_kernel(T6Params p) {
         int G = 0;   // running channel-group counter (slab buffer = G & 1)
         if constexpr (DEPTH > 0) {
         // ---- raw samples through a cp.async ring, DEPTH channel groups deep.  The input streams from HBM (every sample is used by
-        //      two tiles at most): with one register batch per group in flight an SM had ~16 KB outstanding against ~2 us of latency --
-        //      0.8 TB/s over the chip, 38 % of all stall samples on the first use of the batch (profiles/r2_ncu_conv1d_t6_persistent_*).
+        //      two tiles at most): one register batch per group in flight leaves too few bytes outstanding to cover HBM latency.
         //      The ring keeps 3-4 groups (50-70 KB) in flight, costs no registers, and runs across tile boundaries.
         float* rawsm = reinterpret_cast<float*>(t6sm + L.raw);
         const int raw_stage = p.raw_vec * 4 * 128;
@@ -1420,9 +1341,8 @@ __global__ void __launch_bounds__(T6_THREADS, 1) conv1d_t6_kernel(T6Params p) {
             src[i] = (dst[i] >= 0 && g >= 0 && g < p.t_in) ? g : -1;
         }
         const float* xb = p.x + (size_t)b * p.c_in * p.t_in;
-        // The raw samples of a channel group are requested as one batch into registers and consumed afterwards: the first version
-        // loaded, ELU'd (a branch on the loaded value) and stored vector by vector -- 20 dependent L2 round trips per group, 53 % of
-        // all stall samples on that branch, 82 us per CTA (profiles/r2_ncu_conv1d_t6_*).  The next group's batch is requested
+        // The raw samples of a channel group are requested as one batch into registers and consumed afterwards (loading, ELU-ing and
+        // storing vector by vector makes every vector a dependent L2 round trip).  The next group's batch is requested
         // before this group is published, so its round trip overlaps the fence / barrier / wait for the buffer.
         float raw[NV][4];
         auto fetch = [&](int cg) {
@@ -1462,107 +1382,81 @@ __global__ void __launch_bounds__(T6_THREADS, 1) conv1d_t6_kernel(T6Params p) {
         }
         }   // tiles
         }   // register path (NV > 12)
-    } else if (warp == 9) {
-        // ================= weight loader: one TMA bulk copy per weight stage =================
-        if (lane == 0) {
-            int it = 0;
-            for (int tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) {
+    } else {
+        // ================= consumers: warpgroup wg issues the MMAs of time steps [64 wg, +64) and owns those output rows =================
+        const int wg = wgi - 1;
+        const uint32_t lbo_a = (uint32_t)(p.S * p.PL * 16), lbo_b = (uint32_t)N * 16u;
+        const uint32_t slab_s = smem_u32_(t6sm + L.slab) + (uint32_t)wg * (64u * 16u), btile_s = smem_u32_(t6sm + L.btile);
+        float acc[N / 2], accr[N / 2];
+        int it = 0, G = 0;
+        // weight loader (thread 128): a cursor over the CTA's weight-stage sequence (tile, channel group, tap block)
+        const bool loader = tid == 128;
+        int ltile = blockIdx.x, lcg = 0, lsb = 0, lit = 0;
+        auto load_next = [&]() {
+            if (ltile >= p.n_tiles) return;
+            const int bs = lit & 1, k0 = lsb * p.TB, ntap = min(p.TB, p.K - k0);
+            t6_mbar_wait(b_empty + bs, ((lit >> 1) & 1) ^ 1);   // both warpgroups are done with the stage's previous use
             const unsigned char* wbase = reinterpret_cast<const unsigned char*>(p.w6) +
-                                         (size_t)((tile / p.t_tiles) % p.n_co) * p.n_cg * p.K * L.b_tap;
-            for (int cg = 0; cg < p.n_cg; ++cg)
-                for (int sb = 0; sb < nstage_b; ++sb, ++it) {
-                    const int bs = it & 1, k0 = sb * p.TB, ntap = min(p.TB, p.K - k0);
-                    t6_mbar_wait(b_empty + bs, ((it >> 1) & 1) ^ 1);
-                    const uint32_t bytes = (uint32_t)ntap * (uint32_t)L.b_tap;
-                    t6_mbar_expect_tx(b_full + bs, bytes);
-                    t6_bulk_g2s(t6sm + L.btile + bs * L.b_stage, wbase + ((size_t)cg * p.K + k0) * L.b_tap, bytes, b_full + bs);
-                }
-            }   // tiles
-        }
-    } else if (warp == 4) {
-        // ================= MMA issuer =================
-        if (lane == 0) {
-            const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(T6_M >> 4) << 24);
-            const uint32_t lbo_a = (uint32_t)(p.S * p.PL * 16), lbo_b = (uint32_t)N * 16u;
-            const uint32_t slab_s = smem_u32_(t6sm + L.slab), btile_s = smem_u32_(t6sm + L.btile);
-            int it = 0, G = 0;
-            for (int tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x)
+                                         (size_t)((ltile / p.t_tiles) % p.n_co) * p.n_cg * p.K * L.b_tap;
+            const uint32_t bytes = (uint32_t)ntap * (uint32_t)L.b_tap;
+            t6_mbar_expect_tx(b_full + bs, bytes);
+            t6_bulk_g2s(t6sm + L.btile + bs * L.b_stage, wbase + ((size_t)lcg * p.K + k0) * L.b_tap, bytes, b_full + bs);
+            ++lit;
+            if (++lsb == nstage_b) { lsb = 0; if (++lcg == p.n_cg) { lcg = 0; ltile += gridDim.x; } }
+        };
+        if (loader) { load_next(); load_next(); }
+        __syncwarp();
+        for (int tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) {
+            const int t0 = (tile % p.t_tiles) * T6_M, co0 = ((tile / p.t_tiles) % p.n_co) * N, b = tile / (p.t_tiles * p.n_co);
+#pragma unroll
+            for (int j = 0; j < N / 2; ++j) accr[j] = 0.f;
             for (int cg = 0; cg < p.n_cg; ++cg, ++G) {
-                const int st = G & 1, acc = G & 1;
-                t6_mbar_wait(acc_empty + acc, ((G >> 1) & 1) ^ 1);
+                const int st = G & 1;
                 t6_mbar_wait(a_full + st, (G >> 1) & 1);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t d_tmem = tmem + (uint32_t)(acc * N);
-                uint32_t accumulate = 0;
+                uint32_t scale_d = 0;   // the first MMA of a channel group overwrites the accumulator
                 for (int sb = 0; sb < nstage_b; ++sb, ++it) {
                     const int bs = it & 1, k0 = sb * p.TB, ntap = min(p.TB, p.K - k0);
                     t6_mbar_wait(b_full + bs, (it >> 1) & 1);
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+                    wgmma_fence();
+                    wgmma_fence_regs(acc);
                     for (int kk = 0; kk < ntap; ++kk) {
                         const int kd = (k0 + kk) * p.D;
                         const uint32_t a_off = (uint32_t)(((kd % p.S) * p.PL + kd / p.S) * 16);
-                        const uint64_t a_hi = t5_desc(slab_s + st * L.slab_stage + a_off, lbo_a);
-                        const uint64_t a_lo = t5_desc(slab_s + st * L.slab_stage + L.slab_term + a_off, lbo_a);
+                        const uint64_t a_hi = wgmma_desc(slab_s + st * L.slab_stage + a_off, lbo_a, 128);
+                        const uint64_t a_lo = wgmma_desc(slab_s + st * L.slab_stage + L.slab_term + a_off, lbo_a, 128);
                         const uint32_t bt = btile_s + bs * L.b_stage + kk * L.b_tap;
-                        const uint64_t b_hi = t5_desc(bt, lbo_b), b_lo = t5_desc(bt + 2 * N * 16, lbo_b);
-                        t5_mma(d_tmem, a_lo, b_hi, idesc, accumulate);   // small cross terms first
-                        t5_mma(d_tmem, a_hi, b_lo, idesc, 1u);
-                        t5_mma(d_tmem, a_hi, b_hi, idesc, 1u);
-                        accumulate = 1u;
+                        const uint64_t b_hi = wgmma_desc(bt, lbo_b, 128), b_lo = wgmma_desc(bt + 2 * N * 16, lbo_b, 128);
+                        wgmma_tf32<N>(acc, a_lo, b_hi, scale_d);   // small cross terms first
+                        wgmma_tf32<N>(acc, a_hi, b_lo, 1u);
+                        wgmma_tf32<N>(acc, a_hi, b_hi, 1u);
+                        scale_d = 1u;
                     }
-                    t6_commit(b_empty + bs);          // the weight stage may be overwritten once these MMAs are done
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                    wgmma_fence_regs(acc);
+                    __syncwarp();
+                    if (lane == 0) t6_mbar_arrive(b_empty + bs);   // the weight stage may be overwritten
+                    if (loader) load_next();                        // ... with the stage two ahead
+                    __syncwarp();
                 }
-                t6_commit(a_empty + st);              // ... and so may the slab
-                t6_commit(acc_full + acc);            // ... and the partial sum is complete
+                if (lane == 0) t6_mbar_arrive(a_empty + st);       // ... and so may the slab
+#pragma unroll
+                for (int j = 0; j < N / 2; ++j) accr[j] += acc[j];  // round-to-nearest fp32 adds
             }
-        }
-    } else {
-        // ================= epilogue warps 5-8: flush partial sums, then bias / residual / store =================
-        const int quarter = warp & 3;                 // TMEM lanes [32*quarter, +32) are the ones this warp may read
-        int G = 0;
-        for (int tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) {
-        const int t0 = (tile % p.t_tiles) * T6_M, co0 = ((tile / p.t_tiles) % p.n_co) * N, b = tile / (p.t_tiles * p.n_co);
-        const int t = t0 + quarter * 32 + lane;
-        float accr[N];
+            // thread (warp w of the warpgroup, lane l): time steps 64 wg + 16 w + l / 4 (+ 8), channels 8 j + 2 (l % 4) (+ 1)
+            const int tr = t0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
 #pragma unroll
-        for (int j = 0; j < N; ++j) accr[j] = 0.f;
-        for (int cg = 0; cg < p.n_cg; ++cg, ++G) {
-            const int acc = G & 1;
-            t6_mbar_wait(acc_full + acc, (G >> 1) & 1);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll
-            for (int c0 = 0; c0 < N; c0 += 16) {
-                uint32_t v[16];
-                const uint32_t taddr = tmem + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * N + c0);
-                asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                             : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-                               "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-                             : "r"(taddr));
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-                for (int j = 0; j < 16; ++j) accr[c0 + j] += __uint_as_float(v[j]);   // round-to-nearest fp32 adds
-            }
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            __syncwarp();
-            if (lane == 0) t6_mbar_arrive(acc_empty + acc);
-        }
-        if (t < p.t_out) {
-#pragma unroll
-            for (int j = 0; j < N; ++j) {
-                const int co = co0 + j;
-                if (co < p.c_out) {
+            for (int j = 0; j < N / 2; ++j) {
+                const int t = tr + ((j >> 1) & 1) * 8, co = co0 + (j >> 2) * 8 + (lane & 3) * 2 + (j & 1);
+                if (t < p.t_out && co < p.c_out) {
                     const size_t o = ((size_t)b * p.c_out + co) * p.t_out + t;
                     float yv = accr[j] + (p.bias ? p.bias[co] : 0.f);
                     if (p.res) yv += p.res[o];
                     p.y[o] = yv;
                 }
             }
-        }
         }   // tiles
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 4) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "n"(2 * N) : "memory");
 }
 
 template <int N, int NV, int DEPTH>
@@ -1572,9 +1466,9 @@ static int launch_t6_one(const T6Params& q, int batch, cudaStream_t s) {
     ACB_CHECK_CUDA(cudaFuncSetAttribute(conv1d_t6_kernel<N, NV, DEPTH>, cudaFuncAttributeMaxDynamicSharedMemorySize, L.total));
     T6Params r = q;
     r.t_tiles = acb_ceil_div(q.t_out, T6_M); r.n_co = q.c_out / N; r.n_tiles = r.t_tiles * r.n_co * batch;
-    int dev = 0, sms = 148;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    int dev = 0, sms = 0;
+    ACB_CHECK_CUDA(cudaGetDevice(&dev));
+    ACB_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     conv1d_t6_kernel<N, NV, DEPTH><<<dim3(min(r.n_tiles, sms)), T6_THREADS, (size_t)L.total, s>>>(r);
     ACB_LAUNCH_CHECK();
     return ACB_OK;
@@ -1714,8 +1608,8 @@ extern "C" int acb_conv1d(const float* x, const float* w_packed, const float* bi
     ACB_REQUIRE(precision >= ACB_CONV_FP32 && precision <= ACB_CONV_TF32X3_MMASYNC, "acb_conv1d: unknown precision %d", precision);
     if ((precision == ACB_CONV_TF32X3 || precision == ACB_CONV_TF32X3_MMASYNC) && c_out >= 32 && c_in * kernel >= 16 &&
         kernel <= T5_RC) {
-        // tcgen05 pays a fixed im2col-tile build per 32 reduction rows: it wins once the tile has >= 128 output channels
-        // to amortise it over; narrower layers are faster on the mma.sync kernel (profiles/r1_perf_encodec_v4*.log)
+        // the tensor-core kernel pays a fixed im2col-tile build per 32 reduction rows: it wins once the tile has >= 128 output channels
+        // to amortise it over; narrower layers go to the mma.sync kernel
         if (precision == ACB_CONV_TF32X3 && c_out >= 128 && c_in * kernel >= 128) return launch_conv1d_t5(p, batch, s);
         return launch_conv1d_tc(p, batch, s);
     }
@@ -1984,7 +1878,7 @@ __global__ void __launch_bounds__(256) lstm_kernel(LstmParams p) {
 // * thread (unit u = tid / 32, item b = tid % 32) owns one cell: its c_t stays in a register for the whole sequence, it adds the
 //   input half of the gates (requested one step ahead), applies the nonlinearities and writes h_t (fragment order) and y.
 // * one grid barrier per step (release arrive / acquire poll), h double-buffered.
-// The fp32 FMA kernel above measures 18.2 us per step at H = 1024 (two 16-item passes, each: stage 64 KB of h, 2 048 FFMA per thread,
+// The fp32 FMA kernel above makes two 16-item passes per step at H = 1024 (each: stage 64 KB of h, 2 048 FFMA per thread,
 // transposing reduction); this one reads h once and does the arithmetic on the tensor pipe.
 // ------------------------------------------------------------------------------------------------
 constexpr int LTC_U = 8, LTC_ROWS = 4 * LTC_U, LTC_B = 32, LTC_NW = 8, LTC_PB = 4;   // 8 warps; B fragments of LTC_PB k-steps requested together
@@ -2035,11 +1929,9 @@ __global__ void __launch_bounds__(LTC_NW * 32, 1) lstm_tc_kernel(LstmParams p) {
 #pragma unroll
                 for (int j = 0; j < 4; ++j) acc[i][j][0] = acc[i][j][1] = acc[i][j][2] = acc[i][j][3] = 0.f;
             const float4* hf4 = reinterpret_cast<const float4*>(hprev);
-            // B fragments are requested LTC_PB k-steps at a time.  Measured per LSTM block (2 layers x 500 steps, H = 1024, 32 items):
-            // 8 warps x 4 k-steps 14.5 ms; 8 warps, all 16 k-steps up front (255 registers) 16.1 ms; 16 warps x all 8 k-steps (128
-            // registers, spills) 17.2 ms; two alternating 16-item halves with their own barriers (barrier and h round trip off the
-            // critical path, but the W_hh split done twice per step) 16.0 ms; fp32 FMA kernel 18.3 ms (profiles/r2_perf_encodec_v3*.log,
-            // v4*.log, v8*.log).  ncu: issue-latency bound (two warps per scheduler, 32 % of the stall samples `wait`, 5 % `math`).
+            // B fragments are requested LTC_PB k-steps at a time (8 warps x 4 k-steps): all k-steps up front needs 255 registers,
+            // 16 warps spill, and two alternating item halves split W_hh twice per step; each of those was measured slower on the
+            // previous GPU generation (not re-measured on the H100).
 #pragma unroll 1
             for (int s0 = 0; s0 < ksteps; s0 += LTC_PB) {
                 float4 b0[LTC_PB], b1[LTC_PB];
@@ -2142,7 +2034,7 @@ __device__ __forceinline__ void split_h2(float v, __half& hi, __half& lo) {
     hi = __float2half_rn(v);
     lo = __float2half_rn((v - __half2float(hi)) * 2048.f);
 }
-constexpr int LH2_PB = 4;   // k16 steps of B fragments requested together (all 8 at once, 254 registers: 12.4 vs 11.5 ms per LSTM block)
+constexpr int LH2_PB = 4;   // k16 steps of B fragments requested together (all 8 at once needs 254 registers and was slower)
 __global__ void __launch_bounds__(LTC_NW * 32, 1) lstm_h2_kernel(LstmParams p) {
     extern __shared__ float smem[];
     const int H = p.H;

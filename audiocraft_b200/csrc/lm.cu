@@ -1,4 +1,4 @@
-// MusicGen LM decode step for B200 (sm_100a).
+// MusicGen LM decode step for H100 (sm_90a).
 //
 // One decode step = LMModel.forward on one token per row (audiocraft/models/lm.py:221-268) + CFG mix + sampling
 // (lm.py:393-418) + the delay-pattern write-back (lm.py:553-562), replayed as ONE CUDA graph per step with every
@@ -45,8 +45,7 @@ __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;"
 
 // Debug timeline: thread 0 of every CTA writes %globaltimer (ns) into its 8-slot record.  Compiled in only with
 // -DACB_TIMELINE (ACB_BUILD_TIMELINE=1 python -m audiocraft_b200.build) and armed with ACB_LM_TIMING=1: at this time
-// scale even the dormant stamps cost (532 kernels x ~0.3 us measured), because every instruction line of a 3 us kernel is
-// fetched cold.
+// scale even dormant stamps cost time, because every instruction line of a few-microsecond kernel is fetched cold.
 #ifdef ACB_TIMELINE
 __device__ __forceinline__ void tl_stamp(unsigned long long* t, int slot) {
     if (t && threadIdx.x == 0) {
@@ -133,8 +132,7 @@ __global__ void __launch_bounds__(256) lm_embed_kernel(const __half* __restrict_
 // ------------------------------------------------------------------------------------------------ residual + LN
 // x[r] += sum_s part[s][r] (fixed order), then h16[r] = LayerNorm(x[r]) * gamma + beta  (eps 1e-5, fp32 statistics).
 // One CTA per row, ONE float4 per thread (d <= 2048): no per-thread loops, so the kernel is ~300 instructions -- at this
-// time scale cold instruction fetch is a first-order cost (the 4-float4-per-thread version was 1 048 instructions and
-// spent 1-2 us before its first load was consumed).  gamma / beta do not depend on the previous kernel and are
+// time scale cold instruction fetch is a first-order cost (a 4-float4-per-thread version was over 1 000 instructions).  gamma / beta do not depend on the previous kernel and are
 // requested before griddepcontrol.wait.
 constexpr int LN_THREADS = 512;
 __global__ void __launch_bounds__(LN_THREADS) lm_ln_kernel(float* __restrict__ x, const float* __restrict__ part, int nsplit,
@@ -202,12 +200,10 @@ struct GemmParams {
 };
 
 // CTA = 4 warps, tile = 16 output features x kslice of K.  The CTA's 16 x kslice weight slab is fetched by ONE thread
-// with 16 TMA bulk copies (one per W row, padded pitch => conflict-free fragment reads) BEFORE griddepcontrol.wait, i.e.
-// while the producer of the activations is still running: under PDL the weight stream of kernel n+1 overlaps kernel n.
+// with 16 TMA bulk copies (one per W row, padded pitch => conflict-free fragment reads) before griddepcontrol.wait (a no-op:
+// the step graph uses plain edges, see acb_lm_begin).
 // FT2 = feature tiles of 16 per CTA.  FT2 = 2 (opt-in per GEMM, see pick_ft2) halves the number of CTAs and therefore
-// the activation traffic out of L2: every CTA re-reads the whole 16 x K activation block, and the in-kernel timeline
-// (profiles/r1_lm_timeline_layer0_kv1_fine.log) shows the k-loop of the big GEMMs bound by exactly that (14 MB of
-// activation reads per 14 MB weight matrix; ~0.8 us per dependent batch of loads).
+// the activation traffic out of L2: every CTA re-reads the whole 16 x K activation block, as many bytes as the weights.
 template <int NT, int EPI, int FT2 = 1>
 __global__ void __launch_bounds__(128) lm_gemm_kernel(GemmParams p) {
 #ifndef ACB_GEMM_U2
@@ -348,8 +344,7 @@ struct AttnParams {
 // Self attention for one query token: CTA = (row, head[, KV third]), 8 warps, ONE pass over K and V with an online softmax.
 // A warp instruction reads 4 consecutive cache positions (4 x 128 B = 512 contiguous bytes); 8 lanes share a position
 // (8 dims each).  4 positions-groups x 4 unrolled iterations of K and V are in flight per lane before any is consumed.
-// Split KV (gridDim.z = 3, opt-in: ACB_LM_ATT_SPLIT=3): rows x heads = 384 CTAs are 2.6 per SM, so SMs holding 3 finish ~25 % after those holding 2
-// (timeline at KV 751: median CTA 16.7 us, last 22.3 us).  Once the context reaches split_min positions it is cut into
+// Split KV (gridDim.z = 3, opt-in: ACB_LM_ATT_SPLIT=3): rows x heads = 384 CTAs are 2.6 per SM, so SMs holding 3 finish well after those holding 2.  Once the context reaches split_min positions it is cut into
 // up to 3 chunks (multiples of the CTA's 128-position stride): 1 152 CTAs = 7.8 per SM.  Every chunk CTA writes its
 // (m, l, acc) record, and the LAST one to arrive (atomic counter, threadfence) merges the records in chunk order, so the
 // result does not depend on arrival order.  Short contexts take the single-CTA path; the idle CTAs exit at once.
@@ -381,8 +376,7 @@ __global__ void __launch_bounds__(ATT_WARPS * 32) lm_attn_kernel(AttnParams p) {
     const int n = p.fixed_len > 0 ? p.fixed_len : p.pos[0] + tok + 1;
     int lo = 0, hi = n, nact = 1;
     if (SPLIT && gridDim.z > 1) {
-        // measured: the record write + atomic + merge costs more than the balance gains below ~750 positions
-        // (KV 376: 2.71 vs 2.57 ms per step; KV 751: equal; KV 1500: 3.62 vs 3.80), hence split_min (default 768)
+        // the record write + atomic + merge costs more than the balance gains at short contexts, hence split_min (default 768)
         const int S = gridDim.z, chunk = n < p.split_min ? n : max(128, ((n + S - 1) / S + 127) & ~127);
         nact = (n + chunk - 1) / chunk;
         if ((int)blockIdx.z >= nact) return;         // CTA-uniform: nothing in this chunk
@@ -514,14 +508,13 @@ __global__ void __launch_bounds__(ATT_WARPS * 32) lm_attn_kernel(AttnParams p) {
     tl_stamp(p.timing, 3);
 }
 
-// Self attention for one query token, deep-prefetch variant (the default decode path since round 2; ACB_LM_ATTN=v1 keeps the kernel
+// Self attention for one query token, deep-prefetch variant (the default decode path; ACB_LM_ATTN=v1 keeps the kernel
 // above, which also serves prefill and split-KV).  Same work split and arithmetic as lm_attn_kernel<false>: CTA = (row, head), 8 warps,
 // a warp instruction covers 4 consecutive cache positions, 8 lanes share a position.  What changes is how K and V get there: every lane
 // copies its 16-byte slices with cp.async into a private slot of a per-warp shared-memory ring, ATT2_DEPTH iterations deep, and reads
-// them back (its own 32 bytes) one iteration at a time.  With register loads a lane had 128 bytes in flight in bursts (4 iterations
-// requested, then all consumed): ~83 KB per SM at 2.6 CTAs per SM, against the ~13 MB that 6.5 TB/s x ~2 us of loaded HBM latency asks
-// of the chip (88 KB per SM): 4.05 TB/s at KV 751.  The ring keeps up to 8 x 32 bytes per lane outstanding continuously, in shared
-// memory instead of registers.
+// them back (its own 32 bytes) one iteration at a time.  With register loads a lane has 128 bytes in flight in bursts (4 iterations
+// requested, then all consumed), less than HBM bandwidth x loaded latency asks of an SM.  The ring keeps up to 8 x 32 bytes per lane
+// outstanding continuously, in shared memory instead of registers.
 constexpr int ATT2_DEPTH = 8;
 __global__ void __launch_bounds__(ATT_WARPS * 32) lm_attn2_kernel(AttnParams p) {
     extern __shared__ __align__(16) unsigned char att2sm[];   // [warp][depth][K | V][32 lanes][16 B]
@@ -921,10 +914,10 @@ struct acb_lm {
     cudaStream_t capture_stream = nullptr;
     cudaGraph_t graph = nullptr;
     cudaGraphExec_t exec = nullptr;
-    int batch = 0, rows = 0, rows_pad = 0, text_len = 0, seq_len = 0, sms = 148;
+    int batch = 0, rows = 0, rows_pad = 0, text_len = 0, seq_len = 0, sms = 132;
     int launches = 0;
     bool has_cross = false;
-    bool pdl = true;          // programmatic dependent launch between the kernels of a step
+    bool pdl = false;         // programmatic dependent launch between the kernels of a step (never enabled: see acb_lm_begin)
     bool attn2 = true;        // deep-prefetch self attention (cp.async ring); ACB_LM_ATTN=v1: register loads
     bool fused = false;       // ACB_LM_STEP=fused / rotary positions: the whole transformer of a step is ONE persistent kernel (lm_step.cu)
     StepLaunch step{};
@@ -1089,14 +1082,10 @@ static int enqueue_step_kernels(acb_lm* lm, cudaStream_t s, float* logits_out, i
         ++nl;
         DBG("lm_embed_kernel", -1);
     }
-    // (An L2 prefetch chain -- every GEMM pulling the NEXT GEMM's weights into L2 with cp.async.bulk.prefetch.L2 -- was
-    //  built and measured: 2.240 vs 2.258 ms per step, i.e. nothing: under PDL the weight slab is already in flight before
-    //  the dependency resolves, weights are not on the critical path.  profiles/r1_perf_step_v5_l2prefetch_no_gain.log)
     enum { G_QKV, G_O, G_CQ, G_CO, G_FF1, G_FF2, G_HEADS };
     // split-KV self attention: records and counters live in the (otherwise chain-mode-only) plan buffer
-    // OFF by default (ACB_LM_ATT_SPLIT=3 enables): measured on the 30 s workload it gains 2.8 % per step at KV 1500 and
-    // 0.5 % at 1126 but the 768 extra (idle) CTAs per launch and the larger kernel cost 1-4 % per step below ~800
-    // positions -- 53.0 vs 54.1 audio-s/s over the whole generation (profiles/r1_perf_step_v8_splitkv_*.log).
+    // OFF by default (ACB_LM_ATT_SPLIT=3 enables): it only pays at the longest contexts, while its extra (idle) CTAs per
+    // launch cost every shorter step (measured on the previous GPU generation; not re-measured on the H100).
     int att_split = env_int("ACB_LM_ATT_SPLIT", 1);
     if (att_split < 1 || att_split > 8 || !B.plan ||
         ACB_PLAN_COUNTER_BYTES + (size_t)rows * H * att_split * 66 * sizeof(float) > ACB_LM_PLAN_BYTES ||
@@ -1359,10 +1348,12 @@ extern "C" int acb_lm_begin(acb_lm_t* lm, const float* cross, int batch, int row
         if (smem > 48 * 1024)
             ACB_CHECK_CUDA(cudaFuncSetAttribute(lm_sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     }
-    // capture one decode step (with programmatic dependent launch edges; plain edges if the driver refuses them)
+    // capture one decode step with plain stream-order edges.  Launched with programmatic dependent launch (griddepcontrol) the
+    // same kernels reproducibly returned wrong logits on the H100 once the KV cache held more than a few positions, for a cause
+    // not found; there is no switch to turn it on, so every launch goes through the configuration the parity tests pass.
+    // (griddepcontrol.launch_dependents / .wait in the kernels are no-ops for a normally launched kernel.)
     {
-        const char* e = getenv("ACB_NO_PDL");
-        lm->pdl = !(e && e[0] == '1');
+        lm->pdl = false;
         if (env_int("ACB_LM_TIMING", 0) && !lm->timing) {
             ACB_CHECK_CUDA(cudaMalloc(&lm->timing, (size_t)ACB_TIMING_MAX_GEMMS * ACB_TIMING_MAX_CTAS * 64));
             ACB_CHECK_CUDA(cudaMemset(lm->timing, 0, (size_t)ACB_TIMING_MAX_GEMMS * ACB_TIMING_MAX_CTAS * 64));
@@ -1373,8 +1364,7 @@ extern "C" int acb_lm_begin(acb_lm_t* lm, const float* cross, int batch, int row
         }
         const char* ev = getenv("ACB_LM_STEP");
         // The persistent fused step (lm_step.cu; needs the packed weights) is OPT-IN: ACB_LM_STEP=fused, or a model with rotary
-        // positions (only built there).  Measured 3.1 ms vs 2.03 ms per step at KV length 1 for the per-phase graph below
-        // (DESIGN.md section 3.1: ~2.3 us of grid barrier + skew per phase against 0.9 us per PDL kernel boundary).
+        // positions (only built there); the per-phase graph below is the default.
         lm->fused = lm->w.wp_qkv != nullptr && ((ev && ev[0] == 'f') || c.positional_embedding != 0);
         ACB_REQUIRE(c.positional_embedding == 0 || lm->fused, "acb_lm_begin: rotary positions are built in the fused decode step only");
         if (lm->fused) {
@@ -1413,11 +1403,8 @@ extern "C" int acb_lm_begin(acb_lm_t* lm, const float* cross, int batch, int row
         cudaGetLastError();
         drop_graph(lm);
         if (lm->fused && lm->step.cooperative && attempt == 0) { lm->step.cooperative = false; continue; }   // plain launch (grid = #SMs is co-resident anyway)
-        if (!lm->pdl || attempt == 1) {
-            if (rc == ACB_OK) acb_set_error("acb_lm_begin: graph capture failed: %s", cudaGetErrorString(e));
-            return rc != ACB_OK ? rc : ACB_ERR_CUDA;
-        }
-        lm->pdl = false;   // retry without programmatic edges
+        if (rc == ACB_OK) acb_set_error("acb_lm_begin: graph capture failed: %s", cudaGetErrorString(e));
+        return rc != ACB_OK ? rc : ACB_ERR_CUDA;
     }
     return ACB_OK;
 }

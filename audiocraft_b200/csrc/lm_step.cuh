@@ -16,7 +16,7 @@ struct StepGemm {
 
 struct StepParams {
     int d, H, L, ffn, n_q, card, rows, R, batch, has_cross, text_len, max_seq, max_text, max_rows;
-    int n_stage, act_bytes, tmem_cols;
+    int n_stage, act_bytes;
     float pos_scale, attn_scale;
     const __half* emb; const float* inv_freq; const float* ln; const float* out_norm;
     StepGemm g[ACB_STEP_GEMMS];

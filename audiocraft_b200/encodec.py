@@ -1,4 +1,4 @@
-"""EnCodec on B200: host-side mirror of ``audiocraft.models.encodec`` over the C-ABI kernels.
+"""EnCodec on H100: host-side mirror of ``audiocraft.models.encodec`` over the C-ABI kernels.
 
 ``CompressionModel`` keeps the reference's abstract surface (audiocraft/models/encodec.py:28-122);
 ``EncodecModel`` keeps ``encode / decode / decode_latent / preprocess / postprocess`` and the properties
@@ -125,7 +125,7 @@ def tf32_round(x: torch.Tensor) -> torch.Tensor:
 def pack_conv_t6(w: torch.Tensor, tile: int) -> torch.Tensor:
     """Weights [c_out][c_in][K] (weight-norm folded) -> the operand layout of the experimental `acb_conv1d_t6`:
     two tf32 terms (hi, lo = tf32(w - hi)) as [c_out/tile][c_in/8][K][term][2][tile][4]: per (tile, 8-channel group, tap)
-    a K-major UMMA B operand (rows = output channels at 16 B pitch, two 4-channel chunks tile*16 B apart)."""
+    a K-major wgmma B operand (rows = output channels at 16 B pitch, two 4-channel chunks tile*16 B apart)."""
     co, ci, K = w.shape
     assert co % tile == 0 and ci % 8 == 0, (w.shape, tile)
     hi = tf32_round(w.float())
@@ -135,21 +135,21 @@ def pack_conv_t6(w: torch.Tensor, tile: int) -> torch.Tensor:
 
 
 class EncodecModel(CompressionModel):
-    """EnCodec (SEANet + RVQ) on B200 behind the reference's ``EncodecModel`` API."""
+    """EnCodec (SEANet + RVQ) on H100 behind the reference's ``EncodecModel`` API."""
 
     def __init__(self, state_dict: tp.Dict[str, torch.Tensor], cfg: dict, device='cuda',
                  encoder_precision: str = 'fp32_tc', decoder_precision: str = 'tf32x3'):
         """encoder_precision / decoder_precision:
           'fp32'         every convolution on fp32 FMA;
           'fp32_tc'      (encoder default) fp32 ACCURACY on the tensor cores: layers with kernel > 1 and >= 128 output channels
-                         run `acb_conv1d_t6` (tcgen05, 3xTF32 operand split, the TMEM accumulator flushed into fp32 registers
-                         every 8 input channels), the rest fp32 FMA.  Latents within 3.0e-6 of the fp32 reference on the 24 /
-                         32 kHz architectures (all-FMA: 3.6e-6), RVQ indices exact (profiles/r2_t6_first_hardware_contact_*.log);
+                         run `acb_conv1d_t6` (wgmma, 3xTF32 operand split, the tensor-core accumulator flushed into fp32 registers
+                         every 8 input channels), the rest fp32 FMA.  RVQ indices equal the fp32 reference's on the 24 / 32 kHz
+                         goldens (tests/test_gpu_fullsize.py);
                          Residual blocks with the identity skip at 64 / 128 / 256 channels run as ONE kernel (`acb_resblock`, both
                          operands split into two fp16 terms = 22 mantissa bits, tensor-core accumulation runs cut every 48 / 16
                          reduction rows) in every precision except 'fp32'; the LSTM's recurrent step uses the same split;
           'tf32x3_flush' the same kernel on every layer it supports (slower on 1x1 convolutions; kept for tests);
-          'tf32x3'       (decoder default, NOT fp32-exact) tcgen05 3xTF32 without flushes: the decoder's output is a waveform
+          'tf32x3'       (decoder default, NOT fp32-exact) wgmma 3xTF32 without flushes: the decoder's output is a waveform
                          checked to a tolerance of 1e-4 (DESIGN.md section 4); as an encoder mode its latents move by 1.5e-4."""
         self.device = _lib.require_cuda(device)
         prec = {'fp32': _lib.CONV_FP32, 'tf32x3': _lib.CONV_TF32X3, 'tf32x3_mmasync': _lib.CONV_TF32X3_MMASYNC,
@@ -213,7 +213,7 @@ class EncodecModel(CompressionModel):
             out['w'] = w.permute(0, 2, 1).contiguous()                  # [Cin][K][Cout]
             cin, cout, k = w.shape
             S = layer['stride']
-            # GEMM operand of the tcgen05 path: [2*Cin][Cout*S], row (ci, k'), column co*S + ph, value w[ci][co][ph + (1-k')*S]
+            # GEMM operand of the tensor-core path: [2*Cin][Cout*S], row (ci, k'), column co*S + ph, value w[ci][co][ph + (1-k')*S]
             out['w_gemm'] = w.view(cin, cout, 2, S).flip(2).permute(0, 2, 1, 3).reshape(cin * 2, cout * S).contiguous()
             out['b'] = sd[p + 'bias'].to(self.device, torch.float32).contiguous()
         else:
@@ -237,8 +237,8 @@ class EncodecModel(CompressionModel):
         left, t_virt, t_out = conv_geometry(T, k, stride, dilation, self.causal, bool(self.reflect))
         y = torch.empty((B, cout, t_out), device=x.device, dtype=torch.float32)
         if prec == _lib.CONV_T6_AUTO:
-            # measured per layer on 32 x 10 s (profiles/r2_perf_encodec_t6_all_layers.log vs r1_perf_encodec_v5_t5pipelined.log):
-            # the implicit-GEMM tcgen05 kernel wins for k > 1 with >= 128 output channels (1.5-4x), loses on 1x1 convolutions
+            # the implicit-GEMM tensor-core kernel is for k > 1 with >= 128 output channels: a 1x1 convolution gives it too little
+            # reduction per staged slab (a routing choice made on the previous GPU generation, not re-measured per layer on the H100)
             prec = _lib.CONV_T6_FLUSH if (k > 1 and cout >= 128) else _lib.CONV_FP32
         if prec == _lib.CONV_T6_FLUSH:
             if w is None and 'w6' in L and cout == L['cout']:
@@ -616,7 +616,7 @@ def hf_encodec_to_reference(hf_state_dict: tp.Dict[str, torch.Tensor], hf_config
 
 
 class HFEncodecCompressionModel(EncodecModel):
-    """`facebook/encodec_*` checkpoints on the B200 kernels: same surface as the reference's wrapper
+    """`facebook/encodec_*` checkpoints on the CUDA kernels: same surface as the reference's wrapper
     (audiocraft/models/encodec.py:323-392), incl. the restriction of `set_num_codebooks` to the bandwidths the
     checkpoint declares."""
 

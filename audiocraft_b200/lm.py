@@ -1,4 +1,4 @@
-"""MusicGen LM on B200: host-side mirror of ``audiocraft.models.lm.LMModel`` over the C-ABI decode kernels.
+"""MusicGen LM on H100: host-side mirror of ``audiocraft.models.lm.LMModel`` over the C-ABI decode kernels.
 
 Keeps ``LMModel.generate``'s signature and semantics (audiocraft/models/lm.py:420-587) and the attributes its callers
 read (``condition_provider, fuser, card, n_q, num_codebooks, special_token_id, cfg_coef``), but the hot loop

@@ -78,7 +78,7 @@ def lm_cfg_from_xp(xp: dict) -> dict:
     if fz.get('cross_attention_pos_emb', False):
         unsupported.append('fuser.cross_attention_pos_emb')
     if unsupported:
-        raise NotImplementedError("this checkpoint's LM is outside what the B200 decode kernels implement: " + ', '.join(unsupported))
+        raise NotImplementedError("this checkpoint's LM is outside what the decode kernels implement: " + ', '.join(unsupported))
     cond_dim = None
     desc = xp.get('conditioners', {}).get('description')
     if desc is not None:

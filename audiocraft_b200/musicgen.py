@@ -1,4 +1,4 @@
-"""Generation API on B200: `MusicGen` / `AudioGen` with the reference's public surface.
+"""Generation API on H100: `MusicGen` / `AudioGen` with the reference's public surface.
 
 Behavioural contract (what callers of `audiocraft.models.MusicGen` / `AudioGen` / `BaseGenModel` rely on,
 audiocraft/models/genmodel.py:28-267, musicgen.py:41-338, audiogen.py:23-93):
@@ -167,10 +167,10 @@ class MusicGen(BaseGenModel):
         self.generation_params['cfg_coef_beta'] = cfg_coef_beta
 
     def set_style_conditioner_params(self, *args, **kwargs):
-        raise NotImplementedError("MusicGen-Style conditioning is not built on the B200 path (SURVEY.md 8f.3)")
+        raise NotImplementedError("MusicGen-Style conditioning is not built on this path (SURVEY.md 8f.3)")
 
     def generate_with_chroma(self, *args, **kwargs):
-        raise NotImplementedError("melody (chroma) conditioning is not built on the B200 path (SURVEY.md 8f.3)")
+        raise NotImplementedError("melody (chroma) conditioning is not built on this path (SURVEY.md 8f.3)")
 
 
 class AudioGen(BaseGenModel):

@@ -4,7 +4,7 @@ There are no pretrained checkpoints (and no network) in the build or GPU image, 
 and bench.py use random-init weights of the named architectures.  Keys and shapes follow the
 reference checkpoints (SURVEY.md section 8b; audiocraft/models/loaders.py:78-126 consumes
 ``best_state`` dicts with exactly this layout), so the same dict loads into the reference modules,
-the CPU oracle and the B200 models.
+the CPU oracle and the CUDA models.
 
 Hyper-parameters restate the reference config tree (read-only source of shapes):
   config/model/encodec/default.yaml + encodec_large_nq4_s640.yaml / encodec_base_causal.yaml,

@@ -1,8 +1,8 @@
 """bench.py -- MusicGen-medium text-conditioned 30 s generation, batch 8 per GPU (BASELINE.json configs[2]), the
-configuration the headline metric `audio-sec/sec` is quoted on; it fits one B200.
+configuration the headline metric `audio-sec/sec` is quoted on; it fits one H100 (80 GB).
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--duration 30] [--batch 8]
-                  [--scaling weak|strong] [--scale small|medium|large] [--workload musicgen|encodec]
+                  [--scaling weak|strong] [--scale small|medium|large] [--workload musicgen|encodec] [--dump-outputs DIR]
   torchrun --nproc-per-node N bench.py --gpus N ...
 
 Defaults = BASELINE configs[2] with `--batch` items PER GPU (`scaling: weak`, as the contract prescribes for a path that shards
@@ -17,8 +17,13 @@ inputs (condition tensors) resident in HBM.  `e2e` = the same through the public
 with host inputs (text-encoder states pinned on the host, copied inside the timed region) and the waveform read back.
 Weights are seeded random (no checkpoints offline), inputs synthetic.
 
+`--dump-outputs DIR` writes what the last timed step computed, as float32 `DIR/<name>.npy` (musicgen: `tokens` [B, K, T] and
+`wav` [B, 1, samples]; encodec: `codes` and `wav`).  Weights, inputs and sampling seeds are fixed, so two builds run with the
+same arguments can be compared output for output.  Arrays beyond 64 MB in all are replaced by a fixed, seeded sample of
+their flattened elements (`<name>.npy` holds the values, `<name>_index.npy` their flat indices).
+
 `--impl reference` times the reference's OWN code on the box's host cores: the unmodified package installed under
-baseline/_ref (baseline/install_ref.sh; it ships with the snapshot), driven through oracle/ref_import.py's third-party
+baseline/_ref (baseline/install_ref.sh), driven through oracle/ref_import.py's third-party
 stubs by baseline/reference_arm.py.  One "step" of that arm is one bounded sample of the same workload (a few decode
 steps of LMModel.generate's loop at KV length 1 and at the final KV length + the EnCodec decode of 1 s of tokens),
 integrated to the full pass; `ms_per_step` is the sample's wall time.  The b200 line carries the same measurement as
@@ -47,11 +52,31 @@ def peaks():
     if os.path.exists(p):
         j = json.load(open(p))
         return dict(hbm_gbs=j['hbm_gbs'], source='measured (MEASURED_PEAKS.json)')
-    return dict(hbm_gbs=6650.0, source='fallback (B200_PROFILING.md)')
+    return dict(hbm_gbs=3350.0, source='H100 SXM data sheet (HBM3, 3.35 TB/s)')
+
+
+DUMP_LIMIT = 64_000_000   # bytes --dump-outputs writes at most (64 MB)
+
+
+def dump_outputs(out_dir, arrays):
+    """Write {name: tensor} as float32 .npy files; beyond DUMP_LIMIT in all, a seeded sample of each array's elements."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {k: v.detach().float().cpu().contiguous() for k, v in arrays.items()}
+    elems = sum(v.numel() for v in arrays.values())
+    for name, v in arrays.items():
+        if elems * 4 <= DUMP_LIMIT:
+            np.save(os.path.join(out_dir, f'{name}.npy'), v.numpy())
+            continue
+        # a kept element costs 12 bytes: its float32 value and its flat index stored as float64
+        n = max(1, v.numel() * (DUMP_LIMIT - 4096 * len(arrays)) // (elems * 12))   # 4096: .npy headers
+        idx = torch.randperm(v.numel(), generator=torch.Generator().manual_seed(0))[:n].sort().values
+        np.save(os.path.join(out_dir, f'{name}.npy'), v.view(-1)[idx].numpy())
+        np.save(os.path.join(out_dir, f'{name}_index.npy'), idx.numpy().astype(np.float64))
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (recipe in B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
 
     def __init__(self, index: int):
         self.index, self.rows, self.proc = index, [], None
@@ -118,13 +143,13 @@ def encodec_roofline(samples: int, ms: float):
     output once (fp32, ELU / residual / padding fused) and 486 kFLOP/sample.  With tensor-core convolutions the per-layer design
     is HBM-bound (101 FLOP/B < the ridge), so the HBM figure is the binding one; the tensor figure is reported beside it."""
     pj = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json'))) if os.path.exists(os.path.join(ROOT, 'MEASURED_PEAKS.json')) else {}
-    hbm = pj.get('hbm_gbs', 6650.0)
-    tf = pj.get('bf16_tflops_sustained', 1400.0)
+    hbm = pj.get('hbm_gbs', 3350.0)                   # H100 SXM data sheet: HBM3 3.35 TB/s, dense BF16 989 TFLOP/s
+    tf = pj.get('bf16_tflops_sustained', 989.0)
     gbs = samples * 4822 / (ms / 1e3) / 1e9
     tfl = samples * 486e3 / (ms / 1e3) / 1e12
     return dict(bound='hbm', achieved=round(gbs, 1), peak=hbm, unit='GB/s', frac=round(gbs / hbm, 4), traffic=None,
-                algorithmic_bytes_per_sample=4822, peak_source='measured (MEASURED_PEAKS.json)' if pj else 'fallback (B200_PROFILING.md)',
-                tensor=dict(achieved=round(tfl, 2), peak=tf, unit='TFLOP/s (fp32-equivalent work vs the measured dense bf16 peak)',
+                algorithmic_bytes_per_sample=4822, peak_source='measured (MEASURED_PEAKS.json)' if pj else 'H100 SXM data sheet',
+                tensor=dict(achieved=round(tfl, 2), peak=tf, unit='TFLOP/s (fp32-equivalent work vs the dense bf16 peak)',
                             frac=round(tfl / tf, 4), flop_per_sample=486000))
 
 
@@ -154,7 +179,7 @@ def run_encodec(args):
         outs = []
         for i in range(0, B, CH):
             codes, scale = cm.encode(x_dev[i:i + CH])
-            outs.append(cm.decode(codes, scale))
+            outs.append((codes, cm.decode(codes, scale)))
         return outs
 
     def step_e2e():
@@ -194,8 +219,10 @@ def run_encodec(args):
         step_device()
         launches = cm.launches - l0
     with ClockSampler(torch.cuda.current_device()) as clk:
-        ms, _ = timed(step_device, args.steps)
+        ms, outs = timed(step_device, args.steps)
     clocks = clk.summary()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, dict(codes=torch.cat([c for c, _ in outs]), wav=torch.cat([w for _, w in outs])))
     ms_e2e, _ = timed(step_e2e, max(1, min(args.steps, 3)))
     n_e2e = max(1, min(args.steps, 3))
     samples_step = total_items * n_samp
@@ -210,7 +237,7 @@ def run_encodec(args):
                   steps=args.steps, warmup=args.warmup, ms_per_step=round(ms / args.steps, 2), higher_is_better=True,
                   scaling=args.scaling, vs_baseline=None, dtype='f32', data='synthetic',
                   config=dict(workload=f'EnCodec 32 kHz, 4 codebooks: encode + decode of {total_items} x 10 s mono, {B} items on this rank '
-                                       f'(launch chains of {CH} items); encoder fp32-accurate (index-exact), decoder 3xTF32 on tcgen05',
+                                       f'(launch chains of {CH} items); encoder fp32-accurate (index-exact), decoder 3xTF32 on wgmma',
                               global_batch=total_items, seq_len=n_samp, parallelism=f'dp{world} (items split, no collective)',
                               l2=f'inputs larger than L2: every layer of a {CH}-item chain reads / writes 0.3-2.6 GB'),
                   clocks=clocks,
@@ -277,8 +304,11 @@ def run_b200(args):
     hid, msk = pinned_encoder(descriptions + [""] * B)
     h2d_bytes = hid.numel() * 4 + msk.numel() * 8
 
+    last = {}
+
     def step_device():
         tokens = lm.generate(None, [], num_samples=B, max_gen_len=T, cross_attention_src=cross, **mg.generation_params)
+        last['tokens'] = tokens
         wav = mg.generate_audio(tokens)
         if strong and world > 1:   # configs[2] read literally: one batch over the ranks, the audio gathered on every rank
             from audiocraft_b200.dist import gather_batch
@@ -325,6 +355,8 @@ def run_b200(args):
     with ClockSampler(torch.cuda.current_device()) as clk:
         ms, wav = timed(step_device, args.steps)
     clocks = clk.summary()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, dict(tokens=last['tokens'], wav=wav))
     audio_s = total_items * dur * args.steps
     value = audio_s / (ms / 1e3)
     n_e2e = max(1, min(args.steps, 3))
@@ -336,7 +368,7 @@ def run_b200(args):
     # Fused step: the dominant kernel IS the step (lm_step_kernel, one launch per decode step); its algorithmic bytes depend
     # on the KV length, so it is timed at 5 pinned lengths and the generation is integrated over them (trapezoid).
     # Per-phase path (ACB_LM_STEP=v5): lm_gemm_kernel, one pass = every weight matrix of a step.
-    # Either way one launch / pass streams W_step = 3.2 GB >> 126 MB L2: no L2 reuse between timed launches.
+    # Either way one launch / pass streams W_step = 3.2 GB >> 50 MB L2: no L2 reuse between timed launches.
     rows = 2 * B
     w_step, kv_tok, total_bytes = algorithmic_bytes(lm, rows, S)
     pk = peaks()
@@ -355,7 +387,6 @@ def run_b200(args):
         torch.cuda.synchronize()
         return e0.elapsed_time(e1) / reps
 
-    traffic = None
     step_ms = ms / args.steps / (S - 1)  # whole generate incl. sampler and EnCodec decode, amortised per decode step
     whole = dict(algorithmic_bytes=total_bytes, achieved=round(total_bytes / (ms / args.steps / 1e3) / 1e9, 1),
                  frac=round(total_bytes / (ms / args.steps / 1e3) / 1e9 / pk['hbm_gbs'], 4), ms_per_decode_step=round(step_ms, 4))
@@ -367,28 +398,17 @@ def run_b200(args):
             byt = w_step + rows * (t + 1) * kv_tok + rows * kv_tok
             pts.append(dict(kv_len=t + 1, ms=round(k_ms, 4), algorithmic_bytes=byt, gbs=round(byt / k_ms / 1e6, 1)))
         tot_ms = sum((pts[i]['ms'] + pts[i + 1]['ms']) / 2 * (pts[i + 1]['kv_len'] - pts[i]['kv_len']) for i in range(len(pts) - 1))
-        mid = pts[len(pts) // 2]
         achieved = total_bytes / (tot_ms / 1e3) / 1e9
-        tp = os.path.join(ROOT, 'profiles', 'r2_step_kernel_dram.json')   # ncu --set full capture of lm_step_kernel at KV 752
-        if os.path.exists(tp) and args.scale == 'medium' and B == 8:
-            tj = json.load(open(tp))
-            traffic = int(tj['dram_bytes_read'] + tj['dram_bytes_write'])
         roofline = dict(bound='hbm', kernel='lm_step_kernel', achieved=round(achieved, 1), peak=pk['hbm_gbs'], unit='GB/s',
-                        frac=round(achieved / pk['hbm_gbs'], 4), traffic=traffic, peak_source=pk['source'],
+                        frac=round(achieved / pk['hbm_gbs'], 4), peak_source=pk['source'],
                         how='algorithmic bytes of the S-1 step launches of one generate / their kernel time, the latter integrated '
-                            'from CUDA-event timings of the isolated kernel at the listed KV lengths; traffic = ncu dram bytes of the '
-                            'launch at kv_len ' + str(mid['kv_len']) + ' (algorithmic ' + str(mid['algorithmic_bytes']) + ' B)',
+                            'from CUDA-event timings of the isolated kernel at the listed KV lengths',
                         launches_per_generate=S - 1, kernel_ms_per_generate=round(tot_ms, 2), per_kv=pts, whole_generate=whole)
     else:
         gemm_ms = time_dominant(20)
-        tp = os.path.join(ROOT, 'profiles', 'r2_step_kv751_dram_summary.json')   # ncu launch list + DRAM bytes of the per-phase kernels (round 2)
-        if os.path.exists(tp) and args.scale == 'medium' and B == 8:
-            tj = json.load(open(tp)).get('lm_gemm_kernel')
-            if tj:
-                traffic = int((tj['dram_read_MB'] + tj['dram_write_MB']) * 1e6)
         achieved = w_step / (gemm_ms / 1e3) / 1e9
         roofline = dict(bound='hbm', kernel='lm_gemm_kernel', achieved=round(achieved, 1), peak=pk['hbm_gbs'], unit='GB/s',
-                        frac=round(achieved / pk['hbm_gbs'], 4), traffic=traffic, peak_source=pk['source'],
+                        frac=round(achieved / pk['hbm_gbs'], 4), peak_source=pk['source'],
                         launches_per_pass=nl.value, bytes_per_pass=w_step, ms_per_pass=round(gemm_ms, 4), whole_generate=whole)
 
     # ---- secondary metric: EnCodec 32 kHz encode+decode MSamples/s (BASELINE configs[3] per-GPU slice, 32 x 10 s)
@@ -407,7 +427,7 @@ def run_b200(args):
         torch.cuda.synchronize()
         enc_ms = e0.elapsed_time(e1) / 3
         secondary = dict(metric='EnCodec 32kHz encode+decode MSamples/sec', value=round(xb.numel() / (enc_ms / 1e3) / 1e6, 2),
-                         unit='MSamples/s', config='32 x 10 s mono per GPU; encoder fp32-accurate and index-exact (3xTF32 with bounded tensor-core accumulation runs: conv1d_t6 on tcgen05, fused residual blocks and the LSTM step on mma.sync; fp32 FMA where neither wins), decoder 3xTF32 (tcgen05 convolutions, fused residual blocks)',
+                         unit='MSamples/s', config='32 x 10 s mono per GPU; encoder fp32-accurate and index-exact (3xTF32 with bounded tensor-core accumulation runs: conv1d_t6 on wgmma, fused residual blocks and the LSTM step on mma.sync; fp32 FMA where neither wins), decoder 3xTF32 (wgmma convolutions, fused residual blocks)',
                          ms=round(enc_ms, 2), roofline=encodec_roofline(xb.numel(), enc_ms))
         # throughput mode: the encoder's convolutions on the tensor cores as well (latents within 1.5e-4 of fp32)
         from audiocraft_b200 import synth as _synth
@@ -431,7 +451,7 @@ def run_b200(args):
     cpu_baseline = None
     reference_gpu = None
     if rank == 0 and args.gpus == 1 and not args.no_ref_gpu:
-        # the reference's own CUDA path on this box (both models stay resident: ~15 GB of 180)
+        # the reference's own CUDA path on this GPU (both models stay resident: ~15 GB of 80)
         from baseline import reference_arm as RA
         if RA.available():
             try:
@@ -485,7 +505,7 @@ def run_reference(args):
         return
     from baseline import reference_arm as RA
     if not RA.available():
-        emit(dict(impl='reference', unavailable='baseline/_ref is not installed (run baseline/install_ref.sh in the build container)'))
+        emit(dict(impl='reference', unavailable='baseline/_ref is not installed (baseline/install_ref.sh)'))
         return
     from oracle import ref_import as R
     ref = RA.CpuReference(args.scale, args.batch, args.duration)
@@ -544,6 +564,8 @@ if __name__ == '__main__':
     ap.add_argument('--no-cpu', action='store_true')
     ap.add_argument('--no-ref-gpu', action='store_true', help='skip timing the reference CUDA path (reference_gpu block)')
     ap.add_argument('--no-encodec', action='store_true')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write the last timed step\'s outputs as float32 DIR/<name>.npy (at most 64 MB in all)')
     a = ap.parse_args()
     if a.impl == 'reference':
         run_reference(a)

@@ -1,5 +1,5 @@
 /*
- * audiocraft_b200 -- C-ABI of the B200 (sm_100a) hot-path library.
+ * audiocraft_b200 -- C-ABI of the H100 (sm_90a) hot-path library.
  *
  * The reference (facebookresearch/audiocraft) is 100% Python and has no FFI layer; its boundary for
  * this path is the Python class API (CompressionModel / LMModel / MusicGen).  This header is the
@@ -63,7 +63,7 @@ int acb_conv1d(const float* x, const float* w_packed, const float* bias, const f
  * operand split into two tf32 terms and three MMAs per product (~2^-22 relative error per product, fp32 accumulate) --
  * layers too small for the MMA tile fall back to fp32 FMA. */
 #define ACB_CONV_FP32 0
-#define ACB_CONV_TF32X3 1          /* tcgen05.mma.kind::tf32, accumulator in TMEM */
+#define ACB_CONV_TF32X3 1          /* wgmma tf32 (3xTF32 split), accumulator in registers */
 #define ACB_CONV_TF32X3_MMASYNC 2  /* same arithmetic on the legacy mma.sync.m16n8k8 path */
 
 /* StreamableConvTranspose1d.forward, audiocraft/modules/conv.py:221-243: transposed conv (kernel = 2*stride)
@@ -75,10 +75,9 @@ int acb_convtr1d(const float* x, const float* w_packed, const float* w_gemm, con
                  int batch, int c_in, int c_out, int t_in, int t_out, int kernel, int stride, int trim_left,
                  int elu_in, int precision, void* stream);
 
-/* The encoder's default for k > 1, >= 128 output channels (validated on B200 in round 2: latents within 3e-6 of fp32, RVQ
- * indices exact on the 10 s goldens): the same convolution as
- * acb_conv1d (StreamableConv1d.forward, modules/conv.py:185-201, + fused ELU / residual) as an implicit GEMM on tcgen05
- * without an im2col tile, the TMEM accumulator flushed into fp32 registers once per 8 input channels (csrc/encodec.cu,
+/* The encoder's default for k > 1, >= 128 output channels (RVQ indices exact on the 10 s goldens): the same convolution as
+ * acb_conv1d (StreamableConv1d.forward, modules/conv.py:185-201, + fused ELU / residual) as an implicit GEMM on wgmma
+ * without an im2col tile, the tensor-core accumulator flushed into fp32 registers once per 8 input channels (csrc/encodec.cu,
  * conv1d_t6_kernel).  c_in % 8 == 0 and c_out % 64 == 0.  w6 = weights split into two tf32 terms and laid out as
  * [c_out / N][c_in / 8][kernel][term hi,lo][2][N][4] with N = acb_conv1d_t6_tile(c_out)
  * (audiocraft_b200.encodec.pack_conv_t6 builds it). */
@@ -98,8 +97,8 @@ int acb_resblock(const float* x, const float* w1, const float* b1, const float* 
 
 /* w_gemm (optional, needed for precision ACB_CONV_TF32X3): the same weights packed as the GEMM operand
  * [2*Cin][Cout*stride], row r = ci*2 + k (k = 0 multiplies x[ti-1], k = 1 multiplies x[ti]), column n' = co*stride + ph,
- * value w[ci][ph + (1-k)*stride][co]: the transposed conv then runs on the tcgen05 kernel as one GEMM whose accumulator
- * row (TMEM lane) ti holds `stride` consecutive output steps of every channel. */
+ * value w[ci][ph + (1-k)*stride][co]: the transposed conv then runs on the tensor-core kernel as one GEMM whose accumulator
+ * row ti holds `stride` consecutive output steps of every channel. */
 
 /* Recurrent half of StreamableLSTM.forward, audiocraft/modules/lstm.py:19-25 (nn.LSTM, gate order i,f,g,o,
  * zero initial state).  The input half (W_ih x_t + b_ih + b_hh for every t) is a 1x1 acb_conv1d producing
@@ -250,12 +249,12 @@ int acb_lm_step_logits(acb_lm_t* lm, float* logits_out, void* stream);
  * order, so bench.py can time the dominant kernel with CUDA events in isolation.  *n_launches = kernels enqueued. */
 int acb_lm_debug_gemms(acb_lm_t* lm, void* stream, int* n_launches);
 
-/* 1 if the captured decode step uses programmatic dependent launch edges (ACB_NO_PDL=1 disables them). */
+/* 1 if the captured decode step uses programmatic dependent launch edges (currently never: plain stream-order edges). */
 int acb_lm_uses_pdl(const acb_lm_t* lm);
 
 /* [N][K] row-major fp16 (N % 128 == 0, K % 64 == 0) -> the packed tile layout of acb_lm_weights.wp_*: tile (nt, kb) =
  * features [128 nt, +128) x K [64 kb, +64) at ((nt * K/64 + kb) * 8192) halves; inside a tile feature f is the 128-byte row
- * at f * 128 and its 16-byte chunk c sits at position c ^ (f & 7) (the canonical 128-byte-swizzled K-major UMMA layout). */
+ * at f * 128 and its 16-byte chunk c sits at position c ^ (f & 7) (the canonical 128-byte-swizzled K-major wgmma layout). */
 int acb_lm_pack_weight(const void* w, void* wp, int n, int k, void* stream);
 
 /* Inspection of the fused step's work decomposition: out[4 g + {0,1,2,3}] = N, K, K-splits, 64-element K blocks per item

@@ -2,7 +2,7 @@
 
 TEST INFRASTRUCTURE ONLY (see oracle/__init__.py).  Plain fp32 torch ops on CPU; no reference
 code is imported here, every function restates the algorithm and cites where it lives in the
-reference (paths relative to /root/reference).
+reference (paths relative to the reference source tree).
 
 Weights come in as a reference-layout ``state_dict`` (SURVEY.md section 8b):
   encoder.model.{i}.conv.conv.{weight_g,weight_v,bias}, encoder.model.{i}.block.{1,3}.conv.conv.*,

@@ -1,7 +1,7 @@
 """CPU oracle for the MusicGen LM decode path (LMModel.forward / _sample_next_token / generate).
 
 TEST INFRASTRUCTURE ONLY (see oracle/__init__.py).  Plain fp32 torch on CPU, restating the
-reference algorithm with citations (paths relative to /root/reference).  Weights come in as a
+reference algorithm with citations (paths relative to the reference source tree).  Weights come in as a
 reference-layout LM ``state_dict`` (SURVEY.md section 8b).
 
 ``half_gemm=True`` emulates the GPU arithmetic of BOTH the reference GPU path (fp16 weights +

@@ -1,11 +1,10 @@
 """Import the real reference modules, unmodified, on CPU or CUDA.
 
 TEST / BASELINE INFRASTRUCTURE ONLY (never imported by the audiocraft_b200 package).  The reference is looked up in
-this order: $AUDIOCRAFT_REFERENCE, /root/reference (build container only), <repo>/baseline/_ref -- the offline
-`pip install --no-deps --target baseline/_ref /root/reference` copy, git-ignored but shipped to the GPU box with the
-gpurun snapshot (recipe: baseline/install_ref.sh).  Used by tests/golden/make_golden.py to generate the committed
-golden vectors, by the tests that cross-check oracle/ and the CUDA path against the reference when it is present, and
-by bench.py's `--impl reference` arm and `reference_gpu` block (the reference's own modules timed on the box).
+this order: $AUDIOCRAFT_REFERENCE (a source tree), <repo>/baseline/_ref -- the offline, git-ignored
+`pip install --no-deps --target baseline/_ref <reference tree>` copy (recipe: baseline/install_ref.sh).  Used by
+tests/golden/make_golden.py to generate the committed golden vectors, and by bench.py's `--impl reference` arm and
+`reference_gpu` block (the reference's own modules timed on the same machine).  The tests read only the golden vectors.
 
 Recipe (SURVEY.md §8c): the reference's hot-path modules import and run on CPU
 once the missing third-party packages are stubbed. Nothing from the reference is
@@ -21,11 +20,11 @@ _REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def _find_root() -> str:
-    cands = [os.environ.get("AUDIOCRAFT_REFERENCE"), "/root/reference", os.path.join(_REPO, "baseline", "_ref")]
+    cands = [os.environ.get("AUDIOCRAFT_REFERENCE"), os.path.join(_REPO, "baseline", "_ref")]
     for c in cands:
         if c and os.path.isdir(os.path.join(c, "audiocraft", "modules")):
             return c
-    return cands[1]
+    return cands[-1]
 
 
 REF_ROOT = _find_root()

@@ -1,7 +1,7 @@
 """Summarise an `ncu --csv --metrics gpu__time_duration.sum,dram__bytes_read.sum,dram__bytes_write.sum` launch list per
 kernel (template arguments and parameter lists stripped): launches, DRAM MB read/written, total time.
 
-    python profiles/summarise_ncu.py gpurun_out/v6_launches_step750.csv [--skip-kernel lm_gemm_kernel<8] > summary.json
+    python profiles/summarise_ncu.py launches.csv [--skip-kernel lm_gemm_kernel<8] > summary.json
 
 `--skip-kernel` drops kernels whose full name contains the given text (e.g. the once-per-generate cross-K/V prefill,
 which is not part of a decode step)."""

@@ -1,10 +1,11 @@
-"""Generate tests/golden/*.pt by running the REAL reference modules (read-only tree at /root/reference) on CPU.
+"""Generate tests/golden/*.pt by running the REAL reference modules (found through oracle/ref_import.py:
+$AUDIOCRAFT_REFERENCE or baseline/_ref) on CPU, and for `fullsize_cuda` on a GPU.
 
-Run in the build container only:  python tests/golden/make_golden.py
+    python tests/golden/make_golden.py [fullsize|fullsize_cuda [out_dir]|rope|two_step]
 The reference's own tests hold no numeric golden vectors for this path (SURVEY.md section 4), so these
-fixtures are what pins the oracle (tests/test_oracle_vs_golden.py) and, on the GPU box where /root/reference
-does not exist, the CUDA path (tests/test_gpu_*.py).  Inputs and weights are regenerated from seeds by
-tests/helpers.py + audiocraft_b200/synth.py; only outputs are stored.
+fixtures are what pins the oracle (tests/test_oracle_vs_golden.py) and the CUDA path (tests/test_gpu_*.py), which
+never import the reference.  Inputs and weights are regenerated from seeds by tests/helpers.py +
+audiocraft_b200/synth.py; only outputs are stored.
 """
 import os
 import sys
@@ -184,6 +185,38 @@ def golden_lm_fullsize(name, batch, t_text=16, T=1500, wseed=0, cseed=3, sseed=1
     print(name, 'fullsize logits', tuple(tv.shape), f'{time.time() - t0:.0f} s')
 
 
+CUDA_SAMPLE = 48   # logits per row kept from the reference's CUDA path (a seeded sample of the card indices)
+
+
+def golden_lm_fullsize_cuda(name, batch, out_dir=None, t_text=16, T=1500, wseed=0, cseed=3, sseed=17):
+    """The reference's OWN CUDA path at the benchmarked shapes (needs a GPU): fp16 weights, one causal forward under fp16
+    autocast with SDPA (audiocraft/models/loaders.py:115-118, genmodel.py:74-78) over the same seeded sequence as
+    golden_lm_fullsize, rows [cond; null] = 2*batch.  Kept at FULLSIZE_STEPS: the per-row logits at CUDA_SAMPLE seeded
+    card indices (fp16, as the reference computes them) and the argmax / top-2 margin of the CFG-mixed logits."""
+    from oracle import ref_models as RM
+    cfg = synth.lm_config(name)
+    sd = synth.synth_lm_state_dict(cfg, seed=wseed, device='cuda', dtype=torch.float16)
+    hid, mask = synth.synth_text_condition(cfg, batch, t_text, seed=cseed)
+    ref, CA = RM.build_ref_lm(cfg, sd, RM.text_table(hid, mask, cfg['cond_dim']), device='cuda', dtype=torch.float16)
+    del sd
+    seq = H.fullsize_sequence(cfg, batch, T, sseed).cuda()
+    S = seq.shape[-1]
+    with torch.no_grad():
+        cc = RM.ref_cfg_conditions(ref, CA, batch)
+        with torch.autocast('cuda', dtype=torch.float16):
+            rl = ref(torch.cat([seq, seq], 0)[..., :S - 1], conditions=[], condition_tensors=cc)   # [2B,K,S-1,card]
+        rl = rl[:, :, FULLSIZE_STEPS, :].float().permute(2, 0, 1, 3).contiguous()                  # [n,2B,K,card]
+    c, u = rl.split(batch, dim=1)
+    mix = u + (c - u) * cfg['cfg_coef']
+    top2 = mix.topk(2, dim=-1).values
+    idx = torch.randperm(cfg['card'], generator=torch.Generator().manual_seed(11))[:CUDA_SAMPLE].sort().values
+    out = dict(name=name, batch=batch, t_text=t_text, T=T, wseed=wseed, cseed=cseed, sseed=sseed, steps=FULLSIZE_STEPS,
+               index=idx, logits=rl[..., idx.cuda()].half().cpu(), mix_argmax=mix.argmax(-1).to(torch.int16).cpu(),
+               mix_margin=(top2[..., 0] - top2[..., 1]).cpu())
+    torch.save(out, os.path.join(out_dir or H.GOLDEN_DIR, f'{name}_cuda.pt'))
+    print(name, 'reference CUDA logits', tuple(out['logits'].shape))
+
+
 def golden_encodec_fullsize():
     """BASELINE config 1 at its real length (10 s = 240 000 samples at 24 kHz: codes [1, n_q, 750] for n_q = 8 and 32)
     and a [2, 1, 320000] slice of config 4 (32 kHz, 4 codebooks): codes from the reference (int16 to keep the fixture small)."""
@@ -268,6 +301,10 @@ if __name__ == '__main__':
         sys.exit(0)
     if len(sys.argv) > 1 and sys.argv[1] == 'rope':
         golden_lm_rope()
+        sys.exit(0)
+    if len(sys.argv) > 1 and sys.argv[1] == 'fullsize_cuda':   # [out_dir]
+        golden_lm_fullsize_cuda('musicgen_medium', 8, *sys.argv[2:3])
+        golden_lm_fullsize_cuda('musicgen_large', 32, *sys.argv[2:3])
         sys.exit(0)
     if len(sys.argv) > 1 and sys.argv[1] == 'fullsize':
         golden_encodec_fullsize()

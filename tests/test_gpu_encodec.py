@@ -57,7 +57,7 @@ def test_conv1d_matches_oracle(cin, cout, k, s, d, causal, L):
     (64, 256, 16, 8, 1, True, 4100), (8, 64, 3, 1, 2, False, 77), (8, 64, 7, 1, 1, False, 3), (512, 1024, 16, 8, 1, False, 4000),
 ])
 def test_experimental_conv1d_t6_matches_oracle(cin, cout, k, s, d, causal, L):
-    """Implicit-GEMM tcgen05 convolution with per-8-channel fp32 flushes of the TMEM accumulator (acb_conv1d_t6): same
+    """Implicit-GEMM wgmma convolution with per-8-channel fp32 flushes of the tensor-core accumulator (acb_conv1d_t6): same
     contract as acb_conv1d; the flush is meant to bring the tensor-core path to fp32-FMA accuracy (atol 2e-5 here, vs 1e-4
     for the un-flushed 3xTF32 kernels one layer deep)."""
     from audiocraft_b200.encodec import conv_geometry, pack_conv_t6
@@ -136,7 +136,7 @@ def test_convtr1d_matches_oracle(cin, cout, s, causal, ratio, L):
     assert tout == ref.shape[-1] == L * s
     xd, wd, bd = _dev(x), _dev(w.permute(0, 2, 1)), _dev(b)   # keep the device tensors alive across the launch
     wg = _dev(w.view(cin, cout, 2, s).flip(2).permute(0, 2, 1, 3).reshape(cin * 2, cout * s))
-    for prec in (0, 1):   # fp32 FMA; 3xTF32 on tcgen05 as one GEMM over virtual channels (when the layer is big enough)
+    for prec in (0, 1):   # fp32 FMA; 3xTF32 on wgmma as one GEMM over virtual channels (when the layer is big enough)
         y = torch.empty(2, cout, tout, device='cuda')
         lib.check(L_.acb_convtr1d(lib.ptr(xd), lib.ptr(wd), lib.ptr(wg), lib.ptr(bd), lib.ptr(y), 2, cin,
                                   cout, L, tout, 2 * s, s, tl, 1, prec, lib.stream()))
@@ -328,7 +328,7 @@ def test_tensor_core_encoder_mode(name):
 
 @pytest.mark.parametrize('name', ['encodec_32k', 'encodec_24k'])
 def test_experimental_flush_encoder_mode(name):
-    """encoder_precision='tf32x3_flush': the implicit-GEMM tcgen05 convs with per-8-channel fp32 flushes are meant to make
+    """encoder_precision='tf32x3_flush': the implicit-GEMM wgmma convs with per-8-channel fp32 flushes are meant to make
     the tensor-core encoder as accurate as the fp32 FMA one (latents atol 2e-5, codes under the exact-encoder rule)."""
     from audiocraft_b200.encodec import EncodecModel
     g = torch.load(os.path.join(H.GOLDEN_DIR, f'{name}.pt'), weights_only=False)

@@ -402,7 +402,7 @@ def test_double_cfg_matches_oracle():
 @pytest.mark.parametrize('name,B', [('lm_mini', 2), ('lm_medium_2l', 8), ('lm_large_2l', 32)])
 def test_fused_step_matches_per_phase_kernels(monkeypatch, name, B):
     """The opt-in persistent fused decode step (ACB_LM_STEP=fused: ONE cooperative kernel per step -- TMA weight ring,
-    tcgen05 swap-AB GEMMs with TMEM accumulators, grid barriers between phases, csrc/lm_step.cu) against the default graph of
+    wgmma swap-AB GEMMs with register accumulators, grid barriers between phases, csrc/lm_step.cu) against the default graph of
     one kernel per phase: same arithmetic up to fp32 summation grouping (4 accumulator chains, different split-K)."""
     monkeypatch.setenv('ACB_LM_STEP', 'fused')          # before the model is built: the packed weights are made at load time
     cfg, sd, m = _model(name, 5)

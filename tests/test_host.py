@@ -62,11 +62,11 @@ def test_fused_residual_block_routing():
     assert fused('encodec_32k', _lib.CONV_T6_AUTO) == []
 
 
-def test_sass_is_sm100a():
+def test_sass_is_sm90a():
     import subprocess
     from audiocraft_b200 import _lib
     out = subprocess.run(['cuobjdump', '-lelf', _lib.LIB_PATH], capture_output=True, text=True).stdout
-    assert 'sm_100a' in out, out
+    assert 'sm_90a' in out, out
 
 
 def test_no_cpu_fallback():

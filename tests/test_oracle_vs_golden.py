@@ -1,5 +1,5 @@
 """Pin the CPU oracle (oracle/) to outputs of the REAL reference modules (tests/golden/*.pt, produced by
-tests/golden/make_golden.py in the build container).  Integer outputs must match exactly; float outputs to
+tests/golden/make_golden.py on the CPU).  Integer outputs must match exactly; float outputs to
 fp32 round-off (tolerances written at each check)."""
 import os
 

@@ -1,8 +1,7 @@
 """CPU emulation of the data layout of the EXPERIMENTAL conv1d_t6 kernel (csrc/encodec.cu): the staged input slab
 [4-channel chunk][stride phase][row][4 channels], the tap = descriptor-start-address rule, and the packed weight operand
-of `pack_conv_t6`.  The kernel itself has not run on hardware yet (no GPU time was left when it was written); this test
-pins the index arithmetic it relies on against the oracle convolution, so that a hardware failure in round 2 can only be
-a tcgen05 / barrier issue, not a layout one."""
+of `pack_conv_t6`.  This test pins the index arithmetic the kernel relies on against the oracle convolution without a
+GPU, so that a failure of the GPU tests points at the tensor-core or barrier code, not at the layout."""
 import math
 
 import numpy as np

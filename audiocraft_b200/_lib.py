@@ -8,7 +8,7 @@ import os
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get('ACB_LIB') or os.path.join(_HERE, 'libaudiocraft_b200.so')   # ACB_LIB: the instrumented (timeline) build, debugging only
+LIB_PATH = os.environ.get('ACB_LIB') or os.path.join(_HERE, 'libaudiocraft_b200.so')   # ACB_LIB: another build (e.g. an ACB_BUILD_VARIANT one) for A/B runs
 
 CONV_FP32, CONV_TF32X3, CONV_TF32X3_MMASYNC = 0, 1, 2
 CONV_T6_FLUSH = 3   # host-side selector only: every layer acb_conv1d_t6 supports goes through it, the rest fp32 FMA
@@ -16,7 +16,6 @@ CONV_T6_AUTO = 4    # host-side selector only: acb_conv1d_t6 where it is faster 
 ACB_LM_MAX_SPLIT = 8
 ACB_LM_PART_SLOTS = 16
 ACB_LM_PREFILL_ROWS = 64
-ACB_LM_PLAN_BYTES = 2 << 20
 
 
 class LMConfig(C.Structure):
@@ -33,8 +32,8 @@ class LMWeights(C.Structure):
 
 class LMBuffers(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ('x', 'h16', 'a16', 'f16', 'q32', 'part', 'logits', 'k_cache', 'v_cache',
-                                           'ck_cache', 'cv_cache', 'cross16', 'seq', 'seq_mask', 'pos', 'noise', 'plan',
-                                           'stats', 'bar')]
+                                           'ck_cache', 'cv_cache', 'cross16', 'seq', 'seq_mask', 'pos', 'noise', 'stats',
+                                           'bar')]
 
 
 class LMSampling(C.Structure):
@@ -84,12 +83,11 @@ def lib():
     L.acb_lm_uses_pdl.argtypes = [vp]
     L.acb_lm_debug_gemms.argtypes = [vp, vp, C.POINTER(ci)]
     L.acb_sample.argtypes = [vp, vp, vp, ci, ci, ci, ci, C.POINTER(LMSampling), C.c_uint64, vp]
-    L.acb_debug_chain_latency.argtypes = [ci, ci, ci, ci, ci, ci, C.POINTER(C.c_float), vp]
     L.acb_debug_grid_barrier.argtypes = [ci, ci, ci, ci, ci, ci, C.POINTER(C.c_float)]
     for name in ('acb_weight_norm_fold', 'acb_conv1d', 'acb_convtr1d', 'acb_lstm_recurrent', 'acb_rvq_encode',
                  'acb_rvq_decode', 'acb_lm_create', 'acb_lm_destroy', 'acb_lm_begin', 'acb_lm_steps',
                  'acb_lm_step_logits', 'acb_lm_launches_per_step', 'acb_lm_rows_pad', 'acb_sample',
-                 'acb_device_sm_count', 'acb_lm_debug_gemms', 'acb_lm_uses_pdl', 'acb_debug_chain_latency',
+                 'acb_device_sm_count', 'acb_lm_debug_gemms', 'acb_lm_uses_pdl',
                  'acb_conv1d_t6', 'acb_conv1d_t6_tile', 'acb_debug_grid_barrier', 'acb_lm_pack_weight', 'acb_lm_debug_step_plan', 'acb_lm_prefill',
                  'acb_resblock', 'acb_resblock_supported'):
         getattr(L, name).restype = ci
@@ -101,7 +99,7 @@ def lib():
 EXPORTS = ['acb_version', 'acb_last_error', 'acb_device_sm_count', 'acb_weight_norm_fold', 'acb_conv1d', 'acb_convtr1d',
            'acb_lstm_recurrent', 'acb_lstm_state_bytes', 'acb_rvq_encode', 'acb_rvq_decode', 'acb_lm_create',
            'acb_lm_destroy', 'acb_lm_begin', 'acb_lm_steps', 'acb_lm_step_logits', 'acb_lm_rows_pad',
-           'acb_lm_launches_per_step', 'acb_lm_debug_gemms', 'acb_lm_uses_pdl', 'acb_sample', 'acb_debug_chain_latency', 'acb_conv1d_t6', 'acb_conv1d_t6_tile',
+           'acb_lm_launches_per_step', 'acb_lm_debug_gemms', 'acb_lm_uses_pdl', 'acb_sample', 'acb_conv1d_t6', 'acb_conv1d_t6_tile',
            'acb_debug_grid_barrier', 'acb_lm_pack_weight', 'acb_lm_debug_step_plan', 'acb_lm_prefill', 'acb_resblock',
            'acb_resblock_supported']
 

@@ -20,17 +20,14 @@ ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
 FLAGS = ['-O3', '-std=c++17', '-lineinfo'] + ARCH + ['-Xcompiler', '-fPIC',
          '-Xptxas', '-v']
 OBJ_SUFFIX = '.o'
+LOG = os.path.join(HERE, 'build.log')
 if os.environ.get('ACB_BUILD_VARIANT'):   # experiment builds: extra -D flags (ACB_BUILD_DEFS) into libaudiocraft_b200_<variant>.so; run with ACB_LIB=<path>
     _v = os.environ['ACB_BUILD_VARIANT']
     FLAGS += os.environ.get('ACB_BUILD_DEFS', '').split()
     LIB = os.path.join(HERE, f'libaudiocraft_b200_{_v}.so')
     STAMP = LIB + '.stamp'
     OBJ_SUFFIX = f'.{_v}.o'
-if os.environ.get('ACB_BUILD_TIMELINE') == '1':   # instrumented build: in-kernel %globaltimer stamps (see csrc/lm.cu tl_stamp)
-    FLAGS.append('-DACB_TIMELINE')               # goes to its own file (never the product library): run with ACB_LIB=<that path>
-    LIB = os.path.join(HERE, 'libaudiocraft_b200_timeline.so')
-    STAMP = LIB + '.stamp'
-    OBJ_SUFFIX = '.tl.o'
+    LOG = os.path.join(HERE, f'build_{_v}.log')
 
 
 def _digest() -> str:
@@ -65,7 +62,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         raise RuntimeError(f'link failed:\n{r.stdout}')
     with open(STAMP, 'w') as fh:
         fh.write(dig)
-    with open(os.path.join(HERE, 'build.log' if OBJ_SUFFIX == '.o' else 'build_timeline.log'), 'w') as fh:
+    with open(LOG, 'w') as fh:
         fh.write('\n'.join(logs))
     if verbose:
         print('\n'.join(logs))

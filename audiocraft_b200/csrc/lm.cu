@@ -5,26 +5,24 @@
 // step-dependent quantity (position, tokens) resident on the device.
 //
 // The step is HBM-bound in bytes (all layer weights, fp16, 3.2 GB for medium, and the KV cache are read once per step at ~rows FLOP/B)
-// and LATENCY-bound in time: 11 dependent kernels per layer.  Design consequences:
-//   * weights stay in the reference's [out][in] fp16 layout; a CTA's 16 (or 32) x kslice slab is fetched with TMA bulk copies BEFORE
-//     griddepcontrol.wait, i.e. while the previous kernel of the graph still runs (programmatic dependent launch); a 16x32 block of W
-//     is the A operand of two m16n8k16 MMAs, the activations (a few KB, L2 resident) are the B operand, so the tile is 16 output
-//     features x (8*NT) rows and nothing is wasted on padding rows up to 128.
+// and LATENCY-bound in time: 11 dependent kernels per layer, chained by plain stream-order edges of the graph.  Design consequences:
+//   * weights stay in the reference's [out][in] fp16 layout; a CTA's 16 (or 32) x kslice slab is fetched with TMA bulk copies
+//     issued before the CTA reads its first activation; a 16x32 block of W is the A operand of two m16n8k16 MMAs, the activations
+//     (a few KB, L2 resident) are the B operand, so the tile is 16 output features x (8*NT) rows and nothing is wasted on padding
+//     rows up to 128.
 //   * every GEMM spreads its weight matrix over >= 2 CTAs per SM; small-N GEMMs split K across CTAs and the partial sums are reduced
 //     (in a fixed order: bit-reproducible) by the consumer kernel, which is the residual add + LayerNorm, so that reduction costs no
 //     extra pass.
 //   * K/V go from the QKV GEMM epilogue straight into the cache; cross-attention K/V are computed once per generate() instead of
 //     every step (the reference recomputes them, transformer.py:355-357).
-//   * attention for one query token: one CTA per (row, head) streaming K and V through a cp.async ring (lm_attn2_kernel).
-// Alternatives that were built and measured slower (persistent fused step, cluster split-K with LayerNorm on load, chain kernels, ...)
-// are listed with their numbers in DESIGN.md section 3.1.
+//   * self attention: one CTA per (query row, head) streaming K and V through a cp.async ring (lm_attn2_kernel), for the decode
+//     step and for prompt prefill alike.
+// The opt-in alternative, one persistent kernel for the whole step, is lm_step.cu (DESIGN.md section 3.1.1).
 #include "common.cuh"
 #include "lm_step.cuh"
 #include <math.h>
 #include <new>
 #include <vector>
-#include <algorithm>
-#include <utility>
 #include <stdio.h>
 #include <stdlib.h>
 
@@ -36,27 +34,6 @@ __device__ __forceinline__ void mma16816(float (&c)[4], uint32_t a0, uint32_t a1
         : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
         : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
 }
-
-// Programmatic dependent launch (PDL): a kernel launched with the programmatic-stream-serialization attribute may
-// start while its predecessor is still running; everything before pdl_wait() must only touch memory no earlier
-// kernel of the step writes (weights).  Both are no-ops for a normally launched kernel.
-__device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-
-// Debug timeline: thread 0 of every CTA writes %globaltimer (ns) into its 8-slot record.  Compiled in only with
-// -DACB_TIMELINE (ACB_BUILD_TIMELINE=1 python -m audiocraft_b200.build) and armed with ACB_LM_TIMING=1: at this time
-// scale even dormant stamps cost time, because every instruction line of a few-microsecond kernel is fetched cold.
-#ifdef ACB_TIMELINE
-__device__ __forceinline__ void tl_stamp(unsigned long long* t, int slot) {
-    if (t && threadIdx.x == 0) {
-        unsigned long long now;
-        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now));
-        t[(((size_t)blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) * 8 + slot] = now;
-    }
-}
-#else
-__device__ __forceinline__ void tl_stamp(unsigned long long*, int) {}
-#endif
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
@@ -109,8 +86,6 @@ __global__ void __launch_bounds__(256) lm_embed_kernel(const __half* __restrict_
                                                        const int64_t* __restrict__ seq, const int* __restrict__ P,
                                                        float* __restrict__ x, int d, int n_q, int card, int max_seq,
                                                        int batch, float pos_scale, int rows_real) {
-    pdl_trigger();
-    pdl_wait();
     const int r = blockIdx.x, b = (PF ? r % rows_real : r) % batch, pos = P[0] + (PF ? r / rows_real : 0);
     __shared__ int tok[16];
     if (threadIdx.x < n_q) {
@@ -132,22 +107,16 @@ __global__ void __launch_bounds__(256) lm_embed_kernel(const __half* __restrict_
 // ------------------------------------------------------------------------------------------------ residual + LN
 // x[r] += sum_s part[s][r] (fixed order), then h16[r] = LayerNorm(x[r]) * gamma + beta  (eps 1e-5, fp32 statistics).
 // One CTA per row, ONE float4 per thread (d <= 2048): no per-thread loops, so the kernel is ~300 instructions -- at this
-// time scale cold instruction fetch is a first-order cost (a 4-float4-per-thread version was over 1 000 instructions).  gamma / beta do not depend on the previous kernel and are
-// requested before griddepcontrol.wait.
+// time scale cold instruction fetch is a first-order cost (a 4-float4-per-thread version was over 1 000 instructions).
 constexpr int LN_THREADS = 512;
 __global__ void __launch_bounds__(LN_THREADS) lm_ln_kernel(float* __restrict__ x, const float* __restrict__ part, int nsplit,
                                                            size_t split_stride, const float* __restrict__ gamma,
-                                                           const float* __restrict__ beta, __half* __restrict__ out, int d,
-                                                           unsigned long long* timing) {
+                                                           const float* __restrict__ beta, __half* __restrict__ out, int d) {
     __shared__ float red[2][32];
     const int r = blockIdx.x, i = threadIdx.x;
     const bool live = i < (d >> 2);
-    tl_stamp(timing, 0);
     float4 gm = make_float4(0.f, 0.f, 0.f, 0.f), bt = gm;
     if (live) { gm = reinterpret_cast<const float4*>(gamma)[i]; bt = reinterpret_cast<const float4*>(beta)[i]; }
-    pdl_trigger();
-    pdl_wait();
-    tl_stamp(timing, 1);
     float4* xr = reinterpret_cast<float4*>(x + (size_t)r * d);
     float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
     if (live) {
@@ -163,16 +132,13 @@ __global__ void __launch_bounds__(LN_THREADS) lm_ln_kernel(float* __restrict__ x
         }
         if (nsplit) xr[i] = a;
     }
-    tl_stamp(timing, 4);
     const float mean = block_sum((a.x + a.y) + (a.z + a.w), red[0]) / d;
-    tl_stamp(timing, 5);
     float q = 0.f;
     if (live) {
         const float cx = a.x - mean, cy = a.y - mean, cz = a.z - mean, cw = a.w - mean;
         q = fmaf(cx, cx, q); q = fmaf(cy, cy, q); q = fmaf(cz, cz, q); q = fmaf(cw, cw, q);
     }
     const float rstd = 1.f / sqrtf(block_sum(q, red[1]) / d + 1e-5f);
-    tl_stamp(timing, 6);
     if (live) {
         __half2 lo = __floats2half2_rn((a.x - mean) * rstd * gm.x + bt.x, (a.y - mean) * rstd * gm.y + bt.y);
         __half2 hi = __floats2half2_rn((a.z - mean) * rstd * gm.z + bt.z, (a.w - mean) * rstd * gm.w + bt.w);
@@ -181,7 +147,6 @@ __global__ void __launch_bounds__(LN_THREADS) lm_ln_kernel(float* __restrict__ x
         pk.y = *reinterpret_cast<uint32_t*>(&hi);
         reinterpret_cast<uint2*>(out + (size_t)r * d)[i] = pk;
     }
-    tl_stamp(timing, 3);
 }
 
 // ------------------------------------------------------------------------------------------------ skinny GEMM
@@ -196,20 +161,16 @@ struct GemmParams {
     float* q32; __half* kc; __half* vc; int d, H, cache_len; const int* pos;  // QKV / CROSSKV
     int text_len, row0;                                                      // CROSSKV
     int rows_real;                                                           // QKV_PF: rows of the generation (GEMM row = tok * rows_real + row)
-    unsigned long long* timing;                 // debug timeline
 };
 
 // CTA = 4 warps, tile = 16 output features x kslice of K.  The CTA's 16 x kslice weight slab is fetched by ONE thread
-// with 16 TMA bulk copies (one per W row, padded pitch => conflict-free fragment reads) before griddepcontrol.wait (a no-op:
-// the step graph uses plain edges, see acb_lm_begin).
+// with 16 TMA bulk copies (one per W row, padded pitch => conflict-free fragment reads), issued before the first activation
+// read so that the weight bytes are in flight while the activations load.
 // FT2 = feature tiles of 16 per CTA.  FT2 = 2 (opt-in per GEMM, see pick_ft2) halves the number of CTAs and therefore
 // the activation traffic out of L2: every CTA re-reads the whole 16 x K activation block, as many bytes as the weights.
 template <int NT, int EPI, int FT2 = 1>
 __global__ void __launch_bounds__(128) lm_gemm_kernel(GemmParams p) {
-#ifndef ACB_GEMM_U2
-#define ACB_GEMM_U2 4   // k-blocks per batch of activation loads at <= 16 rows (experiment builds: -DACB_GEMM_U2=6)
-#endif
-    constexpr int U = NT <= 2 ? ACB_GEMM_U2 : (NT <= 4 ? 2 : 1);
+    constexpr int U = NT <= 2 ? 4 : (NT <= 4 ? 2 : 1);   // k-blocks per batch of activation loads
     constexpr int RP = 8 * NT + 1;
     constexpr int FB = 16 * FT2;                     // output features per CTA
     extern __shared__ __align__(128) unsigned char gsm[];
@@ -221,7 +182,6 @@ __global__ void __launch_bounds__(128) lm_gemm_kernel(GemmParams p) {
     uint64_t* bar = reinterpret_cast<uint64_t*>(gsm + FB * pitch);
     float* red = reinterpret_cast<float*>(gsm + FB * pitch + 16);   // [4][FB][RP]
 
-    tl_stamp(p.timing, 0);
     if (tid == 0) mbar_init(bar, 1);
     __syncthreads();
     if (tid == 0) {
@@ -230,9 +190,6 @@ __global__ void __launch_bounds__(128) lm_gemm_kernel(GemmParams p) {
         for (int r = 0; r < FB; ++r)
             bulk_g2s(gsm + r * pitch, p.W + (size_t)(f0 + r) * p.K + k0, (uint32_t)ks * 2u, bar);
     }
-    pdl_trigger();
-    pdl_wait();   // activations written by the previous kernel are visible from here on
-    tl_stamp(p.timing, 1);
     int cache_pos = 0;
     if (EPI == EPI_QKV || EPI == EPI_QKV_PF) cache_pos = p.pos[0];   // requested now, consumed in the epilogue: off the critical path
 
@@ -258,7 +215,7 @@ __global__ void __launch_bounds__(128) lm_gemm_kernel(GemmParams p) {
             for (int j = 0; j < NT; ++j)
                 xv[u][j] = (kb + u < kb1) ? *reinterpret_cast<const uint4*>(xr + (size_t)(8 * j) * p.K + (size_t)(kb + u) * 32)
                                           : make_uint4(0, 0, 0, 0);
-        if (!w_ready) { mbar_wait(bar, 0); w_ready = true; tl_stamp(p.timing, 4); }
+        if (!w_ready) { mbar_wait(bar, 0); w_ready = true; }
 #pragma unroll
         for (int u = 0; u < U; ++u) {
             if (kb + u < kb1) {
@@ -276,7 +233,6 @@ __global__ void __launch_bounds__(128) lm_gemm_kernel(GemmParams p) {
         }
     }
     if (!w_ready) mbar_wait(bar, 0);   // never leave with a bulk copy in flight
-    tl_stamp(p.timing, 2);
     // cross-warp (split-K inside the CTA) reduction in a fixed order
 #pragma unroll
     for (int ft = 0; ft < FT2; ++ft)
@@ -289,7 +245,6 @@ __global__ void __launch_bounds__(128) lm_gemm_kernel(GemmParams p) {
             r0[8 * RP + 1] = c[ft][j][3];
         }
     __syncthreads();
-    tl_stamp(p.timing, 5);
     for (int idx = tid; idx < FB * 8 * NT; idx += 128) {
         const int row = idx / FB, feat = idx % FB;
         if (row >= p.rows) continue;
@@ -327,7 +282,6 @@ __global__ void __launch_bounds__(128) lm_gemm_kernel(GemmParams p) {
             cache[(((size_t)r * p.H + h) * p.cache_len + tc) * 64 + dd] = __float2half_rn(v);
         }
     }
-    tl_stamp(p.timing, 3);
 }
 
 // ------------------------------------------------------------------------------------------------ attention (1 query)
@@ -335,20 +289,10 @@ struct AttnParams {
     const float* q; int q_nsplit; size_t q_split_stride;  // q[s][row][d] fp32 partial sums
     const __half* kc; const __half* vc; __half* out;
     int H, d, cache_len; const int* pos; int fixed_len; float scale;
-    unsigned long long* timing;   // debug timeline
     int rows_real;                // prefill (PF kernels): rows of the generation
-    float* part; int* counter;    // split-KV self attention (gridDim.z > 1): partial (m, l, acc[64]) records, arrival counters
-    int split_min;                // contexts shorter than this stay on the single-CTA path
 };
 
-// Self attention for one query token: CTA = (row, head[, KV third]), 8 warps, ONE pass over K and V with an online softmax.
-// A warp instruction reads 4 consecutive cache positions (4 x 128 B = 512 contiguous bytes); 8 lanes share a position
-// (8 dims each).  4 positions-groups x 4 unrolled iterations of K and V are in flight per lane before any is consumed.
-// Split KV (gridDim.z = 3, opt-in: ACB_LM_ATT_SPLIT=3): rows x heads = 384 CTAs are 2.6 per SM, so SMs holding 3 finish well after those holding 2.  Once the context reaches split_min positions it is cut into
-// up to 3 chunks (multiples of the CTA's 128-position stride): 1 152 CTAs = 7.8 per SM.  Every chunk CTA writes its
-// (m, l, acc) record, and the LAST one to arrive (atomic counter, threadfence) merges the records in chunk order, so the
-// result does not depend on arrival order.  Short contexts take the single-CTA path; the idle CTAs exit at once.
-constexpr int ATT_WARPS = 8, ATT_UNROLL = 4;   // UNROLL 8 measured slower (98 regs: 2 CTAs/SM instead of 5)
+constexpr int ATT_WARPS = 8;
 
 struct OnlineSM { float m, l, acc[8]; };
 __device__ __forceinline__ void osm_merge(OnlineSM& a, float m2, float l2, const float (&acc2)[8]) {
@@ -360,173 +304,24 @@ __device__ __forceinline__ void osm_merge(OnlineSM& a, float m2, float l2, const
     a.m = mn;
 }
 
-// SPLIT = false (default step): none of the chunk / record / merge code is compiled in.  PF (prompt prefill): blockIdx.y is a
-// (token, row) pair tok * rows_real + r; the query at position pos + tok attends to the cache of row r up to and including
-// its own position (the QKV GEMM of the same pass has already appended every token of the pass: causal within the chunk).
-template <bool SPLIT, bool PF = false>
-__global__ void __launch_bounds__(ATT_WARPS * 32) lm_attn_kernel(AttnParams p) {
-    __shared__ float wm[ATT_WARPS], wl[ATT_WARPS], wacc[ATT_WARPS][64];
-    const int h = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int qrow = blockIdx.y, row = PF ? qrow % p.rows_real : qrow, tok = PF ? qrow / p.rows_real : 0;
-    const int sl = lane & 7, pg = lane >> 3;
-    tl_stamp(p.timing, 0);
-    pdl_trigger();
-    pdl_wait();
-    tl_stamp(p.timing, 1);
-    const int n = p.fixed_len > 0 ? p.fixed_len : p.pos[0] + tok + 1;
-    int lo = 0, hi = n, nact = 1;
-    if (SPLIT && gridDim.z > 1) {
-        // the record write + atomic + merge costs more than the balance gains at short contexts, hence split_min (default 768)
-        const int S = gridDim.z, chunk = n < p.split_min ? n : max(128, ((n + S - 1) / S + 127) & ~127);
-        nact = (n + chunk - 1) / chunk;
-        if ((int)blockIdx.z >= nact) return;         // CTA-uniform: nothing in this chunk
-        lo = blockIdx.z * chunk;
-        hi = min(n, lo + chunk);
-    }
-
-    float q[8];
-    {   // (split-K query partials exist only on the cross-attention path; a rolled/unrolled split loop here cost
-        //  ~1 500 instructions of cold code per launch)
-        const float4* qp = reinterpret_cast<const float4*>(p.q + (size_t)qrow * p.d + h * 64 + sl * 8);
-        const float4 qa = qp[0], qb = qp[1];
-        q[0] = half_round(qa.x) * p.scale; q[1] = half_round(qa.y) * p.scale; q[2] = half_round(qa.z) * p.scale;
-        q[3] = half_round(qa.w) * p.scale; q[4] = half_round(qb.x) * p.scale; q[5] = half_round(qb.y) * p.scale;
-        q[6] = half_round(qb.z) * p.scale; q[7] = half_round(qb.w) * p.scale;
-    }
-    tl_stamp(p.timing, 4);   // n and q consumed
-    const size_t base = ((size_t)row * p.H + h) * p.cache_len * 64 + sl * 8;
-    const __half* kb = p.kc + base;
-    const __half* vb = p.vc + base;
-
-    OnlineSM st;
-    st.m = -INFINITY; st.l = 0.f;
-#pragma unroll
-    for (int e = 0; e < 8; ++e) st.acc[e] = 0.f;
-
-    // warp-uniform loop bound (the shuffles need all 32 lanes)
-    for (int pb = lo + warp * 4; pb < hi; pb += ATT_WARPS * 4 * ATT_UNROLL) {
-        uint4 kv[ATT_UNROLL], vv[ATT_UNROLL];
-#pragma unroll
-        for (int u = 0; u < ATT_UNROLL; ++u) {
-            const int pp = pb + u * ATT_WARPS * 4 + pg;
-            if (pp < hi) {
-                kv[u] = ld_stream_u4(kb + (size_t)pp * 64);
-                vv[u] = ld_stream_u4(vb + (size_t)pp * 64);
-            } else {
-                kv[u] = vv[u] = make_uint4(0, 0, 0, 0);
-            }
-        }
-#pragma unroll
-        for (int u = 0; u < ATT_UNROLL; ++u) {
-            const int pp = pb + u * ATT_WARPS * 4 + pg;
-            const __half2* k2 = reinterpret_cast<const __half2*>(&kv[u]);
-            float s = 0.f;
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                const float2 f = __half22float2(k2[e]);
-                s = fmaf(q[2 * e], f.x, s);
-                s = fmaf(q[2 * e + 1], f.y, s);
-            }
-            s += __shfl_xor_sync(0xffffffffu, s, 1);
-            s += __shfl_xor_sync(0xffffffffu, s, 2);
-            s += __shfl_xor_sync(0xffffffffu, s, 4);
-            if (pp < hi) {
-                const float mn = fmaxf(st.m, s);
-                const float corr = __expf(st.m - mn);   // exp(-inf) = 0 on the first position
-                const float pw = __expf(s - mn);
-                st.l = st.l * corr + pw;
-                const __half2* v2 = reinterpret_cast<const __half2*>(&vv[u]);
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                    const float2 f = __half22float2(v2[e]);
-                    st.acc[2 * e] = fmaf(pw, f.x, st.acc[2 * e] * corr);
-                    st.acc[2 * e + 1] = fmaf(pw, f.y, st.acc[2 * e + 1] * corr);
-                }
-                st.m = mn;
-            }
-        }
-    }
-    tl_stamp(p.timing, 2);   // position loop
-    // merge the 4 position groups of the warp, then the warps
-#pragma unroll
-    for (int o = 8; o <= 16; o <<= 1) {
-        const float m2 = __shfl_xor_sync(0xffffffffu, st.m, o), l2 = __shfl_xor_sync(0xffffffffu, st.l, o);
-        float a2[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) a2[e] = __shfl_xor_sync(0xffffffffu, st.acc[e], o);
-        osm_merge(st, m2, l2, a2);
-    }
-    tl_stamp(p.timing, 5);   // lane merges
-    if (pg == 0) {
-        if (sl == 0) { wm[warp] = st.m; wl[warp] = st.l; }
-#pragma unroll
-        for (int e = 0; e < 8; ++e) wacc[warp][sl * 8 + e] = st.acc[e];
-    }
-    __syncthreads();
-    tl_stamp(p.timing, 6);
-    float mx = -INFINITY, l = 0.f, o = 0.f;
-    if (tid < 64) {
-        mx = wm[0];
-#pragma unroll
-        for (int w = 1; w < ATT_WARPS; ++w) mx = fmaxf(mx, wm[w]);
-#pragma unroll
-        for (int w = 0; w < ATT_WARPS; ++w) {
-            const float cw = wm[w] == -INFINITY ? 0.f : __expf(wm[w] - mx);
-            l = fmaf(wl[w], cw, l);
-            o = fmaf(wacc[w][tid], cw, o);
-        }
-    }
-    if (!SPLIT || nact == 1) {                       // CTA-uniform
-        if (tid < 64) p.out[(size_t)qrow * p.d + h * 64 + tid] = __float2half_rn(o / l);
-    } else {
-        __shared__ int is_last;
-        float* rec = p.part + ((size_t)row * p.H + h) * gridDim.z * 66;
-        if (tid < 64) {
-            rec[blockIdx.z * 66 + 2 + tid] = o;
-            if (tid == 0) { rec[blockIdx.z * 66] = mx; rec[blockIdx.z * 66 + 1] = l; }
-        }
-        __threadfence();
-        __syncthreads();
-        if (tid == 0) is_last = atomicAdd(p.counter + row * p.H + h, 1) == nact - 1;
-        __syncthreads();
-        if (is_last) {
-            __threadfence();
-            if (tid < 64) {
-                float M = -INFINITY;
-                for (int z = 0; z < nact; ++z) M = fmaxf(M, __ldcg(rec + z * 66));
-                float L = 0.f, O = 0.f;
-                for (int z = 0; z < nact; ++z) {     // chunk order: independent of which CTA arrived last
-                    const float cz = __expf(__ldcg(rec + z * 66) - M);
-                    L = fmaf(__ldcg(rec + z * 66 + 1), cz, L);
-                    O = fmaf(__ldcg(rec + z * 66 + 2 + tid), cz, O);
-                }
-                p.out[(size_t)row * p.d + h * 64 + tid] = __float2half_rn(O / L);
-            }
-            if (tid == 0) p.counter[row * p.H + h] = 0;   // ready for the next layer / step
-        }
-    }
-    tl_stamp(p.timing, 3);
-}
-
-// Self attention for one query token, deep-prefetch variant (the default decode path; ACB_LM_ATTN=v1 keeps the kernel
-// above, which also serves prefill and split-KV).  Same work split and arithmetic as lm_attn_kernel<false>: CTA = (row, head), 8 warps,
-// a warp instruction covers 4 consecutive cache positions, 8 lanes share a position.  What changes is how K and V get there: every lane
-// copies its 16-byte slices with cp.async into a private slot of a per-warp shared-memory ring, ATT2_DEPTH iterations deep, and reads
-// them back (its own 32 bytes) one iteration at a time.  With register loads a lane has 128 bytes in flight in bursts (4 iterations
-// requested, then all consumed), less than HBM bandwidth x loaded latency asks of an SM.  The ring keeps up to 8 x 32 bytes per lane
+// Self attention for one query token: CTA = (query row, head), 8 warps, ONE pass over K and V with an online softmax.  A warp
+// instruction covers 4 consecutive cache positions (4 x 128 B = 512 contiguous bytes), 8 lanes share a position (8 dims each).
+// Every lane copies its 16-byte slices of K and V with cp.async into a private slot of a per-warp shared-memory ring,
+// ATT2_DEPTH iterations deep, and reads them back (its own 32 bytes) one iteration at a time: up to 8 x 32 bytes per lane stay
 // outstanding continuously, in shared memory instead of registers.
+// PF (prompt prefill): blockIdx.y is a (token, row) pair tok * rows_real + r; the query at position pos + tok attends to the
+// cache of row r up to and including its own position (the QKV GEMM of the same pass has already appended every token of the
+// pass: causal within the chunk).
 constexpr int ATT2_DEPTH = 8;
+constexpr int ATT2_SMEM = ATT_WARPS * ATT2_DEPTH * 1024;   // the ring, 64 KB
+template <bool PF>
 __global__ void __launch_bounds__(ATT_WARPS * 32) lm_attn2_kernel(AttnParams p) {
     extern __shared__ __align__(16) unsigned char att2sm[];   // [warp][depth][K | V][32 lanes][16 B]
     __shared__ float wm[ATT_WARPS], wl[ATT_WARPS], wacc[ATT_WARPS][64];
     const int h = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int row = blockIdx.y;
+    const int qrow = blockIdx.y, row = PF ? qrow % p.rows_real : qrow, tok = PF ? qrow / p.rows_real : 0;
     const int sl = lane & 7, pg = lane >> 3;
-    tl_stamp(p.timing, 0);
-    pdl_trigger();
-    pdl_wait();
-    tl_stamp(p.timing, 1);
-    const int n = p.fixed_len > 0 ? p.fixed_len : p.pos[0] + 1;
+    const int n = p.fixed_len > 0 ? p.fixed_len : p.pos[0] + tok + 1;
     const size_t base = ((size_t)row * p.H + h) * p.cache_len * 64 + sl * 8;
     const __half* kb = p.kc + base;
     const __half* vb = p.vc + base;
@@ -549,13 +344,12 @@ __global__ void __launch_bounds__(ATT_WARPS * 32) lm_attn2_kernel(AttnParams p) 
 
     float q[8];
     {
-        const float4* qp = reinterpret_cast<const float4*>(p.q + (size_t)row * p.d + h * 64 + sl * 8);
+        const float4* qp = reinterpret_cast<const float4*>(p.q + (size_t)qrow * p.d + h * 64 + sl * 8);
         const float4 qa = qp[0], qb = qp[1];
         q[0] = half_round(qa.x) * p.scale; q[1] = half_round(qa.y) * p.scale; q[2] = half_round(qa.z) * p.scale;
         q[3] = half_round(qa.w) * p.scale; q[4] = half_round(qb.x) * p.scale; q[5] = half_round(qb.y) * p.scale;
         q[6] = half_round(qb.z) * p.scale; q[7] = half_round(qb.w) * p.scale;
     }
-    tl_stamp(p.timing, 4);
     OnlineSM st;
     st.m = -INFINITY; st.l = 0.f;
 #pragma unroll
@@ -598,8 +392,7 @@ __global__ void __launch_bounds__(ATT_WARPS * 32) lm_attn2_kernel(AttnParams p) 
         }
     }
     asm volatile("cp.async.wait_group 0;" ::: "memory");
-    tl_stamp(p.timing, 2);
-    // merge the 4 position groups of the warp, then the warps (as lm_attn_kernel)
+    // merge the 4 position groups of the warp, then the warps
 #pragma unroll
     for (int o = 8; o <= 16; o <<= 1) {
         const float m2 = __shfl_xor_sync(0xffffffffu, st.m, o), l2 = __shfl_xor_sync(0xffffffffu, st.l, o);
@@ -625,9 +418,8 @@ __global__ void __launch_bounds__(ATT_WARPS * 32) lm_attn2_kernel(AttnParams p) 
             l = fmaf(wl[w], cw, l);
             o = fmaf(wacc[w][tid], cw, o);
         }
-        p.out[(size_t)row * p.d + h * 64 + tid] = __float2half_rn(o / l);
+        p.out[(size_t)qrow * p.d + h * 64 + tid] = __float2half_rn(o / l);
     }
-    tl_stamp(p.timing, 3);
 }
 
 // Cross attention over the (short) text condition: one WARP per (row, head), lane = text position for the scores,
@@ -637,10 +429,6 @@ __global__ void __launch_bounds__(256) lm_cross_attn_kernel(AttnParams p, int ro
     __shared__ float qs[8][64];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int pair = blockIdx.x * 8 + warp;          // (row, head) index
-    tl_stamp(p.timing, 0);
-    pdl_trigger();
-    pdl_wait();
-    tl_stamp(p.timing, 1);
     if (pair >= rows * p.H) return;                  // warp-uniform
     const int row = pair / p.H, h = pair % p.H, n = p.fixed_len;
     {
@@ -656,7 +444,6 @@ __global__ void __launch_bounds__(256) lm_cross_attn_kernel(AttnParams p, int ro
         qs[warp][lane * 2 + 1] = half_round(a1) * p.scale;
     }
     __syncwarp();
-    tl_stamp(p.timing, 4);
     const size_t base = ((size_t)(PF ? row % p.rows_real : row) * p.H + h) * p.cache_len * 64;   // K / V of the generation row
     float mx = -INFINITY, l = 0.f, o0 = 0.f, o1 = 0.f;
     for (int t0 = 0; t0 < n; t0 += 32) {             // chunks of 32 text positions (online softmax across chunks)
@@ -677,13 +464,11 @@ __global__ void __launch_bounds__(256) lm_cross_attn_kernel(AttnParams p, int ro
                 }
             }
         }
-        tl_stamp(p.timing, 5);
         const float cm = fmaxf(mx, warp_max(s));
         const float corr = mx == -INFINITY ? 0.f : __expf(mx - cm);
         const float pw = t < n ? __expf(s - cm) : 0.f;
         l = l * corr + warp_sum(pw);
         o0 *= corr; o1 *= corr;
-        tl_stamp(p.timing, 6);
         const int cnt = min(32, n - t0);
         for (int j = 0; j < cnt; ++j) {
             const float wj = __shfl_sync(0xffffffffu, pw, j);
@@ -693,9 +478,7 @@ __global__ void __launch_bounds__(256) lm_cross_attn_kernel(AttnParams p, int ro
         }
         mx = cm;
     }
-    tl_stamp(p.timing, 2);
     *reinterpret_cast<__half2*>(p.out + (size_t)row * p.d + h * 64 + lane * 2) = __floats2half2_rn(o0 / l, o1 / l);
-    tl_stamp(p.timing, 3);
 }
 
 // ------------------------------------------------------------------------------------------------ sampling
@@ -748,8 +531,6 @@ __global__ void __launch_bounds__(1024) lm_sample_kernel(SampleParams p) {
     const float* lc = p.logits + ((size_t)b * p.n_q + k) * card;
     const float* lu = p.logits + ((size_t)((cfg3 ? 2 : 1) * p.batch + b) * p.n_q + k) * card;
     const float* lw = p.logits + ((size_t)(p.batch + b) * p.n_q + k) * card;
-    pdl_trigger();
-    pdl_wait();
     const int cur_pos = p.pos ? p.pos[0] : 0;   // read once: the last block to finish advances it (below)
     const uint32_t step = p.pos ? (uint32_t)cur_pos : p.step;
 
@@ -917,35 +698,10 @@ struct acb_lm {
     int batch = 0, rows = 0, rows_pad = 0, text_len = 0, seq_len = 0, sms = 132;
     int launches = 0;
     bool has_cross = false;
-    bool pdl = false;         // programmatic dependent launch between the kernels of a step (never enabled: see acb_lm_begin)
-    bool attn2 = true;        // deep-prefetch self attention (cp.async ring); ACB_LM_ATTN=v1: register loads
     bool fused = false;       // ACB_LM_STEP=fused / rotary positions: the whole transformer of a step is ONE persistent kernel (lm_step.cu)
     StepLaunch step{};
     unsigned long long* trace = nullptr;   // ACB_LM_STEP_TRACE=1: per-phase %globaltimer stamps of CTA 0
-    // ACB_LM_TIMING=1 (debug): in-kernel time stamps of the layer-0 GEMMs of a directly enqueued step
-    unsigned long long* timing = nullptr;
-    struct TimedGemm { const char* what; int ctas; };
-    std::vector<TimedGemm> timed;
 };
-constexpr int ACB_TIMING_MAX_CTAS = 1024, ACB_TIMING_MAX_GEMMS = 16;
-constexpr size_t ACB_PLAN_COUNTER_BYTES = 4096;   // first bytes of buffers.plan: arrival counters of the split-KV attention
-
-// Launch with (optionally) the programmatic-stream-serialization attribute: the kernel may begin while its
-// predecessor in the stream is still running and synchronises itself with griddepcontrol.wait.
-template <typename... KArgs, typename... Args>
-static cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, bool pdl,
-                            Args... args) {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = s;
-    cudaLaunchAttribute attr[1];
-    if (pdl) {
-        attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[0].val.programmaticStreamSerializationAllowed = 1;
-        cfg.attrs = attr; cfg.numAttrs = 1;
-    }
-    return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
-}
-#define ACB_LAUNCH(...) ACB_CHECK_CUDA(launch_k(__VA_ARGS__))
 
 static int nt_for_rows(int rows) { return rows <= 8 ? 1 : (rows <= 16 ? 2 : (rows <= 32 ? 4 : 8)); }
 
@@ -955,25 +711,26 @@ static size_t gemm_smem_bytes(int nt, int kslice, int ft2 = 1) {
 constexpr int GEMM_MAX_SMEM = 120 * 1024;
 
 template <int EPI, int FT2>
-static int launch_gemm_ft(int nt, const GemmParams& p, int nsplit, cudaStream_t s, bool pdl) {
+static int launch_gemm_ft(int nt, const GemmParams& p, int nsplit, cudaStream_t s) {
     dim3 grid(p.N / (16 * FT2), nsplit);
     const size_t smem = gemm_smem_bytes(nt, p.kslice, FT2);
     ACB_REQUIRE(smem <= (size_t)GEMM_MAX_SMEM && p.N % (16 * FT2) == 0, "lm_gemm: tile does not fit (N=%d kslice=%d ft2=%d)", p.N, p.kslice, FT2);
     switch (nt) {
-        case 1: ACB_LAUNCH((lm_gemm_kernel<1, EPI, FT2>), grid, dim3(128), smem, s, pdl, p); break;
-        case 2: ACB_LAUNCH((lm_gemm_kernel<2, EPI, FT2>), grid, dim3(128), smem, s, pdl, p); break;
-        case 4: ACB_LAUNCH((lm_gemm_kernel<4, EPI, FT2>), grid, dim3(128), smem, s, pdl, p); break;
-        default: ACB_LAUNCH((lm_gemm_kernel<8, EPI, FT2>), grid, dim3(128), smem, s, pdl, p); break;
+        case 1: lm_gemm_kernel<1, EPI, FT2><<<grid, 128, smem, s>>>(p); break;
+        case 2: lm_gemm_kernel<2, EPI, FT2><<<grid, 128, smem, s>>>(p); break;
+        case 4: lm_gemm_kernel<4, EPI, FT2><<<grid, 128, smem, s>>>(p); break;
+        default: lm_gemm_kernel<8, EPI, FT2><<<grid, 128, smem, s>>>(p); break;
     }
+    ACB_LAUNCH_CHECK();
     return ACB_OK;
 }
 template <int EPI>
-static int launch_gemm(int nt, const GemmParams& p, int nsplit, cudaStream_t s, bool pdl, int ft2 = 1) {
+static int launch_gemm(int nt, const GemmParams& p, int nsplit, cudaStream_t s, int ft2 = 1) {
     if (ft2 == 2) {
         if constexpr (EPI == EPI_CROSSKV || EPI == EPI_QKV_PF) { acb_set_error("lm_gemm: this epilogue uses 16-feature tiles"); return ACB_ERR_INVALID; }
-        else return launch_gemm_ft<EPI, 2>(nt, p, nsplit, s, pdl);
+        else return launch_gemm_ft<EPI, 2>(nt, p, nsplit, s);
     }
-    return launch_gemm_ft<EPI, 1>(nt, p, nsplit, s, pdl);
+    return launch_gemm_ft<EPI, 1>(nt, p, nsplit, s);
 }
 
 template <int NT, int EPI, int FT2>
@@ -1071,52 +828,31 @@ static int enqueue_step_kernels(acb_lm* lm, cudaStream_t s, float* logits_out, i
     const size_t kv_layer = (size_t)c.max_rows * H * c.max_seq * 64;
     const size_t ckv_layer = (size_t)c.max_rows * H * c.max_text * 64;
     const float scale = 1.0f / sqrtf(64.f);
-    const bool pdl = lm->pdl;
     int nl = 0, ks = 0;
 
     if (!gemms_only) {
-        if (pf) ACB_LAUNCH(lm_embed_kernel<true>, dim3(rows), dim3(256), 0, s, pdl, (const __half*)lm->w.emb, lm->w.inv_freq,
-                           (const int64_t*)B.seq, (const int*)B.pos, B.x, d, c.n_q, c.card, c.max_seq, lm->batch, c.pos_scale, rows_real);
-        else ACB_LAUNCH(lm_embed_kernel<false>, dim3(rows), dim3(256), 0, s, pdl, (const __half*)lm->w.emb, lm->w.inv_freq,
-                        (const int64_t*)B.seq, (const int*)B.pos, B.x, d, c.n_q, c.card, c.max_seq, lm->batch, c.pos_scale, rows);
+        if (pf) lm_embed_kernel<true><<<rows, 256, 0, s>>>((const __half*)lm->w.emb, lm->w.inv_freq, B.seq, B.pos, B.x, d, c.n_q,
+                                                         c.card, c.max_seq, lm->batch, c.pos_scale, rows_real);
+        else lm_embed_kernel<false><<<rows, 256, 0, s>>>((const __half*)lm->w.emb, lm->w.inv_freq, B.seq, B.pos, B.x, d, c.n_q,
+                                                      c.card, c.max_seq, lm->batch, c.pos_scale, rows);
+        ACB_LAUNCH_CHECK();
         ++nl;
         DBG("lm_embed_kernel", -1);
     }
-    enum { G_QKV, G_O, G_CQ, G_CO, G_FF1, G_FF2, G_HEADS };
-    // split-KV self attention: records and counters live in the (otherwise chain-mode-only) plan buffer
-    // OFF by default (ACB_LM_ATT_SPLIT=3 enables): it only pays at the longest contexts, while its extra (idle) CTAs per
-    // launch cost every shorter step (measured on the previous GPU generation; not re-measured on the H100).
-    int att_split = env_int("ACB_LM_ATT_SPLIT", 1);
-    if (att_split < 1 || att_split > 8 || !B.plan ||
-        ACB_PLAN_COUNTER_BYTES + (size_t)rows * H * att_split * 66 * sizeof(float) > ACB_LM_PLAN_BYTES ||
-        (size_t)rows * H * sizeof(int) > ACB_PLAN_COUNTER_BYTES)
-        att_split = 1;
-    // debug timeline (ACB_LM_TIMING=1): every kernel of layer 0 of a directly enqueued step gets a stamp buffer
-    if (lm->timing && !capturing) lm->timed.clear();
-    auto tl = [&](const char* what, int layer, int ctas) -> unsigned long long* {
-        if (!lm->timing || capturing || gemms_only || layer != 0 || (int)lm->timed.size() >= ACB_TIMING_MAX_GEMMS ||
-            ctas > ACB_TIMING_MAX_CTAS)
-            return nullptr;
-        unsigned long long* t = lm->timing + (size_t)lm->timed.size() * ACB_TIMING_MAX_CTAS * 8;
-        lm->timed.push_back({what, ctas});
-        return t;
-    };
     int pending = 0;  // split-K partial sums waiting to be folded into x by the next LN
     auto ln_launch = [&](const float* gamma, const float* beta, int layer) -> int {
         if (gemms_only) return ACB_OK;
-        ACB_LAUNCH(lm_ln_kernel, dim3(rows), dim3(LN_THREADS), 0, s, pdl, B.x, (const float*)B.part, pending, part_stride, gamma, beta,
-                   (__half*)B.h16, d, tl("ln", layer, rows));
+        lm_ln_kernel<<<rows, LN_THREADS, 0, s>>>(B.x, B.part, pending, part_stride, gamma, beta, (__half*)B.h16, d);
+        ACB_LAUNCH_CHECK();
         ++nl;
         DBG("lm_ln_kernel", layer);
         return ACB_OK;
     };
-    auto partial_gemm = [&](const __half* W, const void* X, int N, int K, int layer, int id) -> int {
+    auto partial_gemm = [&](const __half* W, const void* X, int N, int K, int layer) -> int {
         const int ns = pick_split(N, K, lm->sms, true, &ks);
         GemmParams p = base_gemm(W, X, N, K, rows, ks);
         p.out_f32 = B.part; p.ld_out = N; p.split_stride = part_stride;
-        const int ft2 = pick_ft2(N, K, ns, ks, nt, lm->sms);
-        p.timing = tl(id == G_O ? "gemm_O" : (id == G_CQ ? "gemm_CQ" : (id == G_CO ? "gemm_CO" : "gemm_FFN2")), layer, (N / (16 * ft2)) * ns);
-        ACB_TRY(launch_gemm<EPI_PARTIAL>(nt, p, ns, s, pdl, ft2));
+        ACB_TRY(launch_gemm<EPI_PARTIAL>(nt, p, ns, s, pick_ft2(N, K, ns, ks, nt, lm->sms)));
         ++nl;
         DBG("gemm_EPI_PARTIAL", layer);
         pending = ns;
@@ -1131,48 +867,38 @@ static int enqueue_step_kernels(acb_lm* lm, cudaStream_t s, float* logits_out, i
             GemmParams p = base_gemm((const __half*)lm->w.w_qkv + (size_t)l * 3 * d * d, B.h16, 3 * d, d, rows, ks);
             p.q32 = B.q32; p.kc = (__half*)B.k_cache + l * kv_layer; p.vc = (__half*)B.v_cache + l * kv_layer;
             p.d = d; p.H = H; p.cache_len = c.max_seq; p.pos = B.pos; p.rows_real = rows_real;
-            const int ft2 = pf ? 1 : pick_ft2(3 * d, d, 1, ks, nt, lm->sms);
-            p.timing = tl("gemm_QKV", l, 3 * d / (16 * ft2));
-            if (pf) ACB_TRY(launch_gemm<EPI_QKV_PF>(nt, p, 1, s, pdl, 1));
-            else ACB_TRY(launch_gemm<EPI_QKV>(nt, p, 1, s, pdl, ft2));
+            if (pf) ACB_TRY(launch_gemm<EPI_QKV_PF>(nt, p, 1, s, 1));
+            else ACB_TRY(launch_gemm<EPI_QKV>(nt, p, 1, s, pick_ft2(3 * d, d, 1, ks, nt, lm->sms)));
             ++nl;
             DBG("gemm_EPI_QKV", l);
         }
         if (!gemms_only) {
             AttnParams a{B.q32, 1, 0, (__half*)B.k_cache + l * kv_layer, (__half*)B.v_cache + l * kv_layer, (__half*)B.a16,
-                         H, d, c.max_seq, B.pos, 0, scale};
-            a.timing = tl("attn", l, H * rows * att_split);
-            a.part = reinterpret_cast<float*>((unsigned char*)B.plan + ACB_PLAN_COUNTER_BYTES);
-            a.counter = reinterpret_cast<int*>(B.plan);
-            a.split_min = max(129, env_int("ACB_LM_ATT_SPLIT_MIN", 768));
-            a.rows_real = rows_real;
-            if (pf) ACB_LAUNCH((lm_attn_kernel<false, true>), dim3(H, rows), dim3(ATT_WARPS * 32), 0, s, pdl, a);
-            else if (att_split <= 1 && lm->attn2)
-                ACB_LAUNCH(lm_attn2_kernel, dim3(H, rows), dim3(ATT_WARPS * 32), (size_t)ATT_WARPS * ATT2_DEPTH * 1024, s, pdl, a);
-            else if (att_split > 1) ACB_LAUNCH(lm_attn_kernel<true>, dim3(H, rows, att_split), dim3(ATT_WARPS * 32), 0, s, pdl, a);
-            else ACB_LAUNCH(lm_attn_kernel<false>, dim3(H, rows), dim3(ATT_WARPS * 32), 0, s, pdl, a);
+                         H, d, c.max_seq, B.pos, 0, scale, rows_real};
+            if (pf) lm_attn2_kernel<true><<<dim3(H, rows), ATT_WARPS * 32, ATT2_SMEM, s>>>(a);
+            else lm_attn2_kernel<false><<<dim3(H, rows), ATT_WARPS * 32, ATT2_SMEM, s>>>(a);
+            ACB_LAUNCH_CHECK();
             ++nl;
-            DBG("lm_attn_kernel", l);
+            DBG("lm_attn2_kernel", l);
         }
-        ACB_TRY(partial_gemm((const __half*)lm->w.w_o + (size_t)l * d * d, B.a16, d, d, l, G_O));
+        ACB_TRY(partial_gemm((const __half*)lm->w.w_o + (size_t)l * d * d, B.a16, d, d, l));
         // --- cross attention
         if (lm->has_cross) {
             ACB_TRY(ln_launch(ln + 2 * d, ln + 3 * d, l));
-            ACB_TRY(partial_gemm((const __half*)lm->w.w_cq + (size_t)l * d * d, B.h16, d, d, l, G_CQ));
+            ACB_TRY(partial_gemm((const __half*)lm->w.w_cq + (size_t)l * d * d, B.h16, d, d, l));
             const int nsq = pending;
             pending = 0;   // these partials are the cross-attention queries, not a residual update
             if (!gemms_only) {
                 AttnParams a{B.part, nsq, part_stride, (__half*)B.ck_cache + l * ckv_layer,
                              (__half*)B.cv_cache + l * ckv_layer, (__half*)B.a16, H, d, c.max_text, B.pos, lm->text_len,
-                             scale};
-                a.timing = tl("cross_attn", l, acb_ceil_div(rows * H, 8));
-                a.rows_real = rows_real;
-                if (pf) ACB_LAUNCH(lm_cross_attn_kernel<true>, dim3(acb_ceil_div(rows * H, 8)), dim3(256), 0, s, pdl, a, rows);
-                else ACB_LAUNCH(lm_cross_attn_kernel<false>, dim3(acb_ceil_div(rows * H, 8)), dim3(256), 0, s, pdl, a, rows);
+                             scale, rows_real};
+                if (pf) lm_cross_attn_kernel<true><<<acb_ceil_div(rows * H, 8), 256, 0, s>>>(a, rows);
+                else lm_cross_attn_kernel<false><<<acb_ceil_div(rows * H, 8), 256, 0, s>>>(a, rows);
+                ACB_LAUNCH_CHECK();
                 ++nl;
                 DBG("lm_cross_attn_kernel", l);
             }
-            ACB_TRY(partial_gemm((const __half*)lm->w.w_co + (size_t)l * d * d, B.a16, d, d, l, G_CO));
+            ACB_TRY(partial_gemm((const __half*)lm->w.w_co + (size_t)l * d * d, B.a16, d, d, l));
         }
         // --- feed forward
         ACB_TRY(ln_launch(ln + 4 * d, ln + 5 * d, l));
@@ -1180,12 +906,10 @@ static int enqueue_step_kernels(acb_lm* lm, cudaStream_t s, float* logits_out, i
             pick_split(ffn, d, lm->sms, false, &ks);
             GemmParams p = base_gemm((const __half*)lm->w.w_ff1 + (size_t)l * ffn * d, B.h16, ffn, d, rows, ks);
             p.out_f16 = (__half*)B.f16; p.ld_out = ffn;
-            const int ft2 = pick_ft2(ffn, d, 1, ks, nt, lm->sms);
-            p.timing = tl("gemm_FFN1", l, ffn / (16 * ft2));
-            ACB_TRY(launch_gemm<EPI_GELU>(nt, p, 1, s, pdl, ft2)); ++nl;
+            ACB_TRY(launch_gemm<EPI_GELU>(nt, p, 1, s, pick_ft2(ffn, d, 1, ks, nt, lm->sms))); ++nl;
             DBG("gemm_EPI_GELU", l);
         }
-        ACB_TRY(partial_gemm((const __half*)lm->w.w_ff2 + (size_t)l * d * ffn, B.f16, d, ffn, l, G_FF2));
+        ACB_TRY(partial_gemm((const __half*)lm->w.w_ff2 + (size_t)l * d * ffn, B.f16, d, ffn, l));
     }
     if (pf) {   // no output norm / heads / sampler: the pass only fills the KV cache
         if (n_launch) *n_launch = nl;
@@ -1197,7 +921,7 @@ static int enqueue_step_kernels(acb_lm* lm, cudaStream_t s, float* logits_out, i
         pick_split(N, d, lm->sms, false, &ks);
         GemmParams p = base_gemm(lm->w.heads, B.h16, N, d, rows, ks);
         p.out_f32 = B.logits; p.ld_out = N;
-        ACB_TRY(launch_gemm<EPI_F32>(nt, p, 1, s, pdl, pick_ft2(N, d, 1, ks, nt, lm->sms))); ++nl;
+        ACB_TRY(launch_gemm<EPI_F32>(nt, p, 1, s, pick_ft2(N, d, 1, ks, nt, lm->sms))); ++nl;
         DBG("gemm_EPI_F32", -1);
     }
     if (!gemms_only) {
@@ -1207,7 +931,8 @@ static int enqueue_step_kernels(acb_lm* lm, cudaStream_t s, float* logits_out, i
                         c.max_seq, nullptr, lm->batch, rows, c.n_q, c.card, NP, lm->samp.use_sampling, lm->samp.top_k,
                         lm->samp.temp, lm->samp.top_p, lm->samp.cfg_coef, lm->samp.seed, 0, lm->samp.cfg_coef_beta};
         size_t smem = ((size_t)c.card + 2 * (size_t)NP) * sizeof(float);
-        ACB_LAUNCH(lm_sample_kernel, dim3(c.n_q, lm->batch), dim3(1024), smem, s, pdl, sp);
+        lm_sample_kernel<<<dim3(c.n_q, lm->batch), 1024, smem, s>>>(sp);
+        ACB_LAUNCH_CHECK();
         ++nl;
         DBG("lm_sample_kernel", -1);
     }
@@ -1230,7 +955,8 @@ static int enqueue_step_fused(acb_lm* lm, cudaStream_t s, float* logits_out, int
                         c.max_seq, nullptr, lm->batch, lm->rows, c.n_q, c.card, NP, lm->samp.use_sampling, lm->samp.top_k,
                         lm->samp.temp, lm->samp.top_p, lm->samp.cfg_coef, lm->samp.seed, 0, lm->samp.cfg_coef_beta};
         size_t smem = ((size_t)c.card + 2 * (size_t)NP) * sizeof(float);
-        ACB_LAUNCH(lm_sample_kernel, dim3(c.n_q, lm->batch), dim3(1024), smem, s, false, sp);
+        lm_sample_kernel<<<dim3(c.n_q, lm->batch), 1024, smem, s>>>(sp);
+        ACB_LAUNCH_CHECK();
         ++nl;
         DBG("lm_sample_kernel", -1);
     }
@@ -1262,18 +988,19 @@ extern "C" int acb_lm_create(const acb_lm_config* cfg, const acb_lm_weights* w, 
     cudaDeviceGetAttribute(&lm->sms, cudaDevAttrMultiProcessorCount, dev);
     cudaError_t e = cudaStreamCreateWithFlags(&lm->capture_stream, cudaStreamNonBlocking);
     if (e != cudaSuccess) { delete lm; acb_set_error("acb_lm_create: cudaStreamCreate: %s", cudaGetErrorString(e)); return ACB_ERR_CUDA; }
-    // the GEMMs stage up to ~70 KB of weights per CTA; keep the shared-memory carve-out at its maximum for every kernel
-    // of the step so that co-resident kernels (PDL) never force an L1/shared reconfiguration.
+    // every kernel of the step asks for the maximum shared-memory carve-out: the GEMMs stage up to ~70 KB of weights per CTA and
+    // the attention ring takes 64 KB, and with one L1 / shared split for all of them an SM never changes its configuration
+    // between consecutive kernels of the graph.
     cudaError_t ea = gemm_attr_all<EPI_PARTIAL>();
     if (ea == cudaSuccess) ea = gemm_attr_all<EPI_QKV>();
     if (ea == cudaSuccess) ea = gemm_attr_all<EPI_GELU>();
     if (ea == cudaSuccess) ea = gemm_attr_all<EPI_F32>();
     if (ea == cudaSuccess) ea = gemm_attr_all<EPI_CROSSKV>();
     if (ea == cudaSuccess) ea = gemm_attr_all<EPI_QKV_PF>();
-    if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_attn_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
-    if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_attn_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
-    if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_attn2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_WARPS * ATT2_DEPTH * 1024);
-    if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_attn2_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+    if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_attn2_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT2_SMEM);
+    if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_attn2_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+    if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_attn2_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT2_SMEM);
+    if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_attn2_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_cross_attn_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_ln_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_embed_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
@@ -1297,7 +1024,6 @@ extern "C" int acb_lm_destroy(acb_lm_t* lm) {
     if (!lm) return ACB_OK;
     drop_graph(lm);
     if (lm->capture_stream) cudaStreamDestroy(lm->capture_stream);
-    if (lm->timing) cudaFree(lm->timing);
     if (lm->trace) cudaFree(lm->trace);
     delete lm;
     return ACB_OK;
@@ -1337,7 +1063,7 @@ extern "C" int acb_lm_begin(acb_lm_t* lm, const float* cross, int batch, int row
                                          (const __half*)lm->buf.cross16 + r0 * d, 2 * d, d, (int)min((size_t)64, M - r0), ks);
                 p.kc = (__half*)lm->buf.ck_cache + l * ckv_layer; p.vc = (__half*)lm->buf.cv_cache + l * ckv_layer;
                 p.d = d; p.H = H; p.cache_len = c.max_text; p.text_len = text_len; p.row0 = (int)r0;
-                ACB_TRY(launch_gemm<EPI_CROSSKV>(8, p, 1, s, false));
+                ACB_TRY(launch_gemm<EPI_CROSSKV>(8, p, 1, s));
             }
     }
     // opt in to large dynamic shared memory where needed
@@ -1348,20 +1074,9 @@ extern "C" int acb_lm_begin(acb_lm_t* lm, const float* cross, int batch, int row
         if (smem > 48 * 1024)
             ACB_CHECK_CUDA(cudaFuncSetAttribute(lm_sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     }
-    // capture one decode step with plain stream-order edges.  Launched with programmatic dependent launch (griddepcontrol) the
-    // same kernels reproducibly returned wrong logits on the H100 once the KV cache held more than a few positions, for a cause
-    // not found; there is no switch to turn it on, so every launch goes through the configuration the parity tests pass.
-    // (griddepcontrol.launch_dependents / .wait in the kernels are no-ops for a normally launched kernel.)
+    // capture one decode step; its kernels are chained by plain stream-order edges.  (Launched with programmatic dependent launch,
+    // the same kernels gave wrong logits on the H100 once the KV cache held more than a few positions, for a cause not found.)
     {
-        lm->pdl = false;
-        if (env_int("ACB_LM_TIMING", 0) && !lm->timing) {
-            ACB_CHECK_CUDA(cudaMalloc(&lm->timing, (size_t)ACB_TIMING_MAX_GEMMS * ACB_TIMING_MAX_CTAS * 64));
-            ACB_CHECK_CUDA(cudaMemset(lm->timing, 0, (size_t)ACB_TIMING_MAX_GEMMS * ACB_TIMING_MAX_CTAS * 64));
-        }
-        {
-            const char* ea = getenv("ACB_LM_ATTN");
-            lm->attn2 = !(ea && ea[0] == 'v' && ea[1] == '1');
-        }
         const char* ev = getenv("ACB_LM_STEP");
         // The persistent fused step (lm_step.cu; needs the packed weights) is OPT-IN: ACB_LM_STEP=fused, or a model with rotary
         // positions (only built there); the per-phase graph below is the default.
@@ -1376,7 +1091,6 @@ extern "C" int acb_lm_begin(acb_lm_t* lm, const float* cross, int batch, int row
                 ACB_REQUIRE(lm->step.n_phases + 2 <= 1024, "trace buffer too small");
             }
         }
-        if (lm->buf.plan) ACB_CHECK_CUDA(cudaMemsetAsync(lm->buf.plan, 0, ACB_PLAN_COUNTER_BYTES, s));   // split-KV arrival counters
     }
     for (int attempt = 0; attempt < 2; ++attempt) {
         drop_graph(lm);
@@ -1384,21 +1098,6 @@ extern "C" int acb_lm_begin(acb_lm_t* lm, const float* cross, int batch, int row
         int rc = enqueue_step(lm, lm->capture_stream, nullptr, &lm->launches, false, true);
         cudaError_t e = cudaStreamEndCapture(lm->capture_stream, &lm->graph);
         if (rc == ACB_OK && e == cudaSuccess) e = cudaGraphInstantiate(&lm->exec, lm->graph, 0);
-        if (rc == ACB_OK && e == cudaSuccess && env_int("ACB_LM_GRAPH_INFO", 0)) {   // how many edges are programmatic (PDL)?
-            size_t ne = 0;
-            if (cudaGraphGetEdges_v2(lm->graph, nullptr, nullptr, nullptr, &ne) == cudaSuccess && ne) {
-                std::vector<cudaGraphNode_t> from(ne), to(ne);
-                std::vector<cudaGraphEdgeData> ed(ne);
-                size_t prog = 0, port_prog = 0;
-                if (cudaGraphGetEdges_v2(lm->graph, from.data(), to.data(), ed.data(), &ne) == cudaSuccess)
-                    for (size_t i = 0; i < ne; ++i) {
-                        prog += ed[i].type == cudaGraphDependencyTypeProgrammatic;
-                        port_prog += ed[i].from_port == cudaGraphKernelNodePortProgrammatic;
-                    }
-                fprintf(stderr, "[acb graph] %zu edges, %zu programmatic (from_port programmatic: %zu), pdl=%d\n", ne, prog, port_prog, (int)lm->pdl);
-            }
-            cudaGetLastError();
-        }
         if (rc == ACB_OK && e == cudaSuccess) return ACB_OK;
         cudaGetLastError();
         drop_graph(lm);
@@ -1447,44 +1146,12 @@ extern "C" int acb_lm_prefill(acb_lm_t* lm, int pos0, int n_tokens, void* stream
     return ACB_OK;
 }
 
-extern "C" int acb_lm_uses_pdl(const acb_lm_t* lm) { return lm && lm->pdl ? 1 : 0; }
+extern "C" int acb_lm_uses_pdl(const acb_lm_t*) { return 0; }
 
 extern "C" int acb_lm_steps(acb_lm_t* lm, int n_steps, void* stream) {
     ACB_REQUIRE(lm && lm->exec, "acb_lm_steps: call acb_lm_begin first");
     ACB_REQUIRE(n_steps >= 0, "acb_lm_steps: negative step count");
     for (int i = 0; i < n_steps; ++i) ACB_CHECK_CUDA(cudaGraphLaunch(lm->exec, (cudaStream_t)stream));
-    return ACB_OK;
-}
-
-// Debug timeline of the default step's layer-0 kernels (%globaltimer, ns, relative to the first CTA of the first kernel):
-// CTA starts (first..last), when griddepcontrol.wait returned (median), the kernel's mid stamp (GEMM: weights + k-loop
-// done; median), CTA ends (median..last).
-static int report_timeline(acb_lm* lm, cudaStream_t s) {
-    ACB_CHECK_CUDA(cudaStreamSynchronize(s));
-    std::vector<unsigned long long> h((size_t)ACB_TIMING_MAX_CTAS * 8);
-    unsigned long long t0 = 0;
-    for (size_t gi = 0; gi < lm->timed.size(); ++gi) {
-        const int n = lm->timed[gi].ctas;
-        ACB_CHECK_CUDA(cudaMemcpy(h.data(), lm->timing + gi * ACB_TIMING_MAX_CTAS * 8, (size_t)n * 64, cudaMemcpyDeviceToHost));
-        std::vector<long long> col[8];
-        for (int i = 0; i < n; ++i)
-            for (int sl = 0; sl < 8; ++sl)
-                if (h[i * 8 + sl]) col[sl].push_back((long long)h[i * 8 + sl]);
-        for (auto& v : col) std::sort(v.begin(), v.end());
-        if (col[0].empty() || col[1].empty() || col[3].empty()) continue;
-        if (!t0) t0 = (unsigned long long)col[0].front();
-        const long long w = col[1][col[1].size() / 2];   // median wait-return
-        fprintf(stderr, "[acb timeline] %-10s %4d CTAs  start %6lld..%6lld  wait-returned %6lld  end %6lld (med) %6lld (max) | after wait [ns, median]:",
-                lm->timed[gi].what, n, col[0].front() - (long long)t0, col[0].back() - (long long)t0, w - (long long)t0,
-                col[3][col[3].size() / 2] - (long long)t0, col[3].back() - (long long)t0);
-        static const int order[6] = {4, 5, 6, 7, 2, 3};   // stamps in program order (2 = main loop done, 3 = end)
-        for (int oi = 0; oi < 6; ++oi) {
-            const std::vector<long long>& v = col[order[oi]];
-            if (!v.empty()) fprintf(stderr, "  s%d %lld", order[oi], v[v.size() / 2] - w);
-        }
-        fprintf(stderr, "\n");
-    }
-    ACB_CHECK_CUDA(cudaMemset(lm->timing, 0, (size_t)ACB_TIMING_MAX_GEMMS * ACB_TIMING_MAX_CTAS * 64));
     return ACB_OK;
 }
 
@@ -1554,8 +1221,6 @@ extern "C" int acb_lm_step_logits(acb_lm_t* lm, float* logits_out, void* stream)
     if (lm->fused && lm->trace) lm->step.p.trace = lm->trace;
     ACB_TRY(enqueue_step(lm, (cudaStream_t)stream, logits_out, nullptr));
     if (lm->fused && lm->trace) { lm->step.p.trace = nullptr; ACB_TRY(report_step_trace(lm, (cudaStream_t)stream)); }
-    if (lm->fused) return ACB_OK;
-    if (lm->timing) ACB_TRY(report_timeline(lm, (cudaStream_t)stream));
     return ACB_OK;
 }
 
@@ -1596,54 +1261,4 @@ extern "C" int acb_sample(const float* logits, const float* noise, int64_t* toke
     lm_sample_kernel<<<dim3(n_q, batch), 1024, smem, (cudaStream_t)stream>>>(sp);
     ACB_LAUNCH_CHECK();
     return ACB_OK;
-}
-
-// ------------------------------------------------------------------------------------------------ dependency-latency probe
-// A chain of `n_kernels` dependent EMPTY kernels (grid `ctas` x `threads`, `smem` bytes of dynamic shared memory each)
-// captured in one graph -- with programmatic (PDL) edges when pdl != 0 -- and replayed `reps` times: the time per
-// kernel is the floor any decode step of that many dependent kernels can reach on this GPU.  Measurement aid only.
-__global__ void acb_probe_kernel(int* sink) {
-    pdl_trigger();
-    pdl_wait();
-    if (sink && threadIdx.x == 0 && blockIdx.x == 0) sink[0] += 1;   // a dependent read-modify-write through global memory
-}
-
-extern "C" int acb_debug_chain_latency(int n_kernels, int ctas, int threads, int smem, int pdl, int reps, float* us_per_kernel,
-                                       void* scratch) {
-    ACB_REQUIRE(n_kernels >= 1 && n_kernels <= 4096 && ctas >= 1 && threads >= 32 && threads <= 1024 && reps >= 1 && us_per_kernel,
-                "acb_debug_chain_latency: bad argument");
-    ACB_REQUIRE(smem >= 0 && smem <= 200 * 1024, "acb_debug_chain_latency: smem out of range");
-    if (smem > 48 * 1024)
-        ACB_CHECK_CUDA(cudaFuncSetAttribute(acb_probe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    cudaStream_t s;
-    ACB_CHECK_CUDA(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
-    cudaGraph_t graph = nullptr;
-    cudaGraphExec_t exec = nullptr;
-    cudaEvent_t e0 = nullptr, e1 = nullptr;
-    int rc = ACB_OK;
-    cudaError_t e = cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal);
-    for (int i = 0; i < n_kernels && e == cudaSuccess; ++i)
-        e = launch_k(acb_probe_kernel, dim3(ctas), dim3(threads), (size_t)smem, s, pdl != 0, (int*)scratch);
-    cudaError_t e2 = cudaStreamEndCapture(s, &graph);
-    if (e == cudaSuccess) e = e2;
-    if (e == cudaSuccess) e = cudaGraphInstantiate(&exec, graph, 0);
-    if (e == cudaSuccess) e = cudaEventCreate(&e0);
-    if (e == cudaSuccess) e = cudaEventCreate(&e1);
-    if (e == cudaSuccess) {
-        for (int i = 0; i < 3; ++i) cudaGraphLaunch(exec, s);
-        cudaEventRecord(e0, s);
-        for (int i = 0; i < reps; ++i) cudaGraphLaunch(exec, s);
-        cudaEventRecord(e1, s);
-        e = cudaStreamSynchronize(s);
-        float ms = 0.f;
-        if (e == cudaSuccess) e = cudaEventElapsedTime(&ms, e0, e1);
-        *us_per_kernel = ms * 1e3f / (float)reps / (float)n_kernels;
-    }
-    if (e != cudaSuccess) { acb_set_error("acb_debug_chain_latency: %s", cudaGetErrorString(e)); rc = ACB_ERR_CUDA; cudaGetLastError(); }
-    if (e0) cudaEventDestroy(e0);
-    if (e1) cudaEventDestroy(e1);
-    if (exec) cudaGraphExecDestroy(exec);
-    if (graph) cudaGraphDestroy(graph);
-    cudaStreamDestroy(s);
-    return rc;
 }

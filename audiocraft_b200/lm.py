@@ -190,7 +190,6 @@ class LMModel:
         b['seq_mask'] = torch.zeros((self.n_q, max_seq), device=dev, dtype=torch.uint8)
         b['pos'] = torch.zeros(4, device=dev, dtype=torch.int32)
         b['noise'] = torch.ones((max_batch, self.n_q, self.card), device=dev, dtype=f32)
-        b['plan'] = torch.zeros(_lib.ACB_LM_PLAN_BYTES, device=dev, dtype=torch.uint8)
         self._bufs = b
         cfg = _lib.LMConfig(self.dim, self.num_heads, self.num_layers, self.ffn_dim, self.n_q, self.card,
                             int(self.cross_attention), max_rows, max_seq, max_text,
@@ -201,7 +200,7 @@ class LMModel:
                                                               'wp_o', 'wp_cq', 'wp_co', 'wp_ff1', 'wp_ff2', 'wp_heads', 'rope_freq')])
         bufs = _lib.LMBuffers(*[_lib.ptr(b[n]) for n in ('x', 'h16', 'a16', 'f16', 'q32', 'part', 'logits', 'k_cache',
                                                          'v_cache', 'ck_cache', 'cv_cache', 'cross16', 'seq',
-                                                         'seq_mask', 'pos', 'noise', 'plan', 'stats', 'bar')])
+                                                         'seq_mask', 'pos', 'noise', 'stats', 'bar')])
         handle = C.c_void_p()
         _lib.check(self._lib.acb_lm_create(C.byref(cfg), C.byref(wts), C.byref(bufs), C.byref(handle)), 'lm_create')
         self._handle = handle

@@ -192,7 +192,6 @@ typedef struct {
     uint8_t* seq_mask; /* [n_q][max_seq]     pattern validity mask (codebooks_patterns.py:130-152) */
     int32_t* pos;      /* [4] device ints: pos (tokens in the KV cache), rows, batch, text_len */
     float* noise;      /* [B][n_q][card] Exponential(1) noise, read when sampling.noise_from_buffer != 0 */
-    void* plan;        /* ACB_LM_PLAN_BYTES of scratch (split-KV attention records of the per-phase path) */
     float* stats;      /* [8][rows_pad][2]  LayerNorm (mean, M2) records per d/8 columns (fused step) */
     void* bar;         /* 128 B: grid-barrier counter of the fused step */
 } acb_lm_buffers;
@@ -200,7 +199,6 @@ typedef struct {
 #define ACB_LM_MAX_SPLIT 8
 #define ACB_LM_PART_SLOTS 16
 #define ACB_LM_PREFILL_ROWS 64   /* (token, row) pairs one prefill pass handles = the tallest GEMM tile */
-#define ACB_LM_PLAN_BYTES (2u << 20)
 
 typedef struct {
     int use_sampling;  /* LMModel.generate(use_sampling, temp, top_k, top_p, cfg_coef), lm.py:421-436 */
@@ -249,7 +247,7 @@ int acb_lm_step_logits(acb_lm_t* lm, float* logits_out, void* stream);
  * order, so bench.py can time the dominant kernel with CUDA events in isolation.  *n_launches = kernels enqueued. */
 int acb_lm_debug_gemms(acb_lm_t* lm, void* stream, int* n_launches);
 
-/* 1 if the captured decode step uses programmatic dependent launch edges (currently never: plain stream-order edges). */
+/* Always 0: the captured decode step chains its kernels with plain stream-order edges, not programmatic dependent launch. */
 int acb_lm_uses_pdl(const acb_lm_t* lm);
 
 /* [N][K] row-major fp16 (N % 128 == 0, K % 64 == 0) -> the packed tile layout of acb_lm_weights.wp_*: tile (nt, kb) =
@@ -267,13 +265,6 @@ int acb_lm_rows_pad(int rows);
 
 /* Number of kernel launches one decode step enqueues (bench.py reports gpu_launches from it). */
 int acb_lm_launches_per_step(const acb_lm_t* lm);
-
-/* Measurement aid (no reference counterpart): time per kernel, in microseconds, of a CUDA graph holding a chain of
- * `n_kernels` dependent empty kernels (grid `ctas` x `threads`, `smem` bytes of dynamic shared memory; programmatic
- * dependent-launch edges when pdl != 0), replayed `reps` times.  This is the floor for a decode step of that many
- * dependent kernels (DESIGN.md section 3.1).  `scratch`: one device int the kernels increment, or NULL. */
-int acb_debug_chain_latency(int n_kernels, int ctas, int threads, int smem, int pdl, int reps, float* us_per_kernel,
-                            void* scratch);
 
 /* Measurement aid (no reference counterpart): microseconds per grid-wide barrier of a cooperative kernel of `ctas`
  * co-resident CTAs x `threads` that does nothing but `n_barriers` barriers (`work` dependent FMAs in between).

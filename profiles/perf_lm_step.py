@@ -16,7 +16,7 @@ ap = argparse.ArgumentParser()
 ap.add_argument('--scale', default='medium')
 ap.add_argument('--batch', type=int, default=8)
 ap.add_argument('--one', type=int, default=-1, help='run a single direct (non-graph) step at this KV length and exit')
-ap.add_argument('--reps', type=int, default=1, help='with --one: repeat the step (ACB_LM_TIMING=1 prints stamps each time)')
+ap.add_argument('--reps', type=int, default=1, help='with --one: repeat the step')
 a = ap.parse_args()
 
 lm = load_lm_model(f'synthetic/{a.scale}')
@@ -36,7 +36,7 @@ if a.one >= 0:
         _lib.check(lm._lib.acb_lm_step_logits(lm._handle, None, _lib.stream()))
         torch.cuda.synchronize()
     sys.exit(0)
-print(f'pdl={lm._lib.acb_lm_uses_pdl(lm._handle)} launches/step={lm._lib.acb_lm_launches_per_step(lm._handle)} '
+print(f'launches/step={lm._lib.acb_lm_launches_per_step(lm._handle)} '
       f'W_step={lm.weight_bytes_per_step / 1e9:.2f} GB')
 for t in (0, 375, 750, 1125, 1499):
     reps = 20
@@ -51,7 +51,7 @@ for t in (0, 375, 750, 1125, 1499):
         torch.cuda.synchronize()
     ms = e0.elapsed_time(e1) / reps
     byt = lm.weight_bytes_per_step + 2 * B * (t + 1) * kv_tok
-    # the same step as direct stream launches (no graph): tells whether the graph keeps the PDL overlap
+    # the same step as direct stream launches (no graph): what the graph saves in launch overhead
     for it in range(2):
         torch.cuda.synchronize()
         e0.record()

@@ -215,36 +215,23 @@ def test_musicgen_api_shapes_and_callbacks():
         mg.generate_with_chroma(['x'], None, 16000)
 
 
-def test_long_context_split_kv_attention(monkeypatch):
-    """Long contexts (>= ACB_LM_ATT_SPLIT_MIN positions, default 768; 129 here) cut self attention into up to three KV
-    chunks per (row, head); the last chunk CTA to arrive merges the (m, l, acc) records in chunk order.  420
-    teacher-forced steps (chunk layouts 1 -> 2 -> 3 and the 256-wide chunks after position 384): against the single-CTA
-    path (ACB_LM_ATT_SPLIT=1) and the oracle."""
-    monkeypatch.setenv('ACB_LM_ATT_SPLIT', '3')         # opt-in (measured net-negative on the 30 s workload, see lm.cu)
-    monkeypatch.setenv('ACB_LM_ATT_SPLIT_MIN', '129')   # default 768: split from the first eligible length here
-    cfg, sd, m = _model('lm_mini', 9)
-    B, T = 2, 420
+@pytest.mark.parametrize('name,B,T', [('lm_mini', 2, 420), ('lm_medium_2l', 8, 300)])
+def test_long_context_attention_matches_oracle(name, B, T):
+    """Self attention over long contexts: T teacher-forced steps, so the K / V ring of lm_attn2_kernel (8 warps x 4 positions
+    per iteration, 8 iterations deep) wraps many times; the medium case runs at the bench width (rows 16).  CFG-mixed logits
+    vs the fp16-emulating oracle."""
+    cfg, sd, m = _model(name, 9)
     _, _, cross = H.lm_condition(cfg, sd, B, 5, 4)
     seq = torch.randint(0, cfg['card'], (B, 4, T + 4), generator=torch.Generator().manual_seed(5))
     o = LO.LMOracle(sd, cfg, half_gemm=True)
     rec = []
     o.generate(None, cross, B, T, use_sampling=False, record_logits=rec, teacher=seq)
     ref = torch.stack(rec)
-    split = m.teacher_forced_logits(o.last_sequence, cross, cfg['cfg_coef']).cpu()
-    monkeypatch.setenv('ACB_LM_ATT_SPLIT', '1')
-    single = m.teacher_forced_logits(o.last_sequence, cross, cfg['cfg_coef']).cpu()
-    monkeypatch.setenv('ACB_LM_ATT_SPLIT', '3')
+    lg = m.teacher_forced_logits(o.last_sequence, cross, cfg['cfg_coef']).cpu()
     n = ref.shape[0]
-    print(f'split-KV: max |split - single| {(split - single).abs().max():.2e}, max |split - oracle| '
-          f'{(split[:n] - ref).abs().max():.2e} on |logits| <= {ref.abs().max():.1f}')
-    assert torch.isfinite(split).all()
-    torch.testing.assert_close(split, single, rtol=0, atol=3e-2)
-    torch.testing.assert_close(split[:n], ref, rtol=2e-2, atol=3e-2)
-    # the graph-replayed generation takes the same path
-    out = m.generate(None, [], num_samples=B, max_gen_len=300, use_sampling=False, cross_attention_src=cross).cpu()
-    monkeypatch.setenv('ACB_LM_ATT_SPLIT', '1')
-    out1 = m.generate(None, [], num_samples=B, max_gen_len=300, use_sampling=False, cross_attention_src=cross).cpu()
-    assert (out == out1).float().mean() > 0.9
+    print(f'{name} B={B} T={T}: max |logit diff| vs oracle {(lg[:n] - ref).abs().max():.2e} on |logits| <= {ref.abs().max():.1f}')
+    assert torch.isfinite(lg).all()
+    torch.testing.assert_close(lg[:n], ref, rtol=2e-2, atol=3e-2)
 
 
 @pytest.mark.parametrize('name,B', [('lm_medium_2l', 8), ('lm_large_2l', 4), ('lm_medium_2l', 2)])
@@ -419,21 +406,6 @@ def test_fused_step_matches_per_phase_kernels(monkeypatch, name, B):
     print(f'{name} B={B}: max |fused - per-phase| = {(fused - base).abs().max():.2e} on |logits| <= {base.abs().max():.1f}')
     torch.testing.assert_close(fused, base, rtol=0, atol=4e-2)
     assert (out_f == out_b).float().mean() > 0.9
-
-
-@pytest.mark.parametrize('name,B,T', [('lm_mini', 3, 70), ('lm_medium_2l', 8, 300)])
-def test_cp_async_attention_is_bit_identical_to_register_loads(monkeypatch, name, B, T):
-    """lm_attn2_kernel (K / V through a per-warp cp.async ring, the decode default) visits the cache positions in the same per-lane order
-    and merges them with the same tree as lm_attn_kernel (register loads, ACB_LM_ATTN=v1): the logits must be bit-identical, over
-    contexts long enough to wrap the 8-deep ring many times (T > 32 x 8 positions)."""
-    cfg, sd, m = _model(name, 5)
-    _, _, cross = H.lm_condition(cfg, sd, B, 5, 1)
-    seq = torch.randint(0, cfg['card'], (B, 4, T + 4), generator=torch.Generator().manual_seed(2))
-    keep = [0, 1, 31, 32, 33, T // 2, T - 2, T - 1]
-    a = m.teacher_forced_logits(seq, cross, 3.0, n_steps=T, keep=keep).cpu()
-    monkeypatch.setenv('ACB_LM_ATTN', 'v1')
-    b = m.teacher_forced_logits(seq, cross, 3.0, n_steps=T, keep=keep).cpu()
-    assert torch.equal(a, b), f'max diff {(a - b).abs().max():.3e}'
 
 
 @pytest.mark.parametrize('name,B,T0', [('lm_mini', 2, 9), ('lm_mini', 5, 23), ('lm_medium_2l', 8, 21)])

@@ -67,6 +67,10 @@ def test_sass_is_sm90a():
     from audiocraft_b200 import _lib
     out = subprocess.run(['cuobjdump', '-lelf', _lib.LIB_PATH], capture_output=True, text=True).stdout
     assert 'sm_90a' in out, out
+    # no programmatic-dependent-launch points (griddepcontrol.wait / .launch_dependents): the decode graph uses plain edges
+    sass = subprocess.run(['cuobjdump', '-sass', _lib.LIB_PATH], capture_output=True, text=True, check=True).stdout
+    assert 'lm_gemm_kernel' in sass
+    assert 'ACQBULK' not in sass and 'PREEXIT' not in sass
 
 
 def test_no_cpu_fallback():

@@ -26,14 +26,12 @@ class LMConfig(C.Structure):
 
 class LMWeights(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ('emb', 'inv_freq', 'w_qkv', 'w_o', 'w_cq', 'w_ckv', 'w_co', 'w_ff1',
-                                           'w_ff2', 'ln', 'out_norm', 'heads', 'wp_qkv', 'wp_o', 'wp_cq', 'wp_co',
-                                           'wp_ff1', 'wp_ff2', 'wp_heads', 'rope_freq')]
+                                           'w_ff2', 'ln', 'out_norm', 'heads', 'rope_freq')]
 
 
 class LMBuffers(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ('x', 'h16', 'a16', 'f16', 'q32', 'part', 'logits', 'k_cache', 'v_cache',
-                                           'ck_cache', 'cv_cache', 'cross16', 'seq', 'seq_mask', 'pos', 'noise', 'stats',
-                                           'bar')]
+                                           'ck_cache', 'cv_cache', 'cross16', 'seq', 'seq_mask', 'pos', 'noise')]
 
 
 class LMSampling(C.Structure):
@@ -78,17 +76,14 @@ def lib():
     L.acb_lm_step_logits.argtypes = [vp, vp, vp]
     L.acb_lm_launches_per_step.argtypes = [vp]
     L.acb_lm_rows_pad.argtypes = [ci]
-    L.acb_lm_pack_weight.argtypes = [vp, vp, ci, ci, vp]
-    L.acb_lm_debug_step_plan.argtypes = [vp, C.POINTER(ci)]
     L.acb_lm_uses_pdl.argtypes = [vp]
     L.acb_lm_debug_gemms.argtypes = [vp, vp, C.POINTER(ci)]
     L.acb_sample.argtypes = [vp, vp, vp, ci, ci, ci, ci, C.POINTER(LMSampling), C.c_uint64, vp]
-    L.acb_debug_grid_barrier.argtypes = [ci, ci, ci, ci, ci, ci, C.POINTER(C.c_float)]
     for name in ('acb_weight_norm_fold', 'acb_conv1d', 'acb_convtr1d', 'acb_lstm_recurrent', 'acb_rvq_encode',
                  'acb_rvq_decode', 'acb_lm_create', 'acb_lm_destroy', 'acb_lm_begin', 'acb_lm_steps',
                  'acb_lm_step_logits', 'acb_lm_launches_per_step', 'acb_lm_rows_pad', 'acb_sample',
                  'acb_device_sm_count', 'acb_lm_debug_gemms', 'acb_lm_uses_pdl',
-                 'acb_conv1d_t6', 'acb_conv1d_t6_tile', 'acb_debug_grid_barrier', 'acb_lm_pack_weight', 'acb_lm_debug_step_plan', 'acb_lm_prefill',
+                 'acb_conv1d_t6', 'acb_conv1d_t6_tile', 'acb_lm_prefill',
                  'acb_resblock', 'acb_resblock_supported'):
         getattr(L, name).restype = ci
     _lib = L
@@ -100,8 +95,7 @@ EXPORTS = ['acb_version', 'acb_last_error', 'acb_device_sm_count', 'acb_weight_n
            'acb_lstm_recurrent', 'acb_lstm_state_bytes', 'acb_rvq_encode', 'acb_rvq_decode', 'acb_lm_create',
            'acb_lm_destroy', 'acb_lm_begin', 'acb_lm_steps', 'acb_lm_step_logits', 'acb_lm_rows_pad',
            'acb_lm_launches_per_step', 'acb_lm_debug_gemms', 'acb_lm_uses_pdl', 'acb_sample', 'acb_conv1d_t6', 'acb_conv1d_t6_tile',
-           'acb_debug_grid_barrier', 'acb_lm_pack_weight', 'acb_lm_debug_step_plan', 'acb_lm_prefill', 'acb_resblock',
-           'acb_resblock_supported']
+           'acb_lm_prefill', 'acb_resblock', 'acb_resblock_supported']
 
 
 def check(rc: int, what: str = ''):

@@ -17,12 +17,9 @@
 //     every step (the reference recomputes them, transformer.py:355-357).
 //   * self attention: one CTA per (query row, head) streaming K and V through a cp.async ring (lm_attn2_kernel), for the decode
 //     step and for prompt prefill alike.
-// The opt-in alternative, one persistent kernel for the whole step, is lm_step.cu (DESIGN.md section 3.1.1).
 #include "common.cuh"
-#include "lm_step.cuh"
 #include <math.h>
 #include <new>
-#include <vector>
 #include <stdio.h>
 #include <stdlib.h>
 
@@ -80,12 +77,13 @@ __device__ __forceinline__ float block_max(float v, float* red) {
 
 // ------------------------------------------------------------------------------------------------ embed + sin pos
 // x[r] = sum_k emb_k[seq[b,k,pos]] + pos_scale * [cos(pos/f_i), sin(pos/f_i)]   (lm.py:244, transformer.py:70-89,701-705)
+// The sin term only when sin_pos ('sin' and 'sin_rope'; a 'rope' model has its positions in the QKV epilogue alone).
 // PF (prompt prefill): the grid's rows are (token, row) pairs r = tok * rows_real + row at positions P[0] + tok.
 template <bool PF>
 __global__ void __launch_bounds__(256) lm_embed_kernel(const __half* __restrict__ emb, const float* __restrict__ inv_freq,
                                                        const int64_t* __restrict__ seq, const int* __restrict__ P,
                                                        float* __restrict__ x, int d, int n_q, int card, int max_seq,
-                                                       int batch, float pos_scale, int rows_real) {
+                                                       int batch, float pos_scale, int rows_real, bool sin_pos) {
     const int r = blockIdx.x, b = (PF ? r % rows_real : r) % batch, pos = P[0] + (PF ? r / rows_real : 0);
     __shared__ int tok[16];
     if (threadIdx.x < n_q) {
@@ -97,9 +95,11 @@ __global__ void __launch_bounds__(256) lm_embed_kernel(const __half* __restrict_
     for (int i = threadIdx.x; i < d; i += 256) {   // d % 32 == 0: a warp is entirely inside or outside the row
         float v = 0.f;
         for (int k = 0; k < n_q; ++k) v += __half2float(emb[((size_t)k * (card + 1) + tok[k]) * d + i]);
-        const int j = i < half_d ? i : i - half_d;
-        const float phase = (float)pos / inv_freq[j];
-        v += pos_scale * (i < half_d ? cosf(phase) : sinf(phase));
+        if (sin_pos) {
+            const int j = i < half_d ? i : i - half_d;
+            const float phase = (float)pos / inv_freq[j];
+            v += pos_scale * (i < half_d ? cosf(phase) : sinf(phase));
+        }
         x[(size_t)r * d + i] = v;
     }
 }
@@ -150,18 +150,41 @@ __global__ void __launch_bounds__(LN_THREADS) lm_ln_kernel(float* __restrict__ x
 }
 
 // ------------------------------------------------------------------------------------------------ skinny GEMM
-enum { EPI_PARTIAL = 0, EPI_QKV = 1, EPI_GELU = 2, EPI_F32 = 3, EPI_CROSSKV = 4, EPI_QKV_PF = 5 };   // _PF: prompt prefill, rows are (token, row) pairs
+// _PF: prompt prefill, rows are (token, row) pairs; _ROPE: q and k rotated (rotary positions) before they are stored
+enum { EPI_PARTIAL = 0, EPI_QKV = 1, EPI_GELU = 2, EPI_F32 = 3, EPI_CROSSKV = 4, EPI_QKV_PF = 5, EPI_QKV_ROPE = 6, EPI_QKV_PF_ROPE = 7 };
 
+// The rotary fields live in padding and in a field the QKV epilogues do not use, so the struct keeps its size and offsets:
+// ptxas schedules every instance by the parameter layout, and 16 more bytes made the MusicGen-medium decode GEMM pass 2 %
+// slower (2.68 vs 2.62 ms, H100 80GB HBM3 at a 400 W limit).
 struct GemmParams {
     const __half* W;  // [N][K] fp16, reference layout
     const __half* X;  // [8*NT][K] fp16, rows >= `rows` are zero
     int N, K, rows, kslice;                            // kslice: K elements per CTA (grid.y slices)
-    float* out_f32; int ld_out; size_t split_stride;  // PARTIAL / F32
-    __half* out_f16;                                   // GELU
+    float* out_f32; int ld_out;                        // PARTIAL / F32
+    float pos_scale;                                   // QKV_ROPE / QKV_PF_ROPE: positional_scale
+    size_t split_stride;                               // PARTIAL
+    union {
+        __half* out_f16;                               // GELU
+        const float* rope_freq;                        // QKV_ROPE / QKV_PF_ROPE: [32] RotaryEmbedding.frequencies
+    };
     float* q32; __half* kc; __half* vc; int d, H, cache_len; const int* pos;  // QKV / CROSSKV
     int text_len, row0;                                                      // CROSSKV
     int rows_real;                                                           // QKV_PF: rows of the generation (GEMM row = tok * rows_real + row)
 };
+static_assert(sizeof(GemmParams) == 128, "GemmParams layout");
+
+// RotaryEmbedding.rotate_qk (modules/rope.py:84-125) on one fp16 element of q / k at position pos: the head dim is 32 complex
+// pairs (2i, 2i+1), rotated by pos * max_period^(-2i/64) in fp32 and blended with `pos_scale`; `other` is the pair partner.
+// Out of line: sincosf is large and rotary positions are an option, not the released models' default.
+__device__ __noinline__ float rope_rotate(const float* rope_freq, float pos_scale, float vh, float other, int dd, int pos) {
+    const bool even = (dd & 1) == 0;
+    const float re = even ? vh : other, im = even ? other : vh;
+    const float ang = (float)pos * rope_freq[dd >> 1];
+    float sn, cs;
+    sincosf(ang, &sn, &cs);
+    const float rr = cs * pos_scale + (1.f - pos_scale), ri = sn * pos_scale;
+    return even ? re * rr - im * ri : re * ri + im * rr;
+}
 
 // CTA = 4 warps, tile = 16 output features x kslice of K.  The CTA's 16 x kslice weight slab is fetched by ONE thread
 // with 16 TMA bulk copies (one per W row, padded pitch => conflict-free fragment reads), issued before the first activation
@@ -173,6 +196,8 @@ __global__ void __launch_bounds__(128) lm_gemm_kernel(GemmParams p) {
     constexpr int U = NT <= 2 ? 4 : (NT <= 4 ? 2 : 1);   // k-blocks per batch of activation loads
     constexpr int RP = 8 * NT + 1;
     constexpr int FB = 16 * FT2;                     // output features per CTA
+    constexpr bool ROPE = EPI == EPI_QKV_ROPE || EPI == EPI_QKV_PF_ROPE, PF = EPI == EPI_QKV_PF || EPI == EPI_QKV_PF_ROPE;
+    constexpr bool QKV = EPI == EPI_QKV || PF || ROPE;
     extern __shared__ __align__(128) unsigned char gsm[];
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, c4 = lane & 3;
     const int f0 = blockIdx.x * FB;
@@ -191,7 +216,7 @@ __global__ void __launch_bounds__(128) lm_gemm_kernel(GemmParams p) {
             bulk_g2s(gsm + r * pitch, p.W + (size_t)(f0 + r) * p.K + k0, (uint32_t)ks * 2u, bar);
     }
     int cache_pos = 0;
-    if (EPI == EPI_QKV || EPI == EPI_QKV_PF) cache_pos = p.pos[0];   // requested now, consumed in the epilogue: off the critical path
+    if (QKV) cache_pos = p.pos[0];   // requested now, consumed in the epilogue: off the critical path
 
     float c[FT2][NT][4];
 #pragma unroll
@@ -258,20 +283,19 @@ __global__ void __launch_bounds__(128) lm_gemm_kernel(GemmParams p) {
             p.out_f32[(size_t)row * p.ld_out + n] = v;
         } else if (EPI == EPI_GELU) {
             p.out_f16[(size_t)row * p.ld_out + n] = __float2half_rn(gelu_erf(half_round(v)));
-        } else if (EPI == EPI_QKV) {   // q | k | v blocks of d features each (no integer division: cold code costs here)
+        } else if (QKV) {   // q | k | v blocks of d features each (no integer division: cold code costs here)
+            // prefill: row = tk * rows_real + rr -> cache row rr, position cache_pos + tk
             const int which = n >= 2 * p.d ? 2 : (n >= p.d ? 1 : 0), nn = n - which * p.d;
-            if (which == 0) {
-                p.q32[(size_t)row * p.d + nn] = v;
-            } else {
-                __half* cache = which == 2 ? p.vc : p.kc;
-                cache[(((size_t)row * p.H + (nn >> 6)) * p.cache_len + cache_pos) * 64 + (nn & 63)] = __float2half_rn(v);
+            const int tk = PF ? row / p.rows_real : 0, rr = row - tk * p.rows_real;
+            if (ROPE && which < 2) {   // the pair partner is feature n ^ 1 of the same CTA (f0 % 16 == 0), same warp order
+                float other = 0.f;
+#pragma unroll
+                for (int w = 0; w < 4; ++w) other += red[(w * FB + (feat ^ 1)) * RP + row];
+                v = rope_rotate(p.rope_freq, p.pos_scale, half_round(v), half_round(other), nn & 63, cache_pos + tk);
             }
-        } else if (EPI == EPI_QKV_PF) {   // prefill: row = tok * rows_real + r -> cache row r, position pos + tok
-            const int which = n >= 2 * p.d ? 2 : (n >= p.d ? 1 : 0), nn = n - which * p.d;
             if (which == 0) {
                 p.q32[(size_t)row * p.d + nn] = v;
             } else {
-                const int tk = row / p.rows_real, rr = row - tk * p.rows_real;
                 __half* cache = which == 2 ? p.vc : p.kc;
                 cache[(((size_t)rr * p.H + (nn >> 6)) * p.cache_len + cache_pos + tk) * 64 + (nn & 63)] = __float2half_rn(v);
             }
@@ -698,9 +722,6 @@ struct acb_lm {
     int batch = 0, rows = 0, rows_pad = 0, text_len = 0, seq_len = 0, sms = 132;
     int launches = 0;
     bool has_cross = false;
-    bool fused = false;       // ACB_LM_STEP=fused / rotary positions: the whole transformer of a step is ONE persistent kernel (lm_step.cu)
-    StepLaunch step{};
-    unsigned long long* trace = nullptr;   // ACB_LM_STEP_TRACE=1: per-phase %globaltimer stamps of CTA 0
 };
 
 static int nt_for_rows(int rows) { return rows <= 8 ? 1 : (rows <= 16 ? 2 : (rows <= 32 ? 4 : 8)); }
@@ -727,7 +748,7 @@ static int launch_gemm_ft(int nt, const GemmParams& p, int nsplit, cudaStream_t 
 template <int EPI>
 static int launch_gemm(int nt, const GemmParams& p, int nsplit, cudaStream_t s, int ft2 = 1) {
     if (ft2 == 2) {
-        if constexpr (EPI == EPI_CROSSKV || EPI == EPI_QKV_PF) { acb_set_error("lm_gemm: this epilogue uses 16-feature tiles"); return ACB_ERR_INVALID; }
+        if constexpr (EPI == EPI_CROSSKV || EPI == EPI_QKV_PF || EPI == EPI_QKV_PF_ROPE) { acb_set_error("lm_gemm: this epilogue uses 16-feature tiles"); return ACB_ERR_INVALID; }
         else return launch_gemm_ft<EPI, 2>(nt, p, nsplit, s);
     }
     return launch_gemm_ft<EPI, 1>(nt, p, nsplit, s);
@@ -746,7 +767,7 @@ static cudaError_t gemm_attr_all() {
     if ((e = gemm_attr_one<2, EPI, 1>()) != cudaSuccess) return e;
     if ((e = gemm_attr_one<4, EPI, 1>()) != cudaSuccess) return e;
     if ((e = gemm_attr_one<8, EPI, 1>()) != cudaSuccess) return e;
-    if constexpr (EPI != EPI_CROSSKV && EPI != EPI_QKV_PF) {
+    if constexpr (EPI != EPI_CROSSKV && EPI != EPI_QKV_PF && EPI != EPI_QKV_PF_ROPE) {
         if ((e = gemm_attr_one<1, EPI, 2>()) != cudaSuccess) return e;
         if ((e = gemm_attr_one<2, EPI, 2>()) != cudaSuccess) return e;
         if ((e = gemm_attr_one<4, EPI, 2>()) != cudaSuccess) return e;
@@ -790,11 +811,6 @@ static GemmParams base_gemm(const void* W, const void* X, int N, int K, int rows
     return p;
 }
 
-static int env_int(const char* name, int dflt) {
-    const char* e = getenv(name);
-    return (e && e[0]) ? atoi(e) : dflt;
-}
-
 #define ACB_TRY(expr) do { int rc_ = (expr); if (rc_ != ACB_OK) return rc_; } while (0)
 
 // ACB_DEBUG=1: synchronise and report after every launch of a directly-enqueued step (not during graph capture).
@@ -817,8 +833,8 @@ static int acb_dbg(cudaStream_t s, bool capturing, const char* what, int layer) 
 // the same kernels run on rows * pf_tokens (token, row) pairs -- positions pos .. pos + pf_tokens - 1 of every row at once, causal
 // inside the pass because the QKV GEMM appends all of them to the cache before the attention kernel runs -- and stop after the
 // last layer (no logits: the next decode step consumes the last prompt position).
-static int enqueue_step_kernels(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_launch, bool gemms_only,
-                                bool capturing, int pf_tokens = 0) {
+static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_launch, bool gemms_only = false,
+                        bool capturing = false, int pf_tokens = 0) {
     const acb_lm_config& c = lm->cfg;
     const acb_lm_buffers& B = lm->buf;
     const bool pf = pf_tokens > 0;
@@ -831,10 +847,11 @@ static int enqueue_step_kernels(acb_lm* lm, cudaStream_t s, float* logits_out, i
     int nl = 0, ks = 0;
 
     if (!gemms_only) {
+        const bool sin_pos = c.positional_embedding != 1;
         if (pf) lm_embed_kernel<true><<<rows, 256, 0, s>>>((const __half*)lm->w.emb, lm->w.inv_freq, B.seq, B.pos, B.x, d, c.n_q,
-                                                         c.card, c.max_seq, lm->batch, c.pos_scale, rows_real);
+                                                         c.card, c.max_seq, lm->batch, c.pos_scale, rows_real, sin_pos);
         else lm_embed_kernel<false><<<rows, 256, 0, s>>>((const __half*)lm->w.emb, lm->w.inv_freq, B.seq, B.pos, B.x, d, c.n_q,
-                                                      c.card, c.max_seq, lm->batch, c.pos_scale, rows);
+                                                      c.card, c.max_seq, lm->batch, c.pos_scale, rows, sin_pos);
         ACB_LAUNCH_CHECK();
         ++nl;
         DBG("lm_embed_kernel", -1);
@@ -867,8 +884,11 @@ static int enqueue_step_kernels(acb_lm* lm, cudaStream_t s, float* logits_out, i
             GemmParams p = base_gemm((const __half*)lm->w.w_qkv + (size_t)l * 3 * d * d, B.h16, 3 * d, d, rows, ks);
             p.q32 = B.q32; p.kc = (__half*)B.k_cache + l * kv_layer; p.vc = (__half*)B.v_cache + l * kv_layer;
             p.d = d; p.H = H; p.cache_len = c.max_seq; p.pos = B.pos; p.rows_real = rows_real;
-            if (pf) ACB_TRY(launch_gemm<EPI_QKV_PF>(nt, p, 1, s, 1));
-            else ACB_TRY(launch_gemm<EPI_QKV>(nt, p, 1, s, pick_ft2(3 * d, d, 1, ks, nt, lm->sms)));
+            p.rope_freq = lm->w.rope_freq; p.pos_scale = c.pos_scale;
+            const bool rope = c.positional_embedding != 0;
+            const int ft2 = pf ? 1 : pick_ft2(3 * d, d, 1, ks, nt, lm->sms);
+            if (pf) ACB_TRY(rope ? launch_gemm<EPI_QKV_PF_ROPE>(nt, p, 1, s, ft2) : launch_gemm<EPI_QKV_PF>(nt, p, 1, s, ft2));
+            else ACB_TRY(rope ? launch_gemm<EPI_QKV_ROPE>(nt, p, 1, s, ft2) : launch_gemm<EPI_QKV>(nt, p, 1, s, ft2));
             ++nl;
             DBG("gemm_EPI_QKV", l);
         }
@@ -940,36 +960,6 @@ static int enqueue_step_kernels(acb_lm* lm, cudaStream_t s, float* logits_out, i
     return ACB_OK;
 }
 
-// Fused step: [memset of the barrier counter] -> lm_step_kernel (embed ... logits) -> lm_sample_kernel.
-static int enqueue_step_fused(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_launch, bool step_only, bool capturing) {
-    const acb_lm_config& c = lm->cfg;
-    const acb_lm_buffers& B = lm->buf;
-    int nl = 0;
-    ACB_TRY(lm_step_launch(lm->step, s));
-    ++nl;
-    DBG("lm_step_kernel", -1);
-    if (!step_only) {
-        int NP = 1;
-        while (NP < c.card) NP <<= 1;
-        SampleParams sp{B.logits, lm->samp.noise_from_buffer ? B.noise : nullptr, logits_out, B.seq, B.seq_mask, B.pos,
-                        c.max_seq, nullptr, lm->batch, lm->rows, c.n_q, c.card, NP, lm->samp.use_sampling, lm->samp.top_k,
-                        lm->samp.temp, lm->samp.top_p, lm->samp.cfg_coef, lm->samp.seed, 0, lm->samp.cfg_coef_beta};
-        size_t smem = ((size_t)c.card + 2 * (size_t)NP) * sizeof(float);
-        lm_sample_kernel<<<dim3(c.n_q, lm->batch), 1024, smem, s>>>(sp);
-        ACB_LAUNCH_CHECK();
-        ++nl;
-        DBG("lm_sample_kernel", -1);
-    }
-    if (n_launch) *n_launch = nl;
-    return ACB_OK;
-}
-
-static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_launch, bool gemms_only = false,
-                        bool capturing = false) {
-    if (lm->fused) return enqueue_step_fused(lm, s, logits_out, n_launch, gemms_only, capturing);
-    return enqueue_step_kernels(lm, s, logits_out, n_launch, gemms_only, capturing);
-}
-
 extern "C" int acb_lm_create(const acb_lm_config* cfg, const acb_lm_weights* w, const acb_lm_buffers* buf, acb_lm_t** out) {
     ACB_REQUIRE(cfg && w && buf && out, "acb_lm_create: null argument");
     ACB_REQUIRE(cfg->dim % 64 == 0 && cfg->dim == cfg->num_heads * 64, "acb_lm_create: head_dim must be 64 (dim=%d heads=%d)",
@@ -980,6 +970,9 @@ extern "C" int acb_lm_create(const acb_lm_config* cfg, const acb_lm_weights* w, 
     ACB_REQUIRE(cfg->max_rows >= 1 && cfg->max_rows <= 64, "acb_lm_create: max_rows %d not in [1,64]", cfg->max_rows);
     ACB_REQUIRE(cfg->max_seq >= 2 && cfg->max_seq <= 12000, "acb_lm_create: max_seq %d out of range", cfg->max_seq);
     ACB_REQUIRE(cfg->dim <= 2048, "acb_lm_create: dim %d > 2048: the GEMM stages a 16 x dim weight slab per CTA", cfg->dim);
+    ACB_REQUIRE(cfg->positional_embedding >= 0 && cfg->positional_embedding <= 2, "acb_lm_create: positional_embedding %d not in [0,2]",
+                cfg->positional_embedding);
+    ACB_REQUIRE(cfg->positional_embedding == 0 || w->rope_freq, "acb_lm_create: rotary positions need weights.rope_freq");
     acb_lm* lm = new (std::nothrow) acb_lm();
     ACB_REQUIRE(lm, "acb_lm_create: out of host memory");
     lm->cfg = *cfg; lm->w = *w; lm->buf = *buf;
@@ -997,6 +990,8 @@ extern "C" int acb_lm_create(const acb_lm_config* cfg, const acb_lm_weights* w, 
     if (ea == cudaSuccess) ea = gemm_attr_all<EPI_F32>();
     if (ea == cudaSuccess) ea = gemm_attr_all<EPI_CROSSKV>();
     if (ea == cudaSuccess) ea = gemm_attr_all<EPI_QKV_PF>();
+    if (ea == cudaSuccess) ea = gemm_attr_all<EPI_QKV_ROPE>();
+    if (ea == cudaSuccess) ea = gemm_attr_all<EPI_QKV_PF_ROPE>();
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_attn2_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT2_SMEM);
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_attn2_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_attn2_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT2_SMEM);
@@ -1024,7 +1019,6 @@ extern "C" int acb_lm_destroy(acb_lm_t* lm) {
     if (!lm) return ACB_OK;
     drop_graph(lm);
     if (lm->capture_stream) cudaStreamDestroy(lm->capture_stream);
-    if (lm->trace) cudaFree(lm->trace);
     delete lm;
     return ACB_OK;
 }
@@ -1076,36 +1070,16 @@ extern "C" int acb_lm_begin(acb_lm_t* lm, const float* cross, int batch, int row
     }
     // capture one decode step; its kernels are chained by plain stream-order edges.  (Launched with programmatic dependent launch,
     // the same kernels gave wrong logits on the H100 once the KV cache held more than a few positions, for a cause not found.)
-    {
-        const char* ev = getenv("ACB_LM_STEP");
-        // The persistent fused step (lm_step.cu; needs the packed weights) is OPT-IN: ACB_LM_STEP=fused, or a model with rotary
-        // positions (only built there); the per-phase graph below is the default.
-        lm->fused = lm->w.wp_qkv != nullptr && ((ev && ev[0] == 'f') || c.positional_embedding != 0);
-        ACB_REQUIRE(c.positional_embedding == 0 || lm->fused, "acb_lm_begin: rotary positions are built in the fused decode step only");
-        if (lm->fused) {
-            ACB_TRY(lm_step_prepare(c, lm->w, lm->buf, rows, batch, text_len, lm->has_cross, lm->sms, &lm->step));
-            if (env_int("ACB_LM_COOP", 1) == 0) lm->step.cooperative = false;
-            if (env_int("ACB_LM_STEP_TRACE", 0)) {
-                if (!lm->trace) ACB_CHECK_CUDA(cudaMalloc(&lm->trace, 8192 * sizeof(unsigned long long)));
-                ACB_CHECK_CUDA(cudaMemset(lm->trace, 0, 8192 * sizeof(unsigned long long)));
-                ACB_REQUIRE(lm->step.n_phases + 2 <= 1024, "trace buffer too small");
-            }
-        }
-    }
-    for (int attempt = 0; attempt < 2; ++attempt) {
-        drop_graph(lm);
-        ACB_CHECK_CUDA(cudaStreamBeginCapture(lm->capture_stream, cudaStreamCaptureModeThreadLocal));
-        int rc = enqueue_step(lm, lm->capture_stream, nullptr, &lm->launches, false, true);
-        cudaError_t e = cudaStreamEndCapture(lm->capture_stream, &lm->graph);
-        if (rc == ACB_OK && e == cudaSuccess) e = cudaGraphInstantiate(&lm->exec, lm->graph, 0);
-        if (rc == ACB_OK && e == cudaSuccess) return ACB_OK;
-        cudaGetLastError();
-        drop_graph(lm);
-        if (lm->fused && lm->step.cooperative && attempt == 0) { lm->step.cooperative = false; continue; }   // plain launch (grid = #SMs is co-resident anyway)
-        if (rc == ACB_OK) acb_set_error("acb_lm_begin: graph capture failed: %s", cudaGetErrorString(e));
-        return rc != ACB_OK ? rc : ACB_ERR_CUDA;
-    }
-    return ACB_OK;
+    drop_graph(lm);
+    ACB_CHECK_CUDA(cudaStreamBeginCapture(lm->capture_stream, cudaStreamCaptureModeThreadLocal));
+    int rc = enqueue_step(lm, lm->capture_stream, nullptr, &lm->launches, false, true);
+    cudaError_t e = cudaStreamEndCapture(lm->capture_stream, &lm->graph);
+    if (rc == ACB_OK && e == cudaSuccess) e = cudaGraphInstantiate(&lm->exec, lm->graph, 0);
+    if (rc == ACB_OK && e == cudaSuccess) return ACB_OK;
+    cudaGetLastError();
+    drop_graph(lm);
+    if (rc == ACB_OK) acb_set_error("acb_lm_begin: graph capture failed: %s", cudaGetErrorString(e));
+    return rc != ACB_OK ? rc : ACB_ERR_CUDA;
 }
 
 __global__ void lm_set_pos_kernel(int* pos, int value) { pos[0] = value; }
@@ -1114,7 +1088,6 @@ __global__ void lm_set_pos_kernel(int* pos, int value) { pos[0] = value; }
 // without sampling, ACB_LM_PREFILL_ROWS / rows positions per pass.  Leaves pos = pos0 + n_tokens on the device.
 extern "C" int acb_lm_prefill(acb_lm_t* lm, int pos0, int n_tokens, void* stream) {
     ACB_REQUIRE(lm && lm->rows > 0, "acb_lm_prefill: call acb_lm_begin first");
-    ACB_REQUIRE(!lm->fused, "acb_lm_prefill: the prefill pass is built on the per-phase kernels");
     ACB_REQUIRE(pos0 >= 0 && n_tokens >= 0 && pos0 + n_tokens < lm->seq_len, "acb_lm_prefill: positions [%d, %d) exceed the sequence (%d)",
                 pos0, pos0 + n_tokens, lm->seq_len);
     cudaStream_t s = (cudaStream_t)stream;
@@ -1132,7 +1105,7 @@ extern "C" int acb_lm_prefill(acb_lm_t* lm, int pos0, int n_tokens, void* stream
             ACB_CHECK_CUDA(cudaMemsetAsync((__half*)lm->buf.a16 + (size_t)vrows * d, 0, (size_t)(pad - vrows) * d * sizeof(__half), s));
             ACB_CHECK_CUDA(cudaMemsetAsync((__half*)lm->buf.f16 + (size_t)vrows * c.ffn_dim, 0, (size_t)(pad - vrows) * c.ffn_dim * sizeof(__half), s));
         }
-        ACB_TRY(enqueue_step_kernels(lm, s, nullptr, nullptr, false, false, tc));
+        ACB_TRY(enqueue_step(lm, s, nullptr, nullptr, false, false, tc));
         done += tc;
     }
     lm_set_pos_kernel<<<1, 1, 0, s>>>(lm->buf.pos, pos0 + n_tokens);
@@ -1155,91 +1128,14 @@ extern "C" int acb_lm_steps(acb_lm_t* lm, int n_steps, void* stream) {
     return ACB_OK;
 }
 
-// ACB_LM_STEP_TRACE=1: time between consecutive grid barriers of the fused step as seen by CTA 0 (ns), summed per phase kind.
-static int report_step_trace(acb_lm* lm, cudaStream_t s) {
-    ACB_CHECK_CUDA(cudaStreamSynchronize(s));
-    const int n = lm->step.n_phases;
-    std::vector<unsigned long long> h((size_t)n + 1);
-    ACB_CHECK_CUDA(cudaMemcpy(h.data(), lm->trace, ((size_t)n) * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-    const bool cross = lm->has_cross;
-    const int per = cross ? 12 : 8;
-    static const char* names_c[12] = {"qkv", "attn", "o", "res1", "cq", "xattn", "co", "res2", "ff1", "gelu", "ff2", "res3"};
-    static const char* names_n[8] = {"qkv", "attn", "o", "res1", "ff1", "gelu", "ff2", "res3"};
-    double sum[12] = {0}, mx[12] = {0};
-    for (int l = 0; l < lm->cfg.num_layers; ++l)
-        for (int k = 0; k < per; ++k) {
-            const int i = 1 + l * per + k;     // stamp i is taken after barrier i; phase k of layer l ends at barrier 1 + l*per + k + 1
-            if (i + 1 >= n || !h[i] || !h[i + 1]) continue;
-            const double dt = (double)(h[i + 1] - h[i]);
-            sum[k] += dt; if (dt > mx[k]) mx[k] = dt;
-        }
-    fprintf(stderr, "[acb step trace] rows=%d pos=? total %.1f us (kernel start -> last barrier); embed %.2f us; per-layer mean (max) us:",
-            lm->rows, (double)(h[n - 1] - h[0]) * 1e-3, (double)(h[1] - h[0]) * 1e-3);
-    for (int k = 0; k < per; ++k)
-        fprintf(stderr, "  %s %.2f (%.2f)", cross ? names_c[k] : names_n[k], sum[k] * 1e-3 / lm->cfg.num_layers, mx[k] * 1e-3);
-    fprintf(stderr, "\n");
-    {   // sub-steps of the GEMM phases (the CTA running item 0): ns from phase start to stats / A-load done / MMAs issued / accumulator ready / epilogue done
-        std::vector<unsigned long long> f(8192);
-        ACB_CHECK_CUDA(cudaMemcpy(f.data(), lm->trace, 8192 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-        static const int gk_c[6] = {0, 2, 4, 6, 8, 10}, gk_n[4] = {0, 2, 4, 6};
-        const int ng = cross ? 6 : 4;
-        fprintf(stderr, "[acb step trace] GEMM sub-steps, mean ns after the phase's first stamp [stats, aload, mma-issued, acc-ready, epilogue]; first stamp - barrier stamp:\n");
-        for (int gi = 0; gi < ng; ++gi) {
-            const int k = cross ? gk_c[gi] : gk_n[gi];
-            double acc[6] = {0}; int cnt = 0; double lag = 0;
-            for (int l = 0; l < lm->cfg.num_layers; ++l) {
-                const int ph = 1 + l * per + k;          // barrier count when the phase starts
-                if (1024 + 8 * ph + 5 >= 8192) break;
-                const unsigned long long* q = f.data() + 1024 + 8 * ph;
-                if (!q[0] || !q[5]) continue;
-                for (int j = 1; j < 6; ++j) acc[j] += q[j] ? (double)(q[j] - q[0]) : 0.0;
-                lag += (double)q[0] - (double)h[ph];
-                ++cnt;
-            }
-            if (cnt) fprintf(stderr, "    %-4s  %.0f %.0f %.0f %.0f %.0f   (start lag %.0f ns, %d layers)\n", cross ? names_c[k] : names_n[k],
-                             acc[1] / cnt, acc[2] / cnt, acc[3] / cnt, acc[4] / cnt, acc[5] / cnt, lag / cnt, cnt);
-        }
-    }
-    {   // per-K-block stamps of the layer-1 QKV and FF2 GEMMs: [loop top -> full barrier passed -> MMAs + commit issued]
-        std::vector<unsigned long long> f(8192);
-        ACB_CHECK_CUDA(cudaMemcpy(f.data(), lm->trace, 8192 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-        for (int which = 0; which < 2; ++which) {
-            const unsigned long long* q = f.data() + 6000 + which * 64;
-            if (!q[0]) continue;
-            fprintf(stderr, "[acb step trace] %s layer 1, per K block ns since loop start (top, data ready, issued):", which ? "ff2" : "qkv");
-            for (int kb = 0; kb < 12 && q[3 * kb]; ++kb)
-                fprintf(stderr, "  [%lld %lld %lld]", (long long)(q[3 * kb] - q[0]), (long long)(q[3 * kb + 1] - q[0]), (long long)(q[3 * kb + 2] - q[0]));
-            fprintf(stderr, "\n");
-        }
-    }
-    ACB_CHECK_CUDA(cudaMemset(lm->trace, 0, 8192 * sizeof(unsigned long long)));
-    return ACB_OK;
-}
-
 extern "C" int acb_lm_step_logits(acb_lm_t* lm, float* logits_out, void* stream) {
     ACB_REQUIRE(lm && lm->rows > 0, "acb_lm_step_logits: call acb_lm_begin first");
-    if (lm->fused && lm->trace) lm->step.p.trace = lm->trace;
-    ACB_TRY(enqueue_step(lm, (cudaStream_t)stream, logits_out, nullptr));
-    if (lm->fused && lm->trace) { lm->step.p.trace = nullptr; ACB_TRY(report_step_trace(lm, (cudaStream_t)stream)); }
-    return ACB_OK;
+    return enqueue_step(lm, (cudaStream_t)stream, logits_out, nullptr);
 }
 
 extern "C" int acb_lm_debug_gemms(acb_lm_t* lm, void* stream, int* n_launches) {
     ACB_REQUIRE(lm && lm->rows > 0, "acb_lm_debug_gemms: call acb_lm_begin first");
     return enqueue_step(lm, (cudaStream_t)stream, nullptr, n_launches, true);
-}
-
-extern "C" int acb_lm_debug_step_plan(const acb_lm_t* lm, int* out) {
-    ACB_REQUIRE(lm && out && lm->fused, "acb_lm_debug_step_plan: the fused step is not active");
-    for (int i = 0; i < ACB_STEP_GEMMS; ++i) {
-        const StepGemm& g = lm->step.p.g[i];
-        out[4 * i] = g.N; out[4 * i + 1] = g.K; out[4 * i + 2] = g.ksplit; out[4 * i + 3] = g.kb_per;
-    }
-    out[4 * ACB_STEP_GEMMS] = lm->step.p.n_stage;
-    out[4 * ACB_STEP_GEMMS + 1] = lm->step.p.R;
-    out[4 * ACB_STEP_GEMMS + 2] = lm->step.n_phases;
-    out[4 * ACB_STEP_GEMMS + 3] = (int)lm->step.smem;
-    return ACB_OK;
 }
 
 extern "C" int acb_lm_rows_pad(int rows) { return rows <= 16 ? 16 : 8 * nt_for_rows(rows); }

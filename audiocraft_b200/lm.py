@@ -94,41 +94,10 @@ class LMModel:
         w['ln'] = ln
         w['out_norm'] = torch.stack([sd['out_norm.weight'].float(), sd['out_norm.bias'].float()]).to(dev).contiguous()
         w['heads'] = torch.cat([h(sd[f'linears.{k}.weight']) for k in range(self.n_q)], dim=0).contiguous()
-        # the persistent fused step (opt-in: ACB_LM_STEP=fused, or rotary positions) streams 128 x 64 tiles in the tensor-core
-        # operand layout: re-packed once at load time (acb_lm_pack_weight) when it will be used; shapes that do not tile
-        # (N % 128, K % 64) only have the per-phase kernels
-        import os as _os
-        ffn, NH = self.ffn_dim, self.n_q * self.card
-        self.fused_ok = d % 128 == 0 and ffn % 128 == 0 and NH % 128 == 0
-        want_fused = _os.environ.get('ACB_LM_STEP', '').startswith('f') or cfg.get('positional_embedding', 'sin') != 'sin'
-        if self.fused_ok and want_fused:
-            def pack(name, n, k):
-                src = w[name]
-                if src is None:
-                    return None
-                dst = torch.empty_like(src)
-                layers = 1 if src.dim() == 2 else src.shape[0]
-                for li in range(layers):
-                    _lib.check(self._lib.acb_lm_pack_weight(src[li].data_ptr() if src.dim() == 3 else src.data_ptr(),
-                                                            dst[li].data_ptr() if dst.dim() == 3 else dst.data_ptr(), n, k,
-                                                            _lib.stream()), 'lm_pack_weight')
-                return dst
-            w['wp_qkv'] = pack('w_qkv', 3 * d, d)
-            w['wp_o'] = pack('w_o', d, d)
-            w['wp_cq'] = pack('w_cq', d, d)
-            w['wp_co'] = pack('w_co', d, d)
-            w['wp_ff1'] = pack('w_ff1', ffn, d)
-            w['wp_ff2'] = pack('w_ff2', d, ffn)
-            w['wp_heads'] = pack('heads', NH, d)
-        else:
-            for n in ('wp_qkv', 'wp_o', 'wp_cq', 'wp_co', 'wp_ff1', 'wp_ff2', 'wp_heads'):
-                w[n] = None
         # positional_embedding (transformer.py:632-637): rotary frequencies computed by the same torch ops as rope.py:68-69
         self.positional_embedding = cfg.get('positional_embedding', 'sin')
         assert self.positional_embedding in ('sin', 'rope', 'sin_rope')
         if self.positional_embedding != 'sin':
-            if not self.fused_ok:
-                raise NotImplementedError("rotary positions need the fused decode step (dim, ffn, n_q*card multiples of 128)")
             adim2 = torch.arange(0, 64, 2, dtype=torch.float32)[:32]
             w['rope_freq'] = (1.0 / (float(cfg['max_period']) ** (adim2 / 64))).to(dev).contiguous()
         else:
@@ -136,7 +105,7 @@ class LMModel:
         self._w = w
         self.weight_bytes_per_step = sum(
             t.numel() * t.element_size() for k, t in w.items()
-            if t is not None and k not in ('emb', 'inv_freq', 'w_ckv') and not k.startswith('wp_') and k != 'rope_freq')
+            if t is not None and k not in ('emb', 'inv_freq', 'w_ckv', 'rope_freq'))
 
     # ------------------------------------------------------------------ reference attributes
     @property
@@ -174,8 +143,6 @@ class LMModel:
         b['f16'] = torch.zeros((rp, self.ffn_dim), device=dev, dtype=f16)
         b['q32'] = torch.zeros((rp, d), device=dev, dtype=f32)
         b['part'] = torch.zeros((_lib.ACB_LM_PART_SLOTS, rp, max(3 * d, self.ffn_dim, self.n_q * self.card)), device=dev, dtype=f32)
-        b['stats'] = torch.zeros((8, rp, 2), device=dev, dtype=f32)
-        b['bar'] = torch.zeros(32, device=dev, dtype=torch.int32)
         b['logits'] = torch.zeros((rp, self.n_q * self.card), device=dev, dtype=f32)
         b['k_cache'] = torch.zeros((L, max_rows, H, max_seq, 64), device=dev, dtype=f16)
         b['v_cache'] = torch.zeros((L, max_rows, H, max_seq, 64), device=dev, dtype=f16)
@@ -196,11 +163,10 @@ class LMModel:
                             float(self.cfg_dict.get('positional_scale', 1.0)),
                             {'sin': 0, 'rope': 1, 'sin_rope': 2}[self.positional_embedding])
         wts = _lib.LMWeights(*[_lib.ptr(self._w[n]) for n in ('emb', 'inv_freq', 'w_qkv', 'w_o', 'w_cq', 'w_ckv',
-                                                              'w_co', 'w_ff1', 'w_ff2', 'ln', 'out_norm', 'heads', 'wp_qkv',
-                                                              'wp_o', 'wp_cq', 'wp_co', 'wp_ff1', 'wp_ff2', 'wp_heads', 'rope_freq')])
+                                                              'w_co', 'w_ff1', 'w_ff2', 'ln', 'out_norm', 'heads', 'rope_freq')])
         bufs = _lib.LMBuffers(*[_lib.ptr(b[n]) for n in ('x', 'h16', 'a16', 'f16', 'q32', 'part', 'logits', 'k_cache',
                                                          'v_cache', 'ck_cache', 'cv_cache', 'cross16', 'seq',
-                                                         'seq_mask', 'pos', 'noise', 'stats', 'bar')])
+                                                         'seq_mask', 'pos', 'noise')])
         handle = C.c_void_p()
         _lib.check(self._lib.acb_lm_create(C.byref(cfg), C.byref(wts), C.byref(bufs), C.byref(handle)), 'lm_create')
         self._handle = handle
@@ -218,11 +184,6 @@ class LMModel:
             self._destroy()
         except Exception:
             pass
-
-    def _fused_active(self) -> bool:
-        import os as _os
-        return self._w.get('wp_qkv') is not None and (_os.environ.get('ACB_LM_STEP', '').startswith('f')
-                                                      or self.positional_embedding != 'sin')
 
     # ------------------------------------------------------------------ conditions (lm.py:488-511)
     def _prepare_conditions(self, conditions, two_step_cfg, cfg_coef_beta):
@@ -317,8 +278,7 @@ class LMModel:
             # they go through acb_lm_prefill, several positions per pass, instead of one decode step each.
             first = 0
             import os as _os
-            if (start_offset_sequence - 1 >= 2 and rows <= _lib.ACB_LM_PREFILL_ROWS and not self._fused_active()
-                    and _os.environ.get('ACB_LM_PREFILL', '1') != '0'):
+            if start_offset_sequence - 1 >= 2 and rows <= _lib.ACB_LM_PREFILL_ROWS and _os.environ.get('ACB_LM_PREFILL', '1') != '0':
                 first = start_offset_sequence - 1
                 _lib.check(self._lib.acb_lm_prefill(self._handle, 0, first, _lib.stream()), 'lm_prefill')
             if callback is None and self._debug_noise_fn is None:

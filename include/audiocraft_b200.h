@@ -144,7 +144,7 @@ typedef struct {
     int max_text;     /* cross-attention source length the cross KV cache is sized for */
     float pos_scale;  /* positional_scale */
     int positional_embedding; /* 0 'sin' (released MusicGen), 1 'rope', 2 'sin_rope'  (modules/transformer.py:632-637, 701-705).
-                                 rope needs the fused step (packed weights) */
+                                 rope and sin_rope need weights.rope_freq */
 } acb_lm_config;
 
 /* fp16 matrices in the reference's own [out_features][in_features] layout, stacked over layers. */
@@ -161,16 +161,6 @@ typedef struct {
     const float* ln;      /* [L][6][d] fp32: norm1.w, norm1.b, norm_cross.w, norm_cross.b, norm2.w, norm2.b */
     const float* out_norm;/* [2][d] fp32 */
     const void* heads;    /* [n_q*card][d] fp16  LMModel.linears, lm.py:172 */
-    /* The same matrices re-packed by acb_lm_pack_weight (one call per [N][K] matrix, layers stacked) for the persistent
-     * fused decode step: 128-feature x 64-K tiles in the canonical K-major tensor-core layout, one contiguous 16 KB bulk
-     * copy each.  All NULL: the step runs as one kernel per phase (the round-1 path). */
-    const void* wp_qkv;   /* [L][3d*d] */
-    const void* wp_o;     /* [L][d*d] */
-    const void* wp_cq;    /* [L][d*d] */
-    const void* wp_co;    /* [L][d*d] */
-    const void* wp_ff1;   /* [L][ffn*d] */
-    const void* wp_ff2;   /* [L][d*ffn] */
-    const void* wp_heads; /* [n_q*card*d] */
     const float* rope_freq; /* [32] fp32: 1 / max_period^(2i/64), RotaryEmbedding.frequencies rope.py:68-69 (NULL without rope) */
 } acb_lm_weights;
 
@@ -192,8 +182,6 @@ typedef struct {
     uint8_t* seq_mask; /* [n_q][max_seq]     pattern validity mask (codebooks_patterns.py:130-152) */
     int32_t* pos;      /* [4] device ints: pos (tokens in the KV cache), rows, batch, text_len */
     float* noise;      /* [B][n_q][card] Exponential(1) noise, read when sampling.noise_from_buffer != 0 */
-    float* stats;      /* [8][rows_pad][2]  LayerNorm (mean, M2) records per d/8 columns (fused step) */
-    void* bar;         /* 128 B: grid-barrier counter of the fused step */
 } acb_lm_buffers;
 
 #define ACB_LM_MAX_SPLIT 8
@@ -235,8 +223,7 @@ int acb_lm_steps(acb_lm_t* lm, int n_steps, void* stream);
 /* Prompt prefill = the reference's multi-token first call (modules/transformer.py:240-247, 413-414; models/lm.py:513-534):
  * consume sequence positions [pos0, pos0 + n_tokens) of every row -- their tokens are already in buffers.seq -- without
  * sampling, ACB_LM_PREFILL_ROWS / rows positions per pass (the per-phase kernels on (token, row) pairs, causal inside a pass),
- * and leave the device position at pos0 + n_tokens.  The activation buffers must hold ACB_LM_PREFILL_ROWS rows.
- * Per-phase path only (not with ACB_LM_STEP=fused). */
+ * and leave the device position at pos0 + n_tokens.  The activation buffers must hold ACB_LM_PREFILL_ROWS rows. */
 int acb_lm_prefill(acb_lm_t* lm, int pos0, int n_tokens, void* stream);
 
 /* Teacher-forced / inspection variant of one step: same as acb_lm_steps(1) and additionally leaves the
@@ -250,27 +237,11 @@ int acb_lm_debug_gemms(acb_lm_t* lm, void* stream, int* n_launches);
 /* Always 0: the captured decode step chains its kernels with plain stream-order edges, not programmatic dependent launch. */
 int acb_lm_uses_pdl(const acb_lm_t* lm);
 
-/* [N][K] row-major fp16 (N % 128 == 0, K % 64 == 0) -> the packed tile layout of acb_lm_weights.wp_*: tile (nt, kb) =
- * features [128 nt, +128) x K [64 kb, +64) at ((nt * K/64 + kb) * 8192) halves; inside a tile feature f is the 128-byte row
- * at f * 128 and its 16-byte chunk c sits at position c ^ (f & 7) (the canonical 128-byte-swizzled K-major wgmma layout). */
-int acb_lm_pack_weight(const void* w, void* wp, int n, int k, void* stream);
-
-/* Inspection of the fused step's work decomposition: out[4 g + {0,1,2,3}] = N, K, K-splits, 64-element K blocks per item
- * of GEMM g in {QKV, O, CQ, CO, FF1, FF2, HEADS}; out[28..31] = ring stages, padded rows, phases per step, shared memory
- * bytes.  Fails when the per-phase path is active. */
-int acb_lm_debug_step_plan(const acb_lm_t* lm, int* out);
-
 /* rows the activation buffers must be padded to for `rows` live rows (16, 32 or 64). */
 int acb_lm_rows_pad(int rows);
 
 /* Number of kernel launches one decode step enqueues (bench.py reports gpu_launches from it). */
 int acb_lm_launches_per_step(const acb_lm_t* lm);
-
-/* Measurement aid (no reference counterpart): microseconds per grid-wide barrier of a cooperative kernel of `ctas`
- * co-resident CTAs x `threads` that does nothing but `n_barriers` barriers (`work` dependent FMAs in between).
- * variant 0 = the barrier the persistent decode step uses (csrc/gridbar.cuh), 1 = relaxed polling, 2 = fence + atomicAdd +
- * volatile spin. */
-int acb_debug_grid_barrier(int ctas, int threads, int n_barriers, int variant, int work, int reps, float* us_per_barrier);
 
 /* Stand-alone sampler (tail of _sample_next_token, lm.py:403-418; utils/utils.py:88-141) for unit tests:
  * logits [rows][n_q][card] fp32 ([cond; null] rows when rows == 2*batch), noise optional, tokens [batch][n_q]. */

@@ -1,0 +1,582 @@
+"""GPU parity at the dispatch edges the other test files do not reach: EnCodec at the benchmark's 32-item launch chain, LM GEMM
+row tiles 17-32 (NT = 4) and text conditions longer than one 32-position cross-attention chunk.
+
+EnCodec kernels are compared with float64 restatements of the same operation (the oracle's convolutions called on float64
+tensors, an nn.LSTM restatement below), and every item of a batched launch with the same item launched alone.  LM logits are
+compared with the fp16-emulating oracle (LO.LMOracle(half_gemm=True)), teacher-forced.
+
+Coverage: kernel instances the dispatchers can select, and the test here that executes each against a reference.
+  lm_gemm_kernel<NT, EPI, FT2> (nt_for_rows: NT = 1 / 2 / 4 / 8 for rows <= 8 / 16 / 32 / 64; pick_ft2 gives FT2 = 2 only to
+  GEMMs with N x K >= 2M weights whose 32-feature grid covers 90 % of the SMs and whose 32-row slab fits 120 KB):
+    <4, PARTIAL, 1>   lm_mini (out-proj, cross q / out, FFN2)      test_lm_rows_17_to_32_match_oracle[lm_mini-*]
+    <4, PARTIAL, 2>   medium and large: out-proj, cross q / out, FFN2
+                                                                   test_lm_rows_17_to_32_match_oracle[lm_medium_2l-*, lm_large_2l-12]
+    <4, QKV, 1>       lm_mini, lm_large_2l (slab too big for FT2)  test_lm_rows_17_to_32_match_oracle[lm_mini-*, lm_large_2l-12]
+    <4, QKV, 2>       lm_medium_2l                                 test_lm_rows_17_to_32_match_oracle[lm_medium_2l-*]
+    <4, GELU, 1>      lm_mini, lm_large_2l                         test_lm_rows_17_to_32_match_oracle[lm_mini-*, lm_large_2l-12]
+    <4, GELU, 2>      lm_medium_2l                                 test_lm_rows_17_to_32_match_oracle[lm_medium_2l-*]
+    <4, F32, 1>       lm_mini, lm_large_2l heads                   test_lm_rows_17_to_32_match_oracle[lm_mini-*, lm_large_2l-12]
+    <4, F32, 2>       lm_medium_2l heads                           test_lm_rows_17_to_32_match_oracle[lm_medium_2l-*]
+    <4, QKV_ROPE, 2>  lm_medium_2l with rotary positions           test_lm_rows_17_to_32_match_oracle[lm_medium_2l-12-rope]
+    <4, QKV_PF, 1>    prefill pass of 17-32 (token, row) pairs     test_prefill_tail_passes_equal_token_by_token[lm_mini-2-22]
+    <4, QKV_PF_ROPE, 1>                                            test_prefill_tail_passes_equal_token_by_token[lm_mini-2-22-rope]
+    <1, QKV_PF, 1>    prefill pass of <= 8 pairs                   test_prefill_tail_passes_equal_token_by_token[lm_mini-1-35]
+    <8, *, 1>         double CFG at 33 rows (lm_mini)              test_double_cfg_rows_18_and_33_match_oracle[11]
+    <4, *, 1>         double CFG at 18 rows (lm_mini)              test_double_cfg_rows_18_and_33_match_oracle[6]
+    <8, CROSSKV, 1>   cross K/V projection, 20 chunks of 64 rows, ragged last (16 rows x 77 positions)
+                                                                   test_long_text_cross_attention_matches_oracle[lm_medium_2l-8-77]
+  lm_cross_attn_kernel<false>: 1 chunk (t_text 31, 32), 2 chunks (33 with a 1-position tail, 64), 3 chunks (77),
+    4 chunks (100, 4-position tail)                                test_long_text_cross_attention_matches_oracle
+  lm_cross_attn_kernel<true> (prefill) at 1 chunk only             test_prefill_tail_passes_equal_token_by_token
+  LSTM recurrence (acb_lstm_recurrent), item slots in four groups 0-7, 8-15, 16-23, 24-31 (the four MMA n-tiles):
+    lstm_h2_kernel (H % 128 == 0, B <= 32): H 512 / 1024 x B 16, 17, 24, 31, 32 (groups 1-4), T 1 / 2 / 37, 1 and 2 layers,
+      with and without skip                                        test_lstm_h2_item_slots_match_float64
+    lstm_h2_kernel at the benchmark shape (H 1024, B 32, T 500)    test_lstm_bench_shape_items_equal_batch_one
+    lstm_tc_kernel (H % 64 == 0 and not % 128, or ACB_LSTM_TC=3): H 64 / 192 x B 9, 17, 32, and H 1024 B 32
+                                                                   test_lstm_tc_and_fma_kernels_match_float64[tc-*]
+    lstm_kernel (fp32 FMA; B > 32 or ACB_LSTM_TC=0): H 512 / 1024 x B 33, 48 (3 chunks of LSTM_BC = 16 items, ragged last),
+      and H 1024 B 32 (2 chunks)                                   test_lstm_tc_and_fma_kernels_match_float64[fma-*]
+  EnCodec-32k convolutions at 32 items, every layer of the plan: acb_conv1d_t6, acb_conv1d (prec 0 and 1), acb_convtr1d
+  (prec 0 and 1), acb_resblock (exact 1 and 0)                     test_encodec_layers_at_32_items
+  RVQ encode / decode at 32 x 500 frames                           test_rvq_at_32_items
+  The whole 32 x 10 s encode / decode chain                        test_encodec_bench_chain_at_32_items
+Still not executed against a reference by any test: lm_gemm_kernel<8, QKV_ROPE, 1> and every <NT, QKV_ROPE, 2> except NT = 4
+(rotary positions at 33-64 rows, and at the released widths outside rows 17-32); <1, QKV | GELU | F32, 2> (medium at rows <= 8
+runs them only in test_ft32_tiles_equal_16_feature_tiles, against the 16-feature tiles, not against the oracle); the prefill
+cross-attention kernel over more than 32 text positions; the EnCodec-24k plan at 32 items.
+"""
+import os
+
+import pytest
+import torch
+
+from tests import helpers as H
+from audiocraft_b200 import synth
+from oracle import encodec_oracle as EO
+from oracle import lm_oracle as LO
+
+
+def _lib():
+    from audiocraft_b200 import _lib
+    return _lib, _lib.lib()
+
+
+def _dev(t):
+    return t.cuda().contiguous()
+
+
+# ----------------------------------------------------------------------------- float64 references and comparison helpers
+
+def lstm_f64(x: torch.Tensor, sd: dict, prefix: str, layers: int):
+    """nn.LSTM restated in float64 (gate order i, f, g, o; zero initial state; bias_ih + bias_hh), conv layout [B, H, T] in
+    and out.  Returns the output of every layer (no skip): the model adds the block input to the last one."""
+    inp = x.double().permute(2, 0, 1)                       # [T, B, H]
+    outs = []
+    for n in range(layers):
+        w_ih = sd[f'{prefix}weight_ih_l{n}'].double()
+        w_hh = sd[f'{prefix}weight_hh_l{n}'].double()
+        bias = sd[f'{prefix}bias_ih_l{n}'].double() + sd[f'{prefix}bias_hh_l{n}'].double()
+        hid = w_hh.shape[1]
+        h = torch.zeros(inp.shape[1], hid, dtype=torch.float64)
+        c = torch.zeros_like(h)
+        gx = inp @ w_ih.t() + bias
+        hs = []
+        for t in range(inp.shape[0]):
+            i, f, g, o = (gx[t] + h @ w_hh.t()).split(hid, dim=1)
+            c = torch.sigmoid(f) * c + torch.sigmoid(i) * torch.tanh(g)
+            h = torch.sigmoid(o) * torch.tanh(c)
+            hs.append(h)
+        inp = torch.stack(hs)
+        outs.append(inp.permute(1, 2, 0))
+    return outs
+
+
+def assert_close(got: torch.Tensor, ref: torch.Tensor, rtol: float, atol: float, what: str):
+    """got (any float dtype) vs a reference; prints the max error and the worst element's share of its tolerance."""
+    got, ref = got.detach().cpu().double(), ref.detach().cpu().double()
+    assert got.shape == ref.shape, (what, got.shape, ref.shape)
+    err = (got - ref).abs()
+    frac = (err / (atol + rtol * ref.abs())).max().item()
+    print(f'{what}: max err {err.max().item():.2e}, {frac:.2f} of tolerance (rtol {rtol:g}, atol {atol:g})')
+    torch.testing.assert_close(got, ref, rtol=rtol, atol=atol, msg=lambda m: f'{what}: {m}')
+
+
+def assert_each_item_equal(batched: torch.Tensor, single, what: str):
+    """Item b of a batched launch is bit-identical to the same item launched alone (`single(b)` -> [1, ...])."""
+    bad = [b for b in range(batched.shape[0]) if not torch.equal(batched[b:b + 1], single(b))]
+    assert not bad, f'{what}: items {bad} differ from their batch-1 runs'
+
+
+def codes_match(codes_gpu: torch.Tensor, codes_ref: torch.Tensor, margins: torch.Tensor, what: str, tie: float = 1e-4):
+    """RVQ codes bit-exact, except where the reference's own best / second-best gap is below fp32 summation noise; a flipped
+    code changes every later residual, so only the first differing codebook of a frame is judged."""
+    codes_gpu = codes_gpu.cpu()
+    assert codes_gpu.shape == codes_ref.shape, (what, codes_gpu.shape, codes_ref.shape)
+    neq = codes_gpu != codes_ref
+    if neq.any():
+        first = neq.int().cumsum(1).eq(1) & neq
+        gaps = margins[first]
+        print(f'{what}: {int(first.sum())} near-tie code flips, margins {gaps.tolist()[:8]}')
+        assert (gaps.abs() < tie).all(), f'{what}: RVQ index mismatch with a clear margin'
+
+
+def _swap(t: torch.Tensor, b: int, dim: int = 0) -> torch.Tensor:
+    idx = torch.arange(t.shape[dim])
+    idx[b], idx[b ^ 1] = b ^ 1, b
+    return t.index_select(dim, idx)
+
+
+def test_float64_references_and_helpers_can_fail():
+    """CPU only: the float64 LSTM restatement agrees with the oracle's fp32 block, the oracle convolutions keep float64, and
+    every comparison helper above rejects an output whose items b and b ^ 1 are swapped."""
+    g = torch.Generator().manual_seed(0)
+    Hd, B, T, layers = 8, 3, 6, 2
+    sd = {f'l.{nm}_l{n}': torch.rand(shp, generator=g) * 0.7 - 0.35 for n in range(layers)
+          for nm, shp in [('weight_ih', (4 * Hd, Hd)), ('weight_hh', (4 * Hd, Hd)), ('bias_ih', (4 * Hd,)), ('bias_hh', (4 * Hd,))]}
+    x = torch.randn(B, Hd, T, generator=g)
+    ref64 = lstm_f64(x, sd, 'l.', layers)[-1] + x.double()
+    assert (ref64 - EO.lstm_block(x, sd, 'l.', layers).double()).abs().max() <= 1e-5
+    # the oracle's convolution helpers do not cast: float64 in, float64 out, equal to the float64 torch op
+    xd = torch.randn(2, 4, 33, generator=g, dtype=torch.float64)
+    w = torch.randn(6, 4, 3, generator=g, dtype=torch.float64)
+    b = torch.randn(6, generator=g, dtype=torch.float64)
+    y = EO.sconv1d(EO.elu(xd), w, b, stride=1, dilation=2)
+    assert y.dtype == torch.float64 and EO.elu(xd).dtype == torch.float64
+    assert torch.equal(y, torch.nn.functional.conv1d(EO.pad1d(EO.elu(xd), 2, 2, 'reflect'), w, b, dilation=2))
+    wt = torch.randn(4, 6, 4, generator=g, dtype=torch.float64)
+    assert EO.sconvtr1d(xd, wt, b, 2).dtype == torch.float64
+    # negative checks: every helper fails on swapped items
+    ref = torch.randn(4, 3, 5, generator=g, dtype=torch.float64)
+    got = ref.float()
+    assert_close(got, ref, 1e-4, 2e-5, 'self-check')
+    assert_each_item_equal(got, lambda i: got[i:i + 1], 'self-check')
+    for bi in (0, 3):
+        with pytest.raises(AssertionError):
+            assert_close(_swap(got, bi), ref, 1e-4, 2e-5, 'swapped items')
+        with pytest.raises(AssertionError):
+            assert_each_item_equal(_swap(got, bi), lambda i: got[i:i + 1], 'swapped items')
+    logits = torch.randn(3, 4, 2, 16, generator=g)          # [steps, B, K, card]
+    with pytest.raises(AssertionError):
+        assert_close(_swap(logits, 1, dim=1), logits, 2e-2, 3e-2, 'swapped LM items')
+    codes = torch.randint(0, 64, (4, 4, 7), generator=g)
+    codes_match(codes, codes, torch.ones(4, 4, 7), 'self-check')
+    with pytest.raises(AssertionError):
+        codes_match(_swap(codes, 2), codes, torch.ones(4, 4, 7), 'swapped codes')
+    with pytest.raises(AssertionError):                     # the LSTM comparison: batch-2 float64 reference, items swapped
+        assert_close(_swap(ref64.float(), 0), ref64, 1e-4, 2e-5, 'swapped LSTM items')
+
+
+# ----------------------------------------------------------------------------- EnCodec: LSTM recurrence
+
+def _lstm_weights(hidden: int, layers: int, seed: int) -> dict:
+    g = torch.Generator().manual_seed(seed)
+    bnd = 1.0 / hidden ** 0.5
+    sd = {}
+    for n in range(layers):
+        for nm, shp in [('weight_ih', (4 * hidden, hidden)), ('weight_hh', (4 * hidden, hidden)), ('bias_ih', (4 * hidden,)),
+                        ('bias_hh', (4 * hidden,))]:
+            sd[f'l.{nm}_l{n}'] = (torch.rand(shp, generator=g) * 2 - 1) * bnd
+    return sd
+
+
+def _lstm_gpu(x: torch.Tensor, sd: dict, hidden: int, layers: int, skip: bool) -> torch.Tensor:
+    """EncodecModel._lstm's launch sequence (input half of the gates as a 3xTF32 1x1 conv, then the recurrent kernel per layer),
+    with the block skip optional."""
+    lib, L = _lib()
+    B, _, T = x.shape
+    xd = _dev(x)
+    ws = torch.empty(int(L.acb_lstm_state_bytes(B, hidden)) // 4, device='cuda')
+    inp = xd
+    for n in range(layers):
+        w_ih = _dev(sd[f'l.weight_ih_l{n}'].float().t())
+        w_hh = _dev(sd[f'l.weight_hh_l{n}'].float())
+        bias = _dev(sd[f'l.bias_ih_l{n}'].float() + sd[f'l.bias_hh_l{n}'].float())
+        gx = torch.empty((B, 4 * hidden, T), device='cuda')
+        lib.check(L.acb_conv1d(lib.ptr(inp), lib.ptr(w_ih), lib.ptr(bias), None, lib.ptr(gx), B, hidden, 4 * hidden, T, T, T,
+                               1, 1, 1, 0, 0, 0, lib.CONV_TF32X3, lib.stream()), 'lstm input conv')
+        y = torch.empty((B, hidden, T), device='cuda')
+        sk = xd if (skip and n == layers - 1) else None
+        lib.check(L.acb_lstm_recurrent(lib.ptr(gx), lib.ptr(w_hh), lib.ptr(sk), lib.ptr(y), lib.ptr(ws), B, hidden, T,
+                                       lib.stream()), 'lstm_recurrent')
+        inp = y
+    return inp.cpu()
+
+
+def _lstm_cases(hidden, B, Ts, seed):
+    """Runs T in Ts, 1 and 2 layers, with and without skip, against ONE float64 run of the longest sequence: the recurrence is
+    causal, so a shorter run equals a prefix of it, and layer 1 of the 2-layer reference is the 1-layer reference."""
+    sd = _lstm_weights(hidden, 2, seed)
+    x = torch.randn(B, hidden, max(Ts), generator=torch.Generator().manual_seed(seed + 1))
+    refs = lstm_f64(x, sd, 'l.', 2)
+    for T in Ts:
+        for layers in (1, 2):
+            for skip in (True, False):
+                got = _lstm_gpu(x[..., :T], sd, hidden, layers, skip)
+                ref = refs[layers - 1][..., :T] + (x[..., :T].double() if skip else 0)
+                assert_close(got, ref, 1e-4, 2e-5, f'lstm H={hidden} B={B} T={T} layers={layers} skip={skip}')
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize('B', [16, 17, 24, 31, 32])
+@pytest.mark.parametrize('hidden', [512, 1024])
+def test_lstm_h2_item_slots_match_float64(hidden, B):
+    """lstm_h2_kernel keeps h for 32 item slots in MMA-fragment order: items 0-7, 8-15, 16-23, 24-31 sit in four different
+    n-tiles.  B = 16 fills two groups, 17 / 24 reach the third, 31 / 32 the fourth (32 = the benchmark's chain)."""
+    _lstm_cases(hidden, B, (1, 2, 37), hidden + B)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize('kernel,hidden,B,env', [
+    ('tc', 64, 9, None), ('tc', 64, 17, None), ('tc', 64, 32, None), ('tc', 192, 9, None), ('tc', 192, 17, None),
+    ('tc', 192, 32, None), ('tc', 1024, 32, '3'),
+    ('fma', 512, 33, None), ('fma', 512, 48, None), ('fma', 1024, 33, None), ('fma', 1024, 48, None), ('fma', 1024, 32, '0')])
+def test_lstm_tc_and_fma_kernels_match_float64(monkeypatch, kernel, hidden, B, env):
+    """lstm_tc_kernel (3xTF32, hidden % 64 == 0 but not % 128, or ACB_LSTM_TC=3) across all four slot groups, and the fp32 FMA
+    lstm_kernel (more than 32 items, or ACB_LSTM_TC=0) with 2 and 3 chunks of LSTM_BC = 16 items, the last one ragged."""
+    if env is not None:
+        monkeypatch.setenv('ACB_LSTM_TC', env)
+    _lstm_cases(hidden, B, (2, 37), hidden * 3 + B)
+
+
+@pytest.mark.gpu
+def test_lstm_bench_shape_items_equal_batch_one():
+    """The encoder LSTM at the benchmark's shape (H 1024, 32 items, 500 frames, 2 layers) through EncodecModel._lstm: each item
+    is its own MMA column and no summation order depends on the batch, so every item equals the same item run alone; items of
+    all four slot groups against float64."""
+    from audiocraft_b200.encodec import EncodecModel
+    lib, L = _lib()
+    hidden, B, T = 1024, 32, 500
+    sd = _lstm_weights(hidden, 2, 5)
+    x = torch.randn(B, hidden, T, generator=torch.Generator().manual_seed(6))
+    m = EncodecModel.__new__(EncodecModel)
+    m._lib, m.device, m.launches, m._lstm_prec = L, torch.device('cuda'), 0, lib.CONV_TF32X3
+    layer = m._prepare(dict(kind='lstm', prefix='l.', dim=hidden, layers=2), sd)
+    xd = _dev(x)
+    y = m._lstm(xd, layer, prec=m._lstm_prec).cpu()
+    assert_each_item_equal(y, lambda b: m._lstm(xd[b:b + 1].contiguous(), layer, prec=m._lstm_prec).cpu(), 'lstm batch 32')
+    items = [0, 15, 16, 31]
+    ref = lstm_f64(x[items], sd, 'l.', 2)[-1] + x[items].double()
+    assert_close(y[items], ref, 1e-4, 2e-5, f'lstm H={hidden} B={B} T={T} items {items}')
+
+
+# ----------------------------------------------------------------------------- EnCodec: convolutions at 32 items
+
+ITEMS = [0, 1, 15, 16, 31]
+
+
+def _units(side: str):
+    """The layer plan of encodec_32k split into the launches EncodecModel makes (LSTMs excluded): ('block', a, b) for a residual
+    block acb_resblock takes, ('conv', L) / ('convtr', L) otherwise."""
+    from audiocraft_b200.encodec import EncodecModel
+    lib, L_ = _lib()
+    layers = synth.encodec_layers(synth.ENCODEC_CONFIGS['encodec_32k'])[side]
+    out, i = [], 0
+    while i < len(layers):
+        a = layers[i]
+        if a['kind'] == 'lstm':
+            i += 1
+            continue
+        if EncodecModel._fused_block(_FakeModel(L_), layers, i, lib.CONV_TF32X3, 301):
+            out.append(('block', a, layers[i + 1]))
+            i += 2
+            continue
+        out.append((a['kind'], a))
+        i += 1
+    return out
+
+
+class _FakeModel:
+    """What EncodecModel._fused_block reads."""
+    def __init__(self, L):
+        self._lib, self._fuse_blocks = L, True
+
+
+def _w(sd, L):
+    return EO._conv_weight(sd, L['prefix'])
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize('side', ['encoder', 'decoder'])
+def test_encodec_layers_at_32_items(side):
+    """Every convolution, transposed convolution and fused residual block of the EnCodec-32k plan at 32 items, on the kernel
+    EncodecModel routes it to (encoder: acb_conv1d_t6 for k > 1 and >= 128 output channels, fp32 acb_conv1d otherwise,
+    acb_resblock exact = 1; decoder: 3xTF32 acb_conv1d, acb_convtr1d at prec 1 and 0, acb_resblock exact = 0).  About 300
+    output frames: a few time tiles and a ragged tail.  Items 0, 1, 15, 16, 31 against float64; every item against itself run
+    alone."""
+    from audiocraft_b200.encodec import conv_geometry, convtr_geometry, pack_conv_t6
+    lib, L_ = _lib()
+    cfg = synth.ENCODEC_CONFIGS['encodec_32k']
+    sd = synth.synth_encodec_state_dict(cfg, seed=0)
+    g = torch.Generator().manual_seed(1 if side == 'encoder' else 2)
+    B, T_OUT = 32, 301
+    enc = side == 'encoder'
+    failures = []
+    ran = []
+
+    def check(name, y, ref, tol, single):
+        try:
+            assert_close(y[ITEMS], ref, tol, tol, f'{side} {name}')
+            assert_each_item_equal(y, single, f'{side} {name}')
+        except AssertionError as e:
+            failures.append(str(e).splitlines()[0])
+        ran.append(name)
+
+    for unit in _units(side):
+        kind, L = unit[0], unit[1]
+        if kind == 'block':
+            a, b2 = unit[1], unit[2]
+            w1, b1 = _w(sd, a)
+            w2, bb2 = _w(sd, b2)
+            C, T = a['cin'], T_OUT
+            x = torch.randn(B, C, T, generator=g)
+            left, _, tout = conv_geometry(T, a['k'], 1, a['dilation'], False, True)
+            xs = x[ITEMS].double()
+            hid = EO.sconv1d(EO.elu(xs), w1.double(), b1.double(), dilation=a['dilation'])
+            ref = xs + EO.sconv1d(EO.elu(hid), w2.double(), bb2.double())
+            xd, w1d, b1d, w2d, b2d = _dev(x), _dev(w1.permute(2, 1, 0)), _dev(b1), _dev(w2[:, :, 0].t()), _dev(bb2)
+            exact = 1 if enc else 0
+
+            def run(xx):
+                y = torch.full(xx.shape, float('nan'), device='cuda')
+                lib.check(L_.acb_resblock(lib.ptr(xx), lib.ptr(w1d), lib.ptr(b1d), lib.ptr(w2d), lib.ptr(b2d), lib.ptr(y),
+                                          xx.shape[0], C, T, a['k'], a['dilation'], left, 1, exact, lib.stream()), 'resblock')
+                return y.cpu()
+            check(f'{a["prefix"]} resblock C={C} exact={exact}', run(xd), ref, 2e-5 if exact else 1e-4,
+                  lambda i: run(xd[i:i + 1].contiguous()))
+        elif kind == 'conv':
+            w, b = _w(sd, L)
+            cin, cout, k, s, d = L['cin'], L['cout'], L['k'], L['stride'], L['dilation']
+            T = T_OUT * s - 3 if s > 1 else T_OUT
+            x = torch.randn(B, cin, T, generator=g)
+            left, tv, tout = conv_geometry(T, k, s, d, False, True)
+            res = torch.randn(B, cout, tout, generator=g) if L['res'] == 'out' else None
+            xs = x[ITEMS].double()
+            ref = EO.sconv1d(EO.elu(xs) if L['elu'] else xs, w.double(), b.double(), stride=s, dilation=d)
+            if res is not None:
+                ref = ref + res[ITEMS].double()
+            xd, bd, rd = _dev(x), _dev(b), (_dev(res) if res is not None else None)
+            if enc and k > 1 and cout >= 128:
+                route, tol = 't6', 2e-5
+                wk = _dev(pack_conv_t6(w, int(L_.acb_conv1d_t6_tile(cout))))
+            else:
+                route, tol = ('fp32', 1e-4) if enc else ('3xtf32', 1e-4)
+                wk = _dev(w.permute(1, 2, 0).reshape(cin * k, cout))
+
+            def run(xx, rr):
+                y = torch.full((xx.shape[0], cout, tout), float('nan'), device='cuda')
+                if route == 't6':
+                    lib.check(L_.acb_conv1d_t6(lib.ptr(xx), lib.ptr(wk), lib.ptr(bd), lib.ptr(rr), lib.ptr(y), xx.shape[0], cin,
+                                               cout, T, tv, tout, k, s, d, left, 1, int(L['elu']), lib.stream()), 'conv1d_t6')
+                else:
+                    lib.check(L_.acb_conv1d(lib.ptr(xx), lib.ptr(wk), lib.ptr(bd), lib.ptr(rr), lib.ptr(y), xx.shape[0], cin, cout,
+                                            T, tv, tout, k, s, d, left, 1, int(L['elu']), 0 if route == 'fp32' else 1,
+                                            lib.stream()), 'conv1d')
+                return y.cpu()
+            check(f'{L["prefix"]} conv {cin}->{cout} k{k} s{s} [{route}]', run(xd, rd), ref, tol,
+                  lambda i: run(xd[i:i + 1].contiguous(), rd[i:i + 1].contiguous() if rd is not None else None))
+        else:
+            w, b = _w(sd, L)                           # [Cin][Cout][K]
+            cin, cout, k, s = L['cin'], L['cout'], L['k'], L['stride']
+            T = T_OUT
+            x = torch.randn(B, cin, T, generator=g)
+            tl, tout = convtr_geometry(T, k, s, False, cfg['trim_right_ratio'])
+            ref = EO.sconvtr1d(EO.elu(x[ITEMS].double()), w.double(), b.double(), s)
+            xd, wd, bd = _dev(x), _dev(w.permute(0, 2, 1)), _dev(b)
+            wg = _dev(w.view(cin, cout, 2, s).flip(2).permute(0, 2, 1, 3).reshape(cin * 2, cout * s))
+            for prec in (1, 0):
+                def run(xx, prec=prec):
+                    y = torch.full((xx.shape[0], cout, tout), float('nan'), device='cuda')
+                    lib.check(L_.acb_convtr1d(lib.ptr(xx), lib.ptr(wd), lib.ptr(wg), lib.ptr(bd), lib.ptr(y), xx.shape[0], cin,
+                                              cout, T, tout, k, s, tl, 1, prec, lib.stream()), 'convtr1d')
+                    return y.cpu()
+                check(f'{L["prefix"]} convtr {cin}->{cout} s{s} prec={prec}', run(xd), ref, 1e-4,
+                      lambda i: run(xd[i:i + 1].contiguous()))
+    print(f'{side}: {len(ran)} launches checked')
+    assert ran and not failures, '\n'.join(failures)
+
+
+@pytest.mark.gpu
+def test_rvq_at_32_items():
+    """RVQ encode / decode at the benchmark's 32 x 500 frames (4 codebooks of 2048)."""
+    lib, L_ = _lib()
+    B, D, T, nq, bins = 32, 128, 500, 4, 2048
+    g = torch.Generator().manual_seed(32)
+    z = torch.randn(B, D, T, generator=g) * 0.4
+    cbs = [torch.randn(bins, D, generator=g) * 0.35 * 0.6 ** k for k in range(nq)]
+    ref, margins = EO.rvq_encode(z.double(), [c.double() for c in cbs], return_margin=True)
+    cb = _dev(torch.stack(cbs))
+    codes = torch.empty(B, nq, T, dtype=torch.int64, device='cuda')
+    zd, cbn = _dev(z), cb.pow(2).sum(-1).contiguous()
+    lib.check(L_.acb_rvq_encode(lib.ptr(zd), lib.ptr(cb), lib.ptr(cbn), lib.ptr(codes), B, D, T, nq, bins, lib.stream()))
+    codes_match(codes, ref, margins, 'rvq_encode 32 items')
+    out = torch.empty(B, D, T, device='cuda')
+    refd = _dev(ref)
+    lib.check(L_.acb_rvq_decode(lib.ptr(refd), lib.ptr(cb), lib.ptr(out), B, D, T, nq, bins, lib.stream()))
+    assert_close(out, EO.rvq_decode(ref, [c.double() for c in cbs]), 0, 1e-6, 'rvq_decode 32 items')
+
+
+@pytest.mark.gpu
+def test_encodec_bench_chain_at_32_items():
+    """The benchmark's launch chain: 32 items x 10 s through the default EncodecModel (fp32-accurate encoder, 3xTF32 decoder).
+    The two items of the encodec_32k_10s golden sit in slots 0 and 31 among 30 other seeded clips; their codes must reproduce
+    the golden (near-tie rule) and every item's codes must equal its batch-1 encode.  Decoding a 32-item batch with the golden
+    codes in slots 0 and 31 must reproduce the golden waveform there."""
+    from audiocraft_b200.encodec import EncodecModel
+    g = torch.load(os.path.join(H.GOLDEN_DIR, 'encodec_32k_10s.pt'), weights_only=False)
+    cfg = dict(synth.ENCODEC_CONFIGS[g['name']])
+    sd = synth.synth_encodec_state_dict(cfg, seed=g['wseed'])
+    gold_x = H.audio_input(cfg, g['batch'], g['length'], g['xseed'])
+    assert torch.equal(gold_x[..., :64], g['x_head'])
+    x = torch.cat([gold_x[:1], H.audio_input(cfg, 30, g['length'], 100), gold_x[1:]], 0)
+    del gold_x
+    m = EncodecModel(sd, cfg, 'cuda')
+    xd = _dev(x)
+    codes, _ = m.encode(xd)
+    codes = codes.cpu()
+    want = g['codes'].long()
+    got = codes[[0, 31]]
+    if not torch.equal(got, want):
+        o = EO.EncodecOracle(sd, cfg)
+        lat = o.encode_latent(x[[0, 31]])
+        ocodes, margins = EO.rvq_encode(lat, EO.codebooks_of(sd, cfg['n_q']), return_margin=True)
+        assert torch.equal(ocodes, want), 'oracle and reference golden disagree'
+        codes_match(got, want, margins, 'slots 0 / 31 vs golden')
+    assert_each_item_equal(codes, lambda b: m.encode(xd[b:b + 1])[0].cpu(), 'encode 32 items')
+    del xd, x
+    torch.cuda.empty_cache()
+    dec_codes = codes.clone()
+    dec_codes[0], dec_codes[31] = want[0], want[1]
+    wav = m.decode(_dev(dec_codes))
+    assert wav.shape == (32, 1, g['wav_len'])
+    strided = wav[[0, 31], :, ::g['wav_stride']].cpu()
+    del wav
+    torch.cuda.empty_cache()
+    assert_close(strided, g['wav_strided'], 0, 1e-4, 'decode slots 0 / 31 vs golden')
+
+
+# ----------------------------------------------------------------------------- LM: row tiles 17-32, double CFG, prefill, text
+
+def _lm(name, wseed, **over):
+    from audiocraft_b200.lm import LMModel
+    cfg = synth.lm_config(name)
+    cfg.update(over)
+    sd = synth.synth_lm_state_dict(cfg, seed=wseed)
+    return cfg, sd, LMModel(sd, cfg, None, None)
+
+
+def _teacher_forced_oracle(cfg, sd, cross, B, T, seed):
+    seq = torch.randint(0, cfg['card'], (B, 4, T + 4), generator=torch.Generator().manual_seed(seed))
+    o = LO.LMOracle(sd, cfg, half_gemm=True)
+    rec = []
+    o.generate(None, cross, B, T, use_sampling=False, record_logits=rec, teacher=seq)
+    return o.last_sequence, torch.stack(rec)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize('name,B,pe', [('lm_mini', 9, 'sin'), ('lm_mini', 16, 'sin'), ('lm_medium_2l', 9, 'sin'),
+                                       ('lm_medium_2l', 12, 'sin'), ('lm_medium_2l', 16, 'sin'), ('lm_medium_2l', 12, 'rope'),
+                                       ('lm_large_2l', 12, 'sin')],
+                         ids=['lm_mini-9', 'lm_mini-16', 'lm_medium_2l-9', 'lm_medium_2l-12', 'lm_medium_2l-16',
+                              'lm_medium_2l-12-rope', 'lm_large_2l-12'])
+def test_lm_rows_17_to_32_match_oracle(monkeypatch, name, B, pe):
+    """CFG rows 18-32 run the NT = 4 GEMM instances; at d = 1536 pick_ft2 gives them 32-feature tiles (lm_gemm_kernel<4, *, 2>,
+    117 KB of shared memory), what MusicGen-medium runs at batch 9-16.  Teacher-forced CFG-mixed logits vs the fp16-emulating
+    oracle; at B = 12 also bit-identical to the 16-feature tiles (ACB_LM_FT32=0)."""
+    monkeypatch.delenv('ACB_LM_FT32', raising=False)
+    cfg, sd, m = _lm(name, 11, positional_embedding=pe)
+    _, _, cross = H.lm_condition(cfg, sd, B, 7, 3)
+    seq, ref = _teacher_forced_oracle(cfg, sd, cross, B, 4, B)
+    lg = m.teacher_forced_logits(seq, cross, cfg['cfg_coef']).cpu()
+    # rotary positions: fp16 q / k after the rotation, the tolerance of test_rope_matches_oracle_and_reference_golden
+    assert_close(lg, ref, 2e-2, 4e-2 if pe != 'sin' else 3e-2, f'{name} {pe} rows={2 * B}')
+    if name == 'lm_medium_2l' and B == 12:
+        monkeypatch.setenv('ACB_LM_FT32', '0')
+        narrow = m.teacher_forced_logits(seq, cross, cfg['cfg_coef']).cpu()
+        monkeypatch.delenv('ACB_LM_FT32')
+        assert torch.equal(lg, narrow), f'32- vs 16-feature tiles: max diff {(lg - narrow).abs().max():.3e}'
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize('B', [6, 11])
+def test_double_cfg_rows_18_and_33_match_oracle(B):
+    """cfg_coef_beta with [cond; style-only; null] rows: 3B = 18 rows (NT = 4) and 33 rows (NT = 8), streaming steps vs the
+    oracle's double-CFG logits."""
+    cfg, sd, m = _lm('lm_mini', 3)
+    _, _, cross2 = H.lm_condition(cfg, sd, B, 5, 1)
+    _, _, other = H.lm_condition(cfg, sd, B, 5, 4)
+    cross3 = torch.cat([cross2[:B], other[:B] * 0.5, cross2[B:]], 0)
+    o = LO.LMOracle(sd, cfg, half_gemm=True)
+    cur = torch.full((B, cfg['n_q'], 1), cfg['card'], dtype=torch.long)
+    o.reset()
+    m.streaming_begin(B, cross3, max_len=10, cfg_coef=2.0, cfg_coef_beta=3.0)
+    for i in range(6):
+        tok, lg = o.next_token(cur, cross3, False, 1.0, 0, 0.0, 2.0, None, None, return_logits=True, cfg_coef_beta=3.0)
+        got = m.streaming_step(cur[..., 0]).cpu()
+        assert_close(got, lg, 3e-2, 3e-2, f'double CFG rows={3 * B} step {i}')
+        cur = tok
+
+
+def _prefill_passes(rows, n):
+    per = 64 // rows
+    return [min(per, n - s) * rows for s in range(0, n, per)]
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize('B,T0,pe,last', [(1, 35, 'sin', 6), (2, 22, 'sin', 24), (2, 22, 'rope', 24)],
+                         ids=['lm_mini-1-35', 'lm_mini-2-22', 'lm_mini-2-22-rope'])
+def test_prefill_tail_passes_equal_token_by_token(monkeypatch, B, T0, pe, last):
+    """Prompt prefill whose last pass holds <= 8 (token, row) pairs (NT = 1) or 17-32 pairs (NT = 4): generate prefills
+    start_offset_sequence - 1 = T0 positions, 64 // rows per pass.  Same KV cache and greedy tokens as token-by-token decoding,
+    the assertions of test_prompt_prefill_equals_token_by_token."""
+    cfg, sd, m = _lm('lm_mini', 5, positional_embedding=pe)
+    passes = _prefill_passes(2 * B, T0)
+    print(f'prefill passes (token, row) pairs: {passes}')
+    assert passes[-1] == last and all(p == 64 for p in passes[:-1])
+    T = T0 + 6
+    _, _, cross = H.lm_condition(cfg, sd, B, 5, 1)
+    prompt = torch.randint(0, cfg['card'], (B, 4, T0), generator=torch.Generator().manual_seed(3))
+    out_pf = m.generate(prompt.cuda(), [], num_samples=B, max_gen_len=T, use_sampling=False, cross_attention_src=cross).cpu()
+    kc_pf = m._bufs['k_cache'][:, :2 * B, :, :T0].clone()
+    vc_pf = m._bufs['v_cache'][:, :2 * B, :, :T0].clone()
+    monkeypatch.setenv('ACB_LM_PREFILL', '0')
+    out_ss = m.generate(prompt.cuda(), [], num_samples=B, max_gen_len=T, use_sampling=False, cross_attention_src=cross).cpu()
+    kc_ss = m._bufs['k_cache'][:, :2 * B, :, :T0]
+    vc_ss = m._bufs['v_cache'][:, :2 * B, :, :T0]
+    assert_close(kc_pf.float(), kc_ss.float(), 0, 4e-3, f'{pe} B={B} T0={T0} K cache')
+    assert_close(vc_pf.float(), vc_ss.float(), 0, 4e-3, f'{pe} B={B} T0={T0} V cache')
+    assert torch.equal(out_pf[..., :T0], prompt)
+    agree = (out_pf == out_ss).float().mean()
+    print(f'token agreement {agree:.4f}')
+    assert agree > 0.95
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize('name,B,t_text', [('lm_mini', 2, 31), ('lm_mini', 2, 32), ('lm_mini', 2, 33), ('lm_mini', 2, 64),
+                                           ('lm_mini', 2, 100), ('lm_medium_2l', 8, 77)])
+def test_long_text_cross_attention_matches_oracle(name, B, t_text):
+    """lm_cross_attn_kernel walks the condition in chunks of 32 positions with an online-softmax rescale between chunks and a
+    `cnt < 32` tail; T5 descriptions longer than 32 tokens are ordinary.  The medium case also runs the cross K/V projection in
+    20 chunks of 64 (token, row) pairs with a ragged last one (16 rows x 77 positions).  Padded text positions are exact zeros
+    (synth_text_condition's ragged masks).  Teacher-forced logits vs the oracle; at t_text = 100 also greedy generation."""
+    cfg, sd, m = _lm(name, 13)
+    _, mask, cross = H.lm_condition(cfg, sd, B, t_text, 6)
+    assert (cross[:B][mask == 0] == 0).all() and (mask == 0).any()
+    seq, ref = _teacher_forced_oracle(cfg, sd, cross, B, 4, t_text)
+    lg = m.teacher_forced_logits(seq, cross, cfg['cfg_coef']).cpu()
+    assert_close(lg, ref, 2e-2, 3e-2, f'{name} B={B} t_text={t_text}')
+    if t_text == 100:
+        T = 12
+        o = LO.LMOracle(sd, cfg, half_gemm=True)
+        rec = []
+        want = o.generate(None, cross, B, T, use_sampling=False, record_logits=rec)
+        oseq = o.last_sequence
+        got = m.generate(None, [], num_samples=B, max_gen_len=T, use_sampling=False, cross_attention_src=cross).cpu()
+        if not torch.equal(got, want):
+            # only the first differing sequence step is comparable: the oracle's top-2 gap there must be an fp16-noise near-tie
+            gseq = m.last_sequence.cpu()
+            step = int((gseq != oseq).any(0).any(0).nonzero()[0])
+            top2 = rec[step - 1].topk(2, dim=-1).values
+            diff = (gseq[..., step] != oseq[..., step])
+            gap = (top2[..., 0] - top2[..., 1])[diff]
+            print(f'greedy tokens diverge at sequence step {step}, oracle top-2 gaps {gap.tolist()}')
+            assert (gap < 5e-2).all(), 'greedy token differs from the oracle although its argmax margin is clear'

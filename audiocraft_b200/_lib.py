@@ -71,6 +71,7 @@ def lib():
     L.acb_lm_create.argtypes = [C.POINTER(LMConfig), C.POINTER(LMWeights), C.POINTER(LMBuffers), C.POINTER(vp)]
     L.acb_lm_destroy.argtypes = [vp]
     L.acb_lm_begin.argtypes = [vp, vp, ci, ci, ci, ci, C.POINTER(LMSampling), vp]
+    L.acb_lm_begin_prefix.argtypes = [vp, vp, vp, ci, ci, ci, ci, ci, C.POINTER(LMSampling), vp]
     L.acb_lm_steps.argtypes = [vp, ci, vp]
     L.acb_lm_prefill.argtypes = [vp, ci, ci, vp]
     L.acb_lm_step_logits.argtypes = [vp, vp, vp]
@@ -80,7 +81,7 @@ def lib():
     L.acb_lm_debug_gemms.argtypes = [vp, vp, C.POINTER(ci)]
     L.acb_sample.argtypes = [vp, vp, vp, ci, ci, ci, ci, C.POINTER(LMSampling), C.c_uint64, vp]
     for name in ('acb_weight_norm_fold', 'acb_conv1d', 'acb_convtr1d', 'acb_lstm_recurrent', 'acb_rvq_encode',
-                 'acb_rvq_decode', 'acb_lm_create', 'acb_lm_destroy', 'acb_lm_begin', 'acb_lm_steps',
+                 'acb_rvq_decode', 'acb_lm_create', 'acb_lm_destroy', 'acb_lm_begin', 'acb_lm_begin_prefix', 'acb_lm_steps',
                  'acb_lm_step_logits', 'acb_lm_launches_per_step', 'acb_lm_rows_pad', 'acb_sample',
                  'acb_device_sm_count', 'acb_lm_debug_gemms', 'acb_lm_uses_pdl',
                  'acb_conv1d_t6', 'acb_conv1d_t6_tile', 'acb_lm_prefill',
@@ -93,7 +94,7 @@ def lib():
 # every symbol include/audiocraft_b200.h declares (checked by tests/test_host.py against the header text)
 EXPORTS = ['acb_version', 'acb_last_error', 'acb_device_sm_count', 'acb_weight_norm_fold', 'acb_conv1d', 'acb_convtr1d',
            'acb_lstm_recurrent', 'acb_lstm_state_bytes', 'acb_rvq_encode', 'acb_rvq_decode', 'acb_lm_create',
-           'acb_lm_destroy', 'acb_lm_begin', 'acb_lm_steps', 'acb_lm_step_logits', 'acb_lm_rows_pad',
+           'acb_lm_destroy', 'acb_lm_begin', 'acb_lm_begin_prefix', 'acb_lm_steps', 'acb_lm_step_logits', 'acb_lm_rows_pad',
            'acb_lm_launches_per_step', 'acb_lm_debug_gemms', 'acb_lm_uses_pdl', 'acb_sample', 'acb_conv1d_t6', 'acb_conv1d_t6_tile',
            'acb_lm_prefill', 'acb_resblock', 'acb_resblock_supported']
 

@@ -79,15 +79,16 @@ __device__ __forceinline__ float block_max(float v, float* red) {
 // x[r] = sum_k emb_k[seq[b,k,pos]] + pos_scale * [cos(pos/f_i), sin(pos/f_i)]   (lm.py:244, transformer.py:70-89,701-705)
 // The sin term only when sin_pos ('sin' and 'sin_rope'; a 'rope' model has its positions in the QKV epilogue alone).
 // PF (prompt prefill): the grid's rows are (token, row) pairs r = tok * rows_real + row at positions P[0] + tok.
+// seq_off: length of the condition prefix in front of the tokens; cache position pos reads sequence column pos - seq_off.
 template <bool PF>
 __global__ void __launch_bounds__(256) lm_embed_kernel(const __half* __restrict__ emb, const float* __restrict__ inv_freq,
                                                        const int64_t* __restrict__ seq, const int* __restrict__ P,
                                                        float* __restrict__ x, int d, int n_q, int card, int max_seq,
-                                                       int batch, float pos_scale, int rows_real, bool sin_pos) {
+                                                       int batch, float pos_scale, int rows_real, bool sin_pos, int seq_off) {
     const int r = blockIdx.x, b = (PF ? r % rows_real : r) % batch, pos = P[0] + (PF ? r / rows_real : 0);
     __shared__ int tok[16];
     if (threadIdx.x < n_q) {
-        long long t = seq[((size_t)b * n_q + threadIdx.x) * max_seq + pos];
+        long long t = seq[((size_t)b * n_q + threadIdx.x) * max_seq + pos - seq_off];
         tok[threadIdx.x] = (int)(t < 0 ? card : (t > card ? card : t));
     }
     __syncthreads();
@@ -95,6 +96,26 @@ __global__ void __launch_bounds__(256) lm_embed_kernel(const __half* __restrict_
     for (int i = threadIdx.x; i < d; i += 256) {   // d % 32 == 0: a warp is entirely inside or outside the row
         float v = 0.f;
         for (int k = 0; k < n_q; ++k) v += __half2float(emb[((size_t)k * (card + 1) + tok[k]) * d + i]);
+        if (sin_pos) {
+            const int j = i < half_d ? i : i - half_d;
+            const float phase = (float)pos / inv_freq[j];
+            v += pos_scale * (i < half_d ? cosf(phase) : sinf(phase));
+        }
+        x[(size_t)r * d + i] = v;
+    }
+}
+
+// Condition-prefix prefill (the `prepend` fuser, conditioners.py:1703-1763): the grid's rows are (position, row) pairs
+// r = p * rows_real + row at cache positions P[0] + p, and x[r] = prefix[row][P[0] + p] (rounded to fp16 like the reference's
+// autocast output_proj) + the sin term.  Each row has its own prefix: cond and null rows differ.
+__global__ void __launch_bounds__(256) lm_embed_prefix_kernel(const float* __restrict__ prefix, const float* __restrict__ inv_freq,
+                                                              const int* __restrict__ P, float* __restrict__ x, int d,
+                                                              int prefix_len, float pos_scale, int rows_real, bool sin_pos) {
+    const int r = blockIdx.x, row = r % rows_real, pos = P[0] + r / rows_real;
+    const float* src = prefix + ((size_t)row * prefix_len + pos) * d;
+    const int half_d = d >> 1;
+    for (int i = threadIdx.x; i < d; i += 256) {
+        float v = half_round(src[i]);
         if (sin_pos) {
             const int j = i < half_d ? i : i - half_d;
             const float phase = (float)pos / inv_freq[j];
@@ -535,6 +556,7 @@ struct SampleParams {
     int batch, rows, n_q, card, NP;
     int use_sampling, top_k; float temp, top_p, cfg_coef; uint64_t seed; uint32_t step;
     float cfg_coef_beta;   // rows == 3 * batch: double CFG (lm.py:362-376)
+    int seq_off;           // condition-prefix length: cache position pos is sequence column pos - seq_off
 };
 
 // descending order, ties by ascending index
@@ -556,7 +578,8 @@ __global__ void __launch_bounds__(1024) lm_sample_kernel(SampleParams p) {
     const float* lu = p.logits + ((size_t)((cfg3 ? 2 : 1) * p.batch + b) * p.n_q + k) * card;
     const float* lw = p.logits + ((size_t)(p.batch + b) * p.n_q + k) * card;
     const int cur_pos = p.pos ? p.pos[0] : 0;   // read once: the last block to finish advances it (below)
-    const uint32_t step = p.pos ? (uint32_t)cur_pos : p.step;
+    const int col = cur_pos - p.seq_off;        // sequence column of the token this step consumed
+    const uint32_t step = p.pos ? (uint32_t)col : p.step;
 
     for (int i = tid; i < card; i += nt) {
         float l = lc[i];
@@ -691,7 +714,7 @@ __global__ void __launch_bounds__(1024) lm_sample_kernel(SampleParams p) {
         int tok = sorted_space ? si[bi] : bi;
         if (p.tokens) p.tokens[(size_t)b * p.n_q + k] = tok;
         if (p.seq) {
-            const int off = cur_pos + 1;
+            const int off = col + 1;
             if (off < p.max_seq) {
                 if (!p.seq_mask[(size_t)k * p.max_seq + off]) tok = card;            // lm.py:555-556
                 int64_t* dst = p.seq + ((size_t)b * p.n_q + k) * p.max_seq + off;
@@ -720,6 +743,8 @@ struct acb_lm {
     cudaGraph_t graph = nullptr;
     cudaGraphExec_t exec = nullptr;
     int batch = 0, rows = 0, rows_pad = 0, text_len = 0, seq_len = 0, sms = 132;
+    int prefix_len = 0;            // condition-prefix positions in front of the tokens in the KV cache
+    const float* prefix = nullptr; // [rows][prefix_len][d] fp32, set only while acb_lm_begin_prefix enqueues the prefix passes
     int launches = 0;
     bool has_cross = false;
 };
@@ -833,11 +858,13 @@ static int acb_dbg(cudaStream_t s, bool capturing, const char* what, int layer) 
 // the same kernels run on rows * pf_tokens (token, row) pairs -- positions pos .. pos + pf_tokens - 1 of every row at once, causal
 // inside the pass because the QKV GEMM appends all of them to the cache before the attention kernel runs -- and stop after the
 // last layer (no logits: the next decode step consumes the last prompt position).
+// pf_prefix: the pass embeds condition-prefix vectors (lm->prefix) instead of tokens, otherwise it is a prefill pass like any other.
 static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_launch, bool gemms_only = false,
-                        bool capturing = false, int pf_tokens = 0) {
+                        bool capturing = false, int pf_tokens = 0, bool pf_prefix = false) {
     const acb_lm_config& c = lm->cfg;
     const acb_lm_buffers& B = lm->buf;
     const bool pf = pf_tokens > 0;
+    ACB_REQUIRE(!pf_prefix || (pf && lm->prefix), "enqueue_step: a prefix pass needs the prefix of acb_lm_begin_prefix");
     const int rows_real = lm->rows, rows = pf ? rows_real * pf_tokens : rows_real;
     const int d = c.dim, ffn = c.ffn_dim, L = c.num_layers, H = c.num_heads, nt = nt_for_rows(rows);
     const size_t part_stride = (size_t)(pf ? 8 * nt : lm->rows_pad) * d;
@@ -848,10 +875,13 @@ static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_la
 
     if (!gemms_only) {
         const bool sin_pos = c.positional_embedding != 1;
-        if (pf) lm_embed_kernel<true><<<rows, 256, 0, s>>>((const __half*)lm->w.emb, lm->w.inv_freq, B.seq, B.pos, B.x, d, c.n_q,
-                                                         c.card, c.max_seq, lm->batch, c.pos_scale, rows_real, sin_pos);
+        if (pf && pf_prefix) lm_embed_prefix_kernel<<<rows, 256, 0, s>>>(lm->prefix, lm->w.inv_freq, B.pos, B.x, d, lm->prefix_len,
+                                                                       c.pos_scale, rows_real, sin_pos);
+        else if (pf) lm_embed_kernel<true><<<rows, 256, 0, s>>>((const __half*)lm->w.emb, lm->w.inv_freq, B.seq, B.pos, B.x, d, c.n_q,
+                                                              c.card, c.max_seq, lm->batch, c.pos_scale, rows_real, sin_pos,
+                                                              lm->prefix_len);
         else lm_embed_kernel<false><<<rows, 256, 0, s>>>((const __half*)lm->w.emb, lm->w.inv_freq, B.seq, B.pos, B.x, d, c.n_q,
-                                                      c.card, c.max_seq, lm->batch, c.pos_scale, rows, sin_pos);
+                                                      c.card, c.max_seq, lm->batch, c.pos_scale, rows, sin_pos, lm->prefix_len);
         ACB_LAUNCH_CHECK();
         ++nl;
         DBG("lm_embed_kernel", -1);
@@ -949,7 +979,8 @@ static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_la
         while (NP < c.card) NP <<= 1;
         SampleParams sp{B.logits, lm->samp.noise_from_buffer ? B.noise : nullptr, logits_out, B.seq, B.seq_mask, B.pos,
                         c.max_seq, nullptr, lm->batch, rows, c.n_q, c.card, NP, lm->samp.use_sampling, lm->samp.top_k,
-                        lm->samp.temp, lm->samp.top_p, lm->samp.cfg_coef, lm->samp.seed, 0, lm->samp.cfg_coef_beta};
+                        lm->samp.temp, lm->samp.top_p, lm->samp.cfg_coef, lm->samp.seed, 0, lm->samp.cfg_coef_beta,
+                        lm->prefix_len};
         size_t smem = ((size_t)c.card + 2 * (size_t)NP) * sizeof(float);
         lm_sample_kernel<<<dim3(c.n_q, lm->batch), 1024, smem, s>>>(sp);
         ACB_LAUNCH_CHECK();
@@ -999,6 +1030,7 @@ extern "C" int acb_lm_create(const acb_lm_config* cfg, const acb_lm_weights* w, 
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_cross_attn_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_ln_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_embed_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+    if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_embed_prefix_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_sample_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     if (ea != cudaSuccess) {
         acb_set_error("acb_lm_create: cudaFuncSetAttribute: %s", cudaGetErrorString(ea));
@@ -1023,18 +1055,64 @@ extern "C" int acb_lm_destroy(acb_lm_t* lm) {
     return ACB_OK;
 }
 
+__global__ void lm_set_pos_kernel(int* pos, int value) { pos[0] = value; }
+
+// Prefill passes over cache positions [pos0, pos0 + n) of every row, ACB_LM_PREFILL_ROWS / rows positions per pass: token
+// columns pos - prefix_len of buffers.seq, or (prefix) the condition-prefix vectors.  Leaves pos = pos0 + n on the device and the
+// padded decode rows [rows, rows_pad) of the activation buffers zero.
+static int prefill_passes(acb_lm* lm, cudaStream_t s, int pos0, int n, bool prefix) {
+    const acb_lm_config& c = lm->cfg;
+    const int d = c.dim;
+    int per = ACB_LM_PREFILL_ROWS / lm->rows;
+    ACB_REQUIRE(per >= 1, "acb_lm_prefill: rows %d > %d", lm->rows, ACB_LM_PREFILL_ROWS);
+    // ACB_LM_PREFILL_PER=n: at most n positions per pass (n = 1: one position per pass, the reference order for tests)
+    if (const char* e = getenv("ACB_LM_PREFILL_PER")) { const int cap = atoi(e); if (cap >= 1 && cap < per) per = cap; }
+    int done = 0;
+    while (done < n) {
+        const int tc = n - done < per ? n - done : per;
+        const int vrows = lm->rows * tc, pad = 8 * nt_for_rows(vrows);
+        lm_set_pos_kernel<<<1, 1, 0, s>>>(lm->buf.pos, pos0 + done);
+        ACB_LAUNCH_CHECK();
+        if (pad > vrows) {   // the GEMMs read their activation rows up to the tile height: rows >= vrows must be zero
+            ACB_CHECK_CUDA(cudaMemsetAsync((__half*)lm->buf.h16 + (size_t)vrows * d, 0, (size_t)(pad - vrows) * d * sizeof(__half), s));
+            ACB_CHECK_CUDA(cudaMemsetAsync((__half*)lm->buf.a16 + (size_t)vrows * d, 0, (size_t)(pad - vrows) * d * sizeof(__half), s));
+            ACB_CHECK_CUDA(cudaMemsetAsync((__half*)lm->buf.f16 + (size_t)vrows * c.ffn_dim, 0, (size_t)(pad - vrows) * c.ffn_dim * sizeof(__half), s));
+        }
+        ACB_TRY(enqueue_step(lm, s, nullptr, nullptr, false, false, tc, prefix));
+        done += tc;
+    }
+    lm_set_pos_kernel<<<1, 1, 0, s>>>(lm->buf.pos, pos0 + n);
+    ACB_LAUNCH_CHECK();
+    // back to decode: its padded rows [rows, rows_pad) must be zero again
+    if (lm->rows_pad > lm->rows) {
+        ACB_CHECK_CUDA(cudaMemsetAsync((__half*)lm->buf.h16 + (size_t)lm->rows * d, 0, (size_t)(lm->rows_pad - lm->rows) * d * sizeof(__half), s));
+        ACB_CHECK_CUDA(cudaMemsetAsync((__half*)lm->buf.a16 + (size_t)lm->rows * d, 0, (size_t)(lm->rows_pad - lm->rows) * d * sizeof(__half), s));
+        ACB_CHECK_CUDA(cudaMemsetAsync((__half*)lm->buf.f16 + (size_t)lm->rows * c.ffn_dim, 0, (size_t)(lm->rows_pad - lm->rows) * c.ffn_dim * sizeof(__half), s));
+    }
+    return ACB_OK;
+}
+
 extern "C" int acb_lm_begin(acb_lm_t* lm, const float* cross, int batch, int rows, int text_len, int seq_len,
                             const acb_lm_sampling* sampling, void* stream) {
+    return acb_lm_begin_prefix(lm, cross, nullptr, 0, batch, rows, text_len, seq_len, sampling, stream);
+}
+
+extern "C" int acb_lm_begin_prefix(acb_lm_t* lm, const float* cross, const float* prefix, int prefix_len, int batch, int rows,
+                                   int text_len, int seq_len, const acb_lm_sampling* sampling, void* stream) {
     ACB_REQUIRE(lm && sampling, "acb_lm_begin: null argument");
     const acb_lm_config& c = lm->cfg;
     ACB_REQUIRE(batch >= 1 && (rows == batch || rows == 2 * batch || rows == 3 * batch), "acb_lm_begin: rows must be batch, 2*batch (CFG) or 3*batch (double CFG)");
     ACB_REQUIRE(rows <= c.max_rows, "acb_lm_begin: rows %d > max_rows %d", rows, c.max_rows);
-    ACB_REQUIRE(seq_len >= 2 && seq_len <= c.max_seq, "acb_lm_begin: seq_len %d > max_seq %d", seq_len, c.max_seq);
+    ACB_REQUIRE(prefix_len >= 0 && (prefix_len == 0 || prefix), "acb_lm_begin: prefix_len %d without a prefix tensor", prefix_len);
+    ACB_REQUIRE(seq_len >= 2 && prefix_len + seq_len <= c.max_seq, "acb_lm_begin: prefix %d + seq_len %d > max_seq %d", prefix_len,
+                seq_len, c.max_seq);
+    ACB_REQUIRE(prefix_len == 0 || rows <= ACB_LM_PREFILL_ROWS, "acb_lm_begin: a condition prefix needs rows <= %d", ACB_LM_PREFILL_ROWS);
     ACB_REQUIRE(!c.cross_attention || cross, "acb_lm_begin: the model has cross attention, a condition tensor is required"
                 " (the reference asserts the same, transformer.py:553-556)");
     ACB_REQUIRE(!cross || (text_len >= 1 && text_len <= c.max_text), "acb_lm_begin: text_len %d out of range", text_len);
     cudaStream_t s = (cudaStream_t)stream;
     lm->batch = batch; lm->rows = rows; lm->rows_pad = 8 * nt_for_rows(rows); lm->text_len = text_len; lm->seq_len = seq_len;
+    lm->prefix_len = prefix_len; lm->prefix = prefix;
     lm->samp = *sampling;
     lm->has_cross = c.cross_attention && cross;
     const int d = c.dim, H = c.num_heads;
@@ -1060,6 +1138,10 @@ extern "C" int acb_lm_begin(acb_lm_t* lm, const float* cross, int batch, int row
                 ACB_TRY(launch_gemm<EPI_CROSSKV>(8, p, 1, s));
             }
     }
+    // the condition prefix fills cache positions [0, prefix_len) once per generate (after the cross K/V: the passes attend to
+    // them); decode and prompt prefill then run at cache position prefix_len + sequence column
+    if (prefix_len > 0) ACB_TRY(prefill_passes(lm, s, 0, prefix_len, true));
+    lm->prefix = nullptr;   // read only by the passes just enqueued: the caller's tensor is not referenced after this call
     // opt in to large dynamic shared memory where needed
     {
         int NP = 1;
@@ -1082,41 +1164,14 @@ extern "C" int acb_lm_begin(acb_lm_t* lm, const float* cross, int batch, int row
     return rc != ACB_OK ? rc : ACB_ERR_CUDA;
 }
 
-__global__ void lm_set_pos_kernel(int* pos, int value) { pos[0] = value; }
-
-// Prompt prefill: consume sequence positions [pos0, pos0 + n_tokens) of every row (their tokens are already in buffers.seq)
-// without sampling, ACB_LM_PREFILL_ROWS / rows positions per pass.  Leaves pos = pos0 + n_tokens on the device.
+// Prompt prefill: consume sequence columns [pos0, pos0 + n_tokens) of every row (their tokens are already in buffers.seq)
+// without sampling, ACB_LM_PREFILL_ROWS / rows positions per pass, at cache positions prefix_len + column.  Leaves
+// pos = prefix_len + pos0 + n_tokens on the device.
 extern "C" int acb_lm_prefill(acb_lm_t* lm, int pos0, int n_tokens, void* stream) {
     ACB_REQUIRE(lm && lm->rows > 0, "acb_lm_prefill: call acb_lm_begin first");
     ACB_REQUIRE(pos0 >= 0 && n_tokens >= 0 && pos0 + n_tokens < lm->seq_len, "acb_lm_prefill: positions [%d, %d) exceed the sequence (%d)",
                 pos0, pos0 + n_tokens, lm->seq_len);
-    cudaStream_t s = (cudaStream_t)stream;
-    const acb_lm_config& c = lm->cfg;
-    const int d = c.dim, per = ACB_LM_PREFILL_ROWS / lm->rows;
-    ACB_REQUIRE(per >= 1, "acb_lm_prefill: rows %d > %d", lm->rows, ACB_LM_PREFILL_ROWS);
-    int done = 0;
-    while (done < n_tokens) {
-        const int tc = n_tokens - done < per ? n_tokens - done : per;
-        const int vrows = lm->rows * tc, pad = 8 * nt_for_rows(vrows);
-        lm_set_pos_kernel<<<1, 1, 0, s>>>(lm->buf.pos, pos0 + done);
-        ACB_LAUNCH_CHECK();
-        if (pad > vrows) {   // the GEMMs read their activation rows up to the tile height: rows >= vrows must be zero
-            ACB_CHECK_CUDA(cudaMemsetAsync((__half*)lm->buf.h16 + (size_t)vrows * d, 0, (size_t)(pad - vrows) * d * sizeof(__half), s));
-            ACB_CHECK_CUDA(cudaMemsetAsync((__half*)lm->buf.a16 + (size_t)vrows * d, 0, (size_t)(pad - vrows) * d * sizeof(__half), s));
-            ACB_CHECK_CUDA(cudaMemsetAsync((__half*)lm->buf.f16 + (size_t)vrows * c.ffn_dim, 0, (size_t)(pad - vrows) * c.ffn_dim * sizeof(__half), s));
-        }
-        ACB_TRY(enqueue_step(lm, s, nullptr, nullptr, false, false, tc));
-        done += tc;
-    }
-    lm_set_pos_kernel<<<1, 1, 0, s>>>(lm->buf.pos, pos0 + n_tokens);
-    ACB_LAUNCH_CHECK();
-    // back to decode: its padded rows [rows, rows_pad) must be zero again
-    if (lm->rows_pad > lm->rows) {
-        ACB_CHECK_CUDA(cudaMemsetAsync((__half*)lm->buf.h16 + (size_t)lm->rows * d, 0, (size_t)(lm->rows_pad - lm->rows) * d * sizeof(__half), s));
-        ACB_CHECK_CUDA(cudaMemsetAsync((__half*)lm->buf.a16 + (size_t)lm->rows * d, 0, (size_t)(lm->rows_pad - lm->rows) * d * sizeof(__half), s));
-        ACB_CHECK_CUDA(cudaMemsetAsync((__half*)lm->buf.f16 + (size_t)lm->rows * c.ffn_dim, 0, (size_t)(lm->rows_pad - lm->rows) * c.ffn_dim * sizeof(__half), s));
-    }
-    return ACB_OK;
+    return prefill_passes(lm, (cudaStream_t)stream, lm->prefix_len + pos0, n_tokens, false);
 }
 
 extern "C" int acb_lm_uses_pdl(const acb_lm_t*) { return 0; }
@@ -1150,7 +1205,7 @@ extern "C" int acb_sample(const float* logits, const float* noise, int64_t* toke
     while (NP < card) NP <<= 1;
     SampleParams sp{logits, sampling->noise_from_buffer ? noise : nullptr, nullptr, nullptr, nullptr, nullptr, 0, tokens, batch, rows, n_q, card, NP,
                     sampling->use_sampling, sampling->top_k, sampling->temp, sampling->top_p, sampling->cfg_coef,
-                    sampling->seed, (uint32_t)step, sampling->cfg_coef_beta};
+                    sampling->seed, (uint32_t)step, sampling->cfg_coef_beta, 0};
     size_t smem = ((size_t)card + 2 * (size_t)NP) * sizeof(float);
     if (smem > 48 * 1024)
         ACB_CHECK_CUDA(cudaFuncSetAttribute(lm_sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

@@ -36,6 +36,8 @@ class LMModel:
         self.pattern_provider = DelayedPatternProvider(self.n_q, delays=cfg['delays'])
         self.condition_provider = condition_provider
         self.fuser = fuser if fuser is not None else ConditionFuser({'cross': ['description']})
+        # `prepend` fuser (MusicGen-melody): the conditions run as a prefix of the sequence, prefilled into the KV cache
+        self.has_prefix = bool(self.fuser.fuse2cond.get('prepend'))
         if self.condition_provider is not None:
             self.condition_provider.to(self.device)
             cp = {k[len('condition_provider.'):]: v for k, v in state_dict.items() if k.startswith('condition_provider.')}
@@ -187,8 +189,12 @@ class LMModel:
 
     # ------------------------------------------------------------------ conditions (lm.py:488-511)
     def _prepare_conditions(self, conditions, two_step_cfg, cfg_coef_beta):
+        return self._condition_tensors(conditions, cfg_coef_beta)[0]
+
+    def _condition_tensors(self, conditions, cfg_coef_beta=None):
+        """(cross_attention_src, prefix) of [conditions; null conditions], each None when the fuser produces none."""
         if not conditions:
-            return None
+            return None, None
         assert self.condition_provider is not None, "conditions given but the model has no condition_provider"
         if cfg_coef_beta is not None:
             # lm.py:490-496: [conditions; conditions without their description; null conditions].  The style-only rows need
@@ -202,7 +208,27 @@ class LMModel:
         null_conditions = nullify_all(conditions)
         tokenized = self.condition_provider.tokenize(list(conditions) + null_conditions)
         tensors = self.condition_provider(tokenized)
-        return self.fuser.cross_source(tensors)
+        return self.fuser.cross_source(tensors), self.fuser.prefix_source(tensors)
+
+    def _check_prefix(self, prefix, rows, two_step_cfg=False, cfg_coef_beta=None):
+        """The condition prefix as the contiguous fp32 CUDA tensor [rows, P, d] acb_lm_begin_prefix takes (None: P = 0)."""
+        if prefix is None:
+            return None, 0
+        if two_step_cfg:
+            raise NotImplementedError("two_step_cfg with a condition prefix (prepend fuser) is not built")
+        if cfg_coef_beta is not None:
+            raise NotImplementedError("double CFG (cfg_coef_beta) with a condition prefix (prepend fuser) is not built")
+        prefix = prefix.to(self.device, torch.float32).contiguous()
+        assert prefix.dim() == 3 and prefix.shape[2] == self.dim and prefix.shape[0] == rows, \
+            f"prefix must be [rows={rows}, P, {self.dim}], got {tuple(prefix.shape)}"
+        if prefix.shape[1] == 0:
+            return None, 0
+        assert rows <= _lib.ACB_LM_PREFILL_ROWS, f"a condition prefix needs rows <= {_lib.ACB_LM_PREFILL_ROWS}"
+        return prefix, prefix.shape[1]
+
+    def _begin(self, cross, prefix, P, B, rows, text_len, S, samp):
+        _lib.check(self._lib.acb_lm_begin_prefix(self._handle, _lib.ptr(cross), _lib.ptr(prefix), P, B, rows, text_len, S,
+                                                 C.byref(samp), _lib.stream()), 'lm_begin')
 
     # ------------------------------------------------------------------ generation
     @torch.no_grad()
@@ -213,9 +239,11 @@ class LMModel:
                  cfg_coef_beta: tp.Optional[float] = None, two_step_cfg: tp.Optional[bool] = None,
                  remove_prompts: bool = False, check: bool = False,
                  callback: tp.Optional[tp.Callable[[int, int], None]] = None,
-                 cross_attention_src: tp.Optional[torch.Tensor] = None) -> torch.Tensor:
+                 cross_attention_src: tp.Optional[torch.Tensor] = None,
+                 prefix: tp.Optional[torch.Tensor] = None) -> torch.Tensor:
         """Same contract as LMModel.generate (lm.py:420-587).  ``cross_attention_src`` is an extension: a pre-computed
-        [2B,T,d] (or [B,T,d] without CFG) condition tensor, bypassing the host conditioners."""
+        [2B,T,d] (or [B,T,d] without CFG) condition tensor, bypassing the host conditioners.  ``prefix`` likewise: a
+        pre-computed [rows,P,d] condition prefix (the `prepend` fuser's output, one per row) for a model that has one."""
         if num_samples is None:
             if prompt is not None:
                 num_samples = prompt.shape[0]
@@ -226,8 +254,14 @@ class LMModel:
             else:
                 num_samples = 1
         two_step_cfg = self.two_step_cfg if two_step_cfg is None else two_step_cfg
-        cross = cross_attention_src if cross_attention_src is not None else \
-            self._prepare_conditions(conditions, two_step_cfg, cfg_coef_beta)
+        if self.has_prefix and two_step_cfg:
+            raise NotImplementedError("two_step_cfg with a condition prefix (prepend fuser) is not built")
+        if self.has_prefix and cfg_coef_beta is not None:
+            raise NotImplementedError("double CFG (cfg_coef_beta) with a condition prefix (prepend fuser) is not built")
+        if cross_attention_src is not None or prefix is not None:
+            cross = cross_attention_src
+        else:
+            cross, prefix = self._condition_tensors(conditions, cfg_coef_beta)
         B, K = num_samples, self.n_q
         # lm.py:387 quirk: the two-step branch uses self.cfg_coef, not the argument.  (With exact-zero null rows the
         # two passes are numerically the batched pass: V = 0 makes the null branch independent of its padding.)
@@ -261,7 +295,11 @@ class LMModel:
                 assert (cross.shape[0] == 3 * B) == (cfg_coef_beta is not None), \
                     "cfg_coef_beta goes with 3B condition rows (lm.py:362-376)"
                 rows, text_len = cross.shape[0], cross.shape[1]
-            self._ensure(rows, S, text_len, B)
+            elif prefix is not None:
+                rows = prefix.shape[0]
+                assert rows in (B, 2 * B), "prefix rows must be B (no CFG) or 2B ([cond; null])"
+            prefix, P = self._check_prefix(prefix, rows, two_step_cfg, cfg_coef_beta)
+            self._ensure(rows, P + S, text_len, B)
             bufs = self._bufs
             bufs['seq'][:B, :, :S] = gen_sequence
             bufs['seq_mask'][:, :S] = mask.to(torch.uint8)
@@ -269,8 +307,7 @@ class LMModel:
             samp = _lib.LMSampling(int(bool(use_sampling)), float(temp), int(top_k), float(top_p), float(coef), seed,
                                    1 if self._debug_noise_fn is not None else 0,
                                    float(cfg_coef_beta) if cfg_coef_beta is not None else 0.0)
-            _lib.check(self._lib.acb_lm_begin(self._handle, _lib.ptr(cross), B, rows, text_len, S, C.byref(samp),
-                                              _lib.stream()), 'lm_begin')
+            self._begin(cross, prefix, P, B, rows, text_len, S, samp)
             self.launches_per_step = self._lib.acb_lm_launches_per_step(self._handle)
             n_steps = S - 1
             # Prompt prefill (the reference's multi-token first call, lm.py:513-534, transformer.py:240-247): positions
@@ -312,16 +349,21 @@ class LMModel:
     # them to run two_step_cfg (lm.py:376-391).  Here the same observable state lives in the device KV cache + the device
     # position counter; the methods below expose it under the reference's key names.
     def streaming_begin(self, batch: int, cross: tp.Optional[torch.Tensor], max_len: int, cfg_coef: tp.Optional[float] = None,
-                        cfg_coef_beta: tp.Optional[float] = None, **sampling):
+                        cfg_coef_beta: tp.Optional[float] = None, prefix: tp.Optional[torch.Tensor] = None, **sampling):
         """Enter streaming mode for `batch` items (what `with lm.streaming():` + the first forward do in the reference):
         allocates / resets the caches, precomputes the cross-attention K/V of `cross` ([rows,T,d] rows = batch, 2*batch or
-        3*batch) and captures the step graph.  Then `streaming_step(tokens)` consumes one [B,K] column per call."""
+        3*batch), prefills the condition `prefix` ([rows,P,d], the first call's prepended conditions) and captures the step
+        graph.  Then `streaming_step(tokens)` consumes one [B,K] column per call; offsets count the prefix, as the
+        reference's transformer offsets do."""
         with torch.cuda.device(self.device):
             rows, text_len = batch, 0
             if cross is not None:
                 cross = cross.to(self.device, torch.float32).contiguous()
                 rows, text_len = cross.shape[0], cross.shape[1]
-            self._ensure(rows, max_len + 1, text_len, batch)
+            elif prefix is not None:
+                rows = prefix.shape[0]
+            prefix, P = self._check_prefix(prefix, rows, False, cfg_coef_beta)
+            self._ensure(rows, P + max_len + 1, text_len, batch)
             b = self._bufs
             b['seq'][:batch].fill_(-1)
             b['seq_mask'].fill_(1)
@@ -329,9 +371,8 @@ class LMModel:
                                    int(sampling.get('top_k', 0)), float(sampling.get('top_p', 0.0)),
                                    float(self.cfg_coef if cfg_coef is None else cfg_coef), int(sampling.get('seed', 0)), 0,
                                    float(cfg_coef_beta) if cfg_coef_beta is not None else 0.0)
-            _lib.check(self._lib.acb_lm_begin(self._handle, _lib.ptr(cross), batch, rows, text_len, max_len + 1, C.byref(samp),
-                                              _lib.stream()), 'lm_begin')
-            self._stream = dict(batch=batch, rows=rows, max_len=max_len)
+            self._begin(cross, prefix, P, batch, rows, text_len, max_len + 1, samp)
+            self._stream = dict(batch=batch, rows=rows, max_len=max_len, prefix_len=P)
 
     @torch.no_grad()
     def streaming_step(self, tokens: torch.Tensor) -> torch.Tensor:
@@ -339,7 +380,7 @@ class LMModel:
         [B,K,card]; the KV cache grows by one position."""
         st = self._stream
         with torch.cuda.device(self.device):
-            pos = int(self._bufs['pos'][0].item())
+            pos = int(self._bufs['pos'][0].item()) - st['prefix_len']   # sequence column
             assert pos < st['max_len'], "streaming_begin(max_len) exceeded"
             self._bufs['seq'][:st['batch'], :, pos] = tokens.to(self.device, torch.long)
             self._bufs['seq'][:st['batch'], :, pos + 1] = -1
@@ -375,20 +416,23 @@ class LMModel:
             b['k_cache'][li, :rows, :, :pos] = k
             b['v_cache'][li, :rows, :, :pos] = v
         assert len(state) == 0, list(state.keys())
+        assert pos >= st['prefix_len'], "the state must include the condition prefix"
         b['pos'][0] = pos
 
     def reset_streaming(self):
-        """StreamingModule.reset_streaming (streaming.py:64-70): forget the cached positions."""
-        self._bufs['pos'][0] = 0
+        """StreamingModule.reset_streaming (streaming.py:64-70): forget the cached positions.  A condition prefix stays
+        cached: the reference prepends it again on the first call after a reset, which is the same cache content."""
+        self._bufs['pos'][0] = self._stream.get('prefix_len', 0) if getattr(self, '_stream', None) else 0
 
     @torch.no_grad()
     def teacher_forced_logits(self, sequence: torch.Tensor, cross: tp.Optional[torch.Tensor], cfg_coef: float,
                               n_steps: tp.Optional[int] = None, keep: tp.Optional[tp.Sequence[int]] = None,
-                              raw: bool = False):
+                              raw: bool = False, prefix: tp.Optional[torch.Tensor] = None):
         """Feed a fully known delay-pattern sequence [B,K,S] token by token and return the (CFG-mixed when cross has
         2B rows) next-token logits [n_steps,B,K,card] -- LMModel.forward in streaming mode (lm.py:221-268), the
         quantity the parity tests compare against the oracle.  ``keep``: only these step indices are returned (in that
-        order; every step still runs).  ``raw``: also return the un-mixed per-row logits [n,rows,K,card] ([cond; null])."""
+        order; every step still runs).  ``raw``: also return the un-mixed per-row logits [n,rows,K,card] ([cond; null]).
+        ``prefix``: [rows,P,d] condition prefix prefilled in front of the sequence (its logits are not returned)."""
         with torch.cuda.device(self.device):
             sequence = sequence.to(self.device, torch.long)
             B, K, S = sequence.shape
@@ -396,13 +440,15 @@ class LMModel:
             if cross is not None:
                 cross = cross.to(self.device, torch.float32).contiguous()
                 rows, text_len = cross.shape[0], cross.shape[1]
-            self._ensure(rows, S, text_len, B)
+            elif prefix is not None:
+                rows = prefix.shape[0]
+            prefix, P = self._check_prefix(prefix, rows)
+            self._ensure(rows, P + S, text_len, B)
             bufs = self._bufs
             bufs['seq'][:B, :, :S] = sequence
             bufs['seq_mask'][:, :S] = 1
             samp = _lib.LMSampling(0, 1.0, 0, 0.0, float(cfg_coef), 0, 0)
-            _lib.check(self._lib.acb_lm_begin(self._handle, _lib.ptr(cross), B, rows, text_len, S, C.byref(samp),
-                                              _lib.stream()), 'lm_begin')
+            self._begin(cross, prefix, P, B, rows, text_len, S, samp)
             self.launches_per_step = self._lib.acb_lm_launches_per_step(self._handle)
             n = S - 1 if n_steps is None else n_steps
             slot = {i: j for j, i in enumerate(range(n) if keep is None else keep)}

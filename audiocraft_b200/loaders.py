@@ -12,11 +12,12 @@ import typing as tp
 import torch
 
 from . import synth
-from .conditioners import ConditionFuser, ConditioningProvider, PrecomputedTextConditioner
+from .conditioners import (ChromaStemConditioner, ConditionFuser, ConditioningProvider, PrecomputedTextConditioner,
+                           identity_stem_separator)
 from .encodec import EncodecModel
 from .lm import LMModel
 
-_SCALES = {'small': 'musicgen_small', 'medium': 'musicgen_medium', 'large': 'musicgen_large'}
+_SCALES = {'small': 'musicgen_small', 'medium': 'musicgen_medium', 'large': 'musicgen_large', 'melody': 'musicgen_melody'}
 
 
 def _cfg_from_yaml(text: str) -> dict:
@@ -70,15 +71,32 @@ def lm_cfg_from_xp(xp: dict) -> dict:
     if xp.get('codebooks_pattern', {}).get('modeling', 'delay') != 'delay':
         unsupported.append(f"codebooks_pattern.modeling={xp['codebooks_pattern'].get('modeling')}")
     fz = xp.get('fuser', {})
-    for how in ('sum', 'prepend', 'input_interpolate'):
+    for how in ('sum', 'input_interpolate'):
         if fz.get(how):
             unsupported.append(f'fuser.{how}={fz[how]}')
+    prepend = list(fz.get('prepend') or [])
+    if prepend and (prepend not in (['self_wav', 'description'], ['self_wav'])):
+        unsupported.append(f'fuser.prepend={prepend} (only the melody layouts [self_wav, description] / [self_wav])')
     if list(fz.get('cross', [])) not in (['description'], []):
         unsupported.append(f"fuser.cross={fz.get('cross')}")
     if fz.get('cross_attention_pos_emb', False):
         unsupported.append('fuser.cross_attention_pos_emb')
     if unsupported:
         raise NotImplementedError("this checkpoint's LM is outside what the decode kernels implement: " + ', '.join(unsupported))
+    chroma = None
+    if 'self_wav' in prepend:
+        sw = xp.get('conditioners', {}).get('self_wav') or {}
+        if sw.get('model') != 'chroma_stem':
+            raise NotImplementedError(f"self_wav conditioner '{sw.get('model')}' is not built (only chroma_stem)")
+        cs = sw['chroma_stem']
+        if cs.get('eval_wavs') is not None:
+            raise NotImplementedError("chroma_stem.eval_wavs (evaluation wavs from a dataset) is not built")
+        if cs.get('cache_path') is not None:
+            raise NotImplementedError("chroma_stem.cache_path (the chroma embedding cache) is not built")
+        chroma = dict(n_chroma=int(cs['n_chroma']), radix2_exp=int(cs['radix2_exp']), argmax=bool(cs.get('argmax', True)),
+                      match_len_on_eval=bool(cs.get('match_len_on_eval', True)),
+                      sample_rate=int(cs.get('sample_rate') or xp['sample_rate']),
+                      duration=float(xp['dataset']['segment_duration']))   # builders.py: duration = segment_duration
     cond_dim = None
     desc = xp.get('conditioners', {}).get('description')
     if desc is not None:
@@ -92,7 +110,19 @@ def lm_cfg_from_xp(xp: dict) -> dict:
                 max_period=float(tl.get('max_period', 10000.0)), positional_scale=float(tl.get('positional_scale', 1.0)),
                 positional_embedding=pe, cross_attention=bool(fz.get('cross')),
                 cfg_coef=xp['classifier_free_guidance']['inference_coef'], cond_dim=cond_dim,
-                two_step_cfg=tl.get('two_step_cfg', False))
+                two_step_cfg=tl.get('two_step_cfg', False), prepend=prepend, chroma=chroma)
+
+
+def _melody_parts(cfg: dict, text_encoder, stem_separator, device):
+    """Provider and fuser of a prepend (melody) model: description (when prepended) + chroma_stem self_wav."""
+    ch = cfg['chroma']
+    conds = {}
+    if 'description' in cfg['prepend']:
+        conds['description'] = PrecomputedTextConditioner(cfg['cond_dim'], cfg['dim'], text_encoder)
+    conds['self_wav'] = ChromaStemConditioner(cfg['dim'], ch['sample_rate'], ch['n_chroma'], ch['radix2_exp'], ch['duration'],
+                                              match_len_on_eval=ch['match_len_on_eval'], argmax=ch['argmax'],
+                                              stem_separator=stem_separator)
+    return ConditioningProvider(conds), ConditionFuser({'prepend': list(cfg['prepend']), 'cross': []})
 
 
 def load_compression_model(name: str, device='cuda', seed: int = 0) -> EncodecModel:
@@ -142,12 +172,20 @@ def hash_str(s: str) -> int:
     return h
 
 
-def load_lm_model(name: str, device='cuda', seed: int = 0, text_encoder=None) -> LMModel:
+def load_lm_model(name: str, device='cuda', seed: int = 0, text_encoder=None, stem_separator=None) -> LMModel:
+    """`stem_separator`: callable (wav [B,C,T], sample_rate) -> melody stems [B,1,T] standing in for Demucs in a melody
+    checkpoint; `synthetic/melody` uses `identity_stem_separator` (the mono mix is the melody) when none is given."""
     if name.startswith('synthetic/'):
         arch = name.split('/', 1)[1]
         cfg = synth.lm_config(_SCALES.get(arch, arch))
         sd = synth.synth_lm_state_dict(cfg, seed, device=device, dtype=torch.float16)
         enc = text_encoder or synthetic_text_encoder(cfg)
+        if cfg.get('n_chroma'):
+            cfg = dict(cfg, prepend=['self_wav', 'description'],
+                       chroma=dict(n_chroma=cfg['n_chroma'], radix2_exp=cfg['radix2_exp'], argmax=True, match_len_on_eval=False,
+                                   sample_rate=cfg['sample_rate'], duration=cfg['duration']))
+            provider, fuser = _melody_parts(cfg, enc, stem_separator or identity_stem_separator, device)
+            return LMModel(sd, cfg, provider, fuser, device)
         provider = ConditioningProvider({'description': PrecomputedTextConditioner(cfg['cond_dim'], cfg['dim'], enc)})
         return LMModel(sd, cfg, provider, ConditionFuser({'cross': ['description']}), device)
     if os.path.isfile(name):
@@ -155,6 +193,16 @@ def load_lm_model(name: str, device='cuda', seed: int = 0, text_encoder=None) ->
         xp = _cfg_from_yaml(pkg['xp.cfg']) if isinstance(pkg['xp.cfg'], str) else pkg['xp.cfg']
         cfg = lm_cfg_from_xp(xp)
         provider = None
+        if cfg['prepend']:
+            if stem_separator is None:
+                raise RuntimeError("this checkpoint is melody-conditioned: pass stem_separator=<callable (wav [B,C,T], "
+                                   "sample_rate) -> melody stems [B,1,T]> standing in for Demucs (htdemucs weights are not "
+                                   "available offline)")
+            if 'description' in cfg['prepend'] and text_encoder is None:
+                raise RuntimeError("this checkpoint is text-conditioned: pass text_encoder=<callable returning the frozen T5 "
+                                   f"hidden states [B,T,{cfg['cond_dim']}] and attention mask>")
+            provider, fuser = _melody_parts(cfg, text_encoder, stem_separator, device)
+            return LMModel(pkg['best_state'], cfg, provider, fuser, device)
         if cfg['cross_attention']:
             if text_encoder is None:
                 raise RuntimeError("this checkpoint is text-conditioned: pass text_encoder=<callable returning the frozen T5 "
@@ -174,18 +222,19 @@ def _wrap_from_xp(cm, lm_ckpt: str):
     return get_wrapped_compression_model(cm, xp.get('interleave_stereo_codebooks'), xp.get('compression_model_n_q'))
 
 
-def load_musicgen(name: str, device=None, seed: int = 0, text_encoder=None):
+def load_musicgen(name: str, device=None, seed: int = 0, text_encoder=None, stem_separator=None):
     """`text_encoder`: callable list[str] -> (hidden [B,T,cond_dim], mask [B,T]) standing in for the frozen T5 when loading
-    a real checkpoint directory (the reference instantiates T5 from the HF hub, conditioners.py:422-515)."""
+    a real checkpoint directory (the reference instantiates T5 from the HF hub, conditioners.py:422-515).
+    `stem_separator`: the Demucs stand-in a melody checkpoint needs (see load_lm_model)."""
     from .musicgen import MusicGen
     device = 'cuda' if device is None else device
     if name.startswith('synthetic/'):
-        lm = load_lm_model(name, device, seed, text_encoder)
+        lm = load_lm_model(name, device, seed, text_encoder, stem_separator)
         cm = load_compression_model('synthetic/encodec_32k', device, seed + 1)
         return MusicGen(name, cm, lm, max_duration=30)
     if os.path.isdir(name):
         lm_path = os.path.join(name, 'state_dict.bin')
-        lm = load_lm_model(lm_path, device, text_encoder=text_encoder)
+        lm = load_lm_model(lm_path, device, text_encoder=text_encoder, stem_separator=stem_separator)
         cm = _wrap_from_xp(load_compression_model(os.path.join(name, 'compression_state_dict.bin'), device), lm_path)
         return MusicGen(name, cm, lm, max_duration=30)
     raise FileNotFoundError(f"MusicGen '{name}': pass a local checkpoint directory or 'synthetic/<small|medium|large>'")

@@ -12,14 +12,15 @@ audiocraft/models/genmodel.py:28-267, musicgen.py:41-338, audiogen.py:23-93):
 * `generate_audio(tokens)` is the codec decode, without trimming the decoder's extra padding.
 
 Everything here is host glue; the two hot loops live behind `LMModel.generate` and `CompressionModel.decode`.
-Melody / style conditioning are conditioner front-ends outside the hot path (SURVEY.md section 8f.3) and raise.
+Melody conditioning (`generate_with_chroma`, musicgen.py:155-249) runs its chroma front-end on the host once per call and
+hands the LM a condition prefix; style conditioning is not built and raises.
 """
 import typing as tp
 
 import torch
 
 from .audio_utils import convert_audio
-from .conditioners import ConditioningAttributes
+from .conditioners import ConditioningAttributes, WavCondition
 from .encodec import CompressionModel
 from .lm import LMModel
 
@@ -125,14 +126,20 @@ class BaseGenModel:
         stride = int(fr * self.extend_stride)
         pieces: tp.List[Tokens] = [] if prompt_tokens is None else [prompt_tokens]
         have = 0 if prompt_tokens is None else prompt_tokens.shape[-1]
+        ref_attributes = attributes
         while done_before_window + have < n_total:
             window_s = min(self.duration - done_before_window / fr, self.max_duration)
+            attributes = self._window_attributes(ref_attributes, done_before_window / fr)
             window = self._lm_generate(prompt_tokens, attributes, int(window_s * fr), callback)
             pieces.append(window if prompt_tokens is None else window[:, :, prompt_tokens.shape[-1]:])
             prompt_tokens = window[:, :, stride:]
             have = prompt_tokens.shape[-1]
             done_before_window += stride
         return torch.cat(pieces, dim=-1)
+
+    def _window_attributes(self, attributes, time_offset: float):
+        """The conditions of the window starting `time_offset` seconds into a generation longer than max_duration."""
+        return attributes
 
 
 def _sampling_params(use_sampling, top_k, top_p, temperature, cfg_coef, two_step_cfg):
@@ -147,15 +154,23 @@ class MusicGen(BaseGenModel):
                  max_duration: tp.Optional[float] = None):
         super().__init__(name, compression_model, lm, max_duration)
         self.set_generation_params(duration=15)  # the reference's default duration
+        if self._has_melody:   # musicgen.py:90-92: at inference the chroma is matched to the training length, unmasked
+            self.lm.condition_provider.conditioners['self_wav'].match_len_on_eval = True
+            self.lm.condition_provider.conditioners['self_wav']._use_masking = False
+
+    @property
+    def _has_melody(self) -> bool:
+        cp = self.lm.condition_provider
+        return cp is not None and 'self_wav' in cp.conditioners
 
     @staticmethod
-    def get_pretrained(name: str = 'facebook/musicgen-medium', device=None, text_encoder=None):
+    def get_pretrained(name: str = 'facebook/musicgen-medium', device=None, text_encoder=None, stem_separator=None):
         """The reference pulls checkpoints from the HF hub (musicgen.py:56-94); offline this accepts a directory holding
         the reference's exported `state_dict.bin` + `compression_state_dict.bin` (then `text_encoder`, a callable returning
         the frozen T5's hidden states and mask, is required: T5 is outside the hot path and not available offline), or
         `synthetic/<small|medium|large>` for seeded random weights of the released architectures."""
         from .loaders import load_musicgen
-        return load_musicgen(name, device=device, text_encoder=text_encoder)
+        return load_musicgen(name, device=device, text_encoder=text_encoder, stem_separator=stem_separator)
 
     def set_generation_params(self, use_sampling: bool = True, top_k: int = 250, top_p: float = 0.0,
                               temperature: float = 1.0, duration: float = 30.0, cfg_coef: float = 3.0,
@@ -169,8 +184,76 @@ class MusicGen(BaseGenModel):
     def set_style_conditioner_params(self, *args, **kwargs):
         raise NotImplementedError("MusicGen-Style conditioning is not built on this path (SURVEY.md 8f.3)")
 
-    def generate_with_chroma(self, *args, **kwargs):
-        raise NotImplementedError("melody (chroma) conditioning is not built on this path (SURVEY.md 8f.3)")
+    def generate_with_chroma(self, descriptions: tp.List[tp.Optional[str]], melody_wavs, melody_sample_rate: int,
+                             progress: bool = False, return_tokens: bool = False):
+        """Generate conditioned on text and melody (musicgen.py:155-189).  melody_wavs: [B,C,T], [C,T] for one
+        description, or a list of [C,T] tensors / None (None: that item has a null melody)."""
+        if not self._has_melody:
+            raise NotImplementedError("this model has no melody ('self_wav') conditioner; use a MusicGen-melody model")
+        if isinstance(melody_wavs, torch.Tensor):
+            if melody_wavs.dim() == 2:
+                melody_wavs = melody_wavs[None]
+            if melody_wavs.dim() != 3:
+                raise ValueError("Melody wavs should have a shape [B, C, T].")
+            melody_wavs = list(melody_wavs)
+        else:
+            for melody in melody_wavs:
+                if melody is not None:
+                    assert melody.dim() == 2, "One melody in the list has the wrong number of dims."
+        melody_wavs = [convert_audio(wav, melody_sample_rate, self.sample_rate, self.audio_channels)
+                       if wav is not None else None for wav in melody_wavs]
+        attributes, prompt_tokens = self._prepare_tokens_and_attributes(descriptions, None, melody_wavs)
+        assert prompt_tokens is None
+        tokens = self._generate_tokens(attributes, prompt_tokens, progress)
+        audio = self.generate_audio(tokens)
+        return (audio, tokens) if return_tokens else audio
+
+    def _null_wav(self) -> WavCondition:
+        return WavCondition(torch.zeros((1, 1, 1), device=self.device), torch.tensor([0], device=self.device),
+                            sample_rate=[self.sample_rate], path=[None])
+
+    @torch.no_grad()
+    def _prepare_tokens_and_attributes(self, descriptions, prompt, melody_wavs=None):
+        """musicgen.py:191-249: on a melody model every item carries a `self_wav` condition, null without a melody."""
+        attributes, prompt_tokens = super()._prepare_tokens_and_attributes(descriptions, prompt)
+        if melody_wavs is None:
+            if self._has_melody:
+                for attr in attributes:
+                    attr.wav['self_wav'] = self._null_wav()
+        else:
+            if not self._has_melody:
+                raise RuntimeError("This model doesn't support melody conditioning. Use the `melody` model.")
+            assert len(melody_wavs) == len(descriptions), \
+                f"number of melody wavs must match number of descriptions! " \
+                f"got melody len={len(melody_wavs)}, and descriptions len={len(descriptions)}"
+            for attr, melody in zip(attributes, melody_wavs):
+                if melody is None:
+                    attr.wav['self_wav'] = self._null_wav()
+                else:
+                    attr.wav['self_wav'] = WavCondition(melody[None].to(device=self.device),
+                                                        torch.tensor([melody.shape[-1]], device=self.device),
+                                                        sample_rate=[self.sample_rate], path=[None])
+        return attributes, prompt_tokens
+
+    def _window_attributes(self, attributes, time_offset: float):
+        """musicgen.py:308-323: each window's melody is max_duration seconds of the original one from time_offset on,
+        wrapped around periodically (positions % length); null melodies stay null."""
+        if not self._has_melody:
+            return attributes
+        out = []
+        for attr in attributes:
+            ref = attr.wav.get('self_wav')
+            attr = ConditioningAttributes(text=dict(attr.text), wav=dict(attr.wav))
+            if ref is not None and int(ref.length.item()) != 0:
+                wav_length = int(ref.length.item())
+                initial_position = int(time_offset * self.sample_rate)
+                wav_target_length = int(self.max_duration * self.sample_rate)
+                positions = torch.arange(initial_position, initial_position + wav_target_length, device=self.device)
+                attr.wav['self_wav'] = WavCondition(ref.wav[..., positions % wav_length],
+                                                    torch.full_like(ref.length, wav_target_length),
+                                                    [self.sample_rate] * ref.wav.size(0), [None], [0.])
+            out.append(attr)
+        return out
 
 
 class AudioGen(BaseGenModel):

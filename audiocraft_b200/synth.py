@@ -183,6 +183,12 @@ LM_CONFIGS: tp.Dict[str, dict] = {
     # the released widths with only 2 layers: exercise the d = 1536 / 2048 GEMM tiling in tests without the full depth
     'lm_medium_2l': dict(dim=1536, num_heads=24, num_layers=2, card=2048, cond_dim=64),
     'lm_large_2l': dict(dim=2048, num_heads=32, num_layers=2, card=2048, cond_dim=64),
+    # MusicGen-melody (config/conditioner/chroma2music.yaml): no cross attention, the prefix [chroma ; T5-base description]
+    # is prepended; 12 chroma bins from a 2^14-sample STFT at 32 kHz, 30 s training segments
+    'musicgen_melody': dict(dim=1536, num_heads=24, num_layers=48, cross_attention=False, cond_dim=768, n_chroma=12,
+                            radix2_exp=14, duration=30.0, sample_rate=32000),
+    'lm_mini_melody': dict(dim=256, num_heads=4, num_layers=3, card=2048, cond_dim=96, cross_attention=False, n_chroma=12,
+                           radix2_exp=14, duration=1.0, sample_rate=32000),
 }
 _LM_COMMON = dict(hidden_scale=4, n_q=4, card=2048, delays=[0, 1, 2, 3], max_period=10000.0,
                   positional_scale=1.0, cross_attention=True, cfg_coef=3.0, cond_dim=768)
@@ -242,6 +248,11 @@ def synth_lm_state_dict(cfg: dict, seed: int = 0, device='cpu', dtype=torch.floa
     sd['condition_provider.conditioners.description.output_proj.weight'] = gauss((d, cd), cd)
     sd['condition_provider.conditioners.description.output_proj.bias'] = \
         (0.05 * torch.randn(d, generator=gen, device=device)).to(dtype)
+    if cfg.get('n_chroma'):   # drawn last: the text-only configurations keep their weights
+        nc = cfg['n_chroma']
+        sd['condition_provider.conditioners.self_wav.output_proj.weight'] = gauss((d, nc), nc)
+        sd['condition_provider.conditioners.self_wav.output_proj.bias'] = \
+            (0.05 * torch.randn(d, generator=gen, device=device)).to(dtype)
     return sd
 
 

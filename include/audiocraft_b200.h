@@ -214,6 +214,15 @@ int acb_lm_destroy(acb_lm_t* lm);
 int acb_lm_begin(acb_lm_t* lm, const float* cross, int batch, int rows, int text_len, int seq_len,
                  const acb_lm_sampling* sampling, void* stream);
 
+/* acb_lm_begin for a model whose fuser prepends conditions to the token embeddings (`prepend`, MusicGen-melody;
+ * conditioners.py:1703-1763).  prefix is fp32 [rows][prefix_len][d], one prefix per row (cond and null rows differ); each value
+ * is rounded to fp16 on the device, as the reference's autocast output_proj rounds it.  The prefix fills KV-cache positions
+ * [0, prefix_len) once, in prefill passes (every layer, cross attention included when the model has it); afterwards sequence
+ * column t runs at cache position prefix_len + t, for decode steps and acb_lm_prefill alike, while acb_lm_prefill still takes
+ * sequence columns.  Needs prefix_len + seq_len <= max_seq and rows <= ACB_LM_PREFILL_ROWS.  prefix_len == 0 is acb_lm_begin. */
+int acb_lm_begin_prefix(acb_lm_t* lm, const float* cross, const float* prefix, int prefix_len, int batch, int rows,
+                        int text_len, int seq_len, const acb_lm_sampling* sampling, void* stream);
+
 /* n_steps iterations of the hot loop of LMModel.generate (lm.py:540-565): for the current offset = pos+1,
  * feed seq[:,:,pos], run the transformer (LMModel.forward lm.py:221-268), CFG-mix, sample
  * (_sample_next_token lm.py:393-418), apply the pattern mask and write seq[:,:,offset] where it is still -1.

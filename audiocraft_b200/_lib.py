@@ -16,6 +16,7 @@ CONV_T6_AUTO = 4    # host-side selector only: acb_conv1d_t6 where it is faster 
 ACB_LM_MAX_SPLIT = 8
 ACB_LM_PART_SLOTS = 16
 ACB_LM_PREFILL_ROWS = 64
+ACB_LM_MAX_ROWS = 256
 
 
 class LMConfig(C.Structure):

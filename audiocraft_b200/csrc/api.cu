@@ -13,7 +13,7 @@ void acb_set_error(const char* fmt, ...) {
 }
 
 extern "C" const char* acb_last_error(void) { return g_err; }
-extern "C" int acb_version(void) { return 103; }
+extern "C" int acb_version(void) { return 104; }
 
 extern "C" int acb_device_sm_count(int device) {
     int sms = 0;

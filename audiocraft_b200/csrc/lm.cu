@@ -18,6 +18,9 @@
 //   * self attention: one CTA per (query row, head) streaming K and V through a cp.async ring (lm_attn2_kernel), for the decode
 //     step and for prompt prefill alike.
 #include "common.cuh"
+#include "wgmma.cuh"
+#include <cooperative_groups.h>
+#include <cudaTypedefs.h>   // CUtensorMap, PFN_cuTensorMapEncodeTiled: types only, the entry point is looked up at run time
 #include <math.h>
 #include <new>
 #include <stdio.h>
@@ -327,6 +330,139 @@ __global__ void __launch_bounds__(128) lm_gemm_kernel(GemmParams p) {
             cache[(((size_t)r * p.H + h) * p.cache_len + tc) * 64 + dd] = __float2half_rn(v);
         }
     }
+}
+
+// ------------------------------------------------------------------------------------------------ wide GEMM (65-256 rows)
+// The decode GEMM for rows > 64, where lm_gemm_kernel's mma.sync tile (8 * NT <= 64 rows in registers) cannot grow.  Swap-AB
+// on wgmma: the output tile is 64 features x all NPAD rows, D = W[64 x k] . X[NPAD x k]^T with the weight slab as the A
+// operand and the activations as the B operand, both K-major in the 128-byte swizzle that tiled TMA writes.  One CTA covers
+// every row of its features, so each weight byte is read from HBM once per step whatever the batch.  The weights stay in the
+// reference's [N][K] layout: one 2-D tensor map per stacked matrix ([L * N][K]), the layer is a row offset.
+// NPAD is 128 (rows 65-128) or 256 (rows 129-256): the padded rows cost MMA issue slots and L2 reads of zero-filled
+// activations, not HBM bytes, and two widths keep the instance count (and the build) small.
+// K is cut into 64-element chunks streamed through an mbarrier ring.  The K split (grid.y) depends only on (N, K, SM count):
+// EPI_PARTIAL writes one `part` slot per slice, the other epilogues split K over a thread-block cluster of grid.y CTAs and
+// add the slices' tiles in rank order through distributed shared memory.  An item's sums are therefore the same in every
+// batch of this range.
+constexpr int WIDE_KC = 64;   // K elements per chunk: one 128-byte swizzle row
+template <int NPAD>
+struct WideCfg {
+    static constexpr int W_BYTES = 64 * WIDE_KC * 2;
+    static constexpr int STAGE = W_BYTES + NPAD * WIDE_KC * 2;
+    static constexpr int STAGES = NPAD <= 128 ? 6 : 5;
+    static constexpr int LDS = 68;   // pitch (floats) of the [NPAD][64] fp32 staging tile: conflict-free fragment stores
+    static constexpr int SMEM = STAGES * STAGE + 1024 + 64;   // ring (1024-aligned) + barriers
+    static_assert(NPAD * LDS * 4 <= STAGES * STAGE, "the staging tile reuses the ring");
+};
+
+__device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
+    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
+                 ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(smem_u32(bar)) : "memory");
+}
+
+// EPI is EPI_PARTIAL, EPI_QKV, EPI_QKV_ROPE, EPI_GELU or EPI_F32.  Prefill passes above 64 rows carry one position per row,
+// so their QKV epilogue is the decode one (token 0 of the pass at position pos).
+template <int NPAD, int EPI>
+__global__ void __launch_bounds__(128, 1) lm_gemm_wide_kernel(const __grid_constant__ CUtensorMap wmap,
+                                                              const __grid_constant__ CUtensorMap xmap, GemmParams p, int w_row0) {
+    using Cfg = WideCfg<NPAD>;
+    constexpr bool ROPE = EPI == EPI_QKV_ROPE, QKV = EPI == EPI_QKV || ROPE;
+    extern __shared__ unsigned char wsm_raw[];
+    unsigned char* wsm = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(wsm_raw) + 1023) & ~(uintptr_t)1023);
+    uint64_t* full = reinterpret_cast<uint64_t*>(wsm + Cfg::STAGES * Cfg::STAGE);
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int f0 = blockIdx.x * 64, k0 = blockIdx.y * p.kslice;
+    const int nch = (min(p.kslice, p.K - k0) + WIDE_KC - 1) / WIDE_KC;   // K past the end is zero-filled by TMA
+
+    if (tid == 0) {
+#pragma unroll
+        for (int s = 0; s < Cfg::STAGES; ++s) mbar_init(&full[s], 1);
+    }
+    __syncthreads();
+    auto load = [&](int c) {
+        const int s = c % Cfg::STAGES;
+        unsigned char* st = wsm + s * Cfg::STAGE;
+        mbar_expect_tx(&full[s], (uint32_t)Cfg::STAGE);
+        tma_load_2d(st, &wmap, k0 + c * WIDE_KC, w_row0 + f0, &full[s]);
+        tma_load_2d(st + Cfg::W_BYTES, &xmap, k0 + c * WIDE_KC, 0, &full[s]);   // rows >= p.rows are zero-filled
+    };
+    if (tid == 0)
+        for (int c = 0; c < min(nch, Cfg::STAGES); ++c) load(c);
+    int cache_pos = 0;
+    if (QKV) cache_pos = p.pos[0];
+
+    float acc[NPAD / 2];
+#pragma unroll
+    for (int i = 0; i < NPAD / 2; ++i) acc[i] = 0.f;
+    for (int c = 0; c < nch; ++c) {
+        const int s = c % Cfg::STAGES;
+        mbar_wait(&full[s], (uint32_t)(c / Cfg::STAGES) & 1u);
+        const uint32_t a = smem_u32(wsm + s * Cfg::STAGE), b = a + Cfg::W_BYTES;
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < WIDE_KC / 16; ++kk)   // a 16-element K step advances the start address by 32 bytes
+            wgmma_f16<NPAD>(acc, wgmma_desc_sw128(a + 32 * kk), wgmma_desc_sw128(b + 32 * kk), 1u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(acc);
+        if (c + Cfg::STAGES < nch) {   // every warp is done with stage s: refill it
+            __syncthreads();
+            if (tid == 0) load(c + Cfg::STAGES);
+        }
+    }
+    __syncthreads();   // the ring is idle: it becomes the staging tile [row][feature]
+    float* tile = reinterpret_cast<float*>(wsm);
+#pragma unroll
+    for (int j = 0; j < NPAD / 8; ++j)
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+            tile[(8 * j + 2 * (lane & 3) + (i & 1)) * Cfg::LDS + 16 * warp + (lane >> 2) + 8 * (i >> 1)] = acc[4 * j + i];
+
+    namespace cg = cooperative_groups;
+    const int cs = EPI == EPI_PARTIAL ? 1 : (int)gridDim.y;   // CTAs of the cluster that share this tile's K
+    const float* src[4] = {tile, tile, tile, tile};
+    int rank = 0;
+    if (cs > 1) {
+        cg::cluster_group cluster = cg::this_cluster();
+        cluster.sync();
+        rank = (int)cluster.block_rank();
+#pragma unroll
+        for (int r = 0; r < 4; ++r)
+            if (r < cs) src[r] = cluster.map_shared_rank(tile, r);
+    } else {
+        __syncthreads();
+    }
+    const int per = (p.rows + cs - 1) / cs, r0 = rank * per, r1 = min(p.rows, r0 + per);   // this CTA's output rows
+    for (int idx = tid; idx < (r1 - r0) * 64; idx += 128) {
+        const int row = r0 + (idx >> 6), feat = idx & 63, n = f0 + feat;
+        float v = 0.f;
+#pragma unroll
+        for (int r = 0; r < 4; ++r)   // fixed order: slice 0 first
+            if (r < cs) v += src[r][row * Cfg::LDS + feat];
+        if (EPI == EPI_PARTIAL) {
+            p.out_f32[blockIdx.y * p.split_stride + (size_t)row * p.ld_out + n] = v;
+        } else if (EPI == EPI_F32) {
+            p.out_f32[(size_t)row * p.ld_out + n] = v;
+        } else if (EPI == EPI_GELU) {
+            p.out_f16[(size_t)row * p.ld_out + n] = __float2half_rn(gelu_erf(half_round(v)));
+        } else if (QKV) {
+            const int which = n >= 2 * p.d ? 2 : (n >= p.d ? 1 : 0), nn = n - which * p.d;
+            if (ROPE && which < 2) {   // the pair partner n ^ 1 is in the same 64-feature tile
+                float other = 0.f;
+#pragma unroll
+                for (int r = 0; r < 4; ++r)
+                    if (r < cs) other += src[r][row * Cfg::LDS + (feat ^ 1)];
+                v = rope_rotate(p.rope_freq, p.pos_scale, half_round(v), half_round(other), nn & 63, cache_pos);
+            }
+            if (which == 0) {
+                p.q32[(size_t)row * p.d + nn] = v;
+            } else {
+                __half* cache = which == 2 ? p.vc : p.kc;
+                cache[(((size_t)row * p.H + (nn >> 6)) * p.cache_len + cache_pos) * 64 + (nn & 63)] = __float2half_rn(v);
+            }
+        }
+    }
+    if (cs > 1) cg::this_cluster().sync();   // the other CTAs read this CTA's tile until here
 }
 
 // ------------------------------------------------------------------------------------------------ attention (1 query)
@@ -747,7 +883,12 @@ struct acb_lm {
     const float* prefix = nullptr; // [rows][prefix_len][d] fp32, set only while acb_lm_begin_prefix enqueues the prefix passes
     int launches = 0;
     bool has_cross = false;
+    // wide GEMM (max_rows > 64): one map per stacked weight matrix [L * N][K] (encoded by acb_lm_create) and per activation
+    // buffer [rows][K] of the current generation (encoded by acb_lm_begin_prefix)
+    CUtensorMap wmap[7];
+    CUtensorMap xmap_h16, xmap_a16, xmap_f16;
 };
+enum { WM_QKV = 0, WM_O, WM_CQ, WM_CO, WM_FF1, WM_FF2, WM_HEADS };
 
 static int nt_for_rows(int rows) { return rows <= 8 ? 1 : (rows <= 16 ? 2 : (rows <= 32 ? 4 : 8)); }
 
@@ -828,6 +969,91 @@ static int pick_split(int N, int K, int sms, bool allow_split, int* kslice) {
     return ns;
 }
 
+// ---- wide GEMM (rows > 64)
+static int wide_npad(int rows) { return rows <= 128 ? 128 : 256; }
+
+// K slices of the wide GEMM (grid.y) from (N, K, SM count) alone, never from rows: the count whose CTAs (one per SM: the ring
+// takes 144-200 KB) fill the largest share of their waves, up to ACB_LM_MAX_SPLIT `part` slots when the consumer reduces
+// partial sums (allow_split), else a cluster of 1, 2 or 4 CTAs.  Sets *kslice (a multiple of WIDE_KC).
+static int pick_split_wide(int N, int K, int sms, bool allow_split, int* kslice) {
+    const int nch = acb_ceil_div(K, WIDE_KC), tiles = N / 64;
+    int best = 1;
+    double best_fill = 0.0;
+    for (int ns = 1; ns <= (allow_split ? ACB_LM_MAX_SPLIT : 4) && ns <= nch; ns = allow_split ? ns + 1 : 2 * ns) {
+        const int ctas = tiles * ns;
+        const double fill = (double)ctas / ((double)sms * acb_ceil_div(ctas, sms));
+        if (fill > best_fill + 1e-9) { best = ns; best_fill = fill; }
+    }
+    const int cps = acb_ceil_div(nch, best);   // chunks per slice; no empty slices
+    *kslice = cps * WIDE_KC;
+    return acb_ceil_div(nch, cps);
+}
+
+static PFN_cuTensorMapEncodeTiled_v12000 tensor_map_encoder() {
+    static PFN_cuTensorMapEncodeTiled_v12000 fn = nullptr;
+    if (!fn) {
+        void* f = nullptr;
+        cudaDriverEntryPointQueryResult q;
+        if (cudaGetDriverEntryPointByVersion("cuTensorMapEncodeTiled", &f, 12000, cudaEnableDefault, &q) == cudaSuccess &&
+            q == cudaDriverEntryPointSuccess)
+            fn = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(f);
+    }
+    return fn;
+}
+
+// Tensor map of a row-major fp16 [outer][inner] matrix read in boxes of box_outer rows x WIDE_KC elements, 128-byte swizzled;
+// boxes past either edge are zero-filled.
+static int encode_map(CUtensorMap* m, const void* base, int inner, int outer, int box_outer) {
+    PFN_cuTensorMapEncodeTiled_v12000 fn = tensor_map_encoder();
+    ACB_REQUIRE(fn, "lm: cuTensorMapEncodeTiled is not available from the CUDA driver");
+    cuuint64_t dims[2] = {(cuuint64_t)inner, (cuuint64_t)outer}, strides[1] = {(cuuint64_t)inner * 2};
+    cuuint32_t box[2] = {(cuuint32_t)WIDE_KC, (cuuint32_t)box_outer}, es[2] = {1, 1};
+    const CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), dims, strides, box, es,
+                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    ACB_REQUIRE(r == CUDA_SUCCESS, "lm: cuTensorMapEncodeTiled failed (%d) for a [%d][%d] fp16 matrix", (int)r, outer, inner);
+    return ACB_OK;
+}
+
+// grid (N / 64, ny); the non-PARTIAL epilogues run ny as one cluster that reduces the K slices
+template <int EPI>
+static int launch_wide(const CUtensorMap& wm, const CUtensorMap& xm, int w_row0, const GemmParams& p, int ny, cudaStream_t s) {
+    ACB_REQUIRE(p.N % 64 == 0 && p.rows <= 256, "lm_gemm_wide: N=%d rows=%d", p.N, p.rows);
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(p.N / 64, ny);
+    cfg.blockDim = dim3(128);
+    cfg.stream = s;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeClusterDimension;
+    at[0].val.clusterDim.x = 1;
+    at[0].val.clusterDim.y = EPI == EPI_PARTIAL ? 1 : ny;
+    at[0].val.clusterDim.z = 1;
+    cfg.attrs = at;
+    cfg.numAttrs = 1;
+    cudaError_t e;
+    if (wide_npad(p.rows) == 128) {
+        cfg.dynamicSmemBytes = WideCfg<128>::SMEM;
+        e = cudaLaunchKernelEx(&cfg, lm_gemm_wide_kernel<128, EPI>, wm, xm, p, w_row0);
+    } else {
+        cfg.dynamicSmemBytes = WideCfg<256>::SMEM;
+        e = cudaLaunchKernelEx(&cfg, lm_gemm_wide_kernel<256, EPI>, wm, xm, p, w_row0);
+    }
+    ACB_CHECK_CUDA(e);
+    return ACB_OK;
+}
+
+template <int NPAD, int EPI>
+static cudaError_t wide_attr_one() {
+    cudaError_t e = cudaFuncSetAttribute(lm_gemm_wide_kernel<NPAD, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, WideCfg<NPAD>::SMEM);
+    if (e != cudaSuccess) return e;
+    return cudaFuncSetAttribute(lm_gemm_wide_kernel<NPAD, EPI>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+}
+template <int EPI>
+static cudaError_t wide_attr_all() {
+    cudaError_t e = wide_attr_one<128, EPI>();
+    return e != cudaSuccess ? e : wide_attr_one<256, EPI>();
+}
+
 static GemmParams base_gemm(const void* W, const void* X, int N, int K, int rows, int kslice) {
     GemmParams p{};
     p.W = (const __half*)W;
@@ -867,7 +1093,9 @@ static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_la
     ACB_REQUIRE(!pf_prefix || (pf && lm->prefix), "enqueue_step: a prefix pass needs the prefix of acb_lm_begin_prefix");
     const int rows_real = lm->rows, rows = pf ? rows_real * pf_tokens : rows_real;
     const int d = c.dim, ffn = c.ffn_dim, L = c.num_layers, H = c.num_heads, nt = nt_for_rows(rows);
-    const size_t part_stride = (size_t)(pf ? 8 * nt : lm->rows_pad) * d;
+    // rows > 64 (then rows_real > 64 and a prefill pass holds one position per row): every GEMM but EPI_CROSSKV on the wide kernel
+    const bool wide = rows > 64;
+    const size_t part_stride = (size_t)(pf && !wide ? 8 * nt : lm->rows_pad) * d;
     const size_t kv_layer = (size_t)c.max_rows * H * c.max_seq * 64;
     const size_t ckv_layer = (size_t)c.max_rows * H * c.max_text * 64;
     const float scale = 1.0f / sqrtf(64.f);
@@ -895,11 +1123,12 @@ static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_la
         DBG("lm_ln_kernel", layer);
         return ACB_OK;
     };
-    auto partial_gemm = [&](const __half* W, const void* X, int N, int K, int layer) -> int {
-        const int ns = pick_split(N, K, lm->sms, true, &ks);
+    auto partial_gemm = [&](const __half* W, const void* X, int N, int K, int layer, int wm, const CUtensorMap& xm) -> int {
+        const int ns = wide ? pick_split_wide(N, K, lm->sms, true, &ks) : pick_split(N, K, lm->sms, true, &ks);
         GemmParams p = base_gemm(W, X, N, K, rows, ks);
         p.out_f32 = B.part; p.ld_out = N; p.split_stride = part_stride;
-        ACB_TRY(launch_gemm<EPI_PARTIAL>(nt, p, ns, s, pick_ft2(N, K, ns, ks, nt, lm->sms)));
+        if (wide) ACB_TRY(launch_wide<EPI_PARTIAL>(lm->wmap[wm], xm, layer * N, p, ns, s));
+        else ACB_TRY(launch_gemm<EPI_PARTIAL>(nt, p, ns, s, pick_ft2(N, K, ns, ks, nt, lm->sms)));
         ++nl;
         DBG("gemm_EPI_PARTIAL", layer);
         pending = ns;
@@ -910,14 +1139,16 @@ static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_la
         // --- self attention
         ACB_TRY(ln_launch(ln, ln + d, l));
         {
-            pick_split(3 * d, d, lm->sms, false, &ks);
+            const int ns = wide ? pick_split_wide(3 * d, d, lm->sms, false, &ks) : pick_split(3 * d, d, lm->sms, false, &ks);
             GemmParams p = base_gemm((const __half*)lm->w.w_qkv + (size_t)l * 3 * d * d, B.h16, 3 * d, d, rows, ks);
             p.q32 = B.q32; p.kc = (__half*)B.k_cache + l * kv_layer; p.vc = (__half*)B.v_cache + l * kv_layer;
             p.d = d; p.H = H; p.cache_len = c.max_seq; p.pos = B.pos; p.rows_real = rows_real;
             p.rope_freq = lm->w.rope_freq; p.pos_scale = c.pos_scale;
             const bool rope = c.positional_embedding != 0;
             const int ft2 = pf ? 1 : pick_ft2(3 * d, d, 1, ks, nt, lm->sms);
-            if (pf) ACB_TRY(rope ? launch_gemm<EPI_QKV_PF_ROPE>(nt, p, 1, s, ft2) : launch_gemm<EPI_QKV_PF>(nt, p, 1, s, ft2));
+            if (wide) ACB_TRY(rope ? launch_wide<EPI_QKV_ROPE>(lm->wmap[WM_QKV], lm->xmap_h16, l * 3 * d, p, ns, s)
+                                   : launch_wide<EPI_QKV>(lm->wmap[WM_QKV], lm->xmap_h16, l * 3 * d, p, ns, s));
+            else if (pf) ACB_TRY(rope ? launch_gemm<EPI_QKV_PF_ROPE>(nt, p, 1, s, ft2) : launch_gemm<EPI_QKV_PF>(nt, p, 1, s, ft2));
             else ACB_TRY(rope ? launch_gemm<EPI_QKV_ROPE>(nt, p, 1, s, ft2) : launch_gemm<EPI_QKV>(nt, p, 1, s, ft2));
             ++nl;
             DBG("gemm_EPI_QKV", l);
@@ -931,11 +1162,11 @@ static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_la
             ++nl;
             DBG("lm_attn2_kernel", l);
         }
-        ACB_TRY(partial_gemm((const __half*)lm->w.w_o + (size_t)l * d * d, B.a16, d, d, l));
+        ACB_TRY(partial_gemm((const __half*)lm->w.w_o + (size_t)l * d * d, B.a16, d, d, l, WM_O, lm->xmap_a16));
         // --- cross attention
         if (lm->has_cross) {
             ACB_TRY(ln_launch(ln + 2 * d, ln + 3 * d, l));
-            ACB_TRY(partial_gemm((const __half*)lm->w.w_cq + (size_t)l * d * d, B.h16, d, d, l));
+            ACB_TRY(partial_gemm((const __half*)lm->w.w_cq + (size_t)l * d * d, B.h16, d, d, l, WM_CQ, lm->xmap_h16));
             const int nsq = pending;
             pending = 0;   // these partials are the cross-attention queries, not a residual update
             if (!gemms_only) {
@@ -948,18 +1179,20 @@ static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_la
                 ++nl;
                 DBG("lm_cross_attn_kernel", l);
             }
-            ACB_TRY(partial_gemm((const __half*)lm->w.w_co + (size_t)l * d * d, B.a16, d, d, l));
+            ACB_TRY(partial_gemm((const __half*)lm->w.w_co + (size_t)l * d * d, B.a16, d, d, l, WM_CO, lm->xmap_a16));
         }
         // --- feed forward
         ACB_TRY(ln_launch(ln + 4 * d, ln + 5 * d, l));
         {
-            pick_split(ffn, d, lm->sms, false, &ks);
+            const int ns = wide ? pick_split_wide(ffn, d, lm->sms, false, &ks) : pick_split(ffn, d, lm->sms, false, &ks);
             GemmParams p = base_gemm((const __half*)lm->w.w_ff1 + (size_t)l * ffn * d, B.h16, ffn, d, rows, ks);
             p.out_f16 = (__half*)B.f16; p.ld_out = ffn;
-            ACB_TRY(launch_gemm<EPI_GELU>(nt, p, 1, s, pick_ft2(ffn, d, 1, ks, nt, lm->sms))); ++nl;
+            if (wide) ACB_TRY(launch_wide<EPI_GELU>(lm->wmap[WM_FF1], lm->xmap_h16, l * ffn, p, ns, s));
+            else ACB_TRY(launch_gemm<EPI_GELU>(nt, p, 1, s, pick_ft2(ffn, d, 1, ks, nt, lm->sms)));
+            ++nl;
             DBG("gemm_EPI_GELU", l);
         }
-        ACB_TRY(partial_gemm((const __half*)lm->w.w_ff2 + (size_t)l * d * ffn, B.f16, d, ffn, l));
+        ACB_TRY(partial_gemm((const __half*)lm->w.w_ff2 + (size_t)l * d * ffn, B.f16, d, ffn, l, WM_FF2, lm->xmap_f16));
     }
     if (pf) {   // no output norm / heads / sampler: the pass only fills the KV cache
         if (n_launch) *n_launch = nl;
@@ -968,10 +1201,12 @@ static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_la
     ACB_TRY(ln_launch(lm->w.out_norm, lm->w.out_norm + d, -1));
     {
         const int N = c.n_q * c.card;
-        pick_split(N, d, lm->sms, false, &ks);
+        const int ns = wide ? pick_split_wide(N, d, lm->sms, false, &ks) : pick_split(N, d, lm->sms, false, &ks);
         GemmParams p = base_gemm(lm->w.heads, B.h16, N, d, rows, ks);
         p.out_f32 = B.logits; p.ld_out = N;
-        ACB_TRY(launch_gemm<EPI_F32>(nt, p, 1, s, pick_ft2(N, d, 1, ks, nt, lm->sms))); ++nl;
+        if (wide) ACB_TRY(launch_wide<EPI_F32>(lm->wmap[WM_HEADS], lm->xmap_h16, 0, p, ns, s));
+        else ACB_TRY(launch_gemm<EPI_F32>(nt, p, 1, s, pick_ft2(N, d, 1, ks, nt, lm->sms)));
+        ++nl;
         DBG("gemm_EPI_F32", -1);
     }
     if (!gemms_only) {
@@ -998,7 +1233,8 @@ extern "C" int acb_lm_create(const acb_lm_config* cfg, const acb_lm_weights* w, 
     ACB_REQUIRE(cfg->dim <= 4 * LN_THREADS, "acb_lm_create: dim %d too large for the LayerNorm kernel", cfg->dim);
     ACB_REQUIRE(cfg->ffn_dim % 32 == 0 && cfg->card % 16 == 0 && cfg->n_q >= 1 && cfg->n_q <= 16, "acb_lm_create: bad ffn/card/n_q");
     ACB_REQUIRE(cfg->card <= 4096, "acb_lm_create: card %d > 4096 not built", cfg->card);
-    ACB_REQUIRE(cfg->max_rows >= 1 && cfg->max_rows <= 64, "acb_lm_create: max_rows %d not in [1,64]", cfg->max_rows);
+    ACB_REQUIRE(cfg->max_rows >= 1 && cfg->max_rows <= ACB_LM_MAX_ROWS, "acb_lm_create: max_rows %d not in [1,%d]", cfg->max_rows,
+                ACB_LM_MAX_ROWS);
     ACB_REQUIRE(cfg->max_seq >= 2 && cfg->max_seq <= 12000, "acb_lm_create: max_seq %d out of range", cfg->max_seq);
     ACB_REQUIRE(cfg->dim <= 2048, "acb_lm_create: dim %d > 2048: the GEMM stages a 16 x dim weight slab per CTA", cfg->dim);
     ACB_REQUIRE(cfg->positional_embedding >= 0 && cfg->positional_embedding <= 2, "acb_lm_create: positional_embedding %d not in [0,2]",
@@ -1032,11 +1268,33 @@ extern "C" int acb_lm_create(const acb_lm_config* cfg, const acb_lm_weights* w, 
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_embed_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_embed_prefix_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_sample_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+    if (cfg->max_rows > 64) {
+        if (ea == cudaSuccess) ea = wide_attr_all<EPI_PARTIAL>();
+        if (ea == cudaSuccess) ea = wide_attr_all<EPI_QKV>();
+        if (ea == cudaSuccess) ea = wide_attr_all<EPI_QKV_ROPE>();
+        if (ea == cudaSuccess) ea = wide_attr_all<EPI_GELU>();
+        if (ea == cudaSuccess) ea = wide_attr_all<EPI_F32>();
+    }
     if (ea != cudaSuccess) {
         acb_set_error("acb_lm_create: cudaFuncSetAttribute: %s", cudaGetErrorString(ea));
         cudaStreamDestroy(lm->capture_stream);
         delete lm;
         return ACB_ERR_CUDA;
+    }
+    if (cfg->max_rows > 64) {   // the wide GEMM's weight maps: each stacked matrix as [L * N][K], 64-row boxes
+        const int d = cfg->dim, ffn = cfg->ffn_dim, L = cfg->num_layers;
+        int rc = encode_map(&lm->wmap[WM_QKV], w->w_qkv, d, L * 3 * d, 64);
+        if (rc == ACB_OK) rc = encode_map(&lm->wmap[WM_O], w->w_o, d, L * d, 64);
+        if (rc == ACB_OK && cfg->cross_attention) rc = encode_map(&lm->wmap[WM_CQ], w->w_cq, d, L * d, 64);
+        if (rc == ACB_OK && cfg->cross_attention) rc = encode_map(&lm->wmap[WM_CO], w->w_co, d, L * d, 64);
+        if (rc == ACB_OK) rc = encode_map(&lm->wmap[WM_FF1], w->w_ff1, d, L * ffn, 64);
+        if (rc == ACB_OK) rc = encode_map(&lm->wmap[WM_FF2], w->w_ff2, ffn, L * d, 64);
+        if (rc == ACB_OK) rc = encode_map(&lm->wmap[WM_HEADS], w->heads, d, cfg->n_q * cfg->card, 64);
+        if (rc != ACB_OK) {
+            cudaStreamDestroy(lm->capture_stream);
+            delete lm;
+            return rc;
+        }
     }
     *out = lm;
     return ACB_OK;
@@ -1057,14 +1315,14 @@ extern "C" int acb_lm_destroy(acb_lm_t* lm) {
 
 __global__ void lm_set_pos_kernel(int* pos, int value) { pos[0] = value; }
 
-// Prefill passes over cache positions [pos0, pos0 + n) of every row, ACB_LM_PREFILL_ROWS / rows positions per pass: token
-// columns pos - prefix_len of buffers.seq, or (prefix) the condition-prefix vectors.  Leaves pos = pos0 + n on the device and the
-// padded decode rows [rows, rows_pad) of the activation buffers zero.
+// Prefill passes over cache positions [pos0, pos0 + n) of every row, ACB_LM_PREFILL_ROWS / rows positions per pass (one above
+// 64 rows: the wide GEMM already shares each weight byte among all rows): token columns pos - prefix_len of buffers.seq, or
+// (prefix) the condition-prefix vectors.  Leaves pos = pos0 + n on the device and the padded decode rows [rows, rows_pad) of
+// the activation buffers zero.
 static int prefill_passes(acb_lm* lm, cudaStream_t s, int pos0, int n, bool prefix) {
     const acb_lm_config& c = lm->cfg;
     const int d = c.dim;
-    int per = ACB_LM_PREFILL_ROWS / lm->rows;
-    ACB_REQUIRE(per >= 1, "acb_lm_prefill: rows %d > %d", lm->rows, ACB_LM_PREFILL_ROWS);
+    int per = lm->rows > ACB_LM_PREFILL_ROWS ? 1 : ACB_LM_PREFILL_ROWS / lm->rows;
     // ACB_LM_PREFILL_PER=n: at most n positions per pass (n = 1: one position per pass, the reference order for tests)
     if (const char* e = getenv("ACB_LM_PREFILL_PER")) { const int cap = atoi(e); if (cap >= 1 && cap < per) per = cap; }
     int done = 0;
@@ -1106,16 +1364,26 @@ extern "C" int acb_lm_begin_prefix(acb_lm_t* lm, const float* cross, const float
     ACB_REQUIRE(prefix_len >= 0 && (prefix_len == 0 || prefix), "acb_lm_begin: prefix_len %d without a prefix tensor", prefix_len);
     ACB_REQUIRE(seq_len >= 2 && prefix_len + seq_len <= c.max_seq, "acb_lm_begin: prefix %d + seq_len %d > max_seq %d", prefix_len,
                 seq_len, c.max_seq);
-    ACB_REQUIRE(prefix_len == 0 || rows <= ACB_LM_PREFILL_ROWS, "acb_lm_begin: a condition prefix needs rows <= %d", ACB_LM_PREFILL_ROWS);
+    if (rows > 64 && (c.ffn_dim % 64 != 0 || (c.n_q * c.card) % 64 != 0)) {
+        acb_set_error("acb_lm_begin: rows %d > 64 run the wide GEMM, which needs ffn_dim (%d) and n_q * card (%d) to be multiples of 64",
+                      rows, c.ffn_dim, c.n_q * c.card);
+        return ACB_ERR_UNSUPPORTED;
+    }
     ACB_REQUIRE(!c.cross_attention || cross, "acb_lm_begin: the model has cross attention, a condition tensor is required"
                 " (the reference asserts the same, transformer.py:553-556)");
     ACB_REQUIRE(!cross || (text_len >= 1 && text_len <= c.max_text), "acb_lm_begin: text_len %d out of range", text_len);
     cudaStream_t s = (cudaStream_t)stream;
-    lm->batch = batch; lm->rows = rows; lm->rows_pad = 8 * nt_for_rows(rows); lm->text_len = text_len; lm->seq_len = seq_len;
+    const int d = c.dim, H = c.num_heads;
+    if (rows > 64) {   // the wide GEMM's activation maps: rows past `rows` of a box are zero-filled
+        const int npad = wide_npad(rows);
+        ACB_TRY(encode_map(&lm->xmap_h16, lm->buf.h16, d, rows, npad));
+        ACB_TRY(encode_map(&lm->xmap_a16, lm->buf.a16, d, rows, npad));
+        ACB_TRY(encode_map(&lm->xmap_f16, lm->buf.f16, c.ffn_dim, rows, npad));
+    }
+    lm->batch = batch; lm->rows = rows; lm->rows_pad = rows > 64 ? wide_npad(rows) : 8 * nt_for_rows(rows); lm->text_len = text_len; lm->seq_len = seq_len;
     lm->prefix_len = prefix_len; lm->prefix = prefix;
     lm->samp = *sampling;
     lm->has_cross = c.cross_attention && cross;
-    const int d = c.dim, H = c.num_heads;
     // zero the padded activation rows once; kernels only ever write rows < `rows`
     ACB_CHECK_CUDA(cudaMemsetAsync(lm->buf.h16, 0, (size_t)lm->rows_pad * d * sizeof(__half), s));
     ACB_CHECK_CUDA(cudaMemsetAsync(lm->buf.a16, 0, (size_t)lm->rows_pad * d * sizeof(__half), s));
@@ -1193,7 +1461,11 @@ extern "C" int acb_lm_debug_gemms(acb_lm_t* lm, void* stream, int* n_launches) {
     return enqueue_step(lm, (cudaStream_t)stream, nullptr, n_launches, true);
 }
 
-extern "C" int acb_lm_rows_pad(int rows) { return rows <= 16 ? 16 : 8 * nt_for_rows(rows); }
+extern "C" int acb_lm_rows_pad(int rows) {
+    ACB_REQUIRE(rows <= ACB_LM_MAX_ROWS, "acb_lm_rows_pad: rows %d > %d", rows, ACB_LM_MAX_ROWS);
+    if (rows > 64) return wide_npad(rows);
+    return rows <= 16 ? 16 : 8 * nt_for_rows(rows);
+}
 
 extern "C" int acb_lm_launches_per_step(const acb_lm_t* lm) { return lm ? lm->launches : 0; }
 

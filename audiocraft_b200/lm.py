@@ -135,8 +135,12 @@ class LMModel:
         max_seq = seq_len if shape is None else max(seq_len, shape[1])
         max_text = max(1, text_len if shape is None else max(text_len, shape[2]))
         max_batch = batch if shape is None else max(batch, shape[3])
-        # activation buffers also hold the (token, row) pairs of a prompt-prefill pass (acb_lm_prefill)
-        rp = max(self._lib.acb_lm_rows_pad(max_rows), _lib.ACB_LM_PREFILL_ROWS)
+        # activation buffers also hold the (token, row) pairs of a prompt-prefill pass (acb_lm_prefill): up to
+        # ACB_LM_PREFILL_ROWS, or one position of every row above that
+        rp = self._lib.acb_lm_rows_pad(max_rows)
+        if rp < 0:
+            _lib.check(rp, 'lm_rows_pad')
+        rp = max(rp, _lib.ACB_LM_PREFILL_ROWS)
         f16, f32 = torch.float16, torch.float32
         b = {}
         b['x'] = torch.zeros((rp, d), device=dev, dtype=f32)
@@ -223,7 +227,6 @@ class LMModel:
             f"prefix must be [rows={rows}, P, {self.dim}], got {tuple(prefix.shape)}"
         if prefix.shape[1] == 0:
             return None, 0
-        assert rows <= _lib.ACB_LM_PREFILL_ROWS, f"a condition prefix needs rows <= {_lib.ACB_LM_PREFILL_ROWS}"
         return prefix, prefix.shape[1]
 
     def _begin(self, cross, prefix, P, B, rows, text_len, S, samp):
@@ -315,7 +318,7 @@ class LMModel:
             # they go through acb_lm_prefill, several positions per pass, instead of one decode step each.
             first = 0
             import os as _os
-            if start_offset_sequence - 1 >= 2 and rows <= _lib.ACB_LM_PREFILL_ROWS and _os.environ.get('ACB_LM_PREFILL', '1') != '0':
+            if start_offset_sequence - 1 >= 2 and _os.environ.get('ACB_LM_PREFILL', '1') != '0':
                 first = start_offset_sequence - 1
                 _lib.check(self._lib.acb_lm_prefill(self._handle, 0, first, _lib.stream()), 'lm_prefill')
             if callback is None and self._debug_noise_fn is None:

@@ -139,7 +139,10 @@ typedef struct {
     int n_q;          /* codebooks (4) */
     int card;         /* cardinality (2048); special token id == card */
     int cross_attention; /* 1: layers have cross attention to the text condition */
-    int max_rows;     /* rows = B (no CFG) or 2B (CFG: [cond rows; null rows]) the buffers are sized for */
+    int max_rows;     /* rows = B (no CFG) or 2B (CFG: [cond rows; null rows]) the buffers are sized for, 1 .. ACB_LM_MAX_ROWS.
+                         Up to 64 rows every GEMM of the step is the mma.sync kernel; above 64 rows the wgmma kernel
+                         (lm_gemm_wide_kernel), which needs ffn_dim and n_q * card to be multiples of 64 (else acb_lm_begin
+                         returns ACB_ERR_UNSUPPORTED) */
     int max_seq;      /* S = T + max_delay + 1, KV cache length */
     int max_text;     /* cross-attention source length the cross KV cache is sized for */
     float pos_scale;  /* positional_scale */
@@ -186,7 +189,9 @@ typedef struct {
 
 #define ACB_LM_MAX_SPLIT 8
 #define ACB_LM_PART_SLOTS 16
-#define ACB_LM_PREFILL_ROWS 64   /* (token, row) pairs one prefill pass handles = the tallest GEMM tile */
+#define ACB_LM_PREFILL_ROWS 64   /* (token, row) pairs one prefill pass handles = the tallest GEMM tile; above 64 rows a pass
+                                    holds one position of every row */
+#define ACB_LM_MAX_ROWS 256      /* rows one handle decodes: the widest wgmma tile (N = 256) */
 
 typedef struct {
     int use_sampling;  /* LMModel.generate(use_sampling, temp, top_k, top_p, cfg_coef), lm.py:421-436 */
@@ -219,7 +224,8 @@ int acb_lm_begin(acb_lm_t* lm, const float* cross, int batch, int rows, int text
  * is rounded to fp16 on the device, as the reference's autocast output_proj rounds it.  The prefix fills KV-cache positions
  * [0, prefix_len) once, in prefill passes (every layer, cross attention included when the model has it); afterwards sequence
  * column t runs at cache position prefix_len + t, for decode steps and acb_lm_prefill alike, while acb_lm_prefill still takes
- * sequence columns.  Needs prefix_len + seq_len <= max_seq and rows <= ACB_LM_PREFILL_ROWS.  prefix_len == 0 is acb_lm_begin. */
+ * sequence columns.  Needs prefix_len + seq_len <= max_seq; any rows up to max_rows (above ACB_LM_PREFILL_ROWS the passes
+ * hold one prefix position of every row).  prefix_len == 0 is acb_lm_begin. */
 int acb_lm_begin_prefix(acb_lm_t* lm, const float* cross, const float* prefix, int prefix_len, int batch, int rows,
                         int text_len, int seq_len, const acb_lm_sampling* sampling, void* stream);
 
@@ -231,22 +237,24 @@ int acb_lm_steps(acb_lm_t* lm, int n_steps, void* stream);
 
 /* Prompt prefill = the reference's multi-token first call (modules/transformer.py:240-247, 413-414; models/lm.py:513-534):
  * consume sequence positions [pos0, pos0 + n_tokens) of every row -- their tokens are already in buffers.seq -- without
- * sampling, ACB_LM_PREFILL_ROWS / rows positions per pass (the per-phase kernels on (token, row) pairs, causal inside a pass),
- * and leave the device position at pos0 + n_tokens.  The activation buffers must hold ACB_LM_PREFILL_ROWS rows. */
+ * sampling, ACB_LM_PREFILL_ROWS / rows positions per pass (the per-phase kernels on (token, row) pairs, causal inside a pass;
+ * one position per pass above ACB_LM_PREFILL_ROWS rows), and leave the device position at pos0 + n_tokens.  The activation
+ * buffers must hold max(ACB_LM_PREFILL_ROWS, acb_lm_rows_pad(rows)) rows. */
 int acb_lm_prefill(acb_lm_t* lm, int pos0, int n_tokens, void* stream);
 
 /* Teacher-forced / inspection variant of one step: same as acb_lm_steps(1) and additionally leaves the
  * CFG-mixed logits [batch][n_q][card] fp32 in logits_out (may be NULL). */
 int acb_lm_step_logits(acb_lm_t* lm, float* logits_out, void* stream);
 
-/* Measurement hook: enqueue ONLY the weight-streaming GEMMs (lm_gemm_kernel) of one decode step, all layers in step
+/* Measurement hook: enqueue ONLY the weight-streaming GEMMs (lm_gemm_kernel, lm_gemm_wide_kernel above 64 rows) of one decode step, all layers in step
  * order, so bench.py can time the dominant kernel with CUDA events in isolation.  *n_launches = kernels enqueued. */
 int acb_lm_debug_gemms(acb_lm_t* lm, void* stream, int* n_launches);
 
 /* Always 0: the captured decode step chains its kernels with plain stream-order edges, not programmatic dependent launch. */
 int acb_lm_uses_pdl(const acb_lm_t* lm);
 
-/* rows the activation buffers must be padded to for `rows` live rows (16, 32 or 64). */
+/* rows the activation buffers must be padded to for `rows` live rows: 16, 32 or 64 up to 64 rows, 128 for 65-128 and 256 for
+ * 129-256 (the wide GEMM's tile heights); ACB_ERR_INVALID above ACB_LM_MAX_ROWS. */
 int acb_lm_rows_pad(int rows);
 
 /* Number of kernel launches one decode step enqueues (bench.py reports gpu_launches from it). */

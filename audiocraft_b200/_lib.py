@@ -81,12 +81,15 @@ def lib():
     L.acb_lm_uses_pdl.argtypes = [vp]
     L.acb_lm_debug_gemms.argtypes = [vp, vp, C.POINTER(ci)]
     L.acb_sample.argtypes = [vp, vp, vp, ci, ci, ci, ci, C.POINTER(LMSampling), C.c_uint64, vp]
+    L.acb_lm_forward_workspace_bytes.argtypes = [C.POINTER(LMConfig), ci, ci, ci, ci]
+    L.acb_lm_forward_workspace_bytes.restype = i64
+    L.acb_lm_forward.argtypes = [C.POINTER(LMConfig), C.POINTER(LMWeights), vp, vp, vp, ci, ci, ci, ci, vp, vp, i64, vp]
     for name in ('acb_weight_norm_fold', 'acb_conv1d', 'acb_convtr1d', 'acb_lstm_recurrent', 'acb_rvq_encode',
                  'acb_rvq_decode', 'acb_lm_create', 'acb_lm_destroy', 'acb_lm_begin', 'acb_lm_begin_prefix', 'acb_lm_steps',
                  'acb_lm_step_logits', 'acb_lm_launches_per_step', 'acb_lm_rows_pad', 'acb_sample',
                  'acb_device_sm_count', 'acb_lm_debug_gemms', 'acb_lm_uses_pdl',
                  'acb_conv1d_t6', 'acb_conv1d_t6_tile', 'acb_lm_prefill',
-                 'acb_resblock', 'acb_resblock_supported'):
+                 'acb_resblock', 'acb_resblock_supported', 'acb_lm_forward'):
         getattr(L, name).restype = ci
     _lib = L
     return L
@@ -97,7 +100,7 @@ EXPORTS = ['acb_version', 'acb_last_error', 'acb_device_sm_count', 'acb_weight_n
            'acb_lstm_recurrent', 'acb_lstm_state_bytes', 'acb_rvq_encode', 'acb_rvq_decode', 'acb_lm_create',
            'acb_lm_destroy', 'acb_lm_begin', 'acb_lm_begin_prefix', 'acb_lm_steps', 'acb_lm_step_logits', 'acb_lm_rows_pad',
            'acb_lm_launches_per_step', 'acb_lm_debug_gemms', 'acb_lm_uses_pdl', 'acb_sample', 'acb_conv1d_t6', 'acb_conv1d_t6_tile',
-           'acb_lm_prefill', 'acb_resblock', 'acb_resblock_supported']
+           'acb_lm_prefill', 'acb_resblock', 'acb_resblock_supported', 'acb_lm_forward_workspace_bytes', 'acb_lm_forward']
 
 
 def check(rc: int, what: str = ''):

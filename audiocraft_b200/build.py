@@ -13,8 +13,9 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libaudiocraft_b200.so')
 STAMP = LIB + '.stamp'
-SOURCES = ['api.cu', 'encodec.cu', 'lm.cu']
-HEADERS = ['common.cuh', 'gridbar.cuh', 'wgmma.cuh', os.path.join('..', '..', 'include', 'audiocraft_b200.h')]
+SOURCES = ['api.cu', 'encodec.cu', 'lm.cu', 'lm_forward.cu']
+HEADERS = ['common.cuh', 'gridbar.cuh', 'lm_math.cuh', 'tma.cuh', 'wgmma.cuh',
+           os.path.join('..', '..', 'include', 'audiocraft_b200.h')]
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
 ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
 FLAGS = ['-O3', '-std=c++17', '-lineinfo'] + ARCH + ['-Xcompiler', '-fPIC',

@@ -27,6 +27,8 @@ void acb_set_error(const char* fmt, ...);
 
 #define ACB_LAUNCH_CHECK() ACB_CHECK_CUDA(cudaGetLastError())
 
+#define ACB_TRY(expr) do { int rc_ = (expr); if (rc_ != ACB_OK) return rc_; } while (0)
+
 static inline int acb_ceil_div(int a, int b) { return (a + b - 1) / b; }
 
 // ELU(alpha=1) as torch computes it: x > 0 ? x : exp(x) - 1   (ATen elu kernel; not expm1)

@@ -18,57 +18,22 @@
 //   * self attention: one CTA per (query row, head) streaming K and V through a cp.async ring (lm_attn2_kernel), for the decode
 //     step and for prompt prefill alike.
 #include "common.cuh"
+#include "lm_math.cuh"
+#include "tma.cuh"
 #include "wgmma.cuh"
 #include <cooperative_groups.h>
-#include <cudaTypedefs.h>   // CUtensorMap, PFN_cuTensorMapEncodeTiled: types only, the entry point is looked up at run time
 #include <math.h>
 #include <new>
 #include <stdio.h>
 #include <stdlib.h>
 
 // ------------------------------------------------------------------------------------------------ helpers
-__device__ __forceinline__ void mma16816(float (&c)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0,
-                                         uint32_t b1) {
-    asm volatile(
-        "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-        : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-        : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
-}
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    uint32_t ok = 0;
-    do {
-        asm volatile("{\n .reg .pred p;\n mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n selp.u32 %0, 1, 0, p;\n}"
-                     : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-    } while (!ok);
-}
 // TMA 1-D bulk copy global -> shared, completion signalled on an mbarrier (UBLKCP in SASS). 16 B aligned, size % 16 == 0.
 __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
 
-__device__ __forceinline__ float half_round(float v) { return __half2float(__float2half_rn(v)); }
-__device__ __forceinline__ float gelu_erf(float v) { return 0.5f * v * (1.f + erff(v * 0.70710678118654752440f)); }
-
-// Block reductions: every thread returns the full result; red needs >= 32 floats and may be reused right after
-// the call returns only behind another barrier (callers alternate two scratch arrays).
-__device__ __forceinline__ float block_sum(float v, float* red) {
-    v = warp_sum(v);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
-    if (lane == 0) red[warp] = v;
-    __syncthreads();
-    float t = lane < nw ? red[lane] : 0.f;
-    return warp_sum(t);
-}
 __device__ __forceinline__ float block_max(float v, float* red) {
     v = warp_max(v);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
@@ -345,6 +310,7 @@ __global__ void __launch_bounds__(128) lm_gemm_kernel(GemmParams p) {
 // add the slices' tiles in rank order through distributed shared memory.  An item's sums are therefore the same in every
 // batch of this range.
 constexpr int WIDE_KC = 64;   // K elements per chunk: one 128-byte swizzle row
+static_assert(WIDE_KC == TMA_BOX_K, "the tensor maps (encode_map) deliver one chunk per box");
 template <int NPAD>
 struct WideCfg {
     static constexpr int W_BYTES = 64 * WIDE_KC * 2;
@@ -354,11 +320,6 @@ struct WideCfg {
     static constexpr int SMEM = STAGES * STAGE + 1024 + 64;   // ring (1024-aligned) + barriers
     static_assert(NPAD * LDS * 4 <= STAGES * STAGE, "the staging tile reuses the ring");
 };
-
-__device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
-    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
-                 ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(smem_u32(bar)) : "memory");
-}
 
 // EPI is EPI_PARTIAL, EPI_QKV, EPI_QKV_ROPE, EPI_GELU or EPI_F32.  Prefill passes above 64 rows carry one position per row,
 // so their QKV epilogue is the decode one (token 0 of the pass at position pos).
@@ -989,32 +950,6 @@ static int pick_split_wide(int N, int K, int sms, bool allow_split, int* kslice)
     return acb_ceil_div(nch, cps);
 }
 
-static PFN_cuTensorMapEncodeTiled_v12000 tensor_map_encoder() {
-    static PFN_cuTensorMapEncodeTiled_v12000 fn = nullptr;
-    if (!fn) {
-        void* f = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPointByVersion("cuTensorMapEncodeTiled", &f, 12000, cudaEnableDefault, &q) == cudaSuccess &&
-            q == cudaDriverEntryPointSuccess)
-            fn = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(f);
-    }
-    return fn;
-}
-
-// Tensor map of a row-major fp16 [outer][inner] matrix read in boxes of box_outer rows x WIDE_KC elements, 128-byte swizzled;
-// boxes past either edge are zero-filled.
-static int encode_map(CUtensorMap* m, const void* base, int inner, int outer, int box_outer) {
-    PFN_cuTensorMapEncodeTiled_v12000 fn = tensor_map_encoder();
-    ACB_REQUIRE(fn, "lm: cuTensorMapEncodeTiled is not available from the CUDA driver");
-    cuuint64_t dims[2] = {(cuuint64_t)inner, (cuuint64_t)outer}, strides[1] = {(cuuint64_t)inner * 2};
-    cuuint32_t box[2] = {(cuuint32_t)WIDE_KC, (cuuint32_t)box_outer}, es[2] = {1, 1};
-    const CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), dims, strides, box, es,
-                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    ACB_REQUIRE(r == CUDA_SUCCESS, "lm: cuTensorMapEncodeTiled failed (%d) for a [%d][%d] fp16 matrix", (int)r, outer, inner);
-    return ACB_OK;
-}
-
 // grid (N / 64, ny); the non-PARTIAL epilogues run ny as one cluster that reduces the K slices
 template <int EPI>
 static int launch_wide(const CUtensorMap& wm, const CUtensorMap& xm, int w_row0, const GemmParams& p, int ny, cudaStream_t s) {
@@ -1062,7 +997,6 @@ static GemmParams base_gemm(const void* W, const void* X, int N, int K, int rows
     return p;
 }
 
-#define ACB_TRY(expr) do { int rc_ = (expr); if (rc_ != ACB_OK) return rc_; } while (0)
 
 // ACB_DEBUG=1: synchronise and report after every launch of a directly-enqueued step (not during graph capture).
 static bool acb_debug_on() {

@@ -10,6 +10,7 @@ Weights: reference-layout LM ``state_dict`` (SURVEY.md section 8b), cast to fp16
 softmax are fp32.  No CPU path exists.
 """
 import typing as tp
+from dataclasses import dataclass
 
 import torch
 
@@ -18,6 +19,13 @@ from .conditioners import (ConditionFuser, ConditioningAttributes, ConditioningP
 from .patterns import DelayedPatternProvider
 
 import ctypes as C
+
+
+@dataclass
+class LMOutput:
+    """audiocraft/models/lm.py:95-101: logits [B,K,T,card] (NaN where the pattern gives no prediction) and mask [B,K,T]."""
+    logits: torch.Tensor
+    mask: torch.Tensor
 
 
 class LMModel:
@@ -124,6 +132,16 @@ class LMModel:
     def eval(self):
         return self
 
+    def _config(self, max_rows: int = 1, max_seq: int = 2, max_text: int = 1) -> _lib.LMConfig:
+        return _lib.LMConfig(self.dim, self.num_heads, self.num_layers, self.ffn_dim, self.n_q, self.card,
+                             int(self.cross_attention), max_rows, max_seq, max_text,
+                             float(self.cfg_dict.get('positional_scale', 1.0)),
+                             {'sin': 0, 'rope': 1, 'sin_rope': 2}[self.positional_embedding])
+
+    def _weights(self) -> _lib.LMWeights:
+        return _lib.LMWeights(*[_lib.ptr(self._w[n]) for n in ('emb', 'inv_freq', 'w_qkv', 'w_o', 'w_cq', 'w_ckv',
+                                                              'w_co', 'w_ff1', 'w_ff2', 'ln', 'out_norm', 'heads', 'rope_freq')])
+
     # ------------------------------------------------------------------ device state
     def _ensure(self, rows: int, seq_len: int, text_len: int, batch: int):
         shape = self._shape
@@ -164,12 +182,8 @@ class LMModel:
         b['pos'] = torch.zeros(4, device=dev, dtype=torch.int32)
         b['noise'] = torch.ones((max_batch, self.n_q, self.card), device=dev, dtype=f32)
         self._bufs = b
-        cfg = _lib.LMConfig(self.dim, self.num_heads, self.num_layers, self.ffn_dim, self.n_q, self.card,
-                            int(self.cross_attention), max_rows, max_seq, max_text,
-                            float(self.cfg_dict.get('positional_scale', 1.0)),
-                            {'sin': 0, 'rope': 1, 'sin_rope': 2}[self.positional_embedding])
-        wts = _lib.LMWeights(*[_lib.ptr(self._w[n]) for n in ('emb', 'inv_freq', 'w_qkv', 'w_o', 'w_cq', 'w_ckv',
-                                                              'w_co', 'w_ff1', 'w_ff2', 'ln', 'out_norm', 'heads', 'rope_freq')])
+        cfg = self._config(max_rows, max_seq, max_text)
+        wts = self._weights()
         bufs = _lib.LMBuffers(*[_lib.ptr(b[n]) for n in ('x', 'h16', 'a16', 'f16', 'q32', 'part', 'logits', 'k_cache',
                                                          'v_cache', 'ck_cache', 'cv_cache', 'cross16', 'seq',
                                                          'seq_mask', 'pos', 'noise')])
@@ -465,3 +479,87 @@ class LMModel:
                 if raw and j is not None:
                     raw_out[j].copy_(bufs['logits'][:rows].view(rows, K, self.card))
             return (out, raw_out) if raw else out
+
+    # ------------------------------------------------------------------ full-sequence forward (scoring)
+    @torch.no_grad()
+    def forward(self, sequence: torch.Tensor, conditions: tp.List[ConditioningAttributes] = [],
+                condition_tensors: tp.Optional[tp.Dict[str, tp.Any]] = None, stage: int = -1, *,
+                cross_attention_src: tp.Optional[torch.Tensor] = None,
+                prefix: tp.Optional[torch.Tensor] = None) -> torch.Tensor:
+        """LMModel.forward (lm.py:221-268): sequence [B,K,S] (codes or the special token `card`) -> logits [B,K,S,card], one
+        causal pass over every position on the acb_lm_forward kernels.  The logits are fp32 (the reference returns fp16
+        under CUDA autocast).  Conditions go through condition_provider and fuser without CFG rows, as in the reference;
+        ``cross_attention_src`` [B,T_text,d] and ``prefix`` [B,P,d] are pre-computed condition tensors, as for generate.
+        With a `prepend` fuser the prefix runs as the first P positions and its logits are dropped.  The decode state
+        (KV caches, position, captured step) is neither read nor changed."""
+        if stage >= 0:
+            raise NotImplementedError("stage >= 0 (MAGNeT's per-stage attention masks) is not built")
+        B, K, S = sequence.shape
+        assert K == self.num_codebooks, "Sequence shape must match the specified number of codebooks"
+        cross = cross_attention_src
+        if cross is not None or prefix is not None:
+            if conditions or condition_tensors is not None:
+                raise ValueError("pass the conditions either as conditions / condition_tensors or as the pre-computed "
+                                 "cross_attention_src / prefix, not both")
+        else:
+            if condition_tensors is None:
+                if conditions:
+                    assert self.condition_provider is not None, "conditions given but the model has no condition_provider"
+                    condition_tensors = self.condition_provider(self.condition_provider.tokenize(list(conditions)))
+            else:
+                assert not conditions, "Shouldn't pass both conditions and condition_tensors."
+            if condition_tensors is not None:
+                cross, prefix = self.fuser.cross_source(condition_tensors), self.fuser.prefix_source(condition_tensors)
+        with torch.cuda.device(self.device):
+            seq = sequence.to(self.device, torch.long).contiguous()
+            # the reference's embedding lookup raises on an out-of-range token; the kernels take the range as a precondition
+            if seq.numel() and not bool(((seq >= 0) & (seq <= self.card)).all()):
+                raise IndexError(f"tokens must lie in [0, {self.card}] (card = the special token)")
+            text_len = 0
+            if self.cross_attention:
+                assert cross is not None, "the model has cross attention: conditions or cross_attention_src are required"
+                cross = cross.to(self.device, torch.float32).contiguous()
+                assert cross.dim() == 3 and cross.shape[0] == B and cross.shape[2] == self.dim, \
+                    f"cross_attention_src must be [B={B}, T, {self.dim}], got {tuple(cross.shape)}"
+                text_len = cross.shape[1]
+            else:
+                cross = None
+            prefix, P = self._check_prefix(prefix, B)
+            cfg = self._config()
+            nbytes = self._lib.acb_lm_forward_workspace_bytes(C.byref(cfg), B, P, S, text_len)
+            if nbytes < 0:
+                _lib.check(int(nbytes), 'lm_forward_workspace_bytes')
+            ws = torch.empty(max(int(nbytes), 1), device=self.device, dtype=torch.uint8)
+            logits = torch.empty((B, K, S, self.card), device=self.device, dtype=torch.float32)
+            _lib.check(self._lib.acb_lm_forward(C.byref(cfg), C.byref(self._weights()), _lib.ptr(seq), _lib.ptr(cross),
+                                                _lib.ptr(prefix), B, P, S, text_len, _lib.ptr(logits), _lib.ptr(ws),
+                                                int(nbytes), _lib.stream()), 'lm_forward')
+            return logits
+
+    __call__ = forward
+
+    @torch.no_grad()
+    def compute_predictions(self, codes: torch.Tensor, conditions: tp.List[ConditioningAttributes] = [],
+                            condition_tensors: tp.Optional[tp.Dict[str, tp.Any]] = None, stage: int = -1,
+                            keep_only_valid_steps: bool = True, *,
+                            cross_attention_src: tp.Optional[torch.Tensor] = None,
+                            prefix: tp.Optional[torch.Tensor] = None) -> LMOutput:
+        """LMModel.compute_predictions (lm.py:270-321): codes [B,K,T] -> LMOutput(logits [B,K,T,card], mask [B,K,T]); the
+        logits of timestep t predict codes[..., t] and are NaN where the mask is 0."""
+        if stage >= 0:
+            raise NotImplementedError("stage >= 0 (MAGNeT's per-stage attention masks) is not built")
+        B, K, T = codes.shape
+        codes = codes.to(self.device).contiguous()
+        pattern = self.pattern_provider.get_pattern(T)
+        sequence_codes, _, _ = pattern.build_pattern_sequence(codes, self.special_token_id,
+                                                              keep_only_valid_steps=keep_only_valid_steps)
+        logits = self.forward(sequence_codes, conditions, condition_tensors, stage,
+                              cross_attention_src=cross_attention_src, prefix=prefix)   # [B, K, S, card]
+        S = logits.shape[2]
+        # revert_pattern_logits' index table applied to [B, K, S, card] directly, without the [B, card, K, S] permuted copy
+        idx, mask = pattern.logits_tables(S, keep_only_valid_steps)
+        idx_t = torch.from_numpy(idx).to(self.device)
+        flat = torch.cat([logits.reshape(B, K * S, self.card),
+                          torch.full((B, 1, self.card), float('nan'), device=self.device, dtype=logits.dtype)], dim=1)
+        out = flat[:, idx_t.reshape(-1)].reshape(B, K, T, self.card)
+        return LMOutput(out, torch.from_numpy(mask).to(self.device)[None].expand(B, -1, -1))

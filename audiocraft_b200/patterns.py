@@ -68,6 +68,30 @@ class Pattern:
         values = flat[:, idx_t.reshape(-1)].reshape(B, K, T)
         return values, idx_t, torch.from_numpy(mask).to(s.device)
 
+    def logits_tables(self, S: int, keep_only_valid_steps: bool = False):
+        """_build_reverted_sequence_scatter_indexes with is_model_output=True (codebooks_patterns.py:181-223): the logits at
+        sequence step s predict the token at step s + 1, so timestep t of codebook q reads step t + delays[q].  Returns
+        (indexes [K,T] into the flattened [K*S] steps, K*S = the special value; mask [K,T])."""
+        layout_len = self.timesteps + (0 if keep_only_valid_steps else self.max_delay) + 1
+        assert S <= layout_len, f"sequence to revert is longer than the defined pattern: {S} > {layout_len}"
+        t = np.arange(self.timesteps)[None, :]
+        step = t + np.asarray(self.delays)[:, None]
+        mask = (step < S) & (step < layout_len - 1)
+        idx = np.where(mask, step + np.arange(self.n_q)[:, None] * S, self.n_q * S).astype(np.int64)
+        return idx, mask
+
+    def revert_pattern_logits(self, logits: torch.Tensor, special_token: float, keep_only_valid_steps: bool = False):
+        """codebooks_patterns.py:250-269: model logits [B,card,K,S] -> (values [B,card,K,T], indexes [K,T], mask [K,T]);
+        positions without a prediction hold `special_token`."""
+        B, card, K, S = logits.shape
+        assert K == self.n_q
+        idx, mask = self.logits_tables(S, keep_only_valid_steps)
+        idx_t = torch.from_numpy(idx).to(logits.device)
+        flat = torch.cat([logits.reshape(B, card, -1),
+                          torch.full((B, card, 1), special_token, dtype=logits.dtype, device=logits.device)], dim=-1)
+        values = flat[:, :, idx_t.reshape(-1)].reshape(B, card, K, idx.shape[1])
+        return values, idx_t, torch.from_numpy(mask).to(logits.device)
+
 
 class DelayedPatternProvider:
     """codebooks_patterns.py:305-356 (flatten_first / empty_initial are 0 for every released MusicGen)."""

@@ -260,6 +260,27 @@ int acb_lm_rows_pad(int rows);
 /* Number of kernel launches one decode step enqueues (bench.py reports gpu_launches from it). */
 int acb_lm_launches_per_step(const acb_lm_t* lm);
 
+/* ---------------------------------------------------------------- MusicGen: LM full-sequence forward -- */
+
+/* LMModel.forward on whole sequences (audiocraft/models/lm.py:221-268; the computation under compute_predictions,
+ * lm.py:270-321): causal self attention over every position, no KV cache and no acb_lm_t.  Stateless: it neither reads nor
+ * writes any decode handle.
+ *   seq     [batch][n_q][seq_len] int64 tokens.  Precondition (not checked on the device, which would break graph capture):
+ *           every token lies in [0, card] (card = the special token).
+ *   cross   [batch][text_len][d] fp32 condition tensor (cross_attention_src; padded positions are zeros and are attended to,
+ *           as in the reference), required exactly when cfg->cross_attention; no CFG rows are added.
+ *   prefix  [batch][prefix_len][d] fp32 condition prefix of a `prepend` fuser (MusicGen-melody) or NULL with prefix_len 0: it
+ *           runs as the first prefix_len positions (each value rounded to fp16 first) and its logits are not written.
+ *   logits  [batch][n_q][seq_len][card] fp32 (the reference returns fp16 under CUDA autocast).
+ *   workspace: at least acb_lm_forward_workspace_bytes(...) bytes of device memory, 256-byte aligned.
+ * cfg->max_rows, max_seq and max_text are ignored.  Needs dim = 64 * num_heads <= 2048, ffn_dim % 8 == 0, even card,
+ * n_q <= 16.  Every output element is summed in one fixed order (no split-K): an item's logits are bit-identical whatever
+ * batch it is in.  Tensor maps are encoded per call; all work is on `stream`. */
+int64_t acb_lm_forward_workspace_bytes(const acb_lm_config* cfg, int batch, int prefix_len, int seq_len, int text_len);
+int acb_lm_forward(const acb_lm_config* cfg, const acb_lm_weights* w, const int64_t* seq, const float* cross,
+                   const float* prefix, int batch, int prefix_len, int seq_len, int text_len, float* logits,
+                   void* workspace, int64_t workspace_bytes, void* stream);
+
 /* Stand-alone sampler (tail of _sample_next_token, lm.py:403-418; utils/utils.py:88-141) for unit tests:
  * logits [rows][n_q][card] fp32 ([cond; null] rows when rows == 2*batch), noise optional, tokens [batch][n_q]. */
 int acb_sample(const float* logits, const float* noise, int64_t* tokens, int batch, int rows, int n_q, int card,

@@ -40,10 +40,11 @@ Coverage: kernel instances the dispatchers can select, and the test here that ex
   (prec 0 and 1), acb_resblock (exact 1 and 0)                     test_encodec_layers_at_32_items
   RVQ encode / decode at 32 x 500 frames                           test_rvq_at_32_items
   The whole 32 x 10 s encode / decode chain                        test_encodec_bench_chain_at_32_items
-Still not executed against a reference by any test: lm_gemm_kernel<8, QKV_ROPE, 1> and every <NT, QKV_ROPE, 2> except NT = 4
-(rotary positions at 33-64 rows, and at the released widths outside rows 17-32); <1, QKV | GELU | F32, 2> (medium at rows <= 8
-runs them only in test_ft32_tiles_equal_16_feature_tiles, against the 16-feature tiles, not against the oracle); the prefill
-cross-attention kernel over more than 32 text positions; the EnCodec-24k plan at 32 items.
+  lm_gemm_kernel<8, QKV_ROPE, 1>, <1 | 2, QKV_ROPE, 2> and <1, QKV | GELU | F32, 2> (and every other decode GEMM instance the
+  released widths select, with the wide GEMM) against float64 on their own inputs: test_gpu_kernels_f64.py (coverage table
+  there).  <8, QKV_ROPE, 2> is selected at none of the released widths on a 132-SM H100.
+Still not executed against a reference by any test: the prefill cross-attention kernel over more than 32 text positions; the
+EnCodec-24k plan at 32 items.
 """
 import os
 

@@ -40,6 +40,16 @@ class LMSampling(C.Structure):
                 ('cfg_coef', C.c_float), ('seed', C.c_uint64), ('noise_from_buffer', C.c_int), ('cfg_coef_beta', C.c_float)]
 
 
+class T5Config(C.Structure):
+    _fields_ = [('d_model', C.c_int), ('d_kv', C.c_int), ('num_heads', C.c_int), ('num_layers', C.c_int), ('d_ff', C.c_int),
+                ('vocab_size', C.c_int), ('num_buckets', C.c_int), ('out_dim', C.c_int), ('eps', C.c_float)]
+
+
+class T5Weights(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in ('shared', 'w_qkv', 'w_o', 'w_i', 'w_fo', 'ln', 'final_ln', 'rel_bias', 'proj_w',
+                                           'proj_b')]
+
+
 _lib = None
 
 
@@ -84,12 +94,15 @@ def lib():
     L.acb_lm_forward_workspace_bytes.argtypes = [C.POINTER(LMConfig), ci, ci, ci, ci]
     L.acb_lm_forward_workspace_bytes.restype = i64
     L.acb_lm_forward.argtypes = [C.POINTER(LMConfig), C.POINTER(LMWeights), vp, vp, vp, ci, ci, ci, ci, vp, vp, i64, vp]
+    L.acb_t5_workspace_bytes.argtypes = [C.POINTER(T5Config), ci, ci]
+    L.acb_t5_workspace_bytes.restype = i64
+    L.acb_t5_encode.argtypes = [C.POINTER(T5Config), C.POINTER(T5Weights), vp, vp, vp, ci, ci, vp, vp, vp, i64, vp]
     for name in ('acb_weight_norm_fold', 'acb_conv1d', 'acb_convtr1d', 'acb_lstm_recurrent', 'acb_rvq_encode',
                  'acb_rvq_decode', 'acb_lm_create', 'acb_lm_destroy', 'acb_lm_begin', 'acb_lm_begin_prefix', 'acb_lm_steps',
                  'acb_lm_step_logits', 'acb_lm_launches_per_step', 'acb_lm_rows_pad', 'acb_sample',
                  'acb_device_sm_count', 'acb_lm_debug_gemms', 'acb_lm_uses_pdl',
                  'acb_conv1d_t6', 'acb_conv1d_t6_tile', 'acb_lm_prefill',
-                 'acb_resblock', 'acb_resblock_supported', 'acb_lm_forward'):
+                 'acb_resblock', 'acb_resblock_supported', 'acb_lm_forward', 'acb_t5_encode'):
         getattr(L, name).restype = ci
     _lib = L
     return L
@@ -100,7 +113,8 @@ EXPORTS = ['acb_version', 'acb_last_error', 'acb_device_sm_count', 'acb_weight_n
            'acb_lstm_recurrent', 'acb_lstm_state_bytes', 'acb_rvq_encode', 'acb_rvq_decode', 'acb_lm_create',
            'acb_lm_destroy', 'acb_lm_begin', 'acb_lm_begin_prefix', 'acb_lm_steps', 'acb_lm_step_logits', 'acb_lm_rows_pad',
            'acb_lm_launches_per_step', 'acb_lm_debug_gemms', 'acb_lm_uses_pdl', 'acb_sample', 'acb_conv1d_t6', 'acb_conv1d_t6_tile',
-           'acb_lm_prefill', 'acb_resblock', 'acb_resblock_supported', 'acb_lm_forward_workspace_bytes', 'acb_lm_forward']
+           'acb_lm_prefill', 'acb_resblock', 'acb_resblock_supported', 'acb_lm_forward_workspace_bytes', 'acb_lm_forward',
+           'acb_t5_workspace_bytes', 'acb_t5_encode']
 
 
 def check(rc: int, what: str = ''):

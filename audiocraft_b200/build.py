@@ -13,8 +13,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libaudiocraft_b200.so')
 STAMP = LIB + '.stamp'
-SOURCES = ['api.cu', 'encodec.cu', 'lm.cu', 'lm_forward.cu']
-HEADERS = ['common.cuh', 'gridbar.cuh', 'lm_math.cuh', 'tma.cuh', 'wgmma.cuh',
+SOURCES = ['api.cu', 'encodec.cu', 'lm.cu', 'lm_forward.cu', 't5.cu']
+HEADERS = ['common.cuh', 'fwd_attn.cuh', 'fwd_gemm.cuh', 'gridbar.cuh', 'lm_math.cuh', 'tma.cuh', 'wgmma.cuh',
            os.path.join('..', '..', 'include', 'audiocraft_b200.h')]
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
 ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']

@@ -1,7 +1,7 @@
 """Conditioning plumbing at the LM boundary (host code).
 
-The hot path consumes ``(cond[B,T,D], mask[B,T])`` tensors; everything that produces them (T5, chroma, CLAP...) stays
-host PyTorch / HF and runs once per ``generate`` call (SURVEY.md section 2 #12, section 8f.3).  This module mirrors
+The hot path consumes ``(cond[B,T,D], mask[B,T])`` tensors, produced once per ``generate`` call: the T5 text encoder runs
+in the package's kernels (``T5Conditioner``, csrc/t5.cu), the chroma front-end in host PyTorch.  This module mirrors
 just the contract ``LMModel.generate`` relies on: ``ConditioningAttributes`` (conditioners.py:83-123),
 ``BaseConditioner`` / ``TextConditioner`` (:345-384), ``ConditioningProvider.tokenize/forward`` (:1501-1545),
 ``ClassifierFreeGuidanceDropout`` at p=1 as used for the null conditions (lm.py:499, conditioners.py:1427-1466) and
@@ -82,8 +82,8 @@ class TextConditioner(BaseConditioner):
 class PrecomputedTextConditioner(TextConditioner):
     """Text conditioner whose encoder output is supplied by the caller: ``encoder(list[str]) -> (hidden [B,T,dim],
     mask [B,T])``.  It reproduces T5Conditioner's contract (conditioners.py:490-515): None / "" entries get a zero
-    mask, the output is ``output_proj(hidden) * mask`` so null rows are exact zeros.  Used with a T5 encoder when its
-    weights are present, and with seeded synthetic hidden states in tests / bench (no network in this image)."""
+    mask, the output is ``output_proj(hidden) * mask`` so null rows are exact zeros.  Used with any caller-supplied encoder,
+    and with seeded synthetic hidden states in tests / bench."""
 
     def __init__(self, dim: int, output_dim: int, encoder: tp.Callable[[tp.List[str]], ConditionType]):
         super().__init__(dim, output_dim)
@@ -103,6 +103,44 @@ class PrecomputedTextConditioner(TextConditioner):
         mask = inputs['attention_mask'].to(w.device)
         embeds = self.output_proj(inputs['hidden'].to(w))
         return embeds * mask.unsqueeze(-1).to(embeds.dtype), mask
+
+
+class T5Conditioner(TextConditioner):
+    """conditioners.py:422-515 on the device: transformers' T5Tokenizer on the host, then the frozen T5 encoder, output_proj
+    and the mask in one acb_t5_encode call (csrc/t5.cu).  `path` is a local T5 directory in Hugging Face layout
+    (audiocraft_b200.t5).  output_proj stays an nn.Linear so the LM checkpoint's `condition_provider.*` entries fill it; the
+    T5 weights are kept out of the module's parameters and state dict, as the reference keeps them
+    (`self.__dict__['t5']`).  Rows whose mask is all zero (None / "" entries, the whole null half of CFG) are exact zeros
+    and skip the encoder.  word_dropout applies only in training, which is not built here."""
+
+    def __init__(self, path: str, output_dim: int, finetune: bool = False, device='cuda',
+                 autocast_dtype: tp.Optional[str] = 'float32', word_dropout: float = 0., normalize_text: bool = False):
+        if finetune:
+            raise NotImplementedError("T5Conditioner finetune=True (training T5) is not built: the encoder is frozen")
+        if normalize_text:
+            raise NotImplementedError("T5Conditioner normalize_text=True is not built (it needs spaCy's lemmatizer)")
+        from .t5 import T5Encoder, load_tokenizer
+        t5 = T5Encoder(path, device)
+        super().__init__(t5.d_model, output_dim)
+        self.device, self.finetune, self.word_dropout, self.normalize_text = device, finetune, word_dropout, normalize_text
+        self.t5_tokenizer = load_tokenizer(path)
+        self.__dict__['t5'] = t5
+
+    def tokenize(self, x: tp.List[tp.Optional[str]]) -> tp.Dict[str, torch.Tensor]:
+        entries = [xi if xi is not None else "" for xi in x]
+        empty_idx = torch.LongTensor([i for i, xi in enumerate(entries) if xi == ""])
+        inputs = self.t5_tokenizer(entries, return_tensors='pt', padding=True)
+        inputs['attention_mask'][empty_idx, :] = 0
+        return {'input_ids': inputs['input_ids'], 'attention_mask': inputs['attention_mask']}
+
+    def forward(self, inputs: tp.Dict[str, torch.Tensor]) -> ConditionType:
+        ids, mask = inputs['input_ids'], inputs['attention_mask']
+        w = self.output_proj.weight
+        out = torch.zeros((ids.shape[0], ids.shape[1], self.output_dim), dtype=torch.float32, device=w.device)
+        live = mask.cpu().any(dim=1).nonzero().flatten()
+        if len(live):
+            out[live.to(w.device)] = self.t5.encode(ids[live], mask[live], w, self.output_proj.bias)[0]
+        return out, mask.to(w.device)
 
 
 def length_to_mask(lengths: torch.Tensor, max_len: tp.Optional[int] = None) -> torch.Tensor:

@@ -12,6 +12,13 @@ __device__ __forceinline__ void mma16816(float (&c)[4], uint32_t a0, uint32_t a1
 }
 
 __device__ __forceinline__ float half_round(float v) { return __half2float(__float2half_rn(v)); }
+// v rounded to the nearest TF32 value (10-bit mantissa).  The TF32 wgmma drops an fp32 operand's low 13 bits (truncation);
+// operands rounded first carry half that error.
+__device__ __forceinline__ float tf32_round(float v) {
+    uint32_t r;
+    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(v));
+    return __uint_as_float(r);
+}
 __device__ __forceinline__ float gelu_erf(float v) { return 0.5f * v * (1.f + erff(v * 0.70710678118654752440f)); }
 
 // Block reductions: every thread returns the full result; red needs >= 32 floats and may be reused right after

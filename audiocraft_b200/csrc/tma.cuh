@@ -1,4 +1,4 @@
-// mbarrier and tiled-TMA helpers shared by the LM decode step (lm.cu) and the LM full-sequence forward (lm_forward.cu).
+// mbarrier and tiled-TMA helpers shared by the LM decode step (lm.cu) and the full-sequence forwards (fwd_gemm.cuh).
 #pragma once
 #include <cudaTypedefs.h>   // CUtensorMap, PFN_cuTensorMapEncodeTiled: types only, the entry point is looked up at run time
 #include <stdint.h>
@@ -41,17 +41,28 @@ static PFN_cuTensorMapEncodeTiled_v12000 tensor_map_encoder() {
     return fn;
 }
 
-// Tensor map of a row-major fp16 [outer][inner] matrix read in boxes of box_outer rows x 64 elements (one 128-byte swizzle
-// row), 128-byte swizzled; boxes past either edge are zero-filled.
-constexpr int TMA_BOX_K = 64;
-static int encode_map(CUtensorMap* m, const void* base, int inner, int outer, int box_outer) {
+// Tensor map of a row-major [outer][inner] matrix of `elem_bytes`-byte elements read in boxes of box_outer rows x one 128-byte
+// swizzle row (box_inner elements), 128-byte swizzled; boxes past either edge are zero-filled.
+static int encode_map_typed(CUtensorMap* m, const void* base, int inner, int outer, int box_outer, CUtensorMapDataType dt,
+                            int elem_bytes, int box_inner, const char* what) {
     PFN_cuTensorMapEncodeTiled_v12000 fn = tensor_map_encoder();
     ACB_REQUIRE(fn, "lm: cuTensorMapEncodeTiled is not available from the CUDA driver");
-    cuuint64_t dims[2] = {(cuuint64_t)inner, (cuuint64_t)outer}, strides[1] = {(cuuint64_t)inner * 2};
-    cuuint32_t box[2] = {(cuuint32_t)TMA_BOX_K, (cuuint32_t)box_outer}, es[2] = {1, 1};
-    const CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), dims, strides, box, es,
+    cuuint64_t dims[2] = {(cuuint64_t)inner, (cuuint64_t)outer}, strides[1] = {(cuuint64_t)inner * elem_bytes};
+    cuuint32_t box[2] = {(cuuint32_t)box_inner, (cuuint32_t)box_outer}, es[2] = {1, 1};
+    const CUresult r = fn(m, dt, 2, const_cast<void*>(base), dims, strides, box, es,
                           CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                           CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    ACB_REQUIRE(r == CUDA_SUCCESS, "lm: cuTensorMapEncodeTiled failed (%d) for a [%d][%d] fp16 matrix", (int)r, outer, inner);
+    ACB_REQUIRE(r == CUDA_SUCCESS, "lm: cuTensorMapEncodeTiled failed (%d) for a [%d][%d] %s matrix", (int)r, outer, inner, what);
     return ACB_OK;
+}
+
+// fp16 matrix, boxes of 64 elements
+constexpr int TMA_BOX_K = 64;
+static int encode_map(CUtensorMap* m, const void* base, int inner, int outer, int box_outer) {
+    return encode_map_typed(m, base, inner, outer, box_outer, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, TMA_BOX_K, "fp16");
+}
+// fp32 matrix (a TF32 wgmma operand), boxes of 32 elements
+constexpr int TMA_BOX_K_F32 = 32;
+static int encode_map_f32(CUtensorMap* m, const void* base, int inner, int outer, int box_outer) {
+    return encode_map_typed(m, base, inner, outer, box_outer, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, TMA_BOX_K_F32, "fp32");
 }

@@ -13,7 +13,7 @@ import torch
 
 from . import synth
 from .conditioners import (ChromaStemConditioner, ConditionFuser, ConditioningProvider, PrecomputedTextConditioner,
-                           identity_stem_separator)
+                           T5Conditioner, identity_stem_separator)
 from .encodec import EncodecModel
 from .lm import LMModel
 
@@ -97,20 +97,39 @@ def lm_cfg_from_xp(xp: dict) -> dict:
                       match_len_on_eval=bool(cs.get('match_len_on_eval', True)),
                       sample_rate=int(cs.get('sample_rate') or xp['sample_rate']),
                       duration=float(xp['dataset']['segment_duration']))   # builders.py: duration = segment_duration
-    cond_dim = None
+    cond_dim, t5 = None, None
     desc = xp.get('conditioners', {}).get('description')
     if desc is not None:
         if desc.get('model') != 't5':
-            raise NotImplementedError(f"description conditioner '{desc.get('model')}' is not built (t5 hidden states are precomputed)")
-        cond_dim = _T5_DIMS.get(desc['t5']['name'])
+            raise NotImplementedError(f"description conditioner '{desc.get('model')}' is not built (only t5)")
+        t5 = dict(desc['t5'])
+        cond_dim = _T5_DIMS.get(t5['name'])
         if cond_dim is None:
-            raise NotImplementedError(f"unknown T5 variant {desc['t5']['name']}")
+            raise NotImplementedError(f"unknown T5 variant {t5['name']}")
     return dict(dim=tl['dim'], num_heads=tl['num_heads'], num_layers=tl['num_layers'], hidden_scale=tl.get('hidden_scale', 4),
                 n_q=tl['n_q'], card=tl['card'], delays=list(xp['codebooks_pattern']['delay']['delays']),
                 max_period=float(tl.get('max_period', 10000.0)), positional_scale=float(tl.get('positional_scale', 1.0)),
                 positional_embedding=pe, cross_attention=bool(fz.get('cross')),
                 cfg_coef=xp['classifier_free_guidance']['inference_coef'], cond_dim=cond_dim,
-                two_step_cfg=tl.get('two_step_cfg', False), prepend=prepend, chroma=chroma)
+                two_step_cfg=tl.get('two_step_cfg', False), prepend=prepend, chroma=chroma, t5=t5)
+
+
+def _text_conditioner(cfg: dict, text_encoder, device):
+    """The description conditioner: a T5Conditioner when `text_encoder` is a local T5 directory, else the caller's callable
+    returning (hidden states, mask) behind a PrecomputedTextConditioner."""
+    if isinstance(text_encoder, (str, os.PathLike)):
+        from .t5 import read_config
+        path = os.fspath(text_encoder)
+        if not os.path.isdir(path):
+            raise FileNotFoundError(f"text_encoder '{path}' is not a local T5 directory (names are not resolved on a hub)")
+        d_model = read_config(path)['d_model']
+        if d_model != cfg['cond_dim']:
+            name = (cfg.get('t5') or {}).get('name', 'the checkpoint\'s T5')
+            raise ValueError(f"T5 directory {path} has d_model {d_model}, but {name} has {cfg['cond_dim']}")
+        t5 = cfg.get('t5') or {}
+        return T5Conditioner(path, cfg['dim'], finetune=bool(t5.get('finetune', False)), device=device,
+                             word_dropout=float(t5.get('word_dropout', 0.)), normalize_text=bool(t5.get('normalize_text', False)))
+    return PrecomputedTextConditioner(cfg['cond_dim'], cfg['dim'], text_encoder)
 
 
 def _melody_parts(cfg: dict, text_encoder, stem_separator, device):
@@ -118,7 +137,7 @@ def _melody_parts(cfg: dict, text_encoder, stem_separator, device):
     ch = cfg['chroma']
     conds = {}
     if 'description' in cfg['prepend']:
-        conds['description'] = PrecomputedTextConditioner(cfg['cond_dim'], cfg['dim'], text_encoder)
+        conds['description'] = _text_conditioner(cfg, text_encoder, device)
     conds['self_wav'] = ChromaStemConditioner(cfg['dim'], ch['sample_rate'], ch['n_chroma'], ch['radix2_exp'], ch['duration'],
                                               match_len_on_eval=ch['match_len_on_eval'], argmax=ch['argmax'],
                                               stem_separator=stem_separator)
@@ -186,7 +205,7 @@ def load_lm_model(name: str, device='cuda', seed: int = 0, text_encoder=None, st
                                    sample_rate=cfg['sample_rate'], duration=cfg['duration']))
             provider, fuser = _melody_parts(cfg, enc, stem_separator or identity_stem_separator, device)
             return LMModel(sd, cfg, provider, fuser, device)
-        provider = ConditioningProvider({'description': PrecomputedTextConditioner(cfg['cond_dim'], cfg['dim'], enc)})
+        provider = ConditioningProvider({'description': _text_conditioner(cfg, enc, device)})
         return LMModel(sd, cfg, provider, ConditionFuser({'cross': ['description']}), device)
     if os.path.isfile(name):
         pkg = _load_pkg(name)
@@ -199,16 +218,16 @@ def load_lm_model(name: str, device='cuda', seed: int = 0, text_encoder=None, st
                                    "sample_rate) -> melody stems [B,1,T]> standing in for Demucs (htdemucs weights are not "
                                    "available offline)")
             if 'description' in cfg['prepend'] and text_encoder is None:
-                raise RuntimeError("this checkpoint is text-conditioned: pass text_encoder=<callable returning the frozen T5 "
-                                   f"hidden states [B,T,{cfg['cond_dim']}] and attention mask>")
+                raise RuntimeError("this checkpoint is text-conditioned: pass text_encoder=<local T5 directory> or <callable "
+                                   f"returning the frozen T5 hidden states [B,T,{cfg['cond_dim']}] and attention mask>")
             provider, fuser = _melody_parts(cfg, text_encoder, stem_separator, device)
             return LMModel(pkg['best_state'], cfg, provider, fuser, device)
         if cfg['cross_attention']:
             if text_encoder is None:
-                raise RuntimeError("this checkpoint is text-conditioned: pass text_encoder=<callable returning the frozen T5 "
-                                   f"hidden states [B,T,{cfg['cond_dim']}] and attention mask> (T5 itself is outside the hot path "
-                                   "and its weights are not available offline)")
-            provider = ConditioningProvider({'description': PrecomputedTextConditioner(cfg['cond_dim'], cfg['dim'], text_encoder)})
+                raise RuntimeError("this checkpoint is text-conditioned: pass text_encoder=<local T5 directory in Hugging Face "
+                                   "layout> or <callable returning the frozen T5 hidden states "
+                                   f"[B,T,{cfg['cond_dim']}] and attention mask>")
+            provider = ConditioningProvider({'description': _text_conditioner(cfg, text_encoder, device)})
         return LMModel(pkg['best_state'], cfg, provider, ConditionFuser({'cross': ['description']}), device)
     raise FileNotFoundError(f"LM '{name}': not a local checkpoint and not 'synthetic/<scale>'")
 
@@ -223,8 +242,9 @@ def _wrap_from_xp(cm, lm_ckpt: str):
 
 
 def load_musicgen(name: str, device=None, seed: int = 0, text_encoder=None, stem_separator=None):
-    """`text_encoder`: callable list[str] -> (hidden [B,T,cond_dim], mask [B,T]) standing in for the frozen T5 when loading
-    a real checkpoint directory (the reference instantiates T5 from the HF hub, conditioners.py:422-515).
+    """`text_encoder`: a local T5 directory in Hugging Face layout (config.json, model.safetensors or pytorch_model.bin,
+    spiece.model), run on the device by T5Conditioner, or a callable list[str] -> (hidden [B,T,cond_dim], mask [B,T]) giving
+    the frozen T5's output (the reference instantiates T5 from the HF hub, conditioners.py:422-515).
     `stem_separator`: the Demucs stand-in a melody checkpoint needs (see load_lm_model)."""
     from .musicgen import MusicGen
     device = 'cuda' if device is None else device
@@ -241,7 +261,8 @@ def load_musicgen(name: str, device=None, seed: int = 0, text_encoder=None, stem
 
 
 def load_audiogen(name: str, device=None, seed: int = 0, text_encoder=None):
-    """`synthetic/audiogen-medium` (seeded random weights of the released architecture) or a local checkpoint directory."""
+    """`synthetic/audiogen-medium` (seeded random weights of the released architecture) or a local checkpoint directory;
+    `text_encoder` as for load_musicgen."""
     from .musicgen import AudioGen
     device = 'cuda' if device is None else device
     if name.startswith('synthetic/'):

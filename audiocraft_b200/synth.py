@@ -265,3 +265,73 @@ def synth_text_condition(cfg: dict, batch: int, t_text: int, seed: int = 0, devi
     lengths = torch.randint(max(1, t_text // 2), t_text + 1, (batch,), generator=gen)
     mask = (torch.arange(t_text).view(1, -1) < lengths.view(-1, 1)).long()
     return hid.to(device), mask.to(device)
+
+
+# ----------------------------------------------------------------------------- T5 text encoder
+
+# transformers' T5Config of the released checkpoints the conditioners name (config/conditioner/text2music.yaml: t5-base,
+# text2sound.yaml: t5-large)
+T5_CONFIGS: tp.Dict[str, dict] = {
+    't5-small': dict(d_model=512, d_kv=64, d_ff=2048, num_heads=8, num_layers=6),
+    't5-base': dict(d_model=768, d_kv=64, d_ff=3072, num_heads=12, num_layers=12),
+    't5-large': dict(d_model=1024, d_kv=64, d_ff=4096, num_heads=16, num_layers=24),
+}
+
+
+def t5_config(name: str) -> dict:
+    """The config.json fields of a released T5 (relu feed-forward, 32128-token vocabulary, 32 buckets up to distance 128)."""
+    cfg = dict(model_type='t5', vocab_size=32128, relative_attention_num_buckets=32, relative_attention_max_distance=128,
+               layer_norm_epsilon=1e-6, feed_forward_proj='relu', dropout_rate=0.1, initializer_factor=1.0,
+               is_encoder_decoder=True, pad_token_id=0, eos_token_id=1, decoder_start_token_id=0)
+    cfg.update(T5_CONFIGS[name])
+    cfg['num_decoder_layers'] = cfg['num_layers']
+    return cfg
+
+
+def synth_t5_state_dict(cfg: dict, seed: int = 0, wi_scale: float = 1.0) -> tp.Dict[str, torch.Tensor]:
+    """Seeded fp32 T5 encoder weights in transformers' key layout, drawn with transformers' T5 init scales (q: (d d_kv)^-1/2;
+    k, v, o, wi, relative bias: d^-1/2; wo: d_ff^-1/2; embedding 1; norms 1).  Unscaled N(0, 1) weights would be meaningless
+    without T5's attention scale, which the init folds into q.  wi_scale multiplies every wi (tests of large activations)."""
+    gen = torch.Generator()
+    gen.manual_seed(seed)
+    d, dkv, ff, H, L = cfg['d_model'], cfg['d_kv'], cfg['d_ff'], cfg['num_heads'], cfg['num_layers']
+
+    def normal(shape, std):
+        return torch.randn(shape, generator=gen) * std
+
+    sd = {'shared.weight': normal((cfg['vocab_size'], d), 1.0)}
+    for i in range(L):
+        a, f = f'encoder.block.{i}.layer.0.', f'encoder.block.{i}.layer.1.'
+        sd[a + 'SelfAttention.q.weight'] = normal((H * dkv, d), (d * dkv) ** -0.5)
+        sd[a + 'SelfAttention.k.weight'] = normal((H * dkv, d), d ** -0.5)
+        sd[a + 'SelfAttention.v.weight'] = normal((H * dkv, d), d ** -0.5)
+        sd[a + 'SelfAttention.o.weight'] = normal((d, H * dkv), (H * dkv) ** -0.5)
+        if i == 0:
+            sd[a + 'SelfAttention.relative_attention_bias.weight'] = normal((cfg['relative_attention_num_buckets'], H), d ** -0.5)
+        sd[a + 'layer_norm.weight'] = torch.ones(d)
+        sd[f + 'DenseReluDense.wi.weight'] = normal((ff, d), d ** -0.5) * wi_scale
+        sd[f + 'DenseReluDense.wo.weight'] = normal((d, ff), ff ** -0.5)
+        sd[f + 'layer_norm.weight'] = torch.ones(d)
+    sd['encoder.final_layer_norm.weight'] = torch.ones(d)
+    return sd
+
+
+def write_t5_dir(path: str, cfg: dict, state_dict: tp.Dict[str, torch.Tensor], spiece_model: str, fmt: str = 'safetensors'):
+    """A local T5 directory in Hugging Face layout: config.json, model.safetensors (fmt 'safetensors') or pytorch_model.bin
+    (fmt 'bin'), and a copy of the SentencePiece model `spiece_model` as spiece.model."""
+    import json
+    import os
+    import shutil
+    os.makedirs(path, exist_ok=True)
+    with open(os.path.join(path, 'config.json'), 'w') as fh:
+        json.dump(cfg, fh, indent=1)
+    sd = {k: v.contiguous() for k, v in state_dict.items()}
+    if fmt == 'safetensors':
+        from safetensors.torch import save_file
+        save_file(sd, os.path.join(path, 'model.safetensors'))
+    elif fmt == 'bin':
+        torch.save(sd, os.path.join(path, 'pytorch_model.bin'))
+    else:
+        raise ValueError(f"fmt {fmt!r}: 'safetensors' or 'bin'")
+    shutil.copyfile(spiece_model, os.path.join(path, 'spiece.model'))
+    return path

@@ -281,6 +281,53 @@ int acb_lm_forward(const acb_lm_config* cfg, const acb_lm_weights* w, const int6
                    const float* prefix, int batch, int prefix_len, int seq_len, int text_len, float* logits,
                    void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ---------------------------------------------------------------- T5 text encoder ------------------ */
+
+/* The text conditioner of MusicGen / AudioGen (T5Conditioner, audiocraft/modules/conditioners.py:422-515): transformers'
+ * T5EncoderModel forward (a frozen t5-small / base / large) followed by output_proj and the mask:
+ *   out = (output_proj(T5(ids, mask)) * mask) */
+typedef struct {
+    int d_model;      /* multiple of 64, <= 2048 */
+    int d_kv;         /* must be 64 (t5-3b / t5-11b use 128: refused) */
+    int num_heads;    /* num_heads * d_kv == d_model */
+    int num_layers;
+    int d_ff;         /* multiple of 4; the feed-forward is wo(relu(wi(x))) */
+    int vocab_size;
+    int num_buckets;  /* relative_attention_num_buckets */
+    int out_dim;      /* output_proj out_features, multiple of 4 */
+    float eps;        /* layer_norm_epsilon */
+} acb_t5_config;
+
+/* fp32 matrices in the [out_features][in_features] layout of transformers' T5, stacked over layers; no biases but proj_b. */
+typedef struct {
+    const float* shared;   /* [vocab][d]          shared.weight */
+    const float* w_qkv;    /* [L][3d][d]          layer.0.SelfAttention.{q,k,v}.weight, stacked q, k, v */
+    const float* w_o;      /* [L][d][d]           layer.0.SelfAttention.o.weight */
+    const float* w_i;      /* [L][d_ff][d]        layer.1.DenseReluDense.wi.weight */
+    const float* w_fo;     /* [L][d][d_ff]        layer.1.DenseReluDense.wo.weight */
+    const float* ln;       /* [L][2][d]           layer.0.layer_norm.weight, layer.1.layer_norm.weight */
+    const float* final_ln; /* [d]                 encoder.final_layer_norm.weight */
+    const float* rel_bias; /* [num_buckets][H]    block.0 ... relative_attention_bias.weight, used by every layer */
+    const float* proj_w;   /* [out_dim][d]        the conditioner's output_proj.weight */
+    const float* proj_b;   /* [out_dim]           output_proj.bias */
+} acb_t5_weights;
+
+/* ids     [batch][seq_len] int64 token ids.  Precondition (not checked on the device): every id lies in [0, vocab_size).
+ * mask    [batch][seq_len] int64 attention mask (0 or 1).  Keys with mask 0 are not attended to; output rows with mask 0 are
+ *         exact zeros.  A row whose mask is all zero therefore comes out as exact zeros (its queries attend to nothing).
+ * buckets [2 seq_len - 1] int32: buckets[j - i + seq_len - 1] is the bidirectional relative-position bucket of key j seen from
+ *         query i (T5Attention._relative_position_bucket; audiocraft_b200.t5.relative_position_buckets computes it).
+ * out     [batch][seq_len][out_dim] fp32.
+ * hidden  [batch][seq_len][d] fp32 T5 last_hidden_state, or NULL.
+ * workspace: at least acb_t5_workspace_bytes(...) bytes of device memory, 256-byte aligned.
+ * GEMMs on the TF32 tensor pipe (fp32 operands, fp32 accumulation), q / k / v rounded to fp16 for the attention products,
+ * softmax and everything else fp32.  No split-K: an item's outputs are bit-identical whatever batch it is in and however
+ * far past its length the batch is padded.  Stateless, graph-capturable; all work is on `stream`. */
+int64_t acb_t5_workspace_bytes(const acb_t5_config* cfg, int batch, int seq_len);
+int acb_t5_encode(const acb_t5_config* cfg, const acb_t5_weights* w, const int64_t* ids, const int64_t* mask,
+                  const int32_t* buckets, int batch, int seq_len, float* out, float* hidden, void* workspace,
+                  int64_t workspace_bytes, void* stream);
+
 /* Stand-alone sampler (tail of _sample_next_token, lm.py:403-418; utils/utils.py:88-141) for unit tests:
  * logits [rows][n_q][card] fp32 ([cond; null] rows when rows == 2*batch), noise optional, tokens [batch][n_q]. */
 int acb_sample(const float* logits, const float* noise, int64_t* tokens, int batch, int rows, int n_q, int card,

@@ -17,7 +17,13 @@ from .conditioners import (ChromaStemConditioner, ConditionFuser, ConditioningPr
 from .encodec import EncodecModel
 from .lm import LMModel
 
-_SCALES = {'small': 'musicgen_small', 'medium': 'musicgen_medium', 'large': 'musicgen_large', 'melody': 'musicgen_melody'}
+_SCALES = {'small': 'musicgen_small', 'medium': 'musicgen_medium', 'large': 'musicgen_large', 'melody': 'musicgen_melody',
+           'stereo-small': 'musicgen_stereo_small', 'stereo-medium': 'musicgen_stereo_medium',
+           'stereo-large': 'musicgen_stereo_large', 'stereo-melody': 'musicgen_stereo_melody',
+           'stereo-melody-large': 'musicgen_stereo_melody_large'}
+# the released stereo checkpoints' xp.cfg (config/solver/musicgen/default.yaml:20-29): the codec's codebooks of both channels
+# interleaved as `b (k c) t`, 4 codebooks per channel
+_STEREO_WRAP = dict(interleave_stereo_codebooks={'use': True, 'per_timestep': False}, compression_model_n_q=4)
 
 
 def _cfg_from_yaml(text: str) -> dict:
@@ -81,6 +87,9 @@ def lm_cfg_from_xp(xp: dict) -> dict:
         unsupported.append(f"fuser.cross={fz.get('cross')}")
     if fz.get('cross_attention_pos_emb', False):
         unsupported.append('fuser.cross_attention_pos_emb')
+    isc = xp.get('interleave_stereo_codebooks') or {}
+    if isc.get('use') and isc.get('per_timestep'):
+        unsupported.append('interleave_stereo_codebooks.per_timestep=true (codes interleaved along time)')
     if unsupported:
         raise NotImplementedError("this checkpoint's LM is outside what the decode kernels implement: " + ', '.join(unsupported))
     chroma = None
@@ -251,13 +260,17 @@ def load_musicgen(name: str, device=None, seed: int = 0, text_encoder=None, stem
     if name.startswith('synthetic/'):
         lm = load_lm_model(name, device, seed, text_encoder, stem_separator)
         cm = load_compression_model('synthetic/encodec_32k', device, seed + 1)
+        if name.split('/', 1)[1].startswith('stereo-'):
+            from .encodec import get_wrapped_compression_model
+            cm = get_wrapped_compression_model(cm, **_STEREO_WRAP)
         return MusicGen(name, cm, lm, max_duration=30)
     if os.path.isdir(name):
         lm_path = os.path.join(name, 'state_dict.bin')
         lm = load_lm_model(lm_path, device, text_encoder=text_encoder, stem_separator=stem_separator)
         cm = _wrap_from_xp(load_compression_model(os.path.join(name, 'compression_state_dict.bin'), device), lm_path)
         return MusicGen(name, cm, lm, max_duration=30)
-    raise FileNotFoundError(f"MusicGen '{name}': pass a local checkpoint directory or 'synthetic/<small|medium|large>'")
+    raise FileNotFoundError(f"MusicGen '{name}': pass a local checkpoint directory or 'synthetic/<scale>' "
+                            f"({', '.join(_SCALES)})")
 
 
 def load_audiogen(name: str, device=None, seed: int = 0, text_encoder=None):

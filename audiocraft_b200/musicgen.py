@@ -168,7 +168,8 @@ class MusicGen(BaseGenModel):
         """The reference pulls checkpoints from the HF hub (musicgen.py:56-94); offline this accepts a directory holding
         the reference's exported `state_dict.bin` + `compression_state_dict.bin` (then `text_encoder` is required: a local T5
         directory in Hugging Face layout, run on the device, or a callable returning the frozen T5's hidden states and mask), or
-        `synthetic/<small|medium|large>` for seeded random weights of the released architectures."""
+        `synthetic/<small|medium|large|melody>` and `synthetic/stereo-<small|medium|large|melody|melody-large>` for seeded random
+        weights of the released architectures (the stereo ones on the interleaved stereo codec, 8 codebooks)."""
         from .loaders import load_musicgen
         return load_musicgen(name, device=device, text_encoder=text_encoder, stem_separator=stem_separator)
 

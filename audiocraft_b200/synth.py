@@ -174,6 +174,11 @@ def synth_encodec_state_dict(cfg: dict, seed: int = 0, device='cpu') -> tp.Dict[
 
 # ----------------------------------------------------------------------------- LM
 
+# stereo MusicGen (docs/MUSICGEN.md "Training stereo models", config/solver/musicgen/default.yaml:20-29): the codec's 4
+# codebooks of the left and of the right channel interleaved as `b (k c) t`, both channels of a level on the same delay
+_STEREO = dict(n_q=8, delays=[0, 0, 1, 1, 2, 2, 3, 3])
+_MELODY = dict(cross_attention=False, cond_dim=768, n_chroma=12, radix2_exp=14, duration=30.0, sample_rate=32000)
+
 LM_CONFIGS: tp.Dict[str, dict] = {
     'musicgen_small': dict(dim=1024, num_heads=16, num_layers=24),
     'musicgen_medium': dict(dim=1536, num_heads=24, num_layers=48),
@@ -189,6 +194,16 @@ LM_CONFIGS: tp.Dict[str, dict] = {
                             radix2_exp=14, duration=30.0, sample_rate=32000),
     'lm_mini_melody': dict(dim=256, num_heads=4, num_layers=3, card=2048, cond_dim=96, cross_attention=False, n_chroma=12,
                            radix2_exp=14, duration=1.0, sample_rate=32000),
+    'musicgen_stereo_small': dict(dim=1024, num_heads=16, num_layers=24, **_STEREO),
+    'musicgen_stereo_medium': dict(dim=1536, num_heads=24, num_layers=48, **_STEREO),
+    'musicgen_stereo_large': dict(dim=2048, num_heads=32, num_layers=48, **_STEREO),
+    'musicgen_stereo_melody': dict(dim=1536, num_heads=24, num_layers=48, **_MELODY, **_STEREO),
+    'musicgen_stereo_melody_large': dict(dim=2048, num_heads=32, num_layers=48, **_MELODY, **_STEREO),
+    # stereo test shapes: card 2048 keeps the released heads width n_q * card = 16384
+    'lm_mini_stereo': dict(dim=256, num_heads=4, num_layers=3, card=2048, cond_dim=96, **_STEREO),
+    'lm_medium_2l_stereo': dict(dim=1536, num_heads=24, num_layers=2, card=2048, cond_dim=64, **_STEREO),
+    'lm_mini_melody_stereo': dict(dim=256, num_heads=4, num_layers=3, card=2048, cond_dim=96, cross_attention=False,
+                                  n_chroma=12, radix2_exp=14, duration=1.0, sample_rate=32000, **_STEREO),
 }
 _LM_COMMON = dict(hidden_scale=4, n_q=4, card=2048, delays=[0, 1, 2, 3], max_period=10000.0,
                   positional_scale=1.0, cross_attention=True, cfg_coef=3.0, cond_dim=768)

@@ -27,7 +27,8 @@ Coverage: kernel instances the dispatchers can select, and the test here that ex
                                                                    test_long_text_cross_attention_matches_oracle[lm_medium_2l-8-77]
   lm_cross_attn_kernel<false>: 1 chunk (t_text 31, 32), 2 chunks (33 with a 1-position tail, 64), 3 chunks (77),
     4 chunks (100, 4-position tail)                                test_long_text_cross_attention_matches_oracle
-  lm_cross_attn_kernel<true> (prefill) at 1 chunk only             test_prefill_tail_passes_equal_token_by_token
+  lm_cross_attn_kernel<true> (prefill): 1 chunk (t_text 5), 2 chunks with a 1-position tail (33), 4 chunks (100)
+                                                                   test_prefill_tail_passes_equal_token_by_token
   LSTM recurrence (acb_lstm_recurrent), item slots in four groups 0-7, 8-15, 16-23, 24-31 (the four MMA n-tiles):
     lstm_h2_kernel (H % 128 == 0, B <= 32): H 512 / 1024 x B 16, 17, 24, 31, 32 (groups 1-4), T 1 / 2 / 37, 1 and 2 layers,
       with and without skip                                        test_lstm_h2_item_slots_match_float64
@@ -43,8 +44,9 @@ Coverage: kernel instances the dispatchers can select, and the test here that ex
   lm_gemm_kernel<8, QKV_ROPE, 1>, <1 | 2, QKV_ROPE, 2> and <1, QKV | GELU | F32, 2> (and every other decode GEMM instance the
   released widths select, with the wide GEMM) against float64 on their own inputs: test_gpu_kernels_f64.py (coverage table
   there).  <8, QKV_ROPE, 2> is selected at none of the released widths on a 132-SM H100.
-Still not executed against a reference by any test: the prefill cross-attention kernel over more than 32 text positions; the
-EnCodec-24k plan at 32 items.
+  T5 encoder (csrc/t5.cu): t5_embed_kernel, t5_rmsnorm_kernel, lm_fwd_gemm_kernel<TF32, FE_QKV | FE_RESID | FE_RELU | FE_PROJ>
+  and lm_fwd_attn_kernel<FA_T5>, each against float64 on its own inputs: test_gpu_t5_f64.py (coverage table there).
+Still not executed against a reference by any test: the EnCodec-24k plan at 32 items.
 """
 import os
 
@@ -523,18 +525,23 @@ def _prefill_passes(rows, n):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize('B,T0,pe,last', [(1, 35, 'sin', 6), (2, 22, 'sin', 24), (2, 22, 'rope', 24)],
-                         ids=['lm_mini-1-35', 'lm_mini-2-22', 'lm_mini-2-22-rope'])
-def test_prefill_tail_passes_equal_token_by_token(monkeypatch, B, T0, pe, last):
+@pytest.mark.parametrize('B,T0,pe,last,t_text', [(1, 35, 'sin', 6, 5), (2, 22, 'sin', 24, 5), (2, 22, 'rope', 24, 5),
+                                                 (2, 22, 'sin', 24, 33), (1, 35, 'rope', 6, 100)],
+                         ids=['lm_mini-1-35', 'lm_mini-2-22', 'lm_mini-2-22-rope', 'lm_mini-2-22-text33',
+                              'lm_mini-1-35-rope-text100'])
+def test_prefill_tail_passes_equal_token_by_token(monkeypatch, B, T0, pe, last, t_text):
     """Prompt prefill whose last pass holds <= 8 (token, row) pairs (NT = 1) or 17-32 pairs (NT = 4): generate prefills
     start_offset_sequence - 1 = T0 positions, 64 // rows per pass.  Same KV cache and greedy tokens as token-by-token decoding,
-    the assertions of test_prompt_prefill_equals_token_by_token."""
+    the assertions of test_prompt_prefill_equals_token_by_token.  The prefill pass's cross attention
+    (lm_cross_attn_kernel<true>) walks the text in chunks of 32 positions: one chunk at 5, a 1-position tail chunk at 33 and
+    4 chunks at 100; token-by-token decoding runs lm_cross_attn_kernel<false>, which
+    test_long_text_cross_attention_matches_oracle checks against the oracle at those lengths."""
     cfg, sd, m = _lm('lm_mini', 5, positional_embedding=pe)
     passes = _prefill_passes(2 * B, T0)
     print(f'prefill passes (token, row) pairs: {passes}')
     assert passes[-1] == last and all(p == 64 for p in passes[:-1])
     T = T0 + 6
-    _, _, cross = H.lm_condition(cfg, sd, B, 5, 1)
+    _, _, cross = H.lm_condition(cfg, sd, B, t_text, 1)
     prompt = torch.randint(0, cfg['card'], (B, 4, T0), generator=torch.Generator().manual_seed(3))
     out_pf = m.generate(prompt.cuda(), [], num_samples=B, max_gen_len=T, use_sampling=False, cross_attention_src=cross).cpu()
     kc_pf = m._bufs['k_cache'][:, :2 * B, :, :T0].clone()
@@ -547,7 +554,7 @@ def test_prefill_tail_passes_equal_token_by_token(monkeypatch, B, T0, pe, last):
     assert_close(vc_pf.float(), vc_ss.float(), 0, 4e-3, f'{pe} B={B} T0={T0} V cache')
     assert torch.equal(out_pf[..., :T0], prompt)
     agree = (out_pf == out_ss).float().mean()
-    print(f'token agreement {agree:.4f}')
+    print(f'text {t_text}: token agreement {agree:.4f}')
     assert agree > 0.95
 
 

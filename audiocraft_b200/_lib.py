@@ -79,6 +79,11 @@ def lib():
     L.acb_lstm_state_bytes.restype = i64
     L.acb_rvq_encode.argtypes = [vp, vp, vp, vp, ci, ci, ci, ci, ci, vp]
     L.acb_rvq_decode.argtypes = [vp, vp, vp, ci, ci, ci, ci, ci, vp]
+    L.acb_groupnorm_workspace_bytes.argtypes = [ci, ci, ci]
+    L.acb_groupnorm_workspace_bytes.restype = i64
+    L.acb_groupnorm_stats.argtypes = [vp, vp, vp, ci, ci, ci, cf, vp]
+    L.acb_groupnorm_apply.argtypes = [vp, vp, vp, vp, ci, ci, vp, vp, vp, vp, vp, vp, ci, ci, ci, vp]
+    L.acb_overlap_add.argtypes = [vp, vp, vp, vp] + [ci] * 7 + [vp]
     L.acb_lm_create.argtypes = [C.POINTER(LMConfig), C.POINTER(LMWeights), C.POINTER(LMBuffers), C.POINTER(vp)]
     L.acb_lm_destroy.argtypes = [vp]
     L.acb_lm_begin.argtypes = [vp, vp, ci, ci, ci, ci, C.POINTER(LMSampling), vp]
@@ -102,7 +107,8 @@ def lib():
                  'acb_lm_step_logits', 'acb_lm_launches_per_step', 'acb_lm_rows_pad', 'acb_sample',
                  'acb_device_sm_count', 'acb_lm_debug_gemms', 'acb_lm_uses_pdl',
                  'acb_conv1d_t6', 'acb_conv1d_t6_tile', 'acb_lm_prefill',
-                 'acb_resblock', 'acb_resblock_supported', 'acb_lm_forward', 'acb_t5_encode'):
+                 'acb_resblock', 'acb_resblock_supported', 'acb_lm_forward', 'acb_t5_encode', 'acb_groupnorm_stats',
+                 'acb_groupnorm_apply', 'acb_overlap_add'):
         getattr(L, name).restype = ci
     _lib = L
     return L
@@ -114,7 +120,8 @@ EXPORTS = ['acb_version', 'acb_last_error', 'acb_device_sm_count', 'acb_weight_n
            'acb_lm_destroy', 'acb_lm_begin', 'acb_lm_begin_prefix', 'acb_lm_steps', 'acb_lm_step_logits', 'acb_lm_rows_pad',
            'acb_lm_launches_per_step', 'acb_lm_debug_gemms', 'acb_lm_uses_pdl', 'acb_sample', 'acb_conv1d_t6', 'acb_conv1d_t6_tile',
            'acb_lm_prefill', 'acb_resblock', 'acb_resblock_supported', 'acb_lm_forward_workspace_bytes', 'acb_lm_forward',
-           'acb_t5_workspace_bytes', 'acb_t5_encode']
+           'acb_t5_workspace_bytes', 'acb_t5_encode', 'acb_groupnorm_workspace_bytes', 'acb_groupnorm_stats',
+           'acb_groupnorm_apply', 'acb_overlap_add']
 
 
 def check(rc: int, what: str = ''):

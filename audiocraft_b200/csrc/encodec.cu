@@ -2372,3 +2372,200 @@ extern "C" int acb_rvq_decode(const int64_t* codes, const float* codebooks, floa
     ACB_LAUNCH_CHECK();
     return ACB_OK;
 }
+
+// ------------------------------------------------------------------------------------------------
+// GroupNorm(1, C) of a SEANet layer output (norm='time_group_norm', modules/conv.py:33-42; NormConv1d /
+// NormConvTranspose1d apply it after the convolution and, for the transposed conv, before the trim).
+// Statistics of item b over its C*T elements in two deterministic passes: GN_PART blocks per item
+// (a count that depends on C*T only, never on the batch) each reduce a fixed contiguous slice in a
+// fixed order into fp64 sums of x - x[b][0][0] (shifted by the item's first sample, so a large mean
+// does not cancel the variance), then one warp per item combines the partials in a fixed order.
+// ------------------------------------------------------------------------------------------------
+constexpr int GN_THREADS = 256;
+constexpr int GN_MAX_PARTS = 256;
+
+static int gn_parts(long long n) {
+    long long p = (n + 16383) / 16384;   // >= 16 K elements per block
+    return (int)(p < 1 ? 1 : (p > GN_MAX_PARTS ? GN_MAX_PARTS : p));
+}
+
+__global__ void __launch_bounds__(GN_THREADS) groupnorm_partial_kernel(const float* __restrict__ x, double2* __restrict__ part,
+                                                                        long long n, int parts) {
+    __shared__ double2 red[GN_THREADS / 32];
+    const int p = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
+    const float* xb = x + (size_t)b * n;
+    const long long chunk = (n + parts - 1) / parts;
+    const long long lo = (long long)p * chunk, hi = min(n, lo + chunk);
+    const double shift = (double)__ldg(xb);
+    double s1 = 0.0, s2 = 0.0;
+    long long i = lo + tid;
+    for (; i + 3 * GN_THREADS < hi; i += 4 * GN_THREADS) {   // four independent loads in flight per thread
+        float v[4];
+#pragma unroll
+        for (int u = 0; u < 4; ++u) v[u] = __ldg(xb + i + u * GN_THREADS);
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+            const double d = (double)v[u] - shift;
+            s1 += d;
+            s2 = fma(d, d, s2);
+        }
+    }
+    for (; i < hi; i += GN_THREADS) {
+        const double d = (double)__ldg(xb + i) - shift;
+        s1 += d;
+        s2 = fma(d, d, s2);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+        s2 += __shfl_xor_sync(0xffffffffu, s2, o);
+    }
+    if ((tid & 31) == 0) red[tid >> 5] = make_double2(s1, s2);
+    __syncthreads();
+    if (tid == 0) {
+        double a = 0.0, q = 0.0;
+        for (int w = 0; w < GN_THREADS / 32; ++w) { a += red[w].x; q += red[w].y; }
+        part[(size_t)b * parts + p] = make_double2(a, q);
+    }
+}
+
+__global__ void groupnorm_finalize_kernel(const float* __restrict__ x, const double2* __restrict__ part, double2* __restrict__ stats,
+                                          long long n, int parts, int batch, float eps) {
+    const int b = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (b >= batch) return;
+    double s1 = 0.0, s2 = 0.0;
+    for (int p = lane; p < parts; p += 32) {
+        const double2 v = part[(size_t)b * parts + p];
+        s1 += v.x;
+        s2 += v.y;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+        s2 += __shfl_xor_sync(0xffffffffu, s2, o);
+    }
+    if (lane == 0) {
+        const double m = s1 / (double)n;
+        const double var = fmax(s2 / (double)n - m * m, 0.0);   // biased variance, as nn.GroupNorm
+        stats[b] = make_double2((double)x[(size_t)b * n] + m, 1.0 / sqrt(var + (double)eps));
+    }
+}
+
+extern "C" int64_t acb_groupnorm_workspace_bytes(int batch, int channels, int t_len) {
+    if (batch <= 0 || channels <= 0 || t_len <= 0) return 0;
+    return (int64_t)batch * gn_parts((long long)channels * t_len) * (int64_t)sizeof(double2);
+}
+
+extern "C" int acb_groupnorm_stats(const float* x, void* workspace, double* stats, int batch, int channels, int t_len, float eps,
+                                   void* stream) {
+    ACB_REQUIRE(x && workspace && stats, "acb_groupnorm_stats: null pointer");
+    ACB_REQUIRE(batch > 0 && batch <= 65535 && channels > 0 && t_len > 0, "acb_groupnorm_stats: bad shape");
+    ACB_REQUIRE(eps >= 0.f, "acb_groupnorm_stats: eps < 0");
+    const long long n = (long long)channels * t_len;
+    const int parts = gn_parts(n);
+    cudaStream_t s = (cudaStream_t)stream;
+    groupnorm_partial_kernel<<<dim3(parts, batch), GN_THREADS, 0, s>>>(x, (double2*)workspace, n, parts);
+    ACB_LAUNCH_CHECK();
+    groupnorm_finalize_kernel<<<acb_ceil_div(batch, 8), 256, 0, s>>>(x, (const double2*)workspace, (double2*)stats, n, parts, batch,
+                                                                   eps);
+    ACB_LAUNCH_CHECK();
+    return ACB_OK;
+}
+
+// y = gamma_c (x[left + t] - mean_b) rstd_b + beta_c, plus either a second GroupNorm output of the same shape (the conv shortcut of a
+// residual block) or a raw tensor (the identity skip).  x - mean in fp64: the mean can be far larger than the spread.
+struct GnApplyParams {
+    const float* x; const double2* st; const float* g; const float* be; int t_src, left;
+    const float* x2; const double2* st2; const float* g2; const float* be2;
+    const float* res; float* y; int C, t_out;
+};
+
+__device__ __forceinline__ float gn_norm(float v, double2 st, float g, float be) {
+    return fmaf(g * (float)st.y, (float)((double)v - st.x), be);
+}
+
+__global__ void __launch_bounds__(256) groupnorm_apply_kernel(GnApplyParams p) {
+    const int c = blockIdx.y, b = blockIdx.z;
+    const size_t row = (size_t)b * p.C + c;
+    const double2 st = p.st[b];
+    const float g = p.g[c], be = p.be[c];
+    const float* xr = p.x + row * p.t_src + p.left;
+    float* yr = p.y + row * p.t_out;
+    double2 st2 = make_double2(0.0, 0.0);
+    float g2 = 0.f, be2 = 0.f;
+    if (p.x2) { st2 = p.st2[b]; g2 = p.g2[c]; be2 = p.be2[c]; }
+    const int t0 = blockIdx.x * (256 * 4) + threadIdx.x;
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+        const int t = t0 + u * 256;
+        if (t >= p.t_out) break;
+        float v = gn_norm(__ldg(xr + t), st, g, be);
+        if (p.x2) v += gn_norm(__ldg(p.x2 + row * p.t_out + t), st2, g2, be2);
+        else if (p.res) v += __ldg(p.res + row * p.t_out + t);
+        yr[t] = v;
+    }
+}
+
+extern "C" int acb_groupnorm_apply(const float* x, const double* stats, const float* gamma, const float* beta, int t_src, int left,
+                                   const float* x2, const double* stats2, const float* gamma2, const float* beta2, const float* residual,
+                                   float* y, int batch, int channels, int t_out, void* stream) {
+    ACB_REQUIRE(x && stats && gamma && beta && y, "acb_groupnorm_apply: null pointer");
+    ACB_REQUIRE(batch > 0 && batch <= 65535 && channels > 0 && channels <= 65535 && t_out > 0, "acb_groupnorm_apply: bad shape");
+    ACB_REQUIRE(left >= 0 && left + t_out <= t_src, "acb_groupnorm_apply: window [%d, %d) outside %d steps", left, left + t_out, t_src);
+    ACB_REQUIRE(!(x2 && residual), "acb_groupnorm_apply: x2 and residual are exclusive");
+    ACB_REQUIRE(!x2 || (stats2 && gamma2 && beta2), "acb_groupnorm_apply: x2 needs stats2, gamma2, beta2");
+    ACB_REQUIRE(y != x && y != x2 && y != residual, "acb_groupnorm_apply: y must not alias an input");
+    GnApplyParams p{x, (const double2*)stats, gamma, beta, t_src, left, x2, (const double2*)stats2, gamma2, beta2, residual, y,
+                    channels, t_out};
+    groupnorm_apply_kernel<<<dim3(acb_ceil_div(t_out, 256 * 4), channels, batch), 256, 0, (cudaStream_t)stream>>>(p);
+    ACB_LAUNCH_CHECK();
+    return ACB_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// Overlap-add of independently decoded chunks (transformers EncodecModel._linear_overlap_add, as the reference's
+// HFEncodecCompressionModel runs the 48 kHz codec): chunk i starts at i*stride, is multiplied by its scale, weighted by the
+// triangle w(j) = 0.5 - |(j+1)/(L+1) - 0.5| (L = length of the first chunk) and the sum is divided by the summed weights.
+// frames = chunks 0 .. n-2, [n-1][B][C][t_frame]; last = chunk n-1, [B][C][t_last]; scales [n][B] or NULL.
+// ------------------------------------------------------------------------------------------------
+struct OlaParams {
+    const float* frames; const float* last; const float* scales; float* y;
+    int n, B, C, t_frame, t_last, stride, t_total, L;
+};
+
+__global__ void __launch_bounds__(256) overlap_add_kernel(OlaParams p) {
+    const int t = blockIdx.x * 256 + threadIdx.x, c = blockIdx.y, b = blockIdx.z;
+    if (t >= p.t_total) return;
+    const double inv = 1.0 / (double)(p.L + 1);
+    float acc = 0.f, wsum = 0.f;
+    for (int i = min(p.n - 1, t / p.stride); i >= 0; --i) {
+        const int j = t - i * p.stride;
+        const bool is_last = i == p.n - 1;
+        if (j >= (is_last ? p.t_last : p.t_frame)) {
+            if (j >= p.t_frame) break;   // every earlier chunk ends earlier still
+            continue;
+        }
+        const float w = (float)(0.5 - fabs((double)(j + 1) * inv - 0.5));
+        const float v = is_last ? __ldg(p.last + ((size_t)b * p.C + c) * p.t_last + j)
+                                : __ldg(p.frames + (((size_t)i * p.B + b) * p.C + c) * p.t_frame + j);
+        const float sc = p.scales ? __ldg(p.scales + (size_t)i * p.B + b) : 1.f;
+        acc = fmaf(w, v * sc, acc);
+        wsum += w;
+    }
+    p.y[((size_t)b * p.C + c) * p.t_total + t] = acc / wsum;
+}
+
+extern "C" int acb_overlap_add(const float* frames, const float* last, const float* scales, float* y, int n_chunks, int batch,
+                               int channels, int t_frame, int t_last, int stride, int t_total, void* stream) {
+    ACB_REQUIRE(last && y && (n_chunks == 1 || frames), "acb_overlap_add: null pointer");
+    ACB_REQUIRE(n_chunks >= 1 && batch > 0 && batch <= 65535 && channels > 0 && channels <= 65535 && stride > 0 && t_last > 0,
+                "acb_overlap_add: bad shape");
+    ACB_REQUIRE(n_chunks == 1 || (t_frame >= t_last && t_frame >= stride),
+                "acb_overlap_add: chunks of %d steps at stride %d leave gaps (last %d)", t_frame, stride, t_last);
+    ACB_REQUIRE((long long)stride * (n_chunks - 1) + t_last == t_total, "acb_overlap_add: t_total != stride*(n-1) + t_last");
+    OlaParams p{frames, last, scales, y, n_chunks, batch, channels, n_chunks > 1 ? t_frame : t_last, t_last, stride, t_total,
+                n_chunks > 1 ? t_frame : t_last};
+    overlap_add_kernel<<<dim3(acb_ceil_div(t_total, 256), channels, batch), 256, 0, (cudaStream_t)stream>>>(p);
+    ACB_LAUNCH_CHECK();
+    return ACB_OK;
+}

@@ -10,6 +10,7 @@ PyTorch here is plumbing only (device memory, streams).  There is no CPU path: w
 or a GPU, construction raises.
 """
 import math
+import os
 import typing as tp
 from abc import ABC, abstractmethod
 
@@ -71,7 +72,11 @@ class CompressionModel(ABC):
     def get_pretrained(name: str, device='cuda') -> 'CompressionModel':
         """The reference downloads checkpoints from the HF hub (encodec.py:87-122).  There is no network here:
         `name` may be a local checkpoint file in the reference's export format
-        ({'best_state', 'xp.cfg'} -- audiocraft/utils/export.py:20-79) or one of the synthetic architectures."""
+        ({'best_state', 'xp.cfg'} -- audiocraft/utils/export.py:20-79), a local directory holding a transformers EnCodec
+        snapshot (config.json + weights, what the reference reaches for `facebook/encodec_*`), or one of the synthetic
+        architectures."""
+        if os.path.isdir(name) and os.path.isfile(os.path.join(name, 'config.json')):
+            return HFEncodecCompressionModel.from_pretrained_dir(name, device=device)
         from .loaders import load_compression_model
         return load_compression_model(name, device=device)
 
@@ -134,6 +139,21 @@ def pack_conv_t6(w: torch.Tensor, tile: int) -> torch.Tensor:
     return t.permute(1, 3, 6, 0, 4, 2, 5).contiguous()                      # tile, cg, k, term, c, n, j
 
 
+def check_norm(cfg: dict) -> float:
+    """The conv normalisations the kernels run (CONV_NORMALIZATIONS, audiocraft/modules/conv.py:17-42): 'weight_norm'
+    (folded at load), 'none', and 'time_group_norm' = GroupNorm(1, C) after every convolution, which the reference refuses
+    on a causal model.  Anything else raises here rather than running the codec without its norm.  Returns the GroupNorm eps."""
+    norm = cfg.get('norm', 'weight_norm')
+    params = dict(cfg.get('norm_params') or {})
+    if norm not in ('weight_norm', 'none', 'time_group_norm'):
+        raise NotImplementedError(f"conv norm '{norm}' is not built (weight_norm, none and time_group_norm are)")
+    if norm == 'time_group_norm' and cfg['causal']:
+        raise ValueError("GroupNorm doesn't support causal evaluation.")   # get_norm_module, conv.py:37-38
+    if set(params) - {'eps'}:
+        raise NotImplementedError(f"norm_params {sorted(set(params) - {'eps'})} are not built (only eps)")
+    return float(params.get('eps', 1e-5))
+
+
 class EncodecModel(CompressionModel):
     """EnCodec (SEANet + RVQ) on H100 behind the reference's ``EncodecModel`` API."""
 
@@ -151,6 +171,7 @@ class EncodecModel(CompressionModel):
           'tf32x3_flush' the same kernel on every layer it supports (slower on 1x1 convolutions; kept for tests);
           'tf32x3'       (decoder default, NOT fp32-exact) wgmma 3xTF32 without flushes: the decoder's output is a waveform
                          checked to a tolerance of 1e-4 (DESIGN.md section 4); as an encoder mode its latents move by 1.5e-4."""
+        self._gn_eps = check_norm(cfg)
         self.device = _lib.require_cuda(device)
         prec = {'fp32': _lib.CONV_FP32, 'tf32x3': _lib.CONV_TF32X3, 'tf32x3_mmasync': _lib.CONV_TF32X3_MMASYNC,
                 'tf32x3_flush': _lib.CONV_T6_FLUSH, 'fp32_tc': _lib.CONV_T6_AUTO}
@@ -201,6 +222,14 @@ class EncodecModel(CompressionModel):
     def _prepare(self, layer: dict, sd) -> dict:
         out = dict(layer)
         p = layer['prefix']
+        if layer['kind'] in ('conv', 'convtr'):
+            # NormConv1d / NormConvTranspose1d hold the GroupNorm next to the conv (modules/conv.py:91-137): `...conv.norm.*`.
+            # Read per layer from the weights, so blocks the reference builds with norm='none' (disable_norm_outer_blocks) have none
+            n = p.rsplit('.', 2)[0] + '.norm.'
+            out['gn'] = n + 'weight' in sd
+            if out['gn']:
+                out['gn_g'] = sd[n + 'weight'].to(self.device, torch.float32).contiguous()
+                out['gn_b'] = sd[n + 'bias'].to(self.device, torch.float32).contiguous()
         if layer['kind'] == 'conv':
             w = self._fold(sd, p)                                       # [Cout][Cin][K]
             out['w'] = w.permute(1, 2, 0).reshape(-1, w.shape[0]).contiguous()   # [Cin*K][Cout]
@@ -256,9 +285,12 @@ class EncodecModel(CompressionModel):
         self.launches += 1
         return y
 
-    def _convtr(self, x, L, prec=0):
+    def _convtr(self, x, L, prec=0, trim=True):
+        """trim=False: the full transposed-conv output (the GroupNorm statistics cover the steps the trim drops)."""
         B, cin, T = x.shape
         trim_left, t_out = convtr_geometry(T, L['k'], L['stride'], self.causal, self.cfg['trim_right_ratio'])
+        if not trim:
+            trim_left, t_out = 0, (T - 1) * L['stride'] + L['k']
         y = torch.empty((B, L['cout'], t_out), device=x.device, dtype=torch.float32)
         if prec in (_lib.CONV_T6_FLUSH, _lib.CONV_T6_AUTO):
             prec = _lib.CONV_TF32X3        # transposed convs have no implicit-GEMM variant yet
@@ -312,7 +344,69 @@ class EncodecModel(CompressionModel):
         self.launches += 1
         return y
 
+    def _gn_stats(self, y):
+        B, C, T = y.shape
+        ws = torch.empty(int(self._lib.acb_groupnorm_workspace_bytes(B, C, T)), device=y.device, dtype=torch.uint8)
+        st = torch.empty((B, 2), device=y.device, dtype=torch.float64)
+        _lib.check(self._lib.acb_groupnorm_stats(_lib.ptr(y), _lib.ptr(ws), _lib.ptr(st), B, C, T, self._gn_eps, _lib.stream()),
+                   'groupnorm_stats')
+        self.launches += 2
+        return st
+
+    def _gn_apply(self, y, L, st, left=0, t_out=None, add=None):
+        """GroupNorm of the conv output y (window [left, left + t_out)), plus `add`: a tensor (identity skip) or the
+        (raw output, stats, layer) of a conv shortcut whose GroupNorm is applied here too."""
+        B, C, T = y.shape
+        t_out = T if t_out is None else t_out
+        out = torch.empty((B, C, t_out), device=y.device, dtype=torch.float32)
+        x2 = st2 = g2 = b2 = res = None
+        if isinstance(add, tuple):
+            x2, st2, L2 = add
+            g2, b2 = L2['gn_g'], L2['gn_b']
+        else:
+            res = add
+        _lib.check(self._lib.acb_groupnorm_apply(_lib.ptr(y), _lib.ptr(st), _lib.ptr(L['gn_g']), _lib.ptr(L['gn_b']), T, left,
+                                                 _lib.ptr(x2), _lib.ptr(st2), _lib.ptr(g2), _lib.ptr(b2), _lib.ptr(res),
+                                                 _lib.ptr(out), B, C, t_out, _lib.stream()), 'groupnorm_apply')
+        self.launches += 1
+        return out
+
+    def _run_gn(self, x, layers, prec):
+        """Layer order of a GroupNorm model: each conv runs without its residual epilogue, then the statistics of its output,
+        then the apply kernel, which also adds the block's skip; the skip is added after both GroupNorms
+        (SEANetResnetBlock.forward: shortcut(x) + block(x), modules/seanet.py:59-60)."""
+        skip, have_shortcut = None, False
+        for L in layers:
+            if L['kind'] == 'lstm':
+                x = self._lstm(x, L, prec=self._lstm_prec)
+            elif L['kind'] == 'convtr':
+                if not L['gn']:
+                    x = self._convtr(x, L, prec=prec)
+                    continue
+                left, t_out = convtr_geometry(x.shape[-1], L['k'], L['stride'], self.causal, self.cfg['trim_right_ratio'])
+                full = self._convtr(x, L, prec=prec, trim=False)
+                x = self._gn_apply(full, L, self._gn_stats(full), left=left, t_out=t_out)
+            elif L['res'] == 'shortcut':
+                s = self._conv(x, L, prec=prec)
+                skip = (s, self._gn_stats(s), L) if L['gn'] else s
+                have_shortcut = True
+            else:
+                if L['res'] == 'in':
+                    if not have_shortcut:
+                        skip = x
+                    have_shortcut = False
+                add = skip if L['res'] == 'out' else None
+                if not L['gn']:
+                    assert not isinstance(add, tuple), 'a residual block with a GroupNorm on only one branch'
+                    x = self._conv(x, L, res=add, prec=prec)
+                    continue
+                y = self._conv(x, L, prec=prec)
+                x = self._gn_apply(y, L, self._gn_stats(y), add=add)
+        return x
+
     def _run(self, x, layers, prec=0):
+        if any(L.get('gn') for L in layers):
+            return self._run_gn(x, layers, prec)
         skip, have_shortcut = None, False
         prof = getattr(self, '_profile', None)   # optional per-layer CUDA-event timing (profiles/perf_encodec.py)
         skip_next = False
@@ -412,12 +506,13 @@ class EncodecModel(CompressionModel):
         with torch.cuda.device(self.device):
             return self._run(self._in(x), self.enc, self._enc_prec)
 
-    def quantize(self, emb):
-        """ResidualVectorQuantizer.encode (vq.py:87-96): latent [B,D,T] -> codes [B,n_q,T] int64."""
+    def quantize(self, emb, n_q=None):
+        """ResidualVectorQuantizer.encode (vq.py:87-96): latent [B,D,T] -> codes [B,n_q,T] int64 (n_q: default the active count)."""
         B, D, T = emb.shape
-        codes = torch.empty((B, self.n_q, T), device=emb.device, dtype=torch.int64)
+        n_q = self.n_q if n_q is None else n_q
+        codes = torch.empty((B, n_q, T), device=emb.device, dtype=torch.int64)
         _lib.check(self._lib.acb_rvq_encode(_lib.ptr(emb.contiguous()), _lib.ptr(self.codebooks),
-                                            _lib.ptr(self.cb_sqnorm), _lib.ptr(codes), B, D, T, self.n_q, self.bins,
+                                            _lib.ptr(self.cb_sqnorm), _lib.ptr(codes), B, D, T, n_q, self.bins,
                                             _lib.stream()), 'rvq_encode')
         self.launches += 1
         return codes
@@ -573,12 +668,13 @@ def hf_encodec_to_reference(hf_state_dict: tp.Dict[str, torch.Tensor], hf_config
     """Translate a `transformers.EncodecModel` checkpoint (what the reference loads for `facebook/encodec_*` through
     `HFEncodecCompressionModel`, audiocraft/models/encodec.py:119-121, 323-392) into the reference's own state_dict layout +
     hyper-parameters.  HF's implementation is the same algorithm with renamed modules
-    (transformers/models/encodec/modeling_encodec.py), so the converted weights run on the kernels unchanged."""
+    (transformers/models/encodec/modeling_encodec.py), so the converted weights run on the kernels unchanged.
+    norm_type 'time_group_norm' (the 48 kHz codec) maps `*.norm.{weight,bias}` to the reference's `...conv.norm.*` /
+    `...convtr.norm.*`; its chunking (chunk_length_s / overlap) is carried in cfg as chunk_length / chunk_stride."""
     c = hf_config
-    if getattr(c, 'norm_type', 'weight_norm') != 'weight_norm':
-        raise NotImplementedError(f"HF EnCodec norm_type '{c.norm_type}' is not built (only weight_norm)")
-    if getattr(c, 'chunk_length_s', None):
-        raise NotImplementedError("chunked HF EnCodec (48 kHz) is not built")
+    norm = getattr(c, 'norm_type', 'weight_norm')
+    if norm not in ('weight_norm', 'time_group_norm'):
+        raise NotImplementedError(f"HF EnCodec norm_type '{norm}' is not built (weight_norm, time_group_norm)")
     hop = int(math.prod(c.upsampling_ratios))
     frame_rate = math.ceil(c.sampling_rate / hop)
     n_qs = [int(bw * 1000 // (frame_rate * math.log2(c.codebook_size))) for bw in c.target_bandwidths]
@@ -586,9 +682,12 @@ def hf_encodec_to_reference(hf_state_dict: tp.Dict[str, torch.Tensor], hf_config
                n_residual_layers=c.num_residual_layers, ratios=list(c.upsampling_ratios), kernel_size=c.kernel_size,
                last_kernel_size=c.last_kernel_size, residual_kernel_size=c.residual_kernel_size,
                dilation_base=c.dilation_growth_rate, causal=c.use_causal_conv, pad_mode=c.pad_mode, compress=c.compress,
-               lstm=c.num_lstm_layers, norm='weight_norm', trim_right_ratio=c.trim_right_ratio,
+               lstm=c.num_lstm_layers, norm=norm, trim_right_ratio=c.trim_right_ratio,
                sample_rate=c.sampling_rate, n_q=max(n_qs), bins=c.codebook_size, renormalize=c.normalize,
-               true_skip=not c.use_conv_shortcut, possible_num_codebooks=n_qs)
+               true_skip=not c.use_conv_shortcut, possible_num_codebooks=n_qs,
+               target_bandwidths=list(c.target_bandwidths), chunk_length=c.chunk_length, chunk_stride=c.chunk_stride)
+    if norm == 'time_group_norm':
+        cfg['norm_params'] = dict(eps=1e-5)   # nn.GroupNorm's default, which transformers' EncodecConv1d keeps
     plan = encodec_layers(cfg)
     kinds = {}
     for layer in plan['encoder'] + plan['decoder']:
@@ -603,28 +702,60 @@ def hf_encodec_to_reference(hf_state_dict: tp.Dict[str, torch.Tensor], hf_config
             rest = rest.replace('parametrizations.weight.original0', 'weight_g').replace('parametrizations.weight.original1', 'weight_v')
             if rest.startswith('lstm.'):
                 sd[f'{side}.model.{idx}.{rest}'] = v
-            elif rest.startswith(('block.', 'shortcut.')):
-                head, tail = rest.split('.conv.', 1)
-                sd[f'{side}.model.{idx}.{head}.conv.conv.{tail}'] = v
-            else:  # rest = 'conv.<param>'
-                tail = rest.split('conv.', 1)[1]
-                inner = 'convtr.convtr' if kinds.get((side, idx)) == 'convtr' else 'conv.conv'
-                sd[f'{side}.model.{idx}.{inner}.{tail}'] = v
+                continue
+            toks = rest.split('.')
+            if toks[0] == 'block':               # block.<j>.{conv,norm}.<param> -> block.<j>.conv.{conv,norm}.<param>
+                outer, mod, tail = f'block.{toks[1]}.conv', toks[2], toks[3:]
+            elif toks[0] == 'shortcut':          # shortcut.{conv,norm}.<param> -> shortcut.conv.{conv,norm}.<param>
+                outer, mod, tail = 'shortcut.conv', toks[1], toks[2:]
+            else:                                # {conv,norm}.<param> -> {conv,convtr}.{conv,convtr,norm}.<param>
+                outer = 'convtr' if kinds.get((side, idx)) == 'convtr' else 'conv'
+                mod, tail = toks[0], toks[1:]
+            inner = outer.split('.')[-1] if mod == 'conv' else 'norm'
+            sd[f'{side}.model.{idx}.{outer}.{inner}.{".".join(tail)}'] = v
         elif parts[0] == 'quantizer':
             sd[f'quantizer.vq.layers.{parts[2]}._codebook.{parts[4]}'] = v
     return sd, cfg
 
 
+def chunk_bounds(length: int, chunk_length: tp.Optional[int], chunk_stride: tp.Optional[int]) -> tp.List[tp.Tuple[int, int]]:
+    """[start, end) of each chunk transformers' EncodecModel.encode cuts: offsets 0, stride, 2*stride, ... < length, each
+    chunk_length long or cut by the end of the input; one chunk when the codec is not chunked."""
+    if chunk_length is None:
+        return [(0, length)]
+    return [(o, min(o + chunk_length, length)) for o in range(0, length, chunk_stride)]
+
+
+class _HFEncodecAPI:
+    """`HFEncodecCompressionModel.model`: transformers' `EncodecModel.encode` / `.decode` (return_dict=False results), on the
+    kernels.  This is what the reference's users call for audio longer than one chunk of a chunked codec."""
+
+    def __init__(self, owner: 'HFEncodecCompressionModel', config):
+        self._m = owner
+        self.config = config
+
+    def encode(self, input_values, padding_mask=None, bandwidth=None):
+        """-> (audio_codes [n_chunks, B, K, frame_len], audio_scales: list of n_chunks [B, 1] (or None), last_frame_pad_length)."""
+        return self._m._encode_chunks(input_values, padding_mask, bandwidth)
+
+    def decode(self, audio_codes, audio_scales, padding_mask=None, last_frame_pad_length=0):
+        """-> (audio_values [B, C, T],)."""
+        return (self._m._decode_chunks(audio_codes, audio_scales, padding_mask, last_frame_pad_length),)
+
+
 class HFEncodecCompressionModel(EncodecModel):
     """`facebook/encodec_*` checkpoints on the CUDA kernels: same surface as the reference's wrapper
     (audiocraft/models/encodec.py:323-392), incl. the restriction of `set_num_codebooks` to the bandwidths the
-    checkpoint declares."""
+    checkpoint declares.  The 48 kHz codec cuts audio into 1 s chunks (stride 47 520) that are renormalised, encoded and
+    decoded independently and joined by a linear overlap-add; all chunks of one length go through the kernels as one batch
+    of items.  `.model.encode` / `.model.decode` take full-length audio, as transformers' model does."""
 
     def __init__(self, hf_state_dict, hf_config, device='cuda', **kw):
         sd, cfg = hf_encodec_to_reference(hf_state_dict, hf_config)
         super().__init__(sd, cfg, device, **kw)
         self.possible_num_codebooks = cfg['possible_num_codebooks']
         self.set_num_codebooks(max(self.possible_num_codebooks))
+        self.model = _HFEncodecAPI(self, hf_config)
 
     @property
     def frame_rate(self):
@@ -634,6 +765,86 @@ class HFEncodecCompressionModel(EncodecModel):
         if n not in self.possible_num_codebooks:
             raise ValueError(f"Allowed values for num codebooks: {self.possible_num_codebooks}")
         self.n_q = n
+
+    def _n_q_for_bandwidth(self, bandwidth):
+        """EncodecResidualVectorQuantizer.get_num_quantizers_for_bandwidth, behind EncodecModel.encode's bandwidth check."""
+        bws = self.cfg['target_bandwidths']
+        if bandwidth is None:
+            bandwidth = bws[0]
+        if bandwidth not in bws:
+            raise ValueError(f"This model doesn't support the bandwidth {bandwidth}. Select one of {bws}.")
+        bw_per_q = math.log2(self.bins) * math.ceil(self.sample_rate / encodec_hop(self.cfg))
+        return int(max(1, math.floor(bandwidth * 1000 / bw_per_q)))
+
+    def _encode_chunks(self, x, padding_mask=None, bandwidth=None):
+        n_q = self._n_q_for_bandwidth(bandwidth)
+        with torch.cuda.device(self.device):
+            x = self._in(x)
+            if padding_mask is not None:
+                x = x * padding_mask.to(self.device).view(x.shape[0], -1, x.shape[-1]).bool()
+            bounds = chunk_bounds(x.shape[-1], self.cfg['chunk_length'], self.cfg['chunk_stride'])
+            codes, scales = [None] * len(bounds), [None] * len(bounds)
+            for length in sorted({e - s for s, e in bounds}, reverse=True):   # one batch of items per chunk length
+                idx = [i for i, (s, e) in enumerate(bounds) if e - s == length]
+                batch = torch.cat([x[..., bounds[i][0]:bounds[i][1]] for i in idx]).contiguous()   # [chunk][item]
+                batch, scale = self.preprocess(batch)
+                c = self.quantize(self._run(batch.contiguous(), self.enc, self._enc_prec), n_q)
+                for j, i in enumerate(idx):
+                    codes[i] = c[j * x.shape[0]:(j + 1) * x.shape[0]]
+                    scales[i] = None if scale is None else scale[j * x.shape[0]:(j + 1) * x.shape[0]]
+            frames = codes[0].shape[-1]
+            if any(c.shape[-1] != frames for c in codes[:-1]):
+                raise ValueError(f"input length {x.shape[-1]} gives chunks of {[c.shape[-1] for c in codes]} frames: every chunk "
+                                 "but the last must have as many frames as the first")
+            pad = frames - codes[-1].shape[-1]
+            if pad > 0:
+                codes[-1] = torch.nn.functional.pad(codes[-1], (0, pad), value=0)
+            return torch.stack(codes), scales, pad
+
+    def _decode_chunks(self, audio_codes, audio_scales, padding_mask=None, last_frame_pad_length=0):
+        n = len(audio_codes)
+        if self.cfg['chunk_length'] is None and n != 1:
+            raise ValueError(f"Expected one frame, got {n}")
+        pad = last_frame_pad_length or 0
+        with torch.cuda.device(self.device):
+            codes = audio_codes.to(self.device, torch.int64)
+            scales = [audio_scales[i] for i in range(n)]
+            last = self._run(self.decode_latent(codes[-1][..., :codes.shape[-1] - pad]), self.dec, self._dec_prec)
+            B = last.shape[0]
+            if self.cfg['chunk_length'] is None:
+                out = last if scales[0] is None else last * scales[0].to(self.device).view(-1, 1, 1)
+            else:
+                full = None
+                if n > 1:
+                    full = self._run(self.decode_latent(codes[:-1].reshape(-1, *codes.shape[2:])), self.dec, self._dec_prec)
+                sc = None
+                if scales[0] is not None:
+                    sc = torch.stack([s.to(self.device, torch.float32).reshape(-1).expand(B) for s in scales]).contiguous()
+                t_frame = full.shape[-1] if full is not None else last.shape[-1]
+                stride = self.cfg['chunk_stride']
+                t_total = stride * (n - 1) + last.shape[-1]
+                out = torch.empty((B, last.shape[1], t_total), device=self.device, dtype=torch.float32)
+                _lib.check(self._lib.acb_overlap_add(_lib.ptr(full), _lib.ptr(last), _lib.ptr(sc), _lib.ptr(out), n, B,
+                                                     last.shape[1], t_frame, last.shape[-1], stride, t_total, _lib.stream()),
+                           'overlap_add')
+                self.launches += 1
+            if padding_mask is not None and padding_mask.shape[-1] < out.shape[-1]:
+                out = out[..., :padding_mask.shape[-1]]
+            return out
+
+    def encode(self, x):
+        """encodec.py:347-353: one chunk only; longer input goes through `.model.encode`."""
+        bandwidth = self.cfg['target_bandwidths'][self.possible_num_codebooks.index(self.num_codebooks)]
+        n = len(chunk_bounds(x.shape[-1], self.cfg['chunk_length'], self.cfg['chunk_stride']))
+        assert n == 1, (f"input of {x.shape[-1]} samples spans {n} chunks of {self.cfg['chunk_length']}: the reference wrapper "
+                        "encodes one chunk (`assert len(res[0]) == 1`); use `.model.encode` / `.model.decode` for longer audio")
+        codes, scales, _ = self.model.encode(x, None, bandwidth)
+        return codes[0], scales[0]
+
+    def decode(self, codes, scale=None):
+        """encodec.py:355-361: `self.model.decode(codes[None], scale)`.  The reference passes the [B, 1] scale where transformers
+        expects one [B, 1] scale per chunk, so chunk 0 takes row 0: item 0's scale is applied to EVERY item (kept as written)."""
+        return self.model.decode(codes[None], [None] if scale is None else scale)[0]
 
     @staticmethod
     def from_pretrained_dir(path: str, device='cuda'):

@@ -156,7 +156,7 @@ def _melody_parts(cfg: dict, text_encoder, stem_separator, device):
 def load_compression_model(name: str, device='cuda', seed: int = 0) -> EncodecModel:
     if name.startswith('synthetic/'):
         arch = name.split('/', 1)[1]
-        cfg = synth.ENCODEC_CONFIGS[arch]
+        cfg = synth.ENCODEC_CONFIGS.get(arch) or synth.ENCODEC_GN_CONFIGS[arch]
         return EncodecModel(synth.synth_encodec_state_dict(cfg, seed), cfg, device)
     if os.path.isfile(name):
         pkg = _load_pkg(name)
@@ -169,7 +169,7 @@ def load_compression_model(name: str, device='cuda', seed: int = 0) -> EncodecMo
                    kernel_size=sea['kernel_size'], last_kernel_size=sea['last_kernel_size'],
                    residual_kernel_size=sea['residual_kernel_size'], dilation_base=sea['dilation_base'],
                    causal=xp['encodec']['causal'], pad_mode=sea['pad_mode'], compress=sea['compress'],
-                   lstm=sea['lstm'], norm=sea['norm'],
+                   lstm=sea['lstm'], norm=sea['norm'], norm_params=dict(sea.get('norm_params') or {}),
                    trim_right_ratio=(sea.get('decoder') or {}).get('trim_right_ratio', 1.0),   # seanet.decoder.* (encodec/default.yaml)
                    sample_rate=xp['sample_rate'], n_q=rvq['n_q'], bins=rvq['bins'],
                    renormalize=xp['encodec']['renormalize'])

@@ -49,6 +49,18 @@ ENCODEC_CONFIGS: tp.Dict[str, dict] = {
                                 latent_sigma=0.35),
 }
 
+# GroupNorm codecs (norm='time_group_norm'): their state dicts hold each conv's GroupNorm next to it (`...conv.norm.*`,
+# `...convtr.norm.*`), outside the conv prefixes of the layer plan.
+ENCODEC_GN_CONFIGS: tp.Dict[str, dict] = {
+    # facebook/encodec_48khz (transformers EncodecConfig of that repo): 48 kHz stereo, hop 320 (150 Hz), 16 x 1024 codes,
+    # GroupNorm(1, C) after every convolution, 1x1 conv shortcuts; transformers cuts its input into 1 s chunks
+    'encodec_48k': dict(channels=2, dimension=128, n_filters=32, n_residual_layers=1, ratios=[8, 5, 4, 2],
+                        kernel_size=7, last_kernel_size=7, residual_kernel_size=3, dilation_base=2,
+                        causal=False, pad_mode='reflect', compress=2, lstm=2, norm='time_group_norm', true_skip=False,
+                        trim_right_ratio=1.0, sample_rate=48000, n_q=16, bins=1024, renormalize=True,
+                        latent_sigma=0.35),
+}
+
 
 def encodec_hop(cfg: dict) -> int:
     return int(math.prod(cfg['ratios']))
@@ -131,7 +143,8 @@ def _uniform(gen, shape, bound, device, dtype=torch.float32):
 
 def synth_encodec_state_dict(cfg: dict, seed: int = 0, device='cpu') -> tp.Dict[str, torch.Tensor]:
     """Seeded random EnCodec weights (variance-preserving conv init, weight-norm g perturbed so that the
-    fold g*v/|v| is exercised, codebooks scaled to the latent statistics)."""
+    fold g*v/|v| is exercised, codebooks scaled to the latent statistics).  norm='time_group_norm' adds each conv's GroupNorm
+    gamma / beta (`...conv.norm.*`, `...convtr.norm.*`) drawn around 1 / 0, so a transposed gamma or a dropped beta shows."""
     gen = torch.Generator(device=device)
     gen.manual_seed(seed)
     sd: tp.Dict[str, torch.Tensor] = {}
@@ -161,6 +174,10 @@ def synth_encodec_state_dict(cfg: dict, seed: int = 0, device='cpu') -> tp.Dict[
         else:
             sd[p + 'weight'] = v
         sd[p + 'bias'] = _uniform(gen, (cout,), 0.05, device)
+        if cfg['norm'] == 'time_group_norm':
+            n = p.rsplit('.', 2)[0] + '.norm.'
+            sd[n + 'weight'] = 1.0 + 0.2 * torch.randn((cout,), generator=gen, device=device)
+            sd[n + 'bias'] = 0.1 * torch.randn((cout,), generator=gen, device=device)
     sigma = cfg.get('latent_sigma', 1.0)
     for q in range(cfg['n_q']):
         emb = torch.randn((cfg['bins'], cfg['dimension']), generator=gen, device=device) * (sigma * 0.6 ** q)

@@ -129,6 +129,31 @@ int acb_rvq_encode(const float* latent, const float* codebooks, const float* cb_
 int acb_rvq_decode(const int64_t* codes, const float* codebooks, float* latent,
                    int batch, int dim, int t_len, int n_q, int bins, void* stream);
 
+/* ---------------------------------------------------------------- EnCodec: GroupNorm, chunking ----- */
+
+/* Statistics of GroupNorm(1, C) (norm='time_group_norm', audiocraft/modules/conv.py:33-42) over each item of x [B][C][T]:
+ * stats[b] = {mean, 1/sqrt(var + eps)} as two doubles (biased variance over the C*T elements).  Deterministic: an item's
+ * statistics do not depend on the batch it sits in; fp64 sums of x - x[b][0][0], so a large mean does not cancel the variance.
+ * workspace: acb_groupnorm_workspace_bytes(B, C, T) bytes of scratch. */
+int64_t acb_groupnorm_workspace_bytes(int batch, int channels, int t_len);
+int acb_groupnorm_stats(const float* x, void* workspace, double* stats, int batch, int channels, int t_len, float eps, void* stream);
+
+/* y[b,c,t] = gamma[c] (x[b,c,left+t] - mean_b) rstd_b + beta[c] for t in [0, t_out), x being [B][C][t_src] (left > 0 reads the
+ * window the transposed conv's trim keeps: NormConvTranspose1d normalises before StreamableConvTranspose1d trims, conv.py:221-243),
+ *   + the same normalisation of x2 [B][C][t_out] with stats2 / gamma2 / beta2 (a residual block's conv shortcut), or
+ *   + residual [B][C][t_out] (the identity skip); x2 and residual may both be NULL, not both set.  y aliases no input. */
+int acb_groupnorm_apply(const float* x, const double* stats, const float* gamma, const float* beta, int t_src, int left,
+                        const float* x2, const double* stats2, const float* gamma2, const float* beta2, const float* residual,
+                        float* y, int batch, int channels, int t_out, void* stream);
+
+/* Linear overlap-add of the independently decoded chunks of the chunked (48 kHz) codec, transformers
+ * EncodecModel._linear_overlap_add: chunk i starts at i*stride, is multiplied by scales[i][b] (scales NULL: 1), weighted by the
+ * triangle w(j) = 0.5 - |(j+1)/(L+1) - 0.5| with L the first chunk's length, and the weighted sum is divided by the summed weights.
+ * frames: chunks 0 .. n-2 as [n-1][B][C][t_frame] (NULL when n_chunks == 1); last: chunk n-1 as [B][C][t_last];
+ * y [B][C][t_total], t_total = stride*(n_chunks-1) + t_last. */
+int acb_overlap_add(const float* frames, const float* last, const float* scales, float* y, int n_chunks, int batch, int channels,
+                    int t_frame, int t_last, int stride, int t_total, void* stream);
+
 /* ---------------------------------------------------------------- MusicGen: LM decode -------------- */
 
 typedef struct {

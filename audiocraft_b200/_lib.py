@@ -75,6 +75,7 @@ def lib():
     L.acb_resblock_supported.argtypes = [ci, ci, ci]
     L.acb_resblock.argtypes = [vp] * 6 + [ci] * 8 + [vp]
     L.acb_lstm_recurrent.argtypes = [vp, vp, vp, vp, vp, ci, ci, ci, vp]
+    L.acb_lstm_recurrent_carry.argtypes = [vp] * 7 + [ci, ci, ci, vp]
     L.acb_lstm_state_bytes.argtypes = [ci, ci]
     L.acb_lstm_state_bytes.restype = i64
     L.acb_rvq_encode.argtypes = [vp, vp, vp, vp, ci, ci, ci, ci, ci, vp]
@@ -102,7 +103,8 @@ def lib():
     L.acb_t5_workspace_bytes.argtypes = [C.POINTER(T5Config), ci, ci]
     L.acb_t5_workspace_bytes.restype = i64
     L.acb_t5_encode.argtypes = [C.POINTER(T5Config), C.POINTER(T5Weights), vp, vp, vp, ci, ci, vp, vp, vp, i64, vp]
-    for name in ('acb_weight_norm_fold', 'acb_conv1d', 'acb_convtr1d', 'acb_lstm_recurrent', 'acb_rvq_encode',
+    for name in ('acb_weight_norm_fold', 'acb_conv1d', 'acb_convtr1d', 'acb_lstm_recurrent', 'acb_lstm_recurrent_carry',
+                 'acb_rvq_encode',
                  'acb_rvq_decode', 'acb_lm_create', 'acb_lm_destroy', 'acb_lm_begin', 'acb_lm_begin_prefix', 'acb_lm_steps',
                  'acb_lm_step_logits', 'acb_lm_launches_per_step', 'acb_lm_rows_pad', 'acb_sample',
                  'acb_device_sm_count', 'acb_lm_debug_gemms', 'acb_lm_uses_pdl',
@@ -121,7 +123,7 @@ EXPORTS = ['acb_version', 'acb_last_error', 'acb_device_sm_count', 'acb_weight_n
            'acb_lm_launches_per_step', 'acb_lm_debug_gemms', 'acb_lm_uses_pdl', 'acb_sample', 'acb_conv1d_t6', 'acb_conv1d_t6_tile',
            'acb_lm_prefill', 'acb_resblock', 'acb_resblock_supported', 'acb_lm_forward_workspace_bytes', 'acb_lm_forward',
            'acb_t5_workspace_bytes', 'acb_t5_encode', 'acb_groupnorm_workspace_bytes', 'acb_groupnorm_stats',
-           'acb_groupnorm_apply', 'acb_overlap_add']
+           'acb_groupnorm_apply', 'acb_overlap_add', 'acb_lstm_recurrent_carry']
 
 
 def check(rc: int, what: str = ''):

@@ -1737,9 +1737,14 @@ extern "C" int acb_convtr1d(const float* x, const float* w_packed, const float* 
 // h_{t-1} (all units) from L2, computes its 4U x B gate pre-activations, applies the cell update for its
 // units and publishes h_t; a grid-wide barrier separates the steps.
 // ------------------------------------------------------------------------------------------------
+// h_state / c_state ([B][H] fp32, null = zero initial state): read as the state before step 0, overwritten with the state after
+// step T-1.  The state is published into the h buffer the kernel's step 0 reads, in that kernel's own layout and split, behind one
+// extra grid barrier, and step 0 then runs the same recurrent product as every later step: pieces of a sequence run with the
+// state carried between calls give the bits of one call.
 struct LstmParams {
     const float* gx; const float* whh; const float* skip; float* y; float* hbuf; unsigned* bar;
     int B, H, T, U;
+    float* h_state; float* c_state;
 };
 
 __device__ __forceinline__ unsigned ld_acquire_u32(const unsigned* p) {
@@ -1770,10 +1775,25 @@ __global__ void __launch_bounds__(256) lstm_kernel(LstmParams p) {
         reinterpret_cast<float4*>(wsm)[idx] =
             reinterpret_cast<const float4*>(p.whh + ((size_t)gate * H + unit0 + u) * H)[c4];
     }
-    for (int idx = tid; idx < U * p.B; idx += 256) cs[idx] = 0.f;
+    const bool carry = p.h_state != nullptr;
+    for (int idx = tid; idx < U * p.B; idx += 256) {   // cs is [U][B]
+        const size_t st = (size_t)(idx % p.B) * H + unit0 + idx / p.B;
+        cs[idx] = carry ? p.c_state[st] : 0.f;
+        if (carry) __stcg(p.hbuf + st, p.h_state[st]);    // buffer 0, [B][H]: what step 0 reads
+    }
     __syncthreads();
+    const unsigned bar0 = carry ? 1u : 0u;
+    if (carry) {
+        if (tid == 0) {
+            __threadfence();
+            atomicAdd(p.bar, 1u);
+            while (ld_acquire_u32(p.bar) < ncta) { }
+        }
+        __syncthreads();
+    }
 
     for (int t = 0; t < p.T; ++t) {
+        const bool rec = t > 0 || carry;   // step 0 of a zero state has no recurrent term
         const float* hprev = p.hbuf + (size_t)(t & 1) * p.B * H;
         float* hnext = p.hbuf + (size_t)((t + 1) & 1) * p.B * H;
         for (int b0 = 0; b0 < p.B; b0 += LSTM_BC) {
@@ -1787,7 +1807,7 @@ __global__ void __launch_bounds__(256) lstm_kernel(LstmParams p) {
                 for (int g = 0; g < 4; ++g)
                     gxr[g] = __ldg(p.gx + ((size_t)(b0 + pb) * 4 * H + (size_t)g * H + unit0 + pu) * p.T + t);
             }
-            if (t > 0) {
+            if (rec) {
                 for (int idx = tid; idx < LSTM_BC * (H / 4); idx += 256) {
                     int bb = idx / (H / 4), c4 = idx - bb * (H / 4);
                     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -1838,7 +1858,7 @@ __global__ void __launch_bounds__(256) lstm_kernel(LstmParams p) {
             }
             if (pw) {
                 float gi = gxr[0], gf = gxr[1], gg = gxr[2], go = gxr[3];
-                if (t > 0) {
+                if (rec) {
                     gi += gs[(0 * U + pu) * LSTM_BC + pb];
                     gf += gs[(1 * U + pu) * LSTM_BC + pb];
                     gg += gs[(2 * U + pu) * LSTM_BC + pb];
@@ -1851,6 +1871,10 @@ __global__ void __launch_bounds__(256) lstm_kernel(LstmParams p) {
                 __stcg(hnext + (size_t)(b0 + pb) * H + unit0 + pu, h);
                 size_t yo = ((size_t)(b0 + pb) * H + unit0 + pu) * p.T + t;
                 p.y[yo] = p.skip ? h + p.skip[yo] : h;
+                if (carry && t == p.T - 1) {
+                    p.h_state[(size_t)(b0 + pb) * H + unit0 + pu] = h;
+                    p.c_state[(size_t)(b0 + pb) * H + unit0 + pu] = c;
+                }
             }
             __syncthreads();  // gs / hs reused by the next batch chunk
         }
@@ -1858,7 +1882,7 @@ __global__ void __launch_bounds__(256) lstm_kernel(LstmParams p) {
         if (tid == 0) {
             __threadfence();
             atomicAdd(p.bar, 1u);
-            const unsigned target = ncta * (unsigned)(t + 1);
+            const unsigned target = ncta * ((unsigned)t + 1u + bar0);
             while (ld_acquire_u32(p.bar) < target) { }
         }
         __syncthreads();
@@ -1908,6 +1932,21 @@ __global__ void __launch_bounds__(LTC_NW * 32, 1) lstm_tc_kernel(LstmParams p) {
     float cstate = 0.f;
     const int ksteps = H / (8 * LTC_NW);         // k-steps of 8 per warp
     const int kb0 = warp * ksteps;               // first k-block (of 8) of this warp
+    const bool carry = p.h_state != nullptr;
+    const size_t st_cell = (size_t)cb * H + kunit;
+    if (carry) {                                 // the carried h into buffer 0 in B-fragment order, as step t publishes h_t
+        if (cell_live) {
+            cstate = p.c_state[st_cell];
+            __stcg(p.hbuf + hf_cell, p.h_state[st_cell]);
+        }
+        __syncthreads();
+        if (tid == 0) {
+            gridbar_arrive(p.bar);
+            gridbar_wait(p.bar, ncta);
+        }
+        __syncthreads();
+    }
+    const unsigned bar0 = carry ? 1u : 0u;
 
     float gxr[4] = {0.f, 0.f, 0.f, 0.f};
     if (cell_live) {
@@ -1922,7 +1961,7 @@ __global__ void __launch_bounds__(LTC_NW * 32, 1) lstm_tc_kernel(LstmParams p) {
 #pragma unroll
             for (int gt = 0; gt < 4; ++gt) gxr[gt] = __ldg(p.gx + gx_cell + (size_t)gt * H * p.T + t + 1);
         }
-        if (t > 0) {
+        if (t > 0 || carry) {
             float acc[2][4][4];
 #pragma unroll
             for (int i = 0; i < 2; ++i)
@@ -1997,12 +2036,16 @@ __global__ void __launch_bounds__(LTC_NW * 32, 1) lstm_tc_kernel(LstmParams p) {
             const float h = sigmoidf_(go) * tanhf(cstate);
             __stcg(hnext + hf_cell, h);
             p.y[y_cell + t] = p.skip ? h + p.skip[y_cell + t] : h;
+            if (carry && t == p.T - 1) {
+                p.h_state[st_cell] = h;
+                p.c_state[st_cell] = cstate;
+            }
         }
         // grid barrier: everyone has published h_t (and is done with the partial-sum buffer) before anyone reads it
         __syncthreads();
         if (tid == 0) {   // release reduction without a return value + acquire polling (csrc/gridbar.cuh): no membar.gl, no atomic round trip
             gridbar_arrive(p.bar);
-            gridbar_wait(p.bar, ncta * (unsigned)(t + 1));
+            gridbar_wait(p.bar, ncta * ((unsigned)t + 1u + bar0));
         }
         __syncthreads();
     }
@@ -2082,6 +2125,24 @@ __global__ void __launch_bounds__(LTC_NW * 32, 1) lstm_h2_kernel(LstmParams p) {
     const size_t y_cell = ((size_t)cb * H + kunit) * p.T;
     float cstate = 0.f;
     __half* hbuf = reinterpret_cast<__half*>(p.hbuf);
+    const bool carry = p.h_state != nullptr;
+    const size_t st_cell = (size_t)cb * H + kunit;
+    if (carry) {                                 // the carried h into buffer 0, split and ordered as step t publishes h_t
+        if (cell_live) {
+            cstate = p.c_state[st_cell];
+            __half hh, hl;
+            split_h2(p.h_state[st_cell], hh, hl);
+            hbuf[hf_cell] = hh;
+            hbuf[hf_cell + 512] = hl;
+        }
+        __syncthreads();
+        if (tid == 0) {
+            gridbar_arrive(p.bar);
+            gridbar_wait(p.bar, ncta);
+        }
+        __syncthreads();
+    }
+    const unsigned bar0 = carry ? 1u : 0u;
 
     float gxr[4] = {0.f, 0.f, 0.f, 0.f};
     if (cell_live) {
@@ -2096,7 +2157,7 @@ __global__ void __launch_bounds__(LTC_NW * 32, 1) lstm_h2_kernel(LstmParams p) {
 #pragma unroll
             for (int gt = 0; gt < 4; ++gt) gxr[gt] = __ldg(p.gx + gx_cell + (size_t)gt * H * p.T + t + 1);
         }
-        if (t > 0) {
+        if (t > 0 || carry) {
             float acc0[2][4][4], acc1[2][4][4];   // hi.hi | hi.lo + lo.hi (scaled by 2^11)
 #pragma unroll
             for (int i = 0; i < 2; ++i)
@@ -2167,11 +2228,15 @@ __global__ void __launch_bounds__(LTC_NW * 32, 1) lstm_h2_kernel(LstmParams p) {
             hnext[hf_cell] = hh;                 // plain stores: published by the release arrive below
             hnext[hf_cell + 512] = hl;
             p.y[y_cell + t] = p.skip ? h + p.skip[y_cell + t] : h;
+            if (carry && t == p.T - 1) {
+                p.h_state[st_cell] = h;
+                p.c_state[st_cell] = cstate;
+            }
         }
         __syncthreads();
         if (tid == 0) {
             gridbar_arrive(p.bar);
-            gridbar_wait(p.bar, ncta * (unsigned)(t + 1));
+            gridbar_wait(p.bar, ncta * ((unsigned)t + 1u + bar0));
         }
         __syncthreads();
     }
@@ -2182,8 +2247,8 @@ extern "C" int64_t acb_lstm_state_bytes(int batch, int hidden) {
     return ((int64_t)2 * b * hidden + 64) * (int64_t)sizeof(float);
 }
 
-extern "C" int acb_lstm_recurrent(const float* gates_x, const float* w_hh, const float* skip, float* y,
-                                  float* state_ws, int batch, int hidden, int t_len, void* stream) {
+static int lstm_recurrent(const float* gates_x, const float* w_hh, const float* skip, float* y, float* state_ws,
+                          float* h_state, float* c_state, int batch, int hidden, int t_len, void* stream) {
     ACB_REQUIRE(gates_x && w_hh && y && state_ws, "acb_lstm_recurrent: null pointer");
     ACB_REQUIRE(batch > 0 && hidden > 0 && t_len > 0, "acb_lstm_recurrent: empty shape");
     ACB_REQUIRE(hidden % 4 == 0, "acb_lstm_recurrent: hidden must be a multiple of 4");
@@ -2201,7 +2266,8 @@ extern "C" int acb_lstm_recurrent(const float* gates_x, const float* w_hh, const
             if (per_sm * sms >= ncta) {
                 const size_t hfloats = (size_t)2 * LTC_B * hidden;
                 ACB_CHECK_CUDA(cudaMemsetAsync(state_ws, 0, (hfloats + 64) * sizeof(float), s));
-                LstmParams p{gates_x, w_hh, skip, y, state_ws, (unsigned*)(state_ws + hfloats), batch, hidden, t_len, LTC_U};
+                LstmParams p{gates_x, w_hh, skip, y, state_ws, (unsigned*)(state_ws + hfloats), batch, hidden, t_len, LTC_U,
+                             h_state, c_state};
                 void* args[] = {&p};
                 // hidden % 128 == 0: both operands pre-split into fp16 terms (lstm_h2_kernel); ACB_LSTM_TC=3 keeps the 3xTF32 kernel (A/B)
                 const bool h2 = hidden % (16 * LTC_NW) == 0 && !(e && e[0] == '3');
@@ -2228,10 +2294,21 @@ extern "C" int acb_lstm_recurrent(const float* gates_x, const float* w_hh, const
     size_t hbytes = (size_t)2 * batch * hidden * sizeof(float);
     ACB_CHECK_CUDA(cudaMemsetAsync(state_ws, 0, hbytes + 64 * sizeof(float), s));
     LstmParams p{gates_x, w_hh, skip, y, state_ws, (unsigned*)(state_ws + (size_t)2 * batch * hidden), batch, hidden,
-                 t_len, U};
+                 t_len, U, h_state, c_state};
     void* args[] = {&p};
     ACB_CHECK_CUDA(cudaLaunchCooperativeKernel((void*)lstm_kernel, dim3(ncta), dim3(256), args, smem, s));
     return ACB_OK;
+}
+
+extern "C" int acb_lstm_recurrent(const float* gates_x, const float* w_hh, const float* skip, float* y,
+                                  float* state_ws, int batch, int hidden, int t_len, void* stream) {
+    return lstm_recurrent(gates_x, w_hh, skip, y, state_ws, nullptr, nullptr, batch, hidden, t_len, stream);
+}
+
+extern "C" int acb_lstm_recurrent_carry(const float* gates_x, const float* w_hh, const float* skip, float* y, float* state_ws,
+                                        float* h_state, float* c_state, int batch, int hidden, int t_len, void* stream) {
+    ACB_REQUIRE(h_state && c_state && h_state != c_state, "acb_lstm_recurrent_carry: null or aliased state");
+    return lstm_recurrent(gates_x, w_hh, skip, y, state_ws, h_state, c_state, batch, hidden, t_len, stream);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -257,13 +257,17 @@ class EncodecModel(CompressionModel):
 
     # ------------------------------------------------------------------ layer launches
     def _conv(self, x, L, w=None, b=None, res=None, k=None, stride=None, dilation=None, elu=None, cout=None,
-              prec=0):
+              prec=0, valid=False):
+        """valid=True: no padding, the outputs whose window lies inside x (a streaming window, audiocraft_b200/streaming.py)."""
         B, cin, T = x.shape
         k = L['k'] if k is None else k
         stride = L['stride'] if stride is None else stride
         dilation = L['dilation'] if dilation is None else dilation
         cout = L['cout'] if cout is None else cout
-        left, t_virt, t_out = conv_geometry(T, k, stride, dilation, self.causal, bool(self.reflect))
+        if valid:
+            left, t_virt, t_out = 0, T, (T - (k - 1) * dilation - 1) // stride + 1
+        else:
+            left, t_virt, t_out = conv_geometry(T, k, stride, dilation, self.causal, bool(self.reflect))
         y = torch.empty((B, cout, t_out), device=x.device, dtype=torch.float32)
         if prec == _lib.CONV_T6_AUTO:
             # the implicit-GEMM tensor-core kernel is for k > 1 with >= 128 output channels: a 1x1 convolution gives it too little
@@ -285,12 +289,15 @@ class EncodecModel(CompressionModel):
         self.launches += 1
         return y
 
-    def _convtr(self, x, L, prec=0, trim=True):
-        """trim=False: the full transposed-conv output (the GroupNorm statistics cover the steps the trim drops)."""
+    def _convtr(self, x, L, prec=0, trim=True, window=None):
+        """trim=False: the full transposed-conv output (the GroupNorm statistics cover the steps the trim drops).
+        window=(trim_left, t_out): that range of the full output (a streaming window)."""
         B, cin, T = x.shape
         trim_left, t_out = convtr_geometry(T, L['k'], L['stride'], self.causal, self.cfg['trim_right_ratio'])
         if not trim:
             trim_left, t_out = 0, (T - 1) * L['stride'] + L['k']
+        if window is not None:
+            trim_left, t_out = window
         y = torch.empty((B, L['cout'], t_out), device=x.device, dtype=torch.float32)
         if prec in (_lib.CONV_T6_FLUSH, _lib.CONV_T6_AUTO):
             prec = _lib.CONV_TF32X3        # transposed convs have no implicit-GEMM variant yet
@@ -300,9 +307,10 @@ class EncodecModel(CompressionModel):
         self.launches += 1
         return y
 
-    def _lstm(self, x, L, prec=0):
+    def _lstm(self, x, L, prec=0, state=None):
         """y = LSTM(x) + x over frames (audiocraft/modules/lstm.py:19-25): per layer one 1x1 conv for the input
-        half of the gates, then the persistent recurrent kernel."""
+        half of the gates, then the persistent recurrent kernel.  state: per-layer ([B, H], [B, H]) (h, c) to start from,
+        advanced in place (acb_lstm_recurrent_carry)."""
         B, H, T = x.shape
         ws = torch.empty(int(self._lib.acb_lstm_state_bytes(B, H)) // 4, device=x.device, dtype=torch.float32)
         inp = x
@@ -314,8 +322,14 @@ class EncodecModel(CompressionModel):
                        'lstm input conv')
             y = torch.empty((B, H, T), device=x.device, dtype=torch.float32)
             skip = x if n == n_layers - 1 else None
-            _lib.check(self._lib.acb_lstm_recurrent(_lib.ptr(gx), _lib.ptr(L['w_hh'][n]), _lib.ptr(skip), _lib.ptr(y),
-                                                    _lib.ptr(ws), B, H, T, _lib.stream()), 'lstm_recurrent')
+            if state is not None:
+                h, c = state[n]
+                _lib.check(self._lib.acb_lstm_recurrent_carry(_lib.ptr(gx), _lib.ptr(L['w_hh'][n]), _lib.ptr(skip), _lib.ptr(y),
+                                                              _lib.ptr(ws), _lib.ptr(h), _lib.ptr(c), B, H, T, _lib.stream()),
+                           'lstm_recurrent_carry')
+            else:
+                _lib.check(self._lib.acb_lstm_recurrent(_lib.ptr(gx), _lib.ptr(L['w_hh'][n]), _lib.ptr(skip), _lib.ptr(y),
+                                                        _lib.ptr(ws), B, H, T, _lib.stream()), 'lstm_recurrent')
             self.launches += 2
             inp = y
         return inp
@@ -330,16 +344,21 @@ class EncodecModel(CompressionModel):
                 and b['k'] == 1 and b['stride'] == 1 and a['elu'] and b['elu'] and b['cout'] == 2 * a['cout']
                 and bool(self._lib.acb_resblock_supported(b['cout'], a['k'], a['dilation'])))
 
-    def _resblock(self, x, a, b, prec):
+    def _resblock(self, x, a, b, prec, pad_left=None):
+        """pad_left given: zero padding of pad_left steps instead of the layer's own (a streaming window: the caller keeps the
+        outputs that touched no padding)."""
         B, C, T = x.shape
         if 'w1p' not in a:   # [C*k][C/2] (row = ci*k + tap) -> [k][C][C/2]
             a['w1p'] = a['w'].view(C, a['k'], a['cout']).permute(1, 0, 2).contiguous()
         left, _, t_out = conv_geometry(T, a['k'], 1, a['dilation'], self.causal, bool(self.reflect))
         assert t_out == T
+        reflect = self.reflect
+        if pad_left is not None:
+            left, reflect = pad_left, 0
         y = torch.empty_like(x)
         exact = int(prec in (_lib.CONV_T6_FLUSH, _lib.CONV_T6_AUTO))
         _lib.check(self._lib.acb_resblock(_lib.ptr(x), _lib.ptr(a['w1p']), _lib.ptr(a['b']), _lib.ptr(b['w']), _lib.ptr(b['b']),
-                                          _lib.ptr(y), B, C, T, a['k'], a['dilation'], left, self.reflect, exact, _lib.stream()),
+                                          _lib.ptr(y), B, C, T, a['k'], a['dilation'], left, reflect, exact, _lib.stream()),
                    'resblock')
         self.launches += 1
         return y
@@ -549,6 +568,17 @@ class EncodecModel(CompressionModel):
             out = self._run(self.decode_latent(codes), self.dec, self._dec_prec)
             return self.postprocess(out, scale)
 
+    def stream_decoder(self, batch: int, scale=None) -> 'EncodecStreamDecoder':
+        """A stateful decoder for codes that arrive in pieces: `push(codes [B, K, n])` returns the samples no later frame can
+        change, `flush()` the rest, and their concatenation is `decode(all codes)` (same length).  Renormalisation scales are not
+        part of MusicGen decoding and are refused; GroupNorm codecs are refused because their statistics span the whole item."""
+        if self.cfg.get('norm') == 'time_group_norm':
+            raise NotImplementedError("streaming decode of a GroupNorm codec (norm: time_group_norm) is not built: its "
+                                      "statistics span the whole item")
+        if scale is not None:
+            raise NotImplementedError("streaming decode with a renormalisation scale is not built (MusicGen decodes without one)")
+        return EncodecStreamDecoder(self, batch)
+
     def forward(self, x):
         """encodec.py:206-221 (inference part): returns the reconstruction trimmed to the input length and codes."""
         length = x.shape[-1]
@@ -560,6 +590,96 @@ class EncodecModel(CompressionModel):
     @staticmethod
     def from_config_name(name: str, state_dict, device='cuda') -> 'EncodecModel':
         return EncodecModel(state_dict, ENCODEC_CONFIGS[name], device)
+
+
+class _KernelLayers:
+    """The layer operations of audiocraft_b200.streaming.DecoderStream on the decoder's kernels, each on a window that needs
+    no padding."""
+
+    def __init__(self, model: EncodecModel):
+        self.m = model
+        self.prec = model._dec_prec
+
+    def conv(self, L, x):
+        return self.m._conv(x.contiguous(), L, prec=self.prec, valid=True)
+
+    def resblock(self, block, x, pad_left):
+        shortcut, a, b = block
+        m, x = self.m, x.contiguous()
+        n = x.shape[-1] - (a['k'] - 1) * a['dilation']
+        if shortcut is None and m._fused_block([a, b], 0, self.prec, x.shape[-1]):
+            # the fused kernel writes every step of x; those whose window reaches into its zero padding are dropped
+            return m._resblock(x, a, b, self.prec, pad_left=pad_left)[..., pad_left:pad_left + n]
+        skip = x[..., pad_left:pad_left + n].contiguous()
+        if shortcut is not None:
+            skip = m._conv(skip, shortcut, prec=self.prec, valid=True)
+        return m._conv(m._conv(x, a, prec=self.prec, valid=True), b, res=skip, prec=self.prec, valid=True)
+
+    def convtr(self, L, x, trim_left, t_out):
+        return self.m._convtr(x.contiguous(), L, prec=self.prec, window=(trim_left, t_out))
+
+    def lstm_state(self, L, batch):
+        z = lambda: torch.zeros((batch, L['dim']), device=self.m.device, dtype=torch.float32)   # noqa: E731
+        return [(z(), z()) for _ in range(len(L['w_hh']))]
+
+    def lstm(self, L, x, state):
+        return self.m._lstm(x.contiguous(), L, prec=self.m._lstm_prec, state=state)
+
+
+class EncodecStreamDecoder:
+    """`EncodecModel.stream_decoder(batch)`: the SEANet decoder with per-layer context (audiocraft_b200/streaming.py) on the
+    kernels; the LSTM carries (h, c) between pushes."""
+
+    def __init__(self, model: EncodecModel, batch: int):
+        from .streaming import DecoderStream
+        self.model, self.batch = model, batch
+        self._stream = DecoderStream(model.dec, model.cfg, _KernelLayers(model), batch)
+
+    @property
+    def lookahead(self) -> int:
+        """Latent frames past its own that a sample waits for once the stream is running."""
+        return self._stream.lookahead
+
+    def _out(self, y):
+        if y is None:
+            return torch.empty((self.batch, self.model.channels, 0), device=self.model.device, dtype=torch.float32)
+        return y
+
+    def push(self, codes: torch.Tensor) -> torch.Tensor:
+        assert codes.dim() == 3 and codes.shape[0] == self.batch, (tuple(codes.shape), self.batch)
+        with torch.cuda.device(self.model.device):
+            if codes.shape[-1] == 0:
+                return self._out(None)
+            return self._out(self._stream.push(self.model.decode_latent(codes)))
+
+    def flush(self) -> torch.Tensor:
+        with torch.cuda.device(self.model.device):
+            return self._out(self._stream.flush())
+
+
+class _StereoStreamDecoder:
+    """The mono stream decoder over 2B items (left channels, then right), as `InterleaveStereoCompressionModel.decode`."""
+
+    def __init__(self, wrapper: 'InterleaveStereoCompressionModel', inner, batch: int):
+        self.wrapper, self.inner, self.batch = wrapper, inner, batch
+
+    @property
+    def lookahead(self) -> int:
+        return self.inner.lookahead
+
+    def _split(self, audio):
+        return torch.cat([audio[:self.batch], audio[self.batch:]], dim=1)
+
+    def push(self, codes: torch.Tensor) -> torch.Tensor:
+        B, K, T = codes.shape
+        assert B == self.batch and K == self.wrapper.num_codebooks, (tuple(codes.shape), self.batch)
+        if T == 0:
+            return self._split(self.inner.push(codes.new_empty((2 * B, K // 2, 0))))
+        c0, c1 = self.wrapper.get_left_right_codes(codes)
+        return self._split(self.inner.push(torch.cat([c0, c1], dim=0)))
+
+    def flush(self) -> torch.Tensor:
+        return self._split(self.inner.flush())
 
 
 class InterleaveStereoCompressionModel(CompressionModel):
@@ -649,6 +769,16 @@ class InterleaveStereoCompressionModel(CompressionModel):
 
     def decode_latent(self, codes):
         raise NotImplementedError("Not supported by interleaved stereo wrapped models.")
+
+    def stream_decoder(self, batch: int, scale=None):
+        """The wrapped codec's stream decoder over 2B mono items; pieces are [B, 2, m]."""
+        if self.per_timestep:
+            raise NotImplementedError("streaming decode of per-timestep interleaved codes is not built")
+        if not hasattr(self.model, 'stream_decoder'):
+            raise NotImplementedError(f"{type(self.model).__name__} has no stream decoder")
+        if scale is not None:
+            raise NotImplementedError("streaming decode with a renormalisation scale is not built (MusicGen decodes without one)")
+        return _StereoStreamDecoder(self, self.model.stream_decoder(2 * batch), batch)
 
 
 def get_wrapped_compression_model(compression_model: CompressionModel, interleave_stereo_codebooks: tp.Optional[dict] = None,
@@ -840,6 +970,10 @@ class HFEncodecCompressionModel(EncodecModel):
                         "encodes one chunk (`assert len(res[0]) == 1`); use `.model.encode` / `.model.decode` for longer audio")
         codes, scales, _ = self.model.encode(x, None, bandwidth)
         return codes[0], scales[0]
+
+    def stream_decoder(self, batch: int, scale=None):
+        raise NotImplementedError("streaming decode of a transformers EnCodec checkpoint is not built: its chunking is an "
+                                  "overlap-add of independently decoded chunks")
 
     def decode(self, codes, scale=None):
         """encodec.py:355-361: `self.model.decode(codes[None], scale)`.  The reference passes the [B, 1] scale where transformers

@@ -261,6 +261,78 @@ class LMModel:
         """Same contract as LMModel.generate (lm.py:420-587).  ``cross_attention_src`` is an extension: a pre-computed
         [2B,T,d] (or [B,T,d] without CFG) condition tensor, bypassing the host conditioners.  ``prefix`` likewise: a
         pre-computed [rows,P,d] condition prefix (the `prepend` fuser's output, one per row) for a model that has one."""
+        g = self._generate_begin(prompt, conditions, num_samples, max_gen_len, use_sampling, temp, top_k, top_p, cfg_coef,
+                                 cfg_coef_beta, two_step_cfg, cross_attention_src, prefix)
+        with torch.cuda.device(self.device):
+            B, K, bufs, first, n_steps, S, start_offset_sequence = (g[k] for k in ('B', 'K', 'bufs', 'first', 'n_steps', 'S',
+                                                                                   'start_offset_sequence'))
+            if callback is None and self._debug_noise_fn is None:
+                _lib.check(self._lib.acb_lm_steps(self._handle, n_steps - first, _lib.stream()), 'lm_steps')
+            else:
+                for pos in range(first, n_steps):
+                    offset = pos + 1
+                    if self._debug_noise_fn is not None:
+                        bufs['noise'][:B].copy_(self._debug_noise_fn(offset, (B, K, self.card)).reshape(B, K, self.card))
+                    _lib.check(self._lib.acb_lm_steps(self._handle, 1, _lib.stream()), 'lm_steps')
+                    if callback is not None and offset >= start_offset_sequence:
+                        callback(1 + offset - start_offset_sequence, S - start_offset_sequence)
+            return self._generate_end(g, remove_prompts)
+
+    @torch.no_grad()
+    def generate_blocks(self, prompt: tp.Optional[torch.Tensor] = None,
+                        conditions: tp.List[ConditioningAttributes] = [],
+                        num_samples: tp.Optional[int] = None, max_gen_len: int = 256, use_sampling: bool = True,
+                        temp: float = 1.0, top_k: int = 250, top_p: float = 0.0, cfg_coef: tp.Optional[float] = None,
+                        cfg_coef_beta: tp.Optional[float] = None, two_step_cfg: tp.Optional[bool] = None,
+                        callback: tp.Optional[tp.Callable[[int, int], None]] = None,
+                        cross_attention_src: tp.Optional[torch.Tensor] = None,
+                        prefix: tp.Optional[torch.Tensor] = None, block: int = 50) -> tp.Iterator[torch.Tensor]:
+        """`generate` as a stream of frames: the decode steps run `block` at a time, and after each block every frame whose
+        codebooks are all written is yielded as codes [B, K, n] (after step s, frames up to s - max_delay).  The prompt's frames
+        come first.  The seed is drawn once at begin, as in `generate`, so the concatenation is what `generate` returns (with
+        remove_prompts=False) for the same `torch.manual_seed`; the checks of `generate` run on the whole sequence at the end.
+        `callback(done, total)` is called after each block."""
+        assert block >= 1
+        if self._debug_noise_fn is not None:
+            raise NotImplementedError("generate_blocks does not take the per-step debug noise")
+        g = self._generate_begin(prompt, conditions, num_samples, max_gen_len, use_sampling, temp, top_k, top_p, cfg_coef,
+                                 cfg_coef_beta, two_step_cfg, cross_attention_src, prefix)
+        B, bufs, first, n_steps, S, s0 = (g[k] for k in ('B', 'bufs', 'first', 'n_steps', 'S', 'start_offset_sequence'))
+        delays = torch.tensor(g['pattern'].delays, device=self.device)
+        max_delay = int(delays.max())
+        done = 0
+
+        def ready_frames(pos_done: int):      # steps [0, pos_done) have run: sequence steps <= pos_done are written
+            nonlocal done
+            ready = max(0, min(max_gen_len, pos_done - max_delay))
+            if ready <= done:
+                return None
+            t = torch.arange(done, ready, device=self.device)
+            steps = (t[None, :] + 1 + delays[:, None])                                  # [K, n]
+            codes = bufs['seq'][:B].gather(2, steps[None].expand(B, -1, -1)).clone()    # [B, K, n]
+            done = ready
+            return codes
+
+        with torch.cuda.device(self.device):
+            out = ready_frames(first)
+            if out is not None:
+                yield out
+            pos = first
+            while pos < n_steps:
+                n = min(block, n_steps - pos)
+                _lib.check(self._lib.acb_lm_steps(self._handle, n, _lib.stream()), 'lm_steps')
+                pos += n
+                if callback is not None and pos >= s0:
+                    callback(pos - s0 + 1, S - s0)
+                out = ready_frames(pos)
+                if out is not None:
+                    yield out
+            assert done == max_gen_len, (done, max_gen_len)
+            self._generate_end(g, False)
+
+    def _generate_begin(self, prompt, conditions, num_samples, max_gen_len, use_sampling, temp, top_k, top_p, cfg_coef,
+                        cfg_coef_beta, two_step_cfg, cross_attention_src, prefix) -> dict:
+        """generate's set-up: pattern, buffers, the sampler seed, acb_lm_begin_prefix and the prompt prefill."""
         if num_samples is None:
             if prompt is not None:
                 num_samples = prompt.shape[0]
@@ -335,16 +407,14 @@ class LMModel:
             if start_offset_sequence - 1 >= 2 and _os.environ.get('ACB_LM_PREFILL', '1') != '0':
                 first = start_offset_sequence - 1
                 _lib.check(self._lib.acb_lm_prefill(self._handle, 0, first, _lib.stream()), 'lm_prefill')
-            if callback is None and self._debug_noise_fn is None:
-                _lib.check(self._lib.acb_lm_steps(self._handle, n_steps - first, _lib.stream()), 'lm_steps')
-            else:
-                for pos in range(first, n_steps):
-                    offset = pos + 1
-                    if self._debug_noise_fn is not None:
-                        bufs['noise'][:B].copy_(self._debug_noise_fn(offset, (B, K, self.card)).reshape(B, K, self.card))
-                    _lib.check(self._lib.acb_lm_steps(self._handle, 1, _lib.stream()), 'lm_steps')
-                    if callback is not None and offset >= start_offset_sequence:
-                        callback(1 + offset - start_offset_sequence, S - start_offset_sequence)
+            return dict(B=B, K=K, bufs=bufs, first=first, n_steps=n_steps, S=S, pattern=pattern, mask=mask,
+                        start_offset=start_offset, start_offset_sequence=start_offset_sequence, max_gen_len=max_gen_len)
+
+    def _generate_end(self, g: dict, remove_prompts: bool) -> torch.Tensor:
+        """generate's teardown: the checks of lm.py:568-586 and revert_pattern_sequence."""
+        B, bufs, S, pattern, mask = g['B'], g['bufs'], g['S'], g['pattern'], g['mask']
+        start_offset, max_gen_len, unknown_token = g['start_offset'], g['max_gen_len'], -1
+        with torch.cuda.device(self.device):
             gen_sequence = bufs['seq'][:B, :, :S].clone()
 
             # lm.py:568-586

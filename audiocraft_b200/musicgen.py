@@ -102,6 +102,14 @@ class BaseGenModel:
         return self.lm.generate(prompt_tokens, attributes, callback=callback, max_gen_len=n_tokens, **self.generation_params)
 
     def _generate_tokens(self, attributes, prompt_tokens: tp.Optional[Tokens], progress: bool = False) -> Tokens:
+        def window(prompt, attrs, n, callback):
+            yield self._lm_generate(prompt, attrs, n, callback)
+        return torch.cat(list(self._token_windows(attributes, prompt_tokens, progress, window)), dim=-1)
+
+    def _token_windows(self, attributes, prompt_tokens: tp.Optional[Tokens], progress: bool, window) -> tp.Iterator[Tokens]:
+        """The window loop of a generation: yields token pieces whose concatenation is the generation's tokens.
+        `window(prompt, attributes, n_tokens, callback)` runs the LM on one window and yields that window's tokens (its prompt
+        included) in one or more pieces; past max_duration each window's new frames are yielded as they arrive."""
         fr = self.frame_rate
         n_total = int(self.duration * fr)
         done_before_window = 0
@@ -118,28 +126,91 @@ class BaseGenModel:
             assert int(min(self.duration, self.max_duration) * fr) >= prompt_tokens.shape[-1], \
                 "Prompt is longer than audio to generate"
         if self.duration <= self.max_duration:
-            return self._lm_generate(prompt_tokens, attributes, n_total, callback)
+            yield from window(prompt_tokens, attributes, n_total, callback)
+            return
 
         # longer than the model's window: slide by `extend_stride`, each window prompted with the tail of the previous
         assert self.extend_stride is not None, "Stride should be defined to generate beyond max_duration"
         assert self.extend_stride < self.max_duration, "Cannot stride by more than max generation duration."
         stride = int(fr * self.extend_stride)
-        pieces: tp.List[Tokens] = [] if prompt_tokens is None else [prompt_tokens]
+        if prompt_tokens is not None:
+            yield prompt_tokens
         have = 0 if prompt_tokens is None else prompt_tokens.shape[-1]
         ref_attributes = attributes
         while done_before_window + have < n_total:
             window_s = min(self.duration - done_before_window / fr, self.max_duration)
             attributes = self._window_attributes(ref_attributes, done_before_window / fr)
-            window = self._lm_generate(prompt_tokens, attributes, int(window_s * fr), callback)
-            pieces.append(window if prompt_tokens is None else window[:, :, prompt_tokens.shape[-1]:])
-            prompt_tokens = window[:, :, stride:]
+            skip = 0 if prompt_tokens is None else prompt_tokens.shape[-1]   # the window's prompt was yielded already
+            got: tp.List[Tokens] = []
+            seen = 0
+            for piece in window(prompt_tokens, attributes, int(window_s * fr), callback):
+                got.append(piece)
+                new = piece[:, :, max(0, skip - seen):]
+                seen += piece.shape[-1]
+                if new.shape[-1]:
+                    yield new
+            prompt_tokens = torch.cat(got, dim=-1)[:, :, stride:]
             have = prompt_tokens.shape[-1]
             done_before_window += stride
-        return torch.cat(pieces, dim=-1)
 
     def _window_attributes(self, attributes, time_offset: float):
         """The conditions of the window starting `time_offset` seconds into a generation longer than max_duration."""
         return attributes
+
+    # -- streaming
+    def generate_stream(self, descriptions: tp.Optional[tp.List[tp.Optional[str]]] = None, *,
+                        num_samples: tp.Optional[int] = None, prompt: tp.Optional[Waveform] = None,
+                        prompt_sample_rate: tp.Optional[int] = None, melody_wavs=None,
+                        melody_sample_rate: tp.Optional[int] = None, chunk_duration: float = 1.0, progress: bool = False,
+                        return_tokens: bool = False) -> tp.Iterator[tp.Any]:
+        """Generate and decode at the same time: yields waveform pieces [B, C, m] (or (wav, tokens) pairs with return_tokens)
+        as the LM produces frames.  Their concatenation is what `generate` (descriptions), `generate_unconditional`
+        (num_samples), `generate_continuation` (prompt) or `generate_with_chroma` (melody_wavs) returns for the same inputs and
+        seed; a continuation's first pieces are the prompt's audio, as that output contains it.  The LM runs
+        `chunk_duration` seconds of decode steps at a time and each block's finished frames go to the codec's stream decoder;
+        the last piece holds the decoder's tail."""
+        if not chunk_duration > 0:
+            raise ValueError(f"chunk_duration must be > 0, got {chunk_duration}")
+        if not hasattr(self.compression_model, 'stream_decoder'):
+            raise NotImplementedError(f"{type(self.compression_model).__name__} has no stream decoder")
+        if prompt is not None and melody_wavs is not None:
+            raise ValueError("a prompt and melody_wavs together: generate_with_chroma takes no prompt")
+        if descriptions is None:
+            descriptions = [None] * (num_samples if num_samples is not None else
+                                     (len(prompt) if prompt is not None and prompt.dim() == 3 else 1))
+        # the codec refuses before any device work (GroupNorm / transformers checkpoints)
+        decoder = self.compression_model.stream_decoder(len(descriptions))
+        if prompt is not None:
+            if prompt.dim() == 2:
+                prompt = prompt[None]
+            if prompt.dim() != 3:
+                raise ValueError("prompt should have 3 dimensions: [B, C, T] (C = 1).")
+            if prompt_sample_rate is None:
+                raise ValueError("prompt_sample_rate is required with a prompt")
+            prompt = convert_audio(prompt, prompt_sample_rate, self.sample_rate, self.audio_channels)
+        if melody_wavs is not None:
+            attributes, prompt_tokens = self._prepare_melody(descriptions, melody_wavs, melody_sample_rate)
+        else:
+            attributes, prompt_tokens = self._prepare_tokens_and_attributes(descriptions, prompt)
+        block = max(1, int(round(chunk_duration * self.frame_rate)))
+
+        def window(prompt_, attrs, n, callback):
+            return self.lm.generate_blocks(prompt_, attrs, callback=callback, max_gen_len=n, block=block,
+                                           **self.generation_params)
+
+        with torch.no_grad():
+            for tokens in self._token_windows(attributes, prompt_tokens, progress, window):
+                for t0 in range(0, tokens.shape[-1], block):   # a prompt is handed to the codec in blocks too
+                    piece = tokens[:, :, t0:t0 + block]
+                    wav = decoder.push(piece)
+                    if wav.shape[-1] or return_tokens:
+                        yield (wav, piece) if return_tokens else wav
+            wav = decoder.flush()
+            empty = torch.empty((len(descriptions), self.lm.n_q, 0), dtype=torch.long, device=self.device)
+            yield (wav, empty) if return_tokens else wav
+
+    def _prepare_melody(self, descriptions, melody_wavs, melody_sample_rate):
+        raise NotImplementedError("this model has no melody ('self_wav') conditioner; use a MusicGen-melody model")
 
 
 def _sampling_params(use_sampling, top_k, top_p, temperature, cfg_coef, two_step_cfg):
@@ -189,6 +260,14 @@ class MusicGen(BaseGenModel):
                              progress: bool = False, return_tokens: bool = False):
         """Generate conditioned on text and melody (musicgen.py:155-189).  melody_wavs: [B,C,T], [C,T] for one
         description, or a list of [C,T] tensors / None (None: that item has a null melody)."""
+        attributes, prompt_tokens = self._prepare_melody(descriptions, melody_wavs, melody_sample_rate)
+        assert prompt_tokens is None
+        tokens = self._generate_tokens(attributes, prompt_tokens, progress)
+        audio = self.generate_audio(tokens)
+        return (audio, tokens) if return_tokens else audio
+
+    def _prepare_melody(self, descriptions, melody_wavs, melody_sample_rate):
+        """generate_with_chroma's inputs -> (attributes, prompt tokens = None) (musicgen.py:155-189)."""
         if not self._has_melody:
             raise NotImplementedError("this model has no melody ('self_wav') conditioner; use a MusicGen-melody model")
         if isinstance(melody_wavs, torch.Tensor):
@@ -203,11 +282,7 @@ class MusicGen(BaseGenModel):
                     assert melody.dim() == 2, "One melody in the list has the wrong number of dims."
         melody_wavs = [convert_audio(wav, melody_sample_rate, self.sample_rate, self.audio_channels)
                        if wav is not None else None for wav in melody_wavs]
-        attributes, prompt_tokens = self._prepare_tokens_and_attributes(descriptions, None, melody_wavs)
-        assert prompt_tokens is None
-        tokens = self._generate_tokens(attributes, prompt_tokens, progress)
-        audio = self.generate_audio(tokens)
-        return (audio, tokens) if return_tokens else audio
+        return self._prepare_tokens_and_attributes(descriptions, None, melody_wavs)
 
     def _null_wav(self) -> WavCondition:
         return WavCondition(torch.zeros((1, 1, 1), device=self.device), torch.tensor([0], device=self.device),

@@ -112,8 +112,15 @@ int acb_resblock(const float* x, const float* w1, const float* b1, const float* 
  * NOT graph-capturable (cooperative launch). */
 int acb_lstm_recurrent(const float* gates_x, const float* w_hh, const float* skip, float* y, float* state_ws,
                        int batch, int hidden, int t_len, void* stream);
-/* bytes of state_ws needed by acb_lstm_recurrent */
+/* bytes of state_ws needed by acb_lstm_recurrent and acb_lstm_recurrent_carry */
 int64_t acb_lstm_state_bytes(int batch, int hidden);
+/* acb_lstm_recurrent from a carried state, for a sequence decoded in pieces: h_state and c_state are caller-owned [B][H] fp32
+ * arrays, read as the state before step 0 and overwritten with the state after step t_len - 1.  Same kernels, same routing and
+ * the same operations in the same order: running T = t1 + t2 + ... steps as pieces, with the state carried between the calls,
+ * gives y and the final (h, c) bit-identical to one call of T steps.  One more grid barrier than acb_lstm_recurrent publishes
+ * the carried h before step 0. */
+int acb_lstm_recurrent_carry(const float* gates_x, const float* w_hh, const float* skip, float* y, float* state_ws,
+                             float* h_state, float* c_state, int batch, int hidden, int t_len, void* stream);
 
 /* ---------------------------------------------------------------- EnCodec: residual VQ ------------- */
 

@@ -17,6 +17,8 @@ ACB_LM_MAX_SPLIT = 8
 ACB_LM_PART_SLOTS = 16
 ACB_LM_PREFILL_ROWS = 64
 ACB_LM_MAX_ROWS = 256
+ACB_LM_SLOT_STRIDE = 8
+ACB_LM_MAX_SLOTS = 128
 
 
 class LMConfig(C.Structure):
@@ -32,7 +34,8 @@ class LMWeights(C.Structure):
 
 class LMBuffers(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ('x', 'h16', 'a16', 'f16', 'q32', 'part', 'logits', 'k_cache', 'v_cache',
-                                           'ck_cache', 'cv_cache', 'cross16', 'seq', 'seq_mask', 'pos', 'noise')]
+                                           'ck_cache', 'cv_cache', 'cross16', 'seq', 'seq_mask', 'pos', 'noise', 'slot_state',
+                                           'slot_mask')]
 
 
 class LMSampling(C.Structure):
@@ -90,6 +93,9 @@ def lib():
     L.acb_lm_begin.argtypes = [vp, vp, ci, ci, ci, ci, C.POINTER(LMSampling), vp]
     L.acb_lm_begin_prefix.argtypes = [vp, vp, vp, ci, ci, ci, ci, ci, C.POINTER(LMSampling), vp]
     L.acb_lm_steps.argtypes = [vp, ci, vp]
+    L.acb_lm_begin_slots.argtypes = [vp, ci, ci, ci, C.POINTER(LMSampling), vp]
+    L.acb_lm_admit.argtypes = [vp, ci, vp, ci, ci, C.c_uint64, vp]
+    L.acb_lm_slot_status.argtypes = [vp, vp, vp]
     L.acb_lm_prefill.argtypes = [vp, ci, ci, vp]
     L.acb_lm_step_logits.argtypes = [vp, vp, vp]
     L.acb_lm_launches_per_step.argtypes = [vp]
@@ -110,7 +116,7 @@ def lib():
                  'acb_device_sm_count', 'acb_lm_debug_gemms', 'acb_lm_uses_pdl',
                  'acb_conv1d_t6', 'acb_conv1d_t6_tile', 'acb_lm_prefill',
                  'acb_resblock', 'acb_resblock_supported', 'acb_lm_forward', 'acb_t5_encode', 'acb_groupnorm_stats',
-                 'acb_groupnorm_apply', 'acb_overlap_add'):
+                 'acb_groupnorm_apply', 'acb_overlap_add', 'acb_lm_begin_slots', 'acb_lm_admit', 'acb_lm_slot_status'):
         getattr(L, name).restype = ci
     _lib = L
     return L
@@ -123,7 +129,8 @@ EXPORTS = ['acb_version', 'acb_last_error', 'acb_device_sm_count', 'acb_weight_n
            'acb_lm_launches_per_step', 'acb_lm_debug_gemms', 'acb_lm_uses_pdl', 'acb_sample', 'acb_conv1d_t6', 'acb_conv1d_t6_tile',
            'acb_lm_prefill', 'acb_resblock', 'acb_resblock_supported', 'acb_lm_forward_workspace_bytes', 'acb_lm_forward',
            'acb_t5_workspace_bytes', 'acb_t5_encode', 'acb_groupnorm_workspace_bytes', 'acb_groupnorm_stats',
-           'acb_groupnorm_apply', 'acb_overlap_add', 'acb_lstm_recurrent_carry']
+           'acb_groupnorm_apply', 'acb_overlap_add', 'acb_lstm_recurrent_carry', 'acb_lm_begin_slots', 'acb_lm_admit',
+           'acb_lm_slot_status']
 
 
 def check(rc: int, what: str = ''):

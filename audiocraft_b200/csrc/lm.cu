@@ -27,6 +27,12 @@
 #include <stdio.h>
 #include <stdlib.h>
 
+// Slot mode (acb_lm_begin_slots): per-slot device state, ACB_LM_SLOT_STRIDE ints per slot in buffers.slot_state.  The host
+// writes a slot only at admission (lm_slot_admit_kernel); the step's sampler advances POS and sets STATUS to FINISHED.
+enum { ACB_SLOT_POS = 0, ACB_SLOT_STATUS = 1, ACB_SLOT_SEQ_LEN = 2, ACB_SLOT_TEXT_LEN = 3, ACB_SLOT_SEED_LO = 4,
+       ACB_SLOT_SEED_HI = 5, ACB_SLOT_DONE = 6 };
+enum { SLOT_INACTIVE = 0, SLOT_ACTIVE = 1, SLOT_FINISHED = 2 };
+
 // ------------------------------------------------------------------------------------------------ helpers
 // TMA 1-D bulk copy global -> shared, completion signalled on an mbarrier (UBLKCP in SASS). 16 B aligned, size % 16 == 0.
 __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
@@ -46,14 +52,10 @@ __device__ __forceinline__ float block_max(float v, float* red) {
 // ------------------------------------------------------------------------------------------------ embed + sin pos
 // x[r] = sum_k emb_k[seq[b,k,pos]] + pos_scale * [cos(pos/f_i), sin(pos/f_i)]   (lm.py:244, transformer.py:70-89,701-705)
 // The sin term only when sin_pos ('sin' and 'sin_rope'; a 'rope' model has its positions in the QKV epilogue alone).
-// PF (prompt prefill): the grid's rows are (token, row) pairs r = tok * rows_real + row at positions P[0] + tok.
-// seq_off: length of the condition prefix in front of the tokens; cache position pos reads sequence column pos - seq_off.
-template <bool PF>
-__global__ void __launch_bounds__(256) lm_embed_kernel(const __half* __restrict__ emb, const float* __restrict__ inv_freq,
-                                                       const int64_t* __restrict__ seq, const int* __restrict__ P,
-                                                       float* __restrict__ x, int d, int n_q, int card, int max_seq,
-                                                       int batch, float pos_scale, int rows_real, bool sin_pos, int seq_off) {
-    const int r = blockIdx.x, b = (PF ? r % rows_real : r) % batch, pos = P[0] + (PF ? r / rows_real : 0);
+// Shared by the per-generation kernel below and the slot-mode kernel (each row at its own position).
+__device__ __forceinline__ void embed_row(const __half* __restrict__ emb, const float* __restrict__ inv_freq,
+                                          const int64_t* __restrict__ seq, float* __restrict__ x, int r, int b, int pos,
+                                          int d, int n_q, int card, int max_seq, float pos_scale, bool sin_pos, int seq_off) {
     __shared__ int tok[16];
     if (threadIdx.x < n_q) {
         long long t = seq[((size_t)b * n_q + threadIdx.x) * max_seq + pos - seq_off];
@@ -71,6 +73,28 @@ __global__ void __launch_bounds__(256) lm_embed_kernel(const __half* __restrict_
         }
         x[(size_t)r * d + i] = v;
     }
+}
+
+// PF (prompt prefill): the grid's rows are (token, row) pairs r = tok * rows_real + row at positions P[0] + tok.
+// seq_off: length of the condition prefix in front of the tokens; cache position pos reads sequence column pos - seq_off.
+template <bool PF>
+__global__ void __launch_bounds__(256) lm_embed_kernel(const __half* __restrict__ emb, const float* __restrict__ inv_freq,
+                                                       const int64_t* __restrict__ seq, const int* __restrict__ P,
+                                                       float* __restrict__ x, int d, int n_q, int card, int max_seq,
+                                                       int batch, float pos_scale, int rows_real, bool sin_pos, int seq_off) {
+    const int r = blockIdx.x, b = (PF ? r % rows_real : r) % batch, pos = P[0] + (PF ? r / rows_real : 0);
+    embed_row(emb, inv_freq, seq, x, r, b, pos, d, n_q, card, max_seq, pos_scale, sin_pos, seq_off);
+}
+
+// Slot mode (continuous batching): row r belongs to slot r % slots (cond rows [0, slots), null rows [slots, 2 slots)) and
+// reads that slot's sequence at the slot's own position.  An inactive slot embeds a finite, unused row.
+__global__ void __launch_bounds__(256) lm_embed_slot_kernel(const __half* __restrict__ emb, const float* __restrict__ inv_freq,
+                                                            const int64_t* __restrict__ seq, const int* __restrict__ slot_state,
+                                                            float* __restrict__ x, int d, int n_q, int card, int max_seq,
+                                                            int slots, float pos_scale, bool sin_pos) {
+    const int r = blockIdx.x, b = r % slots;
+    embed_row(emb, inv_freq, seq, x, r, b, slot_state[b * ACB_LM_SLOT_STRIDE + ACB_SLOT_POS], d, n_q, card, max_seq, pos_scale,
+              sin_pos, 0);
 }
 
 // Condition-prefix prefill (the `prepend` fuser, conditioners.py:1703-1763): the grid's rows are (position, row) pairs
@@ -426,6 +450,30 @@ __global__ void __launch_bounds__(128, 1) lm_gemm_wide_kernel(const __grid_const
     if (cs > 1) cg::this_cluster().sync();   // the other CTAs read this CTA's tile until here
 }
 
+// Slot mode's QKV epilogue as its own kernel: the QKV GEMM runs with the plain fp32 epilogue (EPI_F32, the same sums as
+// EPI_QKV / EPI_QKV_ROPE) into qkv [rows][3d], and this kernel does what those epilogues do at each row's own position: q to
+// q32 (fp32), k and v to the cache (fp16), q and k rotated first under rotary positions.  Only ACTIVE slots append to the cache.
+__global__ void __launch_bounds__(256) lm_qkv_slot_kernel(const float* __restrict__ qkv, const int* __restrict__ slot_state,
+                                                          float* __restrict__ q32, __half* __restrict__ kc, __half* __restrict__ vc,
+                                                          int d, int H, int cache_len, int slots, const float* __restrict__ rope_freq,
+                                                          float pos_scale, bool rope) {
+    const int row = blockIdx.x, s = row % slots;
+    const int pos = slot_state[s * ACB_LM_SLOT_STRIDE + ACB_SLOT_POS];
+    const bool live = slot_state[s * ACB_LM_SLOT_STRIDE + ACB_SLOT_STATUS] == SLOT_ACTIVE;
+    const float* src = qkv + (size_t)row * 3 * d;
+    for (int n = threadIdx.x; n < 3 * d; n += 256) {
+        const int which = n >= 2 * d ? 2 : (n >= d ? 1 : 0), nn = n - which * d;
+        float v = src[n];
+        if (rope && which < 2) v = rope_rotate(rope_freq, pos_scale, half_round(v), half_round(src[n ^ 1]), nn & 63, pos);
+        if (which == 0) {
+            q32[(size_t)row * d + nn] = v;
+        } else if (live) {
+            __half* cache = which == 2 ? vc : kc;
+            cache[(((size_t)row * H + (nn >> 6)) * cache_len + pos) * 64 + (nn & 63)] = __float2half_rn(v);
+        }
+    }
+}
+
 // ------------------------------------------------------------------------------------------------ attention (1 query)
 struct AttnParams {
     const float* q; int q_nsplit; size_t q_split_stride;  // q[s][row][d] fp32 partial sums
@@ -564,15 +612,128 @@ __global__ void __launch_bounds__(ATT_WARPS * 32) lm_attn2_kernel(AttnParams p) 
     }
 }
 
+
+// Slot mode: lm_attn2_kernel with each row at its own slot's position (a separate copy: the decode kernel stays as it is).
+// Row r of slot r % slots (p.rows_real = slots) attends to its slot's positions [0, pos]; the rows of a slot that is not ACTIVE
+// attend to no key and write zeros.
+__global__ void __launch_bounds__(ATT_WARPS * 32) lm_attn2_slot_kernel(AttnParams p, const int* __restrict__ slot_state) {
+    extern __shared__ __align__(16) unsigned char att2sm[];   // [warp][depth][K | V][32 lanes][16 B]
+    __shared__ float wm[ATT_WARPS], wl[ATT_WARPS], wacc[ATT_WARPS][64];
+    const int h = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int qrow = blockIdx.y, row = qrow;
+    const int sl = lane & 7, pg = lane >> 3;
+    const int* slot = slot_state + (row % p.rows_real) * ACB_LM_SLOT_STRIDE;
+    if (slot[ACB_SLOT_STATUS] != SLOT_ACTIVE) {   // block-uniform
+        if (tid < 64) p.out[(size_t)qrow * p.d + h * 64 + tid] = __float2half_rn(0.f);
+        return;
+    }
+    const int n = slot[ACB_SLOT_POS] + 1;
+    const size_t base = ((size_t)row * p.H + h) * p.cache_len * 64 + sl * 8;
+    const __half* kb = p.kc + base;
+    const __half* vb = p.vc + base;
+    const uint32_t ring = smem_u32(att2sm) + (uint32_t)(warp * ATT2_DEPTH * 1024 + lane * 16);
+    // iteration k of this warp covers positions (k * 8 + warp) * 4 + pg
+    const int n_it = (n + 31 - warp * 4) / 32 > 0 ? (n - warp * 4 + 31) / 32 : 0;   // iterations with at least one live position group
+    auto issue = [&](int k) {
+        if (k < n_it) {
+            const int pp = (k * ATT_WARPS + warp) * 4 + pg;
+            if (pp < n) {
+                const uint32_t d = ring + (uint32_t)((k % ATT2_DEPTH) * 1024);
+                asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d), "l"(kb + (size_t)pp * 64) : "memory");
+                asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d + 512u), "l"(vb + (size_t)pp * 64) : "memory");
+            }
+        }
+        asm volatile("cp.async.commit_group;" ::: "memory");
+    };
+#pragma unroll
+    for (int k = 0; k < ATT2_DEPTH - 1; ++k) issue(k);
+
+    float q[8];
+    {
+        const float4* qp = reinterpret_cast<const float4*>(p.q + (size_t)qrow * p.d + h * 64 + sl * 8);
+        const float4 qa = qp[0], qb = qp[1];
+        q[0] = half_round(qa.x) * p.scale; q[1] = half_round(qa.y) * p.scale; q[2] = half_round(qa.z) * p.scale;
+        q[3] = half_round(qa.w) * p.scale; q[4] = half_round(qb.x) * p.scale; q[5] = half_round(qb.y) * p.scale;
+        q[6] = half_round(qb.z) * p.scale; q[7] = half_round(qb.w) * p.scale;
+    }
+    OnlineSM st;
+    st.m = -INFINITY; st.l = 0.f;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) st.acc[e] = 0.f;
+
+    for (int k = 0; k < n_it; ++k) {                 // warp-uniform trip count (the shuffles need all 32 lanes)
+        issue(k + ATT2_DEPTH - 1);
+        asm volatile("cp.async.wait_group %0;" ::"n"(ATT2_DEPTH - 1) : "memory");   // iteration k's copies of this lane have landed
+        const int pp = (k * ATT_WARPS + warp) * 4 + pg;
+        const uint32_t sa = ring + (uint32_t)((k % ATT2_DEPTH) * 1024);
+        uint4 kv = make_uint4(0, 0, 0, 0), vv = make_uint4(0, 0, 0, 0);
+        if (pp < n) {
+            asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(kv.x), "=r"(kv.y), "=r"(kv.z), "=r"(kv.w) : "r"(sa));
+            asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(vv.x), "=r"(vv.y), "=r"(vv.z), "=r"(vv.w) : "r"(sa + 512u));
+        }
+        const __half2* k2 = reinterpret_cast<const __half2*>(&kv);
+        float s = 0.f;
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            const float2 f = __half22float2(k2[e]);
+            s = fmaf(q[2 * e], f.x, s);
+            s = fmaf(q[2 * e + 1], f.y, s);
+        }
+        s += __shfl_xor_sync(0xffffffffu, s, 1);
+        s += __shfl_xor_sync(0xffffffffu, s, 2);
+        s += __shfl_xor_sync(0xffffffffu, s, 4);
+        if (pp < n) {
+            const float mn = fmaxf(st.m, s);
+            const float corr = __expf(st.m - mn);   // exp(-inf) = 0 on the first position
+            const float pw = __expf(s - mn);
+            st.l = st.l * corr + pw;
+            const __half2* v2 = reinterpret_cast<const __half2*>(&vv);
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const float2 f = __half22float2(v2[e]);
+                st.acc[2 * e] = fmaf(pw, f.x, st.acc[2 * e] * corr);
+                st.acc[2 * e + 1] = fmaf(pw, f.y, st.acc[2 * e + 1] * corr);
+            }
+            st.m = mn;
+        }
+    }
+    asm volatile("cp.async.wait_group 0;" ::: "memory");
+    // merge the 4 position groups of the warp, then the warps
+#pragma unroll
+    for (int o = 8; o <= 16; o <<= 1) {
+        const float m2 = __shfl_xor_sync(0xffffffffu, st.m, o), l2 = __shfl_xor_sync(0xffffffffu, st.l, o);
+        float a2[8];
+#pragma unroll
+        for (int e = 0; e < 8; ++e) a2[e] = __shfl_xor_sync(0xffffffffu, st.acc[e], o);
+        osm_merge(st, m2, l2, a2);
+    }
+    if (pg == 0) {
+        if (sl == 0) { wm[warp] = st.m; wl[warp] = st.l; }
+#pragma unroll
+        for (int e = 0; e < 8; ++e) wacc[warp][sl * 8 + e] = st.acc[e];
+    }
+    __syncthreads();
+    if (tid < 64) {
+        float mx = wm[0];
+#pragma unroll
+        for (int w = 1; w < ATT_WARPS; ++w) mx = fmaxf(mx, wm[w]);
+        float l = 0.f, o = 0.f;
+#pragma unroll
+        for (int w = 0; w < ATT_WARPS; ++w) {
+            const float cw = wm[w] == -INFINITY ? 0.f : __expf(wm[w] - mx);
+            l = fmaf(wl[w], cw, l);
+            o = fmaf(wacc[w][tid], cw, o);
+        }
+        p.out[(size_t)qrow * p.d + h * 64 + tid] = __float2half_rn(o / l);
+    }
+}
+
 // Cross attention over the (short) text condition: one WARP per (row, head), lane = text position for the scores,
 // lane = 2 output dims for the weighted sum.  K/V were computed once per generate() (acb_lm_begin).
-template <bool PF>
-__global__ void __launch_bounds__(256) lm_cross_attn_kernel(AttnParams p, int rows) {
+// The warp's query row `row`, head h attends to the first n >= 1 text positions of cache row `crow`.
+__device__ __forceinline__ void cross_attn_body(const AttnParams& p, int row, int h, int crow, int n) {
     __shared__ float qs[8][64];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int pair = blockIdx.x * 8 + warp;          // (row, head) index
-    if (pair >= rows * p.H) return;                  // warp-uniform
-    const int row = pair / p.H, h = pair % p.H, n = p.fixed_len;
     {
         const float* qp = p.q + (size_t)row * p.d + h * 64 + lane * 2;
         float2 part[ACB_LM_MAX_SPLIT];
@@ -586,7 +747,7 @@ __global__ void __launch_bounds__(256) lm_cross_attn_kernel(AttnParams p, int ro
         qs[warp][lane * 2 + 1] = half_round(a1) * p.scale;
     }
     __syncwarp();
-    const size_t base = ((size_t)(PF ? row % p.rows_real : row) * p.H + h) * p.cache_len * 64;   // K / V of the generation row
+    const size_t base = ((size_t)crow * p.H + h) * p.cache_len * 64;
     float mx = -INFINITY, l = 0.f, o0 = 0.f, o1 = 0.f;
     for (int t0 = 0; t0 < n; t0 += 32) {             // chunks of 32 text positions (online softmax across chunks)
         const int t = t0 + lane;
@@ -621,6 +782,28 @@ __global__ void __launch_bounds__(256) lm_cross_attn_kernel(AttnParams p, int ro
         mx = cm;
     }
     *reinterpret_cast<__half2*>(p.out + (size_t)row * p.d + h * 64 + lane * 2) = __floats2half2_rn(o0 / l, o1 / l);
+}
+
+template <bool PF>
+__global__ void __launch_bounds__(256) lm_cross_attn_kernel(AttnParams p, int rows) {
+    const int pair = blockIdx.x * 8 + (threadIdx.x >> 5);   // (row, head) index
+    if (pair >= rows * p.H) return;                         // warp-uniform
+    const int row = pair / p.H, h = pair % p.H;
+    cross_attn_body(p, row, h, PF ? row % p.rows_real : row, p.fixed_len);   // K / V of the generation row
+}
+
+// Slot mode: row r attends to exactly its slot's own text length (p.rows_real = slots), not to a length shared by the batch,
+// so a request's result does not depend on the other requests' conditions.  A slot never admitted (length 0) writes zeros.
+__global__ void __launch_bounds__(256) lm_cross_attn_slot_kernel(AttnParams p, int rows, const int* __restrict__ slot_state) {
+    const int pair = blockIdx.x * 8 + (threadIdx.x >> 5);
+    if (pair >= rows * p.H) return;
+    const int row = pair / p.H, h = pair % p.H, lane = threadIdx.x & 31;
+    const int n = slot_state[(row % p.rows_real) * ACB_LM_SLOT_STRIDE + ACB_SLOT_TEXT_LEN];
+    if (n <= 0) {
+        *reinterpret_cast<__half2*>(p.out + (size_t)row * p.d + h * 64 + lane * 2) = __floats2half2_rn(0.f, 0.f);
+        return;
+    }
+    cross_attn_body(p, row, h, row, n);
 }
 
 // ------------------------------------------------------------------------------------------------ sampling
@@ -659,7 +842,9 @@ struct SampleParams {
 // descending order, ties by ascending index
 __device__ __forceinline__ bool before(float va, int ia, float vb, int ib) { return va > vb || (va == vb && ia < ib); }
 
-__global__ void __launch_bounds__(1024) lm_sample_kernel(SampleParams p) {
+// lm_sample_kernel and (SLOT) lm_sample_slot_kernel: CFG mix, sampling, first-max argmax and the write-back of block (k, b).
+template <bool SLOT>
+__device__ __forceinline__ void sample_impl(const SampleParams& p, int* slot_state) {
     extern __shared__ float sm[];
     float* pr = sm;                 // [card] logits -> probabilities
     float* sv = pr + p.card;        // [NP] sort values
@@ -669,14 +854,19 @@ __global__ void __launch_bounds__(1024) lm_sample_kernel(SampleParams p) {
     __shared__ int besti[32];
     __shared__ float s_scalar;
     const int k = blockIdx.x, b = blockIdx.y, tid = threadIdx.x, nt = blockDim.x;
+    int* st = SLOT ? slot_state + b * ACB_LM_SLOT_STRIDE : nullptr;
+    if (SLOT && st[ACB_SLOT_STATUS] != SLOT_ACTIVE) return;   // block-uniform
     const int card = p.card;
     const bool cfg = p.rows == 2 * p.batch, cfg3 = p.rows == 3 * p.batch;   // [cond; null] or [cond; style-only; null]
     const float* lc = p.logits + ((size_t)b * p.n_q + k) * card;
     const float* lu = p.logits + ((size_t)((cfg3 ? 2 : 1) * p.batch + b) * p.n_q + k) * card;
     const float* lw = p.logits + ((size_t)(p.batch + b) * p.n_q + k) * card;
-    const int cur_pos = p.pos ? p.pos[0] : 0;   // read once: the last block to finish advances it (below)
+    const int cur_pos = SLOT ? st[ACB_SLOT_POS] : (p.pos ? p.pos[0] : 0);   // read once: the last block to finish advances it
     const int col = cur_pos - p.seq_off;        // sequence column of the token this step consumed
-    const uint32_t step = p.pos ? (uint32_t)col : p.step;
+    const uint32_t step = (SLOT || p.pos) ? (uint32_t)col : p.step;
+    uint64_t slot_seed = 0;
+    if constexpr (SLOT)
+        slot_seed = (uint64_t)(uint32_t)st[ACB_SLOT_SEED_LO] | ((uint64_t)(uint32_t)st[ACB_SLOT_SEED_HI] << 32);
 
     for (int i = tid; i < card; i += nt) {
         float l = lc[i];
@@ -784,7 +974,8 @@ __global__ void __launch_bounds__(1024) lm_sample_kernel(SampleParams p) {
         // torch.multinomial(num_samples=1): argmax_i p_i / q_i, q ~ Exponential(1)
         for (int i = tid; i < card; i += nt) {
             const float qn = p.noise ? p.noise[((size_t)b * p.n_q + k) * card + i]
-                                     : exp1_noise(p.seed, step, (uint32_t)(b * p.n_q + k), (uint32_t)i);
+                                     : exp1_noise(SLOT ? slot_seed : p.seed, step,
+                                                  SLOT ? (uint32_t)k : (uint32_t)(b * p.n_q + k), (uint32_t)i);
             pr[i] = pr[i] / qn;
         }
         __syncthreads();
@@ -809,20 +1000,57 @@ __global__ void __launch_bounds__(1024) lm_sample_kernel(SampleParams p) {
             if (bestv[w] > bv || (bestv[w] == bv && besti[w] < bi)) { bv = bestv[w]; bi = besti[w]; }
         if (bi == 0x7fffffff) bi = 0;
         int tok = sorted_space ? si[bi] : bi;
-        if (p.tokens) p.tokens[(size_t)b * p.n_q + k] = tok;
-        if (p.seq) {
-            const int off = col + 1;
-            if (off < p.max_seq) {
-                if (!p.seq_mask[(size_t)k * p.max_seq + off]) tok = card;            // lm.py:555-556
-                int64_t* dst = p.seq + ((size_t)b * p.n_q + k) * p.max_seq + off;
-                if (*dst == -1) *dst = tok;                                           // lm.py:559-562
-            }
-            // the last (b, k) block to get here advances the position: pos[1] counts finished blocks
+        if constexpr (SLOT) {
+            const int off = col + 1;   // < the slot's seq_len while it is active
+            const size_t at = ((size_t)b * p.n_q + k) * p.max_seq + off;
+            if (!p.seq_mask[at]) tok = card;
+            if (p.seq[at] == -1) p.seq[at] = tok;
             __threadfence();
-            const int done = atomicAdd(p.pos + 1, 1);
-            if (done == (int)(gridDim.x * gridDim.y) - 1) { p.pos[1] = 0; p.pos[0] = cur_pos + 1; }
+            const int done = atomicAdd(st + ACB_SLOT_DONE, 1);
+            if (done == p.n_q - 1) {   // the slot's last block: advance it, and finish it after its last column
+                st[ACB_SLOT_DONE] = 0;
+                st[ACB_SLOT_POS] = off;
+                if (off >= st[ACB_SLOT_SEQ_LEN] - 1) st[ACB_SLOT_STATUS] = SLOT_FINISHED;
+            }
+        } else {
+            if (p.tokens) p.tokens[(size_t)b * p.n_q + k] = tok;
+            if (p.seq) {
+                const int off = col + 1;
+                if (off < p.max_seq) {
+                    if (!p.seq_mask[(size_t)k * p.max_seq + off]) tok = card;            // lm.py:555-556
+                    int64_t* dst = p.seq + ((size_t)b * p.n_q + k) * p.max_seq + off;
+                    if (*dst == -1) *dst = tok;                                           // lm.py:559-562
+                }
+                // the last (b, k) block to get here advances the position: pos[1] counts finished blocks
+                __threadfence();
+                const int done = atomicAdd(p.pos + 1, 1);
+                if (done == (int)(gridDim.x * gridDim.y) - 1) { p.pos[1] = 0; p.pos[0] = cur_pos + 1; }
+            }
         }
     }
+}
+
+__global__ void __launch_bounds__(1024) lm_sample_kernel(SampleParams p) { sample_impl<false>(p, nullptr); }
+
+// Slot mode's sampler: block (k, slot), slots not ACTIVE skipped.  Column, step and seed are the slot's own, and the noise is
+// Philox stream k of (seed, column) -- what lm_sample_kernel draws for item 0 of a generation, so a request samples as if
+// generated alone.  p.seq_mask is [slots][n_q][max_seq].  A known token (!= -1) stays, so a prompt written into the sequence
+// is consumed one column per step.  The last of the slot's n_q blocks advances its position; writing column seq_len - 1
+// finishes the slot.
+__global__ void __launch_bounds__(1024) lm_sample_slot_kernel(SampleParams p, int* __restrict__ slot_state) {
+    sample_impl<true>(p, slot_state);
+}
+
+// Admission: the slot starts at position 0 with its own sequence length, text length and seed.
+__global__ void lm_slot_admit_kernel(int* slot_state, int slot, int seq_len, int text_len, uint32_t seed_lo, uint32_t seed_hi) {
+    int* st = slot_state + slot * ACB_LM_SLOT_STRIDE;
+    st[ACB_SLOT_POS] = 0;
+    st[ACB_SLOT_STATUS] = SLOT_ACTIVE;
+    st[ACB_SLOT_SEQ_LEN] = seq_len;
+    st[ACB_SLOT_TEXT_LEN] = text_len;
+    st[ACB_SLOT_SEED_LO] = (int)seed_lo;
+    st[ACB_SLOT_SEED_HI] = (int)seed_hi;
+    st[ACB_SLOT_DONE] = 0;
 }
 
 __global__ void lm_f32_to_f16_kernel(const float* __restrict__ src, __half* __restrict__ dst, size_t n_valid, size_t n_total) {
@@ -840,6 +1068,7 @@ struct acb_lm {
     cudaGraph_t graph = nullptr;
     cudaGraphExec_t exec = nullptr;
     int batch = 0, rows = 0, rows_pad = 0, text_len = 0, seq_len = 0, sms = 132;
+    int slots = 0;                 // slot mode (acb_lm_begin_slots): batch = slots, rows = 2 * slots, per-slot device state
     int prefix_len = 0;            // condition-prefix positions in front of the tokens in the KV cache
     const float* prefix = nullptr; // [rows][prefix_len][d] fp32, set only while acb_lm_begin_prefix enqueues the prefix passes
     int launches = 0;
@@ -1037,7 +1266,9 @@ static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_la
 
     if (!gemms_only) {
         const bool sin_pos = c.positional_embedding != 1;
-        if (pf && pf_prefix) lm_embed_prefix_kernel<<<rows, 256, 0, s>>>(lm->prefix, lm->w.inv_freq, B.pos, B.x, d, lm->prefix_len,
+        if (lm->slots) lm_embed_slot_kernel<<<rows, 256, 0, s>>>((const __half*)lm->w.emb, lm->w.inv_freq, B.seq, B.slot_state, B.x, d,
+                                                                c.n_q, c.card, c.max_seq, lm->slots, c.pos_scale, sin_pos);
+        else if (pf && pf_prefix) lm_embed_prefix_kernel<<<rows, 256, 0, s>>>(lm->prefix, lm->w.inv_freq, B.pos, B.x, d, lm->prefix_len,
                                                                        c.pos_scale, rows_real, sin_pos);
         else if (pf) lm_embed_kernel<true><<<rows, 256, 0, s>>>((const __half*)lm->w.emb, lm->w.inv_freq, B.seq, B.pos, B.x, d, c.n_q,
                                                               c.card, c.max_seq, lm->batch, c.pos_scale, rows_real, sin_pos,
@@ -1080,17 +1311,34 @@ static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_la
             p.rope_freq = lm->w.rope_freq; p.pos_scale = c.pos_scale;
             const bool rope = c.positional_embedding != 0;
             const int ft2 = pf ? 1 : pick_ft2(3 * d, d, 1, ks, nt, lm->sms);
-            if (wide) ACB_TRY(rope ? launch_wide<EPI_QKV_ROPE>(lm->wmap[WM_QKV], lm->xmap_h16, l * 3 * d, p, ns, s)
+            if (lm->slots) {   // plain fp32 epilogue into part slot 0 (free between the LN and the out projection), then
+                               // the rotary + cache append at each row's own position
+                p.out_f32 = B.part; p.ld_out = 3 * d;
+                if (wide) ACB_TRY(launch_wide<EPI_F32>(lm->wmap[WM_QKV], lm->xmap_h16, l * 3 * d, p, ns, s));
+                else ACB_TRY(launch_gemm<EPI_F32>(nt, p, 1, s, ft2));
+                ++nl;
+                DBG("gemm_EPI_F32 (qkv)", l);
+                if (!gemms_only) {
+                    lm_qkv_slot_kernel<<<rows, 256, 0, s>>>(B.part, B.slot_state, B.q32, p.kc, p.vc, d, H, c.max_seq, lm->slots,
+                                                            lm->w.rope_freq, c.pos_scale, rope);
+                    ACB_LAUNCH_CHECK();
+                    ++nl;
+                    DBG("lm_qkv_slot_kernel", l);
+                }
+            } else if (wide) ACB_TRY(rope ? launch_wide<EPI_QKV_ROPE>(lm->wmap[WM_QKV], lm->xmap_h16, l * 3 * d, p, ns, s)
                                    : launch_wide<EPI_QKV>(lm->wmap[WM_QKV], lm->xmap_h16, l * 3 * d, p, ns, s));
             else if (pf) ACB_TRY(rope ? launch_gemm<EPI_QKV_PF_ROPE>(nt, p, 1, s, ft2) : launch_gemm<EPI_QKV_PF>(nt, p, 1, s, ft2));
             else ACB_TRY(rope ? launch_gemm<EPI_QKV_ROPE>(nt, p, 1, s, ft2) : launch_gemm<EPI_QKV>(nt, p, 1, s, ft2));
-            ++nl;
-            DBG("gemm_EPI_QKV", l);
+            if (!lm->slots) {
+                ++nl;
+                DBG("gemm_EPI_QKV", l);
+            }
         }
         if (!gemms_only) {
             AttnParams a{B.q32, 1, 0, (__half*)B.k_cache + l * kv_layer, (__half*)B.v_cache + l * kv_layer, (__half*)B.a16,
                          H, d, c.max_seq, B.pos, 0, scale, rows_real};
-            if (pf) lm_attn2_kernel<true><<<dim3(H, rows), ATT_WARPS * 32, ATT2_SMEM, s>>>(a);
+            if (lm->slots) { a.rows_real = lm->slots; lm_attn2_slot_kernel<<<dim3(H, rows), ATT_WARPS * 32, ATT2_SMEM, s>>>(a, B.slot_state); }
+            else if (pf) lm_attn2_kernel<true><<<dim3(H, rows), ATT_WARPS * 32, ATT2_SMEM, s>>>(a);
             else lm_attn2_kernel<false><<<dim3(H, rows), ATT_WARPS * 32, ATT2_SMEM, s>>>(a);
             ACB_LAUNCH_CHECK();
             ++nl;
@@ -1107,7 +1355,10 @@ static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_la
                 AttnParams a{B.part, nsq, part_stride, (__half*)B.ck_cache + l * ckv_layer,
                              (__half*)B.cv_cache + l * ckv_layer, (__half*)B.a16, H, d, c.max_text, B.pos, lm->text_len,
                              scale, rows_real};
-                if (pf) lm_cross_attn_kernel<true><<<acb_ceil_div(rows * H, 8), 256, 0, s>>>(a, rows);
+                if (lm->slots) {
+                    a.rows_real = lm->slots;
+                    lm_cross_attn_slot_kernel<<<acb_ceil_div(rows * H, 8), 256, 0, s>>>(a, rows, B.slot_state);
+                } else if (pf) lm_cross_attn_kernel<true><<<acb_ceil_div(rows * H, 8), 256, 0, s>>>(a, rows);
                 else lm_cross_attn_kernel<false><<<acb_ceil_div(rows * H, 8), 256, 0, s>>>(a, rows);
                 ACB_LAUNCH_CHECK();
                 ++nl;
@@ -1151,7 +1402,12 @@ static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_la
                         lm->samp.temp, lm->samp.top_p, lm->samp.cfg_coef, lm->samp.seed, 0, lm->samp.cfg_coef_beta,
                         lm->prefix_len};
         size_t smem = ((size_t)c.card + 2 * (size_t)NP) * sizeof(float);
-        lm_sample_kernel<<<dim3(c.n_q, lm->batch), 1024, smem, s>>>(sp);
+        if (lm->slots) {
+            sp.seq_mask = B.slot_mask; sp.pos = nullptr;
+            lm_sample_slot_kernel<<<dim3(c.n_q, lm->slots), 1024, smem, s>>>(sp, B.slot_state);
+        } else {
+            lm_sample_kernel<<<dim3(c.n_q, lm->batch), 1024, smem, s>>>(sp);
+        }
         ACB_LAUNCH_CHECK();
         ++nl;
         DBG("lm_sample_kernel", -1);
@@ -1197,6 +1453,12 @@ extern "C" int acb_lm_create(const acb_lm_config* cfg, const acb_lm_weights* w, 
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_attn2_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_attn2_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT2_SMEM);
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_attn2_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+    if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_attn2_slot_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT2_SMEM);
+    if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_attn2_slot_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+    if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_cross_attn_slot_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+    if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_embed_slot_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+    if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_qkv_slot_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+    if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_sample_slot_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_cross_attn_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_ln_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_embed_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
@@ -1284,6 +1546,21 @@ static int prefill_passes(acb_lm* lm, cudaStream_t s, int pos0, int n, bool pref
     return ACB_OK;
 }
 
+// Capture one decode step; its kernels are chained by plain stream-order edges.  (Launched with programmatic dependent launch,
+// the same kernels gave wrong logits on the H100 once the KV cache held more than a few positions, for a cause not found.)
+static int capture_step(acb_lm* lm) {
+    drop_graph(lm);
+    ACB_CHECK_CUDA(cudaStreamBeginCapture(lm->capture_stream, cudaStreamCaptureModeThreadLocal));
+    int rc = enqueue_step(lm, lm->capture_stream, nullptr, &lm->launches, false, true);
+    cudaError_t e = cudaStreamEndCapture(lm->capture_stream, &lm->graph);
+    if (rc == ACB_OK && e == cudaSuccess) e = cudaGraphInstantiate(&lm->exec, lm->graph, 0);
+    if (rc == ACB_OK && e == cudaSuccess) return ACB_OK;
+    cudaGetLastError();
+    drop_graph(lm);
+    if (rc == ACB_OK) acb_set_error("acb_lm_begin: graph capture failed: %s", cudaGetErrorString(e));
+    return rc != ACB_OK ? rc : ACB_ERR_CUDA;
+}
+
 extern "C" int acb_lm_begin(acb_lm_t* lm, const float* cross, int batch, int rows, int text_len, int seq_len,
                             const acb_lm_sampling* sampling, void* stream) {
     return acb_lm_begin_prefix(lm, cross, nullptr, 0, batch, rows, text_len, seq_len, sampling, stream);
@@ -1306,6 +1583,7 @@ extern "C" int acb_lm_begin_prefix(acb_lm_t* lm, const float* cross, const float
     ACB_REQUIRE(!c.cross_attention || cross, "acb_lm_begin: the model has cross attention, a condition tensor is required"
                 " (the reference asserts the same, transformer.py:553-556)");
     ACB_REQUIRE(!cross || (text_len >= 1 && text_len <= c.max_text), "acb_lm_begin: text_len %d out of range", text_len);
+    lm->slots = 0;
     cudaStream_t s = (cudaStream_t)stream;
     const int d = c.dim, H = c.num_heads;
     if (rows > 64) {   // the wide GEMM's activation maps: rows past `rows` of a box are zero-filled
@@ -1352,18 +1630,7 @@ extern "C" int acb_lm_begin_prefix(acb_lm_t* lm, const float* cross, const float
         if (smem > 48 * 1024)
             ACB_CHECK_CUDA(cudaFuncSetAttribute(lm_sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     }
-    // capture one decode step; its kernels are chained by plain stream-order edges.  (Launched with programmatic dependent launch,
-    // the same kernels gave wrong logits on the H100 once the KV cache held more than a few positions, for a cause not found.)
-    drop_graph(lm);
-    ACB_CHECK_CUDA(cudaStreamBeginCapture(lm->capture_stream, cudaStreamCaptureModeThreadLocal));
-    int rc = enqueue_step(lm, lm->capture_stream, nullptr, &lm->launches, false, true);
-    cudaError_t e = cudaStreamEndCapture(lm->capture_stream, &lm->graph);
-    if (rc == ACB_OK && e == cudaSuccess) e = cudaGraphInstantiate(&lm->exec, lm->graph, 0);
-    if (rc == ACB_OK && e == cudaSuccess) return ACB_OK;
-    cudaGetLastError();
-    drop_graph(lm);
-    if (rc == ACB_OK) acb_set_error("acb_lm_begin: graph capture failed: %s", cudaGetErrorString(e));
-    return rc != ACB_OK ? rc : ACB_ERR_CUDA;
+    return capture_step(lm);
 }
 
 // Prompt prefill: consume sequence columns [pos0, pos0 + n_tokens) of every row (their tokens are already in buffers.seq)
@@ -1371,9 +1638,104 @@ extern "C" int acb_lm_begin_prefix(acb_lm_t* lm, const float* cross, const float
 // pos = prefix_len + pos0 + n_tokens on the device.
 extern "C" int acb_lm_prefill(acb_lm_t* lm, int pos0, int n_tokens, void* stream) {
     ACB_REQUIRE(lm && lm->rows > 0, "acb_lm_prefill: call acb_lm_begin first");
+    ACB_REQUIRE(!lm->slots, "acb_lm_prefill: a slot session consumes prompts one column per step");
     ACB_REQUIRE(pos0 >= 0 && n_tokens >= 0 && pos0 + n_tokens < lm->seq_len, "acb_lm_prefill: positions [%d, %d) exceed the sequence (%d)",
                 pos0, pos0 + n_tokens, lm->seq_len);
     return prefill_passes(lm, (cudaStream_t)stream, lm->prefix_len + pos0, n_tokens, false);
+}
+
+// ------------------------------------------------------------------------------------------------ slot mode
+extern "C" int acb_lm_begin_slots(acb_lm_t* lm, int slots, int max_text, int seq_len_max, const acb_lm_sampling* sampling,
+                                  void* stream) {
+    ACB_REQUIRE(lm && sampling, "acb_lm_begin_slots: null argument");
+    const acb_lm_config& c = lm->cfg;
+    ACB_REQUIRE(lm->buf.slot_state && lm->buf.slot_mask, "acb_lm_begin_slots: buffers.slot_state and slot_mask are required");
+    ACB_REQUIRE(slots >= 1 && slots <= ACB_LM_MAX_SLOTS && 2 * slots <= c.max_rows, "acb_lm_begin_slots: slots %d not in [1, %d] "
+                "or 2 * slots > max_rows %d", slots, ACB_LM_MAX_SLOTS, c.max_rows);
+    ACB_REQUIRE(seq_len_max >= 2 && seq_len_max <= c.max_seq, "acb_lm_begin_slots: seq_len_max %d not in [2, max_seq %d]",
+                seq_len_max, c.max_seq);
+    ACB_REQUIRE(!c.cross_attention || (max_text >= 1 && max_text <= c.max_text), "acb_lm_begin_slots: max_text %d not in [1, %d]",
+                max_text, c.max_text);
+    if (sampling->cfg_coef_beta != 0.f) {
+        acb_set_error("acb_lm_begin_slots: double CFG (cfg_coef_beta) is not built in slot mode: a session is [cond; null] rows");
+        return ACB_ERR_UNSUPPORTED;
+    }
+    ACB_REQUIRE(!sampling->noise_from_buffer, "acb_lm_begin_slots: slot mode samples with the on-device Philox noise only");
+    const int rows = 2 * slots;
+    if (rows > 64 && (c.ffn_dim % 64 != 0 || (c.n_q * c.card) % 64 != 0)) {
+        acb_set_error("acb_lm_begin_slots: rows %d > 64 run the wide GEMM, which needs ffn_dim (%d) and n_q * card (%d) to be "
+                      "multiples of 64", rows, c.ffn_dim, c.n_q * c.card);
+        return ACB_ERR_UNSUPPORTED;
+    }
+    cudaStream_t s = (cudaStream_t)stream;
+    const int d = c.dim;
+    if (rows > 64) {
+        const int npad = wide_npad(rows);
+        ACB_TRY(encode_map(&lm->xmap_h16, lm->buf.h16, d, rows, npad));
+        ACB_TRY(encode_map(&lm->xmap_a16, lm->buf.a16, d, rows, npad));
+        ACB_TRY(encode_map(&lm->xmap_f16, lm->buf.f16, c.ffn_dim, rows, npad));
+    }
+    lm->slots = slots; lm->batch = slots; lm->rows = rows;
+    lm->rows_pad = rows > 64 ? wide_npad(rows) : 8 * nt_for_rows(rows);
+    lm->text_len = max_text; lm->seq_len = seq_len_max; lm->prefix_len = 0; lm->prefix = nullptr;
+    lm->samp = *sampling;
+    lm->has_cross = c.cross_attention != 0;
+    ACB_CHECK_CUDA(cudaMemsetAsync(lm->buf.h16, 0, (size_t)lm->rows_pad * d * sizeof(__half), s));
+    ACB_CHECK_CUDA(cudaMemsetAsync(lm->buf.a16, 0, (size_t)lm->rows_pad * d * sizeof(__half), s));
+    ACB_CHECK_CUDA(cudaMemsetAsync(lm->buf.f16, 0, (size_t)lm->rows_pad * c.ffn_dim * sizeof(__half), s));
+    ACB_CHECK_CUDA(cudaMemsetAsync(lm->buf.slot_state, 0, (size_t)slots * ACB_LM_SLOT_STRIDE * sizeof(int), s));   // all INACTIVE
+    int NP = 1;
+    while (NP < c.card) NP <<= 1;
+    const size_t smem = ((size_t)c.card + 2 * (size_t)NP) * sizeof(float);
+    if (smem > 48 * 1024)
+        ACB_CHECK_CUDA(cudaFuncSetAttribute(lm_sample_slot_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    return capture_step(lm);
+}
+
+extern "C" int acb_lm_admit(acb_lm_t* lm, int slot, const float* cross, int text_len, int seq_len, uint64_t seed, void* stream) {
+    ACB_REQUIRE(lm && lm->slots > 0, "acb_lm_admit: call acb_lm_begin_slots first");
+    const acb_lm_config& c = lm->cfg;
+    ACB_REQUIRE(slot >= 0 && slot < lm->slots, "acb_lm_admit: slot %d not in [0, %d)", slot, lm->slots);
+    ACB_REQUIRE(seq_len >= 2 && seq_len <= lm->seq_len, "acb_lm_admit: seq_len %d not in [2, %d]", seq_len, lm->seq_len);
+    ACB_REQUIRE(!lm->has_cross || (cross && text_len >= 1 && text_len <= lm->text_len),
+                "acb_lm_admit: the model has cross attention: a condition of 1 .. %d text positions is required (got %d)",
+                lm->text_len, text_len);
+    cudaStream_t s = (cudaStream_t)stream;
+    if (lm->has_cross) {
+        // cross K/V of the slot's cond row (slot) and null row (slots + slot), each staged and projected on its own: the
+        // EPI_CROSSKV epilogue writes cache row R / text_len = 0 of the destination pointer
+        const int d = c.dim, H = c.num_heads;
+        const size_t ckv_layer = (size_t)c.max_rows * H * c.max_text * 64, row_elems = (size_t)H * c.max_text * 64;
+        const size_t M = (size_t)text_len, Mpad = (M + 63) / 64 * 64;
+        for (int half = 0; half < 2; ++half) {
+            const int dst = half ? lm->slots + slot : slot;
+            lm_f32_to_f16_kernel<<<(unsigned)((Mpad * d + 255) / 256), 256, 0, s>>>(cross + (size_t)half * M * d,
+                                                                                   (__half*)lm->buf.cross16, M * d, Mpad * d);
+            ACB_LAUNCH_CHECK();
+            for (int l = 0; l < c.num_layers; ++l)
+                for (size_t r0 = 0; r0 < M; r0 += 64) {
+                    int ks = 0;
+                    pick_split(2 * d, d, lm->sms, false, &ks);
+                    GemmParams p = base_gemm((const __half*)lm->w.w_ckv + (size_t)l * 2 * d * d,
+                                             (const __half*)lm->buf.cross16 + r0 * d, 2 * d, d, (int)min((size_t)64, M - r0), ks);
+                    p.kc = (__half*)lm->buf.ck_cache + l * ckv_layer + dst * row_elems;
+                    p.vc = (__half*)lm->buf.cv_cache + l * ckv_layer + dst * row_elems;
+                    p.d = d; p.H = H; p.cache_len = c.max_text; p.text_len = text_len; p.row0 = (int)r0;
+                    ACB_TRY(launch_gemm<EPI_CROSSKV>(8, p, 1, s));
+                }
+        }
+    }
+    lm_slot_admit_kernel<<<1, 1, 0, s>>>(lm->buf.slot_state, slot, seq_len, lm->has_cross ? text_len : 0, (uint32_t)seed,
+                                         (uint32_t)(seed >> 32));
+    ACB_LAUNCH_CHECK();
+    return ACB_OK;
+}
+
+extern "C" int acb_lm_slot_status(acb_lm_t* lm, int* out, void* stream) {
+    ACB_REQUIRE(lm && lm->slots > 0 && out, "acb_lm_slot_status: call acb_lm_begin_slots first");
+    ACB_CHECK_CUDA(cudaMemcpy2DAsync(out, 2 * sizeof(int), lm->buf.slot_state, ACB_LM_SLOT_STRIDE * sizeof(int), 2 * sizeof(int),
+                                     lm->slots, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+    return ACB_OK;
 }
 
 extern "C" int acb_lm_uses_pdl(const acb_lm_t*) { return 0; }

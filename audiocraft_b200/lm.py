@@ -57,6 +57,7 @@ class LMModel:
         self._shape = None
         self._debug_noise_fn = None
         self.launches_per_step = 0
+        self._session = None      # the batching.SlotSession that owns the decode handle, if any
         with torch.cuda.device(self.device):
             self._load_weights(state_dict, cfg)
 
@@ -148,6 +149,7 @@ class LMModel:
         if shape is not None and rows <= shape[0] and seq_len <= shape[1] and text_len <= shape[2] and batch <= shape[3]:
             return
         self._destroy()
+        self._session = None
         dev, d, H, L = self.device, self.dim, self.num_heads, self.num_layers
         max_rows = rows if shape is None else max(rows, shape[0])
         max_seq = seq_len if shape is None else max(seq_len, shape[1])
@@ -181,12 +183,15 @@ class LMModel:
         b['seq_mask'] = torch.zeros((self.n_q, max_seq), device=dev, dtype=torch.uint8)
         b['pos'] = torch.zeros(4, device=dev, dtype=torch.int32)
         b['noise'] = torch.ones((max_batch, self.n_q, self.card), device=dev, dtype=f32)
+        # slot mode (batching.SlotSession): per-slot device state and per-slot pattern masks, B = slots
+        b['slot_state'] = torch.zeros((max_batch, _lib.ACB_LM_SLOT_STRIDE), device=dev, dtype=torch.int32)
+        b['slot_mask'] = torch.zeros((max_batch, self.n_q, max_seq), device=dev, dtype=torch.uint8)
         self._bufs = b
         cfg = self._config(max_rows, max_seq, max_text)
         wts = self._weights()
         bufs = _lib.LMBuffers(*[_lib.ptr(b[n]) for n in ('x', 'h16', 'a16', 'f16', 'q32', 'part', 'logits', 'k_cache',
                                                          'v_cache', 'ck_cache', 'cv_cache', 'cross16', 'seq',
-                                                         'seq_mask', 'pos', 'noise')])
+                                                         'seq_mask', 'pos', 'noise', 'slot_state', 'slot_mask')])
         handle = C.c_void_p()
         _lib.check(self._lib.acb_lm_create(C.byref(cfg), C.byref(wts), C.byref(bufs), C.byref(handle)), 'lm_create')
         self._handle = handle
@@ -244,6 +249,7 @@ class LMModel:
         return prefix, prefix.shape[1]
 
     def _begin(self, cross, prefix, P, B, rows, text_len, S, samp):
+        self._session = None   # a slot session's captured step is replaced
         _lib.check(self._lib.acb_lm_begin_prefix(self._handle, _lib.ptr(cross), _lib.ptr(prefix), P, B, rows, text_len, S,
                                                  C.byref(samp), _lib.stream()), 'lm_begin')
 

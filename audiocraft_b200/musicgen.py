@@ -212,6 +212,16 @@ class BaseGenModel:
     def _prepare_melody(self, descriptions, melody_wavs, melody_sample_rate):
         raise NotImplementedError("this model has no melody ('self_wav') conditioner; use a MusicGen-melody model")
 
+    # -- continuous batching
+    def continuous(self, slots: int = 32, poll_steps: tp.Optional[int] = None, max_text: int = 64,
+                   return_tokens: bool = False):
+        """A `batching.ContinuousGenerator` over this model: up to `slots` requests decode side by side, each admitted when a
+        slot frees and retired when its last frame is sampled, with the current generation parameters.  `submit(description,
+        duration, prompt, prompt_sample_rate)` returns a request id; `poll()` / `run()` return `(request_id, wav[, tokens])`
+        as requests finish, each equal to that request generated alone.  `max_text` bounds a description's text positions."""
+        from .batching import ContinuousGenerator
+        return ContinuousGenerator(self, slots, poll_steps, max_text, return_tokens)
+
 
 def _sampling_params(use_sampling, top_k, top_p, temperature, cfg_coef, two_step_cfg):
     return {'use_sampling': use_sampling, 'temp': temperature, 'top_k': top_k, 'top_p': top_p, 'cfg_coef': cfg_coef,

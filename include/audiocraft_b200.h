@@ -217,8 +217,13 @@ typedef struct {
     uint8_t* seq_mask; /* [n_q][max_seq]     pattern validity mask (codebooks_patterns.py:130-152) */
     int32_t* pos;      /* [4] device ints: pos (tokens in the KV cache), rows, batch, text_len */
     float* noise;      /* [B][n_q][card] Exponential(1) noise, read when sampling.noise_from_buffer != 0 */
+    /* slot mode only (acb_lm_begin_slots; NULL otherwise), with B = slots in seq above: */
+    int32_t* slot_state; /* [slots][ACB_LM_SLOT_STRIDE] per-slot position, status, lengths and seed (written by the library) */
+    uint8_t* slot_mask;  /* [slots][n_q][max_seq] each slot's pattern validity mask (written by the caller before acb_lm_admit) */
 } acb_lm_buffers;
 
+#define ACB_LM_SLOT_STRIDE 8     /* int32 words of slot_state per slot */
+#define ACB_LM_MAX_SLOTS 128     /* slots of a session: rows = 2 * slots <= ACB_LM_MAX_ROWS */
 #define ACB_LM_MAX_SPLIT 8
 #define ACB_LM_PART_SLOTS 16
 #define ACB_LM_PREFILL_ROWS 64   /* (token, row) pairs one prefill pass handles = the tallest GEMM tile; above 64 rows a pass
@@ -274,8 +279,31 @@ int acb_lm_steps(acb_lm_t* lm, int n_steps, void* stream);
  * buffers must hold max(ACB_LM_PREFILL_ROWS, acb_lm_rows_pad(rows)) rows. */
 int acb_lm_prefill(acb_lm_t* lm, int pos0, int n_tokens, void* stream);
 
+/* Slot mode (continuous batching): a session of `slots` independent requests in the CFG layout, slot s owning rows s (cond)
+ * and slots + s (null), rows = 2 * slots <= max_rows, 1 <= slots <= ACB_LM_MAX_SLOTS.  Requests enter free slots between
+ * steps (acb_lm_admit) and leave when their last column is sampled, while the other slots keep decoding; every slot has its
+ * own position, sequence length, text length and seed.  The GEMMs run on all rows whichever slots are busy, so their regime
+ * and K split are fixed for the session.  Each slot attends to exactly its own text length, and its noise is Philox stream k
+ * of (its seed, column) -- what acb_lm_begin draws for item 0 -- so a request's tokens are those of the same request
+ * generated alone (bit for bit where both run the same GEMM regime, i.e. up to 64 rows).  Needs buffers.slot_state and
+ * buffers.slot_mask.  Shared sampling options; cfg_coef_beta != 0 returns ACB_ERR_UNSUPPORTED and noise_from_buffer is
+ * refused.  Marks every slot inactive and captures the session's step graph, which acb_lm_steps then launches.
+ * max_text <= max_text of the config bounds the admitted conditions, seq_len_max <= max_seq their sequences. */
+int acb_lm_begin_slots(acb_lm_t* lm, int slots, int max_text, int seq_len_max, const acb_lm_sampling* sampling, void* stream);
+
+/* Admit a request into `slot` (free: never used or finished) between steps: writes the slot's cross-attention K/V from cross,
+ * the fp32 condition [2][text_len][d] ([cond; null] rows, NULL without cross attention), and starts the slot at column 0 with
+ * sequence length seq_len and the Philox key seed.  The caller first writes the slot's delay-pattern sequence into
+ * buffers.seq[slot] (-1 where unknown; known prompt tokens are kept and consumed one column per step) and its mask into
+ * buffers.slot_mask[slot].  After seq_len - 1 steps the slot has written column seq_len - 1 and is finished. */
+int acb_lm_admit(acb_lm_t* lm, int slot, const float* cross, int text_len, int seq_len, uint64_t seed, void* stream);
+
+/* out [slots][2] int32 (device): each slot's position (columns consumed) and status (0 never admitted, 1 decoding,
+ * 2 finished). */
+int acb_lm_slot_status(acb_lm_t* lm, int* out, void* stream);
+
 /* Teacher-forced / inspection variant of one step: same as acb_lm_steps(1) and additionally leaves the
- * CFG-mixed logits [batch][n_q][card] fp32 in logits_out (may be NULL). */
+ * CFG-mixed logits [batch][n_q][card] fp32 in logits_out (may be NULL; in slot mode [slots][n_q][card], active slots only). */
 int acb_lm_step_logits(acb_lm_t* lm, float* logits_out, void* stream);
 
 /* Measurement hook: enqueue ONLY the weight-streaming GEMMs (lm_gemm_kernel, lm_gemm_wide_kernel above 64 rows) of one decode step, all layers in step

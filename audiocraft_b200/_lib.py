@@ -18,6 +18,7 @@ ACB_LM_PART_SLOTS = 16
 ACB_LM_PREFILL_ROWS = 64
 ACB_LM_MAX_ROWS = 256
 ACB_LM_SLOT_STRIDE = 8
+ACB_LM_SLOT_SAMPLING_STRIDE = 8
 ACB_LM_MAX_SLOTS = 128
 
 
@@ -34,8 +35,8 @@ class LMWeights(C.Structure):
 
 class LMBuffers(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ('x', 'h16', 'a16', 'f16', 'q32', 'part', 'logits', 'k_cache', 'v_cache',
-                                           'ck_cache', 'cv_cache', 'cross16', 'seq', 'seq_mask', 'pos', 'noise', 'slot_state',
-                                           'slot_mask')]
+                                           'ck_cache', 'cv_cache', 'cross16', 'seq', 'seq_mask', 'pos', 'noise', 'slot_sampling',
+                                           'slot_state', 'slot_mask')]
 
 
 class LMSampling(C.Structure):
@@ -94,7 +95,8 @@ def lib():
     L.acb_lm_begin_prefix.argtypes = [vp, vp, vp, ci, ci, ci, ci, ci, C.POINTER(LMSampling), vp]
     L.acb_lm_steps.argtypes = [vp, ci, vp]
     L.acb_lm_begin_slots.argtypes = [vp, ci, ci, ci, C.POINTER(LMSampling), vp]
-    L.acb_lm_admit.argtypes = [vp, ci, vp, ci, ci, C.c_uint64, vp]
+    L.acb_lm_admit.argtypes = [vp, ci, vp, ci, ci, C.c_uint64, C.POINTER(LMSampling), vp]
+    L.acb_lm_retire.argtypes = [vp, ci, vp]
     L.acb_lm_slot_status.argtypes = [vp, vp, vp]
     L.acb_lm_prefill.argtypes = [vp, ci, ci, vp]
     L.acb_lm_step_logits.argtypes = [vp, vp, vp]
@@ -116,7 +118,7 @@ def lib():
                  'acb_device_sm_count', 'acb_lm_debug_gemms', 'acb_lm_uses_pdl',
                  'acb_conv1d_t6', 'acb_conv1d_t6_tile', 'acb_lm_prefill',
                  'acb_resblock', 'acb_resblock_supported', 'acb_lm_forward', 'acb_t5_encode', 'acb_groupnorm_stats',
-                 'acb_groupnorm_apply', 'acb_overlap_add', 'acb_lm_begin_slots', 'acb_lm_admit', 'acb_lm_slot_status'):
+                 'acb_groupnorm_apply', 'acb_overlap_add', 'acb_lm_begin_slots', 'acb_lm_admit', 'acb_lm_slot_status', 'acb_lm_retire'):
         getattr(L, name).restype = ci
     _lib = L
     return L
@@ -130,7 +132,7 @@ EXPORTS = ['acb_version', 'acb_last_error', 'acb_device_sm_count', 'acb_weight_n
            'acb_lm_prefill', 'acb_resblock', 'acb_resblock_supported', 'acb_lm_forward_workspace_bytes', 'acb_lm_forward',
            'acb_t5_workspace_bytes', 'acb_t5_encode', 'acb_groupnorm_workspace_bytes', 'acb_groupnorm_stats',
            'acb_groupnorm_apply', 'acb_overlap_add', 'acb_lstm_recurrent_carry', 'acb_lm_begin_slots', 'acb_lm_admit',
-           'acb_lm_slot_status']
+           'acb_lm_slot_status', 'acb_lm_retire']
 
 
 def check(rc: int, what: str = ''):

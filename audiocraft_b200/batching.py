@@ -13,12 +13,18 @@ bit-identical to `generate` of that item alone when both run the same GEMM regim
 prompt is not prefilled (``ACB_LM_PREFILL=0``): a session consumes a continuation prompt one column per step (teacher
 forcing), which costs one step per prompt column, where `generate` prefills it several positions per pass.
 
-`ContinuousScheduler` is the host-side policy (FIFO admission, retirement) over any object with the device session's four
-methods, so it is tested without a GPU; `ContinuousGenerator` (``BaseGenModel.continuous``) is the public entry point.
+Each request has its own sampling options (use_sampling, temperature, top-k, top-p, CFG coefficient): admission writes them to
+the slot's record on the device, which the captured step reads, so requests with different options share one session.  A
+request can be cancelled between steps (acb_lm_retire), which frees its slot for the next admission.
+
+`ContinuousScheduler` is the host-side policy (FIFO admission, retirement, cancellation) over any object with the device
+session's methods, so it is tested without a GPU.  `CohortStream` turns a session's progress into audio pieces while the
+requests decode; `ContinuousGenerator` (``BaseGenModel.continuous``) is the public entry point.
 """
 import collections
 import ctypes as C
 import itertools
+import math
 import typing as tp
 from dataclasses import dataclass, field
 
@@ -38,6 +44,29 @@ class Request:
     seed: int = 0
     id: int = -1
     meta: tp.Dict[str, tp.Any] = field(default_factory=dict)   # filled by the session at admission
+    # the request's own sampling options; None takes the session's (SlotSession's constructor arguments)
+    use_sampling: tp.Optional[bool] = None
+    temp: tp.Optional[float] = None
+    top_k: tp.Optional[int] = None
+    top_p: tp.Optional[float] = None
+    cfg_coef: tp.Optional[float] = None
+
+
+SAMPLING_OPTIONS = ('use_sampling', 'temp', 'top_k', 'top_p', 'cfg_coef')
+
+
+def check_sampling(use_sampling, temp, top_k, top_p, cfg_coef):
+    """The options acb_lm_admit accepts: temp >= 0, an integer top_k >= 0, 0 <= top_p <= 1 and a finite cfg_coef."""
+    if not isinstance(use_sampling, (bool, int)):
+        raise ValueError(f"use_sampling must be a bool, got {use_sampling!r}")
+    if not (isinstance(temp, (int, float)) and math.isfinite(temp) and temp >= 0):
+        raise ValueError(f"temperature must be finite and >= 0, got {temp!r}")
+    if isinstance(top_k, bool) or not isinstance(top_k, int) or top_k < 0:
+        raise ValueError(f"top_k must be an integer >= 0, got {top_k!r}")
+    if not (isinstance(top_p, (int, float)) and 0 <= top_p <= 1):
+        raise ValueError(f"top_p must be in [0, 1], got {top_p!r}")
+    if not (isinstance(cfg_coef, (int, float)) and math.isfinite(cfg_coef)):
+        raise ValueError(f"cfg_coef must be finite, got {cfg_coef!r}")
 
 
 def pattern_sequence(lm, prompt: tp.Optional[torch.Tensor], max_gen_len: int, device='cpu'):
@@ -83,8 +112,11 @@ class SlotSession:
         if lm.has_prefix:
             raise NotImplementedError("continuous batching with a condition prefix (prepend fuser, melody) is not built")
         self.lm, self.slots, self.max_gen_len, self.max_text = lm, slots, max_gen_len, max_text
-        self.seq_len_max = pattern_sequence(lm, None, max_gen_len)[0].shape[-1]
+        seq, _, pattern = pattern_sequence(lm, None, max_gen_len)
+        self.seq_len_max, self.delays = seq.shape[-1], list(pattern.delays)
         coef = lm.cfg_coef if cfg_coef is None else cfg_coef
+        self.sampling = dict(use_sampling=bool(use_sampling), temp=float(temp), top_k=int(top_k), top_p=float(top_p),
+                             cfg_coef=float(coef))
         with torch.cuda.device(lm.device):
             lm._ensure(2 * slots, self.seq_len_max, max_text if lm.cross_attention else 0, slots)
             samp = _lib.LMSampling(int(bool(use_sampling)), float(temp), int(top_k), float(top_p), float(coef), 0, 0, 0.0)
@@ -98,12 +130,22 @@ class SlotSession:
         if self.lm._session is not self:
             raise RuntimeError("the LM's decode handle was taken by another generation call; start a new session")
 
+    @property
+    def max_delay(self) -> int:
+        return max(self.delays)
+
     def admit(self, slot: int, req: Request):
-        """Write the request's sequence and mask rows, then its cross K/V and slot state (acb_lm_admit)."""
+        """Write the request's sequence and mask rows, then its sampling options, cross K/V and slot state (acb_lm_admit)."""
         self._check_owner()
         lm = self.lm
         if req.max_gen_len > self.max_gen_len:
             raise ValueError(f"max_gen_len {req.max_gen_len} > the session's {self.max_gen_len}")
+        samp = None
+        if any(getattr(req, k) is not None for k in SAMPLING_OPTIONS):
+            o = {k: self.sampling[k] if getattr(req, k) is None else getattr(req, k) for k in SAMPLING_OPTIONS}
+            check_sampling(**o)
+            samp = C.byref(_lib.LMSampling(int(bool(o['use_sampling'])), float(o['temp']), int(o['top_k']), float(o['top_p']),
+                                           float(o['cfg_coef']), 0, 0, 0.0))
         with torch.cuda.device(lm.device):
             seq, mask, pattern = pattern_sequence(lm, req.prompt, req.max_gen_len, lm.device)
             S = seq.shape[-1]
@@ -122,9 +164,25 @@ class SlotSession:
                 T = cross.shape[1]
                 if not 1 <= T <= self.max_text:
                     raise ValueError(f"condition of {T} text positions: the session holds 1 .. {self.max_text}")
-            _lib.check(lm._lib.acb_lm_admit(lm._handle, slot, _lib.ptr(cross), T, S, C.c_uint64(req.seed), _lib.stream()),
-                       'lm_admit')
+            _lib.check(lm._lib.acb_lm_admit(lm._handle, slot, _lib.ptr(cross), T, S, C.c_uint64(req.seed), samp,
+                                            _lib.stream()), 'lm_admit')
             req.meta.update(S=S, mask=mask, pattern=pattern, keep=cross)   # `keep`: the stream reads cross after this call
+
+    def retire(self, slot: int):
+        """Cancel the slot's request between steps (acb_lm_retire): the slot stops decoding and is free for admission."""
+        self._check_owner()
+        with torch.cuda.device(self.lm.device):
+            _lib.check(self.lm._lib.acb_lm_retire(self.lm._handle, slot, _lib.stream()), 'lm_retire')
+
+    def frames(self, slots: tp.List[int], t0: int, t1: int) -> torch.Tensor:
+        """Codes [len(slots), K, t1 - t0] of frames [t0, t1) of the given slots, read from their delay-pattern sequences (frame t
+        of codebook k is sequence step t + 1 + delays[k]); every frame must be final (below position - max_delay)."""
+        lm = self.lm
+        with torch.cuda.device(lm.device):
+            t = torch.arange(t0, t1, device=lm.device)
+            steps = t[None, :] + 1 + torch.tensor(self.delays, device=lm.device)[:, None]                # [K, n]
+            idx = torch.tensor(slots, device=lm.device)
+            return lm._bufs['seq'][idx].gather(2, steps[None].expand(len(slots), -1, -1))
 
     def steps(self, n: int):
         self._check_owner()
@@ -157,9 +215,10 @@ class SlotSession:
 
 class ContinuousScheduler:
     """FIFO admission and retirement over a device session (`admit(slot, req)`, `steps(n)`, `status()`,
-    `collect(slot, req)`).  Every active slot advances one column per step, so the host knows when each one finishes: a poll
-    admits waiting requests into free slots, runs steps up to the next retirement (at most `poll_steps`), checks the device
-    status once, and returns the finished requests with their codes."""
+    `collect(slot, req)`, and `retire(slot)` for cancellation).  Every active slot advances one column per step, so the host
+    knows when each one finishes: a poll admits waiting requests into free slots, runs steps up to the next retirement (at
+    most `poll_steps`), checks the device status once, and returns the finished requests with their codes.  `last_admitted`
+    holds the (slot, request) pairs the last poll admitted."""
 
     def __init__(self, session, slots: int, poll_steps: tp.Optional[int] = None):
         if poll_steps is not None and poll_steps < 1:
@@ -170,9 +229,25 @@ class ContinuousScheduler:
         self.pos: tp.Dict[int, int] = {}
         self.steps_run = 0
         self.busy_slot_steps = 0     # sum over steps of the active slots: occupancy = busy_slot_steps / (steps_run * slots)
+        self.last_admitted: tp.List[tp.Tuple[int, Request]] = []
 
     def submit(self, req: Request):
         self.waiting.append(req)
+
+    def cancel(self, request_id: int) -> bool:
+        """Drop a waiting request, or retire an active one (its slot is free for the next poll).  False when the id is neither
+        waiting nor decoding (finished, cancelled before or unknown)."""
+        for req in self.waiting:
+            if req.id == request_id:
+                self.waiting.remove(req)
+                return True
+        for slot, req in self.active.items():
+            if req.id == request_id:
+                self.session.retire(slot)
+                del self.active[slot]
+                del self.pos[slot]
+                return True
+        return False
 
     @property
     def pending(self) -> bool:
@@ -182,6 +257,7 @@ class ContinuousScheduler:
         return req.meta['S'] - 1
 
     def poll(self) -> tp.List[tp.Tuple[Request, torch.Tensor]]:
+        self.last_admitted = []
         for slot in range(self.slots):
             if not self.waiting:
                 break
@@ -190,6 +266,7 @@ class ContinuousScheduler:
                 self.session.admit(slot, req)
                 self.active[slot] = req
                 self.pos[slot] = 0
+                self.last_admitted.append((slot, req))
         if not self.active:
             return []
         n = min(self._n_steps(r) - self.pos[s] for s, r in self.active.items())
@@ -219,19 +296,119 @@ class ContinuousScheduler:
         return self.busy_slot_steps / max(1, self.steps_run * self.slots)
 
 
-class ContinuousGenerator:
-    """`model.continuous(slots, poll_steps)`: submit requests at any time, collect waveforms as they finish.
+class _Cohort:
+    """Requests admitted in the same poll: they advance in lock-step and share one stream decoder."""
 
-    `submit(description=None, duration=None, prompt=None, prompt_sample_rate=None)` returns a request id; `poll()` runs one
-    scheduling round and returns the `(request_id, wav)` (or `(request_id, wav, tokens)` with return_tokens) of the requests
-    that finished in it, `run()` polls until every submitted request has finished.  `wav` is [1, C, T] and `tokens`
-    [1, K, T_frames]: what `generate([description])` (or `generate_continuation` / `generate_unconditional`) returns for that
-    request alone after the same `torch.manual_seed`.  Requests beyond `slots` wait in FIFO order.  A continuation prompt costs
-    one decode step per prompt frame.  Refused (NotImplementedError, before any device work): durations beyond
-    max_duration, melody models, two_step_cfg and cfg_coef_beta."""
+    def __init__(self, members: tp.List[tp.Tuple[int, Request]], decoder, start: int):
+        self.members, self.decoder = members, decoder
+        self.start = start           # the scheduler's steps_run when the cohort was admitted
+        self.frames = 0              # frames handed to the decoder
+
+
+class CohortStream:
+    """Audio pieces of a session's requests while they decode, one codec call per cohort and poll.
+
+    `stream_decoder(n)` makes a decoder over n items (`push(codes [n, K, m]) -> [n, C, m']`, `flush()`, `select(items)`).
+    After a poll in which a request has run s steps, its frames below s - max_delay are final (as in
+    `LMModel.generate_blocks`); the scheduler knows every position on the host, so nothing is read back to find them.  Each
+    cohort's new frames go to its decoder in one push.  Members that finish are split out with `select` and flushed together
+    (members of one cohort that finish in the same poll have the same length), the rest keep decoding in the remaining
+    decoder.  A cancelled member is dropped from its cohort the same way.  `poll()` returns `(request_id, piece, tokens, final)`
+    events: `piece` [1, C, m] is the request's next audio, `tokens` [1, K, n] the frames handed to the codec with it, and a
+    request's pieces, concatenated, are the codec's decode of all its frames."""
+
+    def __init__(self, scheduler: ContinuousScheduler, stream_decoder: tp.Callable[[int], tp.Any], max_delay: int):
+        self.scheduler, self.stream_decoder, self.max_delay = scheduler, stream_decoder, max_delay
+        self.cohorts: tp.List[_Cohort] = []
+        self.codec_calls = 0         # pushes and flushes, over all polls
+
+    def cancel(self, request_id: int) -> bool:
+        if not self.scheduler.cancel(request_id):
+            return False
+        for co in self.cohorts:
+            ids = [r.id for _, r in co.members]
+            if request_id in ids:
+                keep = [i for i, rid in enumerate(ids) if rid != request_id]
+                if keep:
+                    co.decoder = co.decoder.select(keep)
+                    co.members = [co.members[i] for i in keep]
+                else:
+                    self.cohorts.remove(co)
+                break
+        return True
+
+    def poll(self) -> tp.List[tp.Tuple[int, torch.Tensor, torch.Tensor, bool]]:
+        sch = self.scheduler
+        start = sch.steps_run
+        done = sch.poll()
+        if sch.last_admitted:
+            self.cohorts.append(_Cohort(list(sch.last_admitted), self.stream_decoder(len(sch.last_admitted)), start))
+        finished = {req.id for req, _ in done}
+        events = []
+        for co in list(self.cohorts):
+            events += self._advance(co, finished)
+        return events
+
+    def _advance(self, co: _Cohort, finished: tp.Set[int]) -> list:
+        members = co.members
+        fin = [i for i, (_, r) in enumerate(members) if r.id in finished]
+        ready = max(0, self.scheduler.steps_run - co.start - self.max_delay)
+        if ready == co.frames:   # no new frame, so no member finished either (its last step makes its last frame final)
+            assert not fin
+            return []
+        codes = self.scheduler.session.frames([slot for slot, _ in members], co.frames, ready)
+        wav = co.decoder.push(codes)
+        co.frames = ready
+        self.codec_calls += 1
+        if fin:
+            assert all(members[i][1].max_gen_len == ready for i in fin)
+            keep = [i for i in range(len(members)) if i not in fin]
+            if keep:
+                tail = co.decoder.select(fin).flush()
+                co.decoder = co.decoder.select(keep)
+                co.members = [members[i] for i in keep]
+            else:
+                tail = co.decoder.flush()
+                self.cohorts.remove(co)
+            self.codec_calls += 1
+        events = []
+        for i, (_, req) in enumerate(members):
+            piece = wav[i:i + 1]
+            if i in fin:
+                j = fin.index(i)
+                piece = torch.cat([piece, tail[j:j + 1]], dim=-1)
+            events.append((req.id, piece, codes[i:i + 1], i in fin))
+        return events
+
+
+class ContinuousGenerator:
+    """`model.continuous(slots, poll_steps, max_text, return_tokens, chunk_duration)`: submit requests at any time, collect
+    their audio as it decodes or when they finish.
+
+    `submit(description=None, duration=None, prompt=None, prompt_sample_rate=None, *, use_sampling=None, top_k=None,
+    top_p=None, temperature=None, cfg_coef=None)` returns a request id.  The sampling options are the request's own; None
+    takes the value of `model.generation_params` when the generator was made.  Requests beyond `slots` wait in FIFO order.  A
+    continuation prompt costs one decode step per prompt frame.  `cancel(request_id)` drops a waiting request or stops a
+    decoding one, whose slot then takes the next waiting request; it returns False for a finished or unknown id, and a
+    cancelled request yields nothing more.  `run()` polls until every submitted request has finished or been cancelled.
+
+    Without `chunk_duration`, `poll()` runs one scheduling round and returns `(request_id, wav)` (or `(request_id, wav,
+    tokens)` with return_tokens) for the requests that finished in it.  `wav` is [1, C, T] and `tokens` [1, K, T_frames]:
+    what `generate([description])` (or `generate_continuation` / `generate_unconditional`) returns for that request alone,
+    with its options, after the same `torch.manual_seed`.
+
+    With `chunk_duration`, a round runs at most `round(chunk_duration * frame_rate)` steps and `poll()` returns
+    `(request_id, piece, final)` (or `(request_id, piece, tokens, final)`) events: `piece` [1, C, m] is the request's next
+    audio, as soon as the codec can produce it, and `final` marks its last event.  A request's pieces, concatenated, are the
+    waveform the generator without chunk_duration returns for it; a continuation's first pieces are its prompt's audio.  The
+    requests admitted in one round share one stream decoder.  Refused before any device work: a codec without a stream
+    decoder (NotImplementedError) and chunk_duration <= 0 (ValueError).
+
+    Refused (NotImplementedError, before any device work): durations beyond max_duration, melody models, two_step_cfg and
+    cfg_coef_beta."""
 
     def __init__(self, model, slots: int = 32, poll_steps: tp.Optional[int] = None, max_text: int = 64,
-                 return_tokens: bool = False):
+                 return_tokens: bool = False, chunk_duration: tp.Optional[float] = None):
         params = dict(model.generation_params)
         if getattr(model, '_has_melody', False) or model.lm.has_prefix:
             raise NotImplementedError("continuous batching of melody-conditioned models (a condition prefix) is not built")
@@ -239,16 +416,30 @@ class ContinuousGenerator:
             raise NotImplementedError("continuous batching with two_step_cfg is not built")
         if params.get('cfg_coef_beta') is not None:
             raise NotImplementedError("continuous batching with cfg_coef_beta (double CFG) is not built")
+        if chunk_duration is not None:
+            if not chunk_duration > 0:
+                raise ValueError(f"chunk_duration must be > 0, got {chunk_duration}")
+            if not hasattr(model.compression_model, 'stream_decoder'):
+                raise NotImplementedError(f"{type(model.compression_model).__name__} has no stream decoder")
+            model.compression_model.stream_decoder(1)   # GroupNorm and transformers' chunked codecs refuse here
+            block = max(1, int(round(chunk_duration * model.frame_rate)))
+            poll_steps = block if poll_steps is None else min(poll_steps, block)
         self.model, self.return_tokens = model, return_tokens
+        self.defaults = dict(use_sampling=params['use_sampling'], temp=params['temp'], top_k=params['top_k'],
+                             top_p=params['top_p'], cfg_coef=params['cfg_coef'])
         max_gen_len = int(model.max_duration * model.frame_rate)
-        self.session = SlotSession(model.lm, slots, max_gen_len, max_text, use_sampling=params['use_sampling'],
-                                   temp=params['temp'], top_k=params['top_k'], top_p=params['top_p'],
-                                   cfg_coef=params['cfg_coef'])
+        self.session = SlotSession(model.lm, slots, max_gen_len, max_text, **self.defaults)
         self.scheduler = ContinuousScheduler(self.session, slots, poll_steps)
+        self.stream = None
+        if chunk_duration is not None:
+            self.stream = CohortStream(self.scheduler, model.compression_model.stream_decoder, self.session.max_delay)
         self._ids = itertools.count()
+        self._cancelled: tp.Set[int] = set()
 
     def submit(self, description: tp.Optional[str] = None, duration: tp.Optional[float] = None,
-               prompt: tp.Optional[torch.Tensor] = None, prompt_sample_rate: tp.Optional[int] = None) -> int:
+               prompt: tp.Optional[torch.Tensor] = None, prompt_sample_rate: tp.Optional[int] = None, *,
+               use_sampling: tp.Optional[bool] = None, top_k: tp.Optional[int] = None, top_p: tp.Optional[float] = None,
+               temperature: tp.Optional[float] = None, cfg_coef: tp.Optional[float] = None) -> int:
         from .audio_utils import convert_audio
         m = self.model
         duration = m.duration if duration is None else float(duration)
@@ -265,6 +456,12 @@ class ContinuousGenerator:
                 prompt = prompt[None]
             if prompt.dim() != 3 or prompt.shape[0] != 1:
                 raise ValueError("prompt should be one item: [C, T] or [1, C, T]")
+        given = dict(use_sampling=use_sampling, temp=temperature, top_k=top_k, top_p=top_p, cfg_coef=cfg_coef)
+        options = {k: self.defaults[k] if v is None else v for k, v in given.items()}
+        if options['cfg_coef'] is None:
+            options['cfg_coef'] = m.lm.cfg_coef
+        check_sampling(**options)
+        if prompt is not None:
             prompt = convert_audio(prompt, prompt_sample_rate, m.sample_rate, m.audio_channels)
         attributes, prompt_tokens = m._prepare_tokens_and_attributes([description], prompt)
         if prompt_tokens is not None and prompt_tokens.shape[-1] >= n:
@@ -274,8 +471,15 @@ class ContinuousGenerator:
             raise ValueError(f"the description has {cross.shape[1]} text positions; the session holds {self.session.max_text}")
         seed = int(torch.randint(0, 2 ** 62, (1,)).item())   # drawn as LMModel.generate draws it
         rid = next(self._ids)
-        self.scheduler.submit(Request(n, cross, prompt_tokens, seed, rid))
+        self.scheduler.submit(Request(n, cross, prompt_tokens, seed, rid, **options))
         return rid
+
+    def cancel(self, request_id: int) -> bool:
+        """Drop a waiting request or stop a decoding one (acb_lm_retire); False for a finished or unknown id."""
+        ok = self.stream.cancel(request_id) if self.stream is not None else self.scheduler.cancel(request_id)
+        if ok:
+            self._cancelled.add(request_id)
+        return ok
 
     @property
     def pending(self) -> bool:
@@ -286,6 +490,12 @@ class ContinuousGenerator:
         return self.scheduler.occupancy
 
     def poll(self) -> tp.List[tuple]:
+        if self.stream is not None:
+            out = []
+            for rid, piece, tokens, final in self.stream.poll():
+                if piece.shape[-1] or final or self.return_tokens:
+                    out.append((rid, piece, tokens, final) if self.return_tokens else (rid, piece, final))
+            return out
         done = self.scheduler.poll()
         out = {}
         by_len: tp.Dict[int, tp.List[tp.Tuple[Request, torch.Tensor]]] = collections.defaultdict(list)
@@ -300,4 +510,6 @@ class ContinuousGenerator:
 
     def run(self) -> tp.Iterator[tuple]:
         while self.pending:
-            yield from self.poll()
+            for ev in self.poll():
+                if ev[0] not in self._cancelled:   # a request cancelled while this round's events are consumed
+                    yield ev

@@ -1036,9 +1036,34 @@ __global__ void __launch_bounds__(1024) lm_sample_kernel(SampleParams p) { sampl
 // Philox stream k of (seed, column) -- what lm_sample_kernel draws for item 0 of a generation, so a request samples as if
 // generated alone.  p.seq_mask is [slots][n_q][max_seq].  A known token (!= -1) stays, so a prompt written into the sequence
 // is consumed one column per step.  The last of the slot's n_q blocks advances its position; writing column seq_len - 1
-// finishes the slot.
-__global__ void __launch_bounds__(1024) lm_sample_slot_kernel(SampleParams p, int* __restrict__ slot_state) {
+// finishes the slot.  The sampling options are the slot's own record in slot_sampling (written at admission), so the captured
+// step serves requests with different options: every choice they drive (CFG coefficient, temperature, top-k radix select or
+// top-p sort, argmax) is uniform over a block.
+__global__ void __launch_bounds__(1024) lm_sample_slot_kernel(SampleParams p, int* __restrict__ slot_state,
+                                                              const int* __restrict__ slot_sampling) {
+    const int* rec = slot_sampling + blockIdx.y * ACB_LM_SLOT_SAMPLING_STRIDE;
+    p.use_sampling = rec[0];
+    p.temp = __int_as_float(rec[1]);
+    p.top_k = rec[2];
+    p.top_p = __int_as_float(rec[3]);
+    p.cfg_coef = __int_as_float(rec[4]);
     sample_impl<true>(p, slot_state);
+}
+
+// Admission of a request's sampling options (the record lm_sample_slot_kernel reads).
+__global__ void lm_slot_sampling_kernel(int* slot_sampling, int slot, int use_sampling, float temp, int top_k, float top_p,
+                                        float cfg_coef) {
+    int* rec = slot_sampling + slot * ACB_LM_SLOT_SAMPLING_STRIDE;
+    rec[0] = use_sampling;
+    rec[1] = __float_as_int(temp);
+    rec[2] = top_k;
+    rec[3] = __float_as_int(top_p);
+    rec[4] = __float_as_int(cfg_coef);
+}
+
+// Cancellation: the slot is skipped from the next step on, as a slot never admitted.
+__global__ void lm_slot_retire_kernel(int* slot_state, int slot) {
+    slot_state[slot * ACB_LM_SLOT_STRIDE + ACB_SLOT_STATUS] = SLOT_INACTIVE;
 }
 
 // Admission: the slot starts at position 0 with its own sequence length, text length and seed.
@@ -1404,7 +1429,7 @@ static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_la
         size_t smem = ((size_t)c.card + 2 * (size_t)NP) * sizeof(float);
         if (lm->slots) {
             sp.seq_mask = B.slot_mask; sp.pos = nullptr;
-            lm_sample_slot_kernel<<<dim3(c.n_q, lm->slots), 1024, smem, s>>>(sp, B.slot_state);
+            lm_sample_slot_kernel<<<dim3(c.n_q, lm->slots), 1024, smem, s>>>(sp, B.slot_state, B.slot_sampling);
         } else {
             lm_sample_kernel<<<dim3(c.n_q, lm->batch), 1024, smem, s>>>(sp);
         }
@@ -1649,7 +1674,8 @@ extern "C" int acb_lm_begin_slots(acb_lm_t* lm, int slots, int max_text, int seq
                                   void* stream) {
     ACB_REQUIRE(lm && sampling, "acb_lm_begin_slots: null argument");
     const acb_lm_config& c = lm->cfg;
-    ACB_REQUIRE(lm->buf.slot_state && lm->buf.slot_mask, "acb_lm_begin_slots: buffers.slot_state and slot_mask are required");
+    ACB_REQUIRE(lm->buf.slot_sampling && lm->buf.slot_state && lm->buf.slot_mask,
+                "acb_lm_begin_slots: buffers.slot_sampling, slot_state and slot_mask are required");
     ACB_REQUIRE(slots >= 1 && slots <= ACB_LM_MAX_SLOTS && 2 * slots <= c.max_rows, "acb_lm_begin_slots: slots %d not in [1, %d] "
                 "or 2 * slots > max_rows %d", slots, ACB_LM_MAX_SLOTS, c.max_rows);
     ACB_REQUIRE(seq_len_max >= 2 && seq_len_max <= c.max_seq, "acb_lm_begin_slots: seq_len_max %d not in [2, max_seq %d]",
@@ -1692,7 +1718,8 @@ extern "C" int acb_lm_begin_slots(acb_lm_t* lm, int slots, int max_text, int seq
     return capture_step(lm);
 }
 
-extern "C" int acb_lm_admit(acb_lm_t* lm, int slot, const float* cross, int text_len, int seq_len, uint64_t seed, void* stream) {
+extern "C" int acb_lm_admit(acb_lm_t* lm, int slot, const float* cross, int text_len, int seq_len, uint64_t seed,
+                            const acb_lm_sampling* sampling, void* stream) {
     ACB_REQUIRE(lm && lm->slots > 0, "acb_lm_admit: call acb_lm_begin_slots first");
     const acb_lm_config& c = lm->cfg;
     ACB_REQUIRE(slot >= 0 && slot < lm->slots, "acb_lm_admit: slot %d not in [0, %d)", slot, lm->slots);
@@ -1700,6 +1727,18 @@ extern "C" int acb_lm_admit(acb_lm_t* lm, int slot, const float* cross, int text
     ACB_REQUIRE(!lm->has_cross || (cross && text_len >= 1 && text_len <= lm->text_len),
                 "acb_lm_admit: the model has cross attention: a condition of 1 .. %d text positions is required (got %d)",
                 lm->text_len, text_len);
+    if (sampling) {
+        if (sampling->cfg_coef_beta != 0.f) {
+            acb_set_error("acb_lm_admit: double CFG (cfg_coef_beta) is not built in slot mode: a session is [cond; null] rows");
+            return ACB_ERR_UNSUPPORTED;
+        }
+        ACB_REQUIRE(!sampling->noise_from_buffer, "acb_lm_admit: slot mode samples with the on-device Philox noise only");
+        ACB_REQUIRE(sampling->temp >= 0.f && sampling->top_k >= 0 && sampling->top_p >= 0.f && sampling->top_p <= 1.f &&
+                    isfinite(sampling->temp) && isfinite(sampling->cfg_coef),
+                    "acb_lm_admit: needs 0 <= temp < inf (got %g), top_k >= 0 (got %d), 0 <= top_p <= 1 (got %g) and a finite "
+                    "cfg_coef (got %g)", sampling->temp, sampling->top_k, sampling->top_p, sampling->cfg_coef);
+    }
+    const acb_lm_sampling& sp = sampling ? *sampling : lm->samp;
     cudaStream_t s = (cudaStream_t)stream;
     if (lm->has_cross) {
         // cross K/V of the slot's cond row (slot) and null row (slots + slot), each staged and projected on its own: the
@@ -1725,8 +1764,19 @@ extern "C" int acb_lm_admit(acb_lm_t* lm, int slot, const float* cross, int text
                 }
         }
     }
+    lm_slot_sampling_kernel<<<1, 1, 0, s>>>(lm->buf.slot_sampling, slot, sp.use_sampling, sp.temp, sp.top_k, sp.top_p,
+                                            sp.cfg_coef);
+    ACB_LAUNCH_CHECK();
     lm_slot_admit_kernel<<<1, 1, 0, s>>>(lm->buf.slot_state, slot, seq_len, lm->has_cross ? text_len : 0, (uint32_t)seed,
                                          (uint32_t)(seed >> 32));
+    ACB_LAUNCH_CHECK();
+    return ACB_OK;
+}
+
+extern "C" int acb_lm_retire(acb_lm_t* lm, int slot, void* stream) {
+    ACB_REQUIRE(lm && lm->slots > 0, "acb_lm_retire: call acb_lm_begin_slots first");
+    ACB_REQUIRE(slot >= 0 && slot < lm->slots, "acb_lm_retire: slot %d not in [0, %d)", slot, lm->slots);
+    lm_slot_retire_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(lm->buf.slot_state, slot);
     ACB_LAUNCH_CHECK();
     return ACB_OK;
 }

@@ -9,6 +9,7 @@ and every layer is one fused kernel (padding, ELU, bias, residual, trim inside).
 PyTorch here is plumbing only (device memory, streams).  There is no CPU path: without the CUDA library
 or a GPU, construction raises.
 """
+import copy
 import math
 import os
 import typing as tp
@@ -625,6 +626,9 @@ class _KernelLayers:
     def lstm(self, L, x, state):
         return self.m._lstm(x.contiguous(), L, prec=self.m._lstm_prec, state=state)
 
+    def lstm_select(self, L, state, items):
+        return [(h[items].contiguous(), c[items].contiguous()) for h, c in state]
+
 
 class EncodecStreamDecoder:
     """`EncodecModel.stream_decoder(batch)`: the SEANet decoder with per-layer context (audiocraft_b200/streaming.py) on the
@@ -644,6 +648,13 @@ class EncodecStreamDecoder:
         if y is None:
             return torch.empty((self.batch, self.model.channels, 0), device=self.model.device, dtype=torch.float32)
         return y
+
+    def select(self, items: tp.List[int]) -> 'EncodecStreamDecoder':
+        """A stream decoder of the given items only, in this one's state (see streaming.DecoderStream.select)."""
+        with torch.cuda.device(self.model.device):
+            out = copy.copy(self)
+            out.batch, out._stream = len(items), self._stream.select(list(items))
+            return out
 
     def push(self, codes: torch.Tensor) -> torch.Tensor:
         assert codes.dim() == 3 and codes.shape[0] == self.batch, (tuple(codes.shape), self.batch)
@@ -669,6 +680,10 @@ class _StereoStreamDecoder:
 
     def _split(self, audio):
         return torch.cat([audio[:self.batch], audio[self.batch:]], dim=1)
+
+    def select(self, items: tp.List[int]) -> '_StereoStreamDecoder':
+        items = list(items)
+        return _StereoStreamDecoder(self.wrapper, self.inner.select(items + [i + self.batch for i in items]), len(items))
 
     def push(self, codes: torch.Tensor) -> torch.Tensor:
         B, K, T = codes.shape

@@ -183,7 +183,8 @@ class LMModel:
         b['seq_mask'] = torch.zeros((self.n_q, max_seq), device=dev, dtype=torch.uint8)
         b['pos'] = torch.zeros(4, device=dev, dtype=torch.int32)
         b['noise'] = torch.ones((max_batch, self.n_q, self.card), device=dev, dtype=f32)
-        # slot mode (batching.SlotSession): per-slot device state and per-slot pattern masks, B = slots
+        # slot mode (batching.SlotSession): per-slot sampling options, device state and pattern masks, B = slots
+        b['slot_sampling'] = torch.zeros((max_batch, _lib.ACB_LM_SLOT_SAMPLING_STRIDE), device=dev, dtype=torch.int32)
         b['slot_state'] = torch.zeros((max_batch, _lib.ACB_LM_SLOT_STRIDE), device=dev, dtype=torch.int32)
         b['slot_mask'] = torch.zeros((max_batch, self.n_q, max_seq), device=dev, dtype=torch.uint8)
         self._bufs = b
@@ -191,7 +192,8 @@ class LMModel:
         wts = self._weights()
         bufs = _lib.LMBuffers(*[_lib.ptr(b[n]) for n in ('x', 'h16', 'a16', 'f16', 'q32', 'part', 'logits', 'k_cache',
                                                          'v_cache', 'ck_cache', 'cv_cache', 'cross16', 'seq',
-                                                         'seq_mask', 'pos', 'noise', 'slot_state', 'slot_mask')])
+                                                         'seq_mask', 'pos', 'noise', 'slot_sampling', 'slot_state',
+                                                         'slot_mask')])
         handle = C.c_void_p()
         _lib.check(self._lib.acb_lm_create(C.byref(cfg), C.byref(wts), C.byref(bufs), C.byref(handle)), 'lm_create')
         self._handle = handle

@@ -214,13 +214,16 @@ class BaseGenModel:
 
     # -- continuous batching
     def continuous(self, slots: int = 32, poll_steps: tp.Optional[int] = None, max_text: int = 64,
-                   return_tokens: bool = False):
+                   return_tokens: bool = False, chunk_duration: tp.Optional[float] = None):
         """A `batching.ContinuousGenerator` over this model: up to `slots` requests decode side by side, each admitted when a
-        slot frees and retired when its last frame is sampled, with the current generation parameters.  `submit(description,
-        duration, prompt, prompt_sample_rate)` returns a request id; `poll()` / `run()` return `(request_id, wav[, tokens])`
-        as requests finish, each equal to that request generated alone.  `max_text` bounds a description's text positions."""
+        slot frees and retired when its last frame is sampled.  `submit(description, duration, prompt, prompt_sample_rate,
+        use_sampling=, top_k=, top_p=, temperature=, cfg_coef=)` returns a request id (options left out take the current
+        generation parameters) and `cancel(request_id)` stops a request.  `poll()` / `run()` return `(request_id, wav[, tokens])`
+        as requests finish, each equal to that request generated alone; with `chunk_duration` (seconds of decode steps per
+        round) they return `(request_id, piece[, tokens], final)` audio pieces while the requests decode.  `max_text` bounds a
+        description's text positions."""
         from .batching import ContinuousGenerator
-        return ContinuousGenerator(self, slots, poll_steps, max_text, return_tokens)
+        return ContinuousGenerator(self, slots, poll_steps, max_text, return_tokens, chunk_duration)
 
 
 def _sampling_params(use_sampling, top_k, top_p, temperature, cfg_coef, two_step_cfg):

@@ -9,6 +9,7 @@ themselves run through a backend with four operations, each on a window that nee
                                       steps [pad_left, pad_left + n_out)
     convtr(L, x, trim_left, t_out)    transposed conv of L with x[-1] = x[t_in] = 0, full-output steps [trim_left, trim_left + t_out)
     lstm(L, x, state)                 the LSTM block (y = LSTM(x) + x) from `state`, which it advances; lstm_state(L, batch) makes one
+                                      and lstm_select(L, state, items) copies the given items of one (only `select` needs it)
 
 `EncodecModel.stream_decoder` plugs in the CUDA kernels; the CPU tests plug in the oracle's layers.
 
@@ -22,6 +23,7 @@ What each layer keeps (reference semantics: audiocraft/modules/conv.py:185-243, 
     u // s - 1, so after n inputs the steps below n * s are final and the last s come at flush (x[n] = 0);
   * the LSTM keeps (h, c) per layer.
 """
+import copy
 import math
 import typing as tp
 
@@ -104,6 +106,12 @@ class _ConvStage:
             self.buf = torch.cat([self.buf, x], dim=-1)
         return self._emit()
 
+    def select(self, items: tp.List[int]) -> '_ConvStage':
+        out = copy.copy(self)
+        out.pending = None if self.pending is None else self.pending[items]
+        out.buf = None if self.buf is None else self.buf[items]
+        return out
+
     def flush(self) -> tp.Optional[torch.Tensor]:
         if self.n_in == 0:
             return None
@@ -143,6 +151,11 @@ class _ConvTrStage:
         self.prev = x[..., -1:]
         return y
 
+    def select(self, items: tp.List[int]) -> '_ConvTrStage':
+        out = copy.copy(self)
+        out.prev = None if self.prev is None else self.prev[items]
+        return out
+
     def flush(self) -> tp.Optional[torch.Tensor]:
         if self.prev is None or self.s == self.right:
             return None
@@ -150,8 +163,11 @@ class _ConvTrStage:
 
 
 class _LstmStage:
-    def __init__(self, run, state):
-        self.run, self.state = run, state
+    def __init__(self, run, state, pick):
+        self.run, self.state, self.pick = run, state, pick
+
+    def select(self, items: tp.List[int]) -> '_LstmStage':
+        return _LstmStage(self.run, self.pick(self.state, items), self.pick)
 
     def last_in(self, o: int) -> int:
         return o
@@ -205,7 +221,8 @@ class DecoderStream:
                 self.stages.append(_ConvTrStage(lambda x, tl, n, L=L: backend.convtr(L, x, tl, n), L['k'], L['stride'], causal,
                                                 cfg['trim_right_ratio']))
             else:
-                self.stages.append(_LstmStage(lambda x, st, L=L: backend.lstm(L, x, st), backend.lstm_state(L, batch)))
+                self.stages.append(_LstmStage(lambda x, st, L=L: backend.lstm(L, x, st), backend.lstm_state(L, batch),
+                                              lambda st, items, L=L: backend.lstm_select(L, st, items)))
 
     @property
     def lookahead(self) -> int:
@@ -219,6 +236,14 @@ class DecoderStream:
                 f = st.last_in(f)
             best = max(best, f - o // self.hop)
         return best
+
+    def select(self, items: tp.List[int]) -> 'DecoderStream':
+        """A stream of the given items only (indices into the batch, in that order), in the same state: every stage's held
+        input, the transposed convolutions' previous step and the LSTM state are copied along the batch.  The items' output
+        continues exactly as in this stream; this stream is unchanged."""
+        out = copy.copy(self)
+        out.stages = [st.select(items) for st in self.stages]
+        return out
 
     def push(self, z: torch.Tensor) -> tp.Optional[torch.Tensor]:
         x = z

@@ -218,11 +218,14 @@ typedef struct {
     int32_t* pos;      /* [4] device ints: pos (tokens in the KV cache), rows, batch, text_len */
     float* noise;      /* [B][n_q][card] Exponential(1) noise, read when sampling.noise_from_buffer != 0 */
     /* slot mode only (acb_lm_begin_slots; NULL otherwise), with B = slots in seq above: */
+    int32_t* slot_sampling; /* [slots][ACB_LM_SLOT_SAMPLING_STRIDE] 32-bit words per slot: use_sampling, temp (fp32 bits), top_k,
+                               top_p (fp32 bits), cfg_coef (fp32 bits), 3 unused (written by the library at admission) */
     int32_t* slot_state; /* [slots][ACB_LM_SLOT_STRIDE] per-slot position, status, lengths and seed (written by the library) */
     uint8_t* slot_mask;  /* [slots][n_q][max_seq] each slot's pattern validity mask (written by the caller before acb_lm_admit) */
 } acb_lm_buffers;
 
 #define ACB_LM_SLOT_STRIDE 8     /* int32 words of slot_state per slot */
+#define ACB_LM_SLOT_SAMPLING_STRIDE 8   /* 32-bit words of slot_sampling per slot */
 #define ACB_LM_MAX_SLOTS 128     /* slots of a session: rows = 2 * slots <= ACB_LM_MAX_ROWS */
 #define ACB_LM_MAX_SPLIT 8
 #define ACB_LM_PART_SLOTS 16
@@ -285,18 +288,31 @@ int acb_lm_prefill(acb_lm_t* lm, int pos0, int n_tokens, void* stream);
  * own position, sequence length, text length and seed.  The GEMMs run on all rows whichever slots are busy, so their regime
  * and K split are fixed for the session.  Each slot attends to exactly its own text length, and its noise is Philox stream k
  * of (its seed, column) -- what acb_lm_begin draws for item 0 -- so a request's tokens are those of the same request
- * generated alone (bit for bit where both run the same GEMM regime, i.e. up to 64 rows).  Needs buffers.slot_state and
- * buffers.slot_mask.  Shared sampling options; cfg_coef_beta != 0 returns ACB_ERR_UNSUPPORTED and noise_from_buffer is
- * refused.  Marks every slot inactive and captures the session's step graph, which acb_lm_steps then launches.
+ * generated alone (bit for bit where both run the same GEMM regime, i.e. up to 64 rows).  Needs buffers.slot_sampling,
+ * buffers.slot_state and buffers.slot_mask.  `sampling` holds the session's default options, which a request admitted without
+ * its own takes; cfg_coef_beta != 0 returns ACB_ERR_UNSUPPORTED and noise_from_buffer is refused.  Marks every slot inactive
+ * and captures the session's step graph, which acb_lm_steps then launches.
  * max_text <= max_text of the config bounds the admitted conditions, seq_len_max <= max_seq their sequences. */
 int acb_lm_begin_slots(acb_lm_t* lm, int slots, int max_text, int seq_len_max, const acb_lm_sampling* sampling, void* stream);
 
-/* Admit a request into `slot` (free: never used or finished) between steps: writes the slot's cross-attention K/V from cross,
- * the fp32 condition [2][text_len][d] ([cond; null] rows, NULL without cross attention), and starts the slot at column 0 with
- * sequence length seq_len and the Philox key seed.  The caller first writes the slot's delay-pattern sequence into
+/* Admit a request into `slot` (free: never used, finished or retired) between steps: writes the slot's cross-attention K/V from
+ * cross, the fp32 condition [2][text_len][d] ([cond; null] rows, NULL without cross attention), and starts the slot at column 0
+ * with sequence length seq_len and the Philox key seed.  The caller first writes the slot's delay-pattern sequence into
  * buffers.seq[slot] (-1 where unknown; known prompt tokens are kept and consumed one column per step) and its mask into
- * buffers.slot_mask[slot].  After seq_len - 1 steps the slot has written column seq_len - 1 and is finished. */
-int acb_lm_admit(acb_lm_t* lm, int slot, const float* cross, int text_len, int seq_len, uint64_t seed, void* stream);
+ * buffers.slot_mask[slot].  After seq_len - 1 steps the slot has written column seq_len - 1 and is finished.
+ * sampling: the request's own use_sampling, temp, top_k, top_p and cfg_coef, written to buffers.slot_sampling[slot], where the
+ * captured step reads them (slots with different options share one step); NULL takes the options of acb_lm_begin_slots.  seed,
+ * noise_from_buffer and cfg_coef_beta of the struct: seed is the argument above, noise_from_buffer != 0 and cfg_coef_beta != 0
+ * are refused (ACB_ERR_INVALID, ACB_ERR_UNSUPPORTED).  Needs temp >= 0, top_k >= 0, 0 <= top_p <= 1 and a finite cfg_coef
+ * (else ACB_ERR_INVALID); as in acb_lm_begin, top_p > 0 samples top-p, else top_k > 0 top-k, and use_sampling == 0 or
+ * temp == 0 takes the argmax. */
+int acb_lm_admit(acb_lm_t* lm, int slot, const float* cross, int text_len, int seq_len, uint64_t seed,
+                 const acb_lm_sampling* sampling, void* stream);
+
+/* Cancel the request in `slot` between steps: an ACTIVE or FINISHED slot becomes INACTIVE (status 0) and the next step skips
+ * it, as it skips a slot never admitted; the slot is free for acb_lm_admit, which overwrites its K/V, mask and state.  One
+ * single-thread kernel on the stream; retiring an INACTIVE slot changes nothing. */
+int acb_lm_retire(acb_lm_t* lm, int slot, void* stream);
 
 /* out [slots][2] int32 (device): each slot's position (columns consumed) and status (0 never admitted, 1 decoding,
  * 2 finished). */

@@ -96,6 +96,7 @@ def lib():
     L.acb_lm_steps.argtypes = [vp, ci, vp]
     L.acb_lm_begin_slots.argtypes = [vp, ci, ci, ci, C.POINTER(LMSampling), vp]
     L.acb_lm_admit.argtypes = [vp, ci, vp, ci, ci, C.c_uint64, C.POINTER(LMSampling), vp]
+    L.acb_lm_admit_prefix.argtypes = [vp, ci, vp, ci, vp, ci, ci, C.c_uint64, C.POINTER(LMSampling), vp]
     L.acb_lm_retire.argtypes = [vp, ci, vp]
     L.acb_lm_slot_status.argtypes = [vp, vp, vp]
     L.acb_lm_prefill.argtypes = [vp, ci, ci, vp]
@@ -118,7 +119,8 @@ def lib():
                  'acb_device_sm_count', 'acb_lm_debug_gemms', 'acb_lm_uses_pdl',
                  'acb_conv1d_t6', 'acb_conv1d_t6_tile', 'acb_lm_prefill',
                  'acb_resblock', 'acb_resblock_supported', 'acb_lm_forward', 'acb_t5_encode', 'acb_groupnorm_stats',
-                 'acb_groupnorm_apply', 'acb_overlap_add', 'acb_lm_begin_slots', 'acb_lm_admit', 'acb_lm_slot_status', 'acb_lm_retire'):
+                 'acb_groupnorm_apply', 'acb_overlap_add', 'acb_lm_begin_slots', 'acb_lm_admit', 'acb_lm_slot_status', 'acb_lm_retire',
+                 'acb_lm_admit_prefix'):
         getattr(L, name).restype = ci
     _lib = L
     return L
@@ -132,7 +134,7 @@ EXPORTS = ['acb_version', 'acb_last_error', 'acb_device_sm_count', 'acb_weight_n
            'acb_lm_prefill', 'acb_resblock', 'acb_resblock_supported', 'acb_lm_forward_workspace_bytes', 'acb_lm_forward',
            'acb_t5_workspace_bytes', 'acb_t5_encode', 'acb_groupnorm_workspace_bytes', 'acb_groupnorm_stats',
            'acb_groupnorm_apply', 'acb_overlap_add', 'acb_lstm_recurrent_carry', 'acb_lm_begin_slots', 'acb_lm_admit',
-           'acb_lm_slot_status', 'acb_lm_retire']
+           'acb_lm_slot_status', 'acb_lm_retire', 'acb_lm_admit_prefix']
 
 
 def check(rc: int, what: str = ''):

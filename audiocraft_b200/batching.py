@@ -13,6 +13,11 @@ bit-identical to `generate` of that item alone when both run the same GEMM regim
 prompt is not prefilled (``ACB_LM_PREFILL=0``): a session consumes a continuation prompt one column per step (teacher
 forcing), which costs one step per prompt column, where `generate` prefills it several positions per pass.
 
+A melody model (the `prepend` fuser: MusicGen-melody) conditions a request on a prefix [2, P, d] of chroma and, in the
+released layout, description positions, whose length P differs from request to request.  Admission prefills it into the
+slot's own cache rows (acb_lm_admit_prefix), in the passes `generate` runs for that request alone, and the slot then runs
+column t at cache position P + t.  A session is sized for `max_prefix` prefix positions.
+
 Each request has its own sampling options (use_sampling, temperature, top-k, top-p, CFG coefficient): admission writes them to
 the slot's record on the device, which the captured step reads, so requests with different options share one session.  A
 request can be cancelled between steps (acb_lm_retire), which frees its slot for the next admission.
@@ -37,7 +42,8 @@ SLOT_INACTIVE, SLOT_ACTIVE, SLOT_FINISHED = 0, 1, 2
 
 @dataclass
 class Request:
-    """One generation request at the LM level: cross [2, T, d] ([cond; null]) or None, prompt codes [1, K, T0] or None."""
+    """One generation request at the LM level: cross [2, T, d] ([cond; null]) or None, prompt codes [1, K, T0] or None, and
+    on a model with a condition prefix its prefix [2, P, d] ([cond; null])."""
     max_gen_len: int
     cross: tp.Optional[torch.Tensor] = None
     prompt: tp.Optional[torch.Tensor] = None
@@ -50,6 +56,7 @@ class Request:
     top_k: tp.Optional[int] = None
     top_p: tp.Optional[float] = None
     cfg_coef: tp.Optional[float] = None
+    prefix: tp.Optional[torch.Tensor] = None
 
 
 SAMPLING_OPTIONS = ('use_sampling', 'temp', 'top_k', 'top_p', 'cfg_coef')
@@ -67,6 +74,19 @@ def check_sampling(use_sampling, temp, top_k, top_p, cfg_coef):
         raise ValueError(f"top_p must be in [0, 1], got {top_p!r}")
     if not (isinstance(cfg_coef, (int, float)) and math.isfinite(cfg_coef)):
         raise ValueError(f"cfg_coef must be finite, got {cfg_coef!r}")
+
+
+def prefix_bound(lm, max_text: int) -> int:
+    """The longest condition prefix a request can have on `lm`: 0 without a `prepend` fuser, else the melody conditioner's
+    chroma_len, plus max_text when the description is prepended too (the released [self_wav, description] layout)."""
+    if not lm.has_prefix:
+        return 0
+    cp = getattr(lm, 'condition_provider', None)
+    chroma = cp.conditioners['self_wav'] if cp is not None and 'self_wav' in cp.conditioners else None
+    if chroma is None or not chroma.match_len_on_eval:
+        raise NotImplementedError("a condition prefix without a melody ('self_wav') conditioner matched to its training length "
+                                  "has no length bound: pass max_prefix")
+    return chroma.chroma_len + (max_text if 'description' in lm.fuser.fuse2cond.get('prepend', []) else 0)
 
 
 def pattern_sequence(lm, prompt: tp.Optional[torch.Tensor], max_gen_len: int, device='cpu'):
@@ -101,24 +121,32 @@ def revert_sequence(lm, gen_sequence: torch.Tensor, mask: torch.Tensor, pattern,
 
 class SlotSession:
     """The device half of continuous batching on one `LMModel`: `slots` requests decoded side by side, in the CFG layout
-    (slot s owns rows s and slots + s).  Holds the model's decode handle until another generation call takes it."""
+    (slot s owns rows s and slots + s).  Holds the model's decode handle until another generation call takes it.
+
+    On a model with a condition prefix every request carries one of at most `max_prefix` positions (None: `prefix_bound`),
+    and the KV cache holds max_prefix + the longest sequence."""
 
     def __init__(self, lm, slots: int, max_gen_len: int, max_text: int = 64, use_sampling: bool = True, temp: float = 1.0,
-                 top_k: int = 250, top_p: float = 0.0, cfg_coef: tp.Optional[float] = None):
+                 top_k: int = 250, top_p: float = 0.0, cfg_coef: tp.Optional[float] = None,
+                 max_prefix: tp.Optional[int] = None):
         if not 1 <= slots <= _lib.ACB_LM_MAX_SLOTS:
             raise ValueError(f"slots must be in [1, {_lib.ACB_LM_MAX_SLOTS}], got {slots}")
         if max_gen_len < 1 or max_text < 1:
             raise ValueError("max_gen_len and max_text must be >= 1")
-        if lm.has_prefix:
-            raise NotImplementedError("continuous batching with a condition prefix (prepend fuser, melody) is not built")
+        if not lm.has_prefix and max_prefix:
+            raise ValueError("max_prefix > 0 needs a model with a condition prefix (prepend fuser)")
+        max_prefix = prefix_bound(lm, max_text) if max_prefix is None else int(max_prefix)
+        if max_prefix < 0:
+            raise ValueError(f"max_prefix must be >= 0, got {max_prefix}")
         self.lm, self.slots, self.max_gen_len, self.max_text = lm, slots, max_gen_len, max_text
+        self.max_prefix = max_prefix
         seq, _, pattern = pattern_sequence(lm, None, max_gen_len)
         self.seq_len_max, self.delays = seq.shape[-1], list(pattern.delays)
         coef = lm.cfg_coef if cfg_coef is None else cfg_coef
         self.sampling = dict(use_sampling=bool(use_sampling), temp=float(temp), top_k=int(top_k), top_p=float(top_p),
                              cfg_coef=float(coef))
         with torch.cuda.device(lm.device):
-            lm._ensure(2 * slots, self.seq_len_max, max_text if lm.cross_attention else 0, slots)
+            lm._ensure(2 * slots, max_prefix + self.seq_len_max, max_text if lm.cross_attention else 0, slots)
             samp = _lib.LMSampling(int(bool(use_sampling)), float(temp), int(top_k), float(top_p), float(coef), 0, 0, 0.0)
             _lib.check(lm._lib.acb_lm_begin_slots(lm._handle, slots, max_text, self.seq_len_max, C.byref(samp),
                                                   _lib.stream()), 'lm_begin_slots')
@@ -135,7 +163,8 @@ class SlotSession:
         return max(self.delays)
 
     def admit(self, slot: int, req: Request):
-        """Write the request's sequence and mask rows, then its sampling options, cross K/V and slot state (acb_lm_admit)."""
+        """Write the request's sequence and mask rows, then its sampling options, cross K/V, condition prefix and slot state
+        (acb_lm_admit_prefix)."""
         self._check_owner()
         lm = self.lm
         if req.max_gen_len > self.max_gen_len:
@@ -146,6 +175,17 @@ class SlotSession:
             check_sampling(**o)
             samp = C.byref(_lib.LMSampling(int(bool(o['use_sampling'])), float(o['temp']), int(o['top_k']), float(o['top_p']),
                                            float(o['cfg_coef']), 0, 0, 0.0))
+        if lm.has_prefix and req.prefix is None:
+            raise ValueError("the model prepends a condition prefix: the request needs its prefix [2, P, d]")
+        if not lm.has_prefix and req.prefix is not None:
+            raise ValueError("the model has no condition prefix (prepend fuser): the request must not carry one")
+        P = 0
+        if req.prefix is not None:
+            if req.prefix.dim() != 3 or req.prefix.shape[0] != 2 or req.prefix.shape[2] != lm.dim:
+                raise ValueError(f"prefix must be [2, P, {lm.dim}] ([cond; null]), got {tuple(req.prefix.shape)}")
+            P = req.prefix.shape[1]
+            if P > self.max_prefix:
+                raise ValueError(f"condition prefix of {P} positions: the session holds 0 .. {self.max_prefix}")
         with torch.cuda.device(lm.device):
             seq, mask, pattern = pattern_sequence(lm, req.prompt, req.max_gen_len, lm.device)
             S = seq.shape[-1]
@@ -164,9 +204,11 @@ class SlotSession:
                 T = cross.shape[1]
                 if not 1 <= T <= self.max_text:
                     raise ValueError(f"condition of {T} text positions: the session holds 1 .. {self.max_text}")
-            _lib.check(lm._lib.acb_lm_admit(lm._handle, slot, _lib.ptr(cross), T, S, C.c_uint64(req.seed), samp,
-                                            _lib.stream()), 'lm_admit')
-            req.meta.update(S=S, mask=mask, pattern=pattern, keep=cross)   # `keep`: the stream reads cross after this call
+            prefix = req.prefix.to(lm.device, torch.float32).contiguous() if P else None
+            _lib.check(lm._lib.acb_lm_admit_prefix(lm._handle, slot, _lib.ptr(cross), T, _lib.ptr(prefix), P, S,
+                                                   C.c_uint64(req.seed), samp, _lib.stream()), 'lm_admit')
+            # `keep`: the stream reads cross and the prefix after this call
+            req.meta.update(S=S, mask=mask, pattern=pattern, keep=(cross, prefix))
 
     def retire(self, slot: int):
         """Cancel the slot's request between steps (acb_lm_retire): the slot stops decoding and is free for admission."""
@@ -385,8 +427,8 @@ class ContinuousGenerator:
     """`model.continuous(slots, poll_steps, max_text, return_tokens, chunk_duration)`: submit requests at any time, collect
     their audio as it decodes or when they finish.
 
-    `submit(description=None, duration=None, prompt=None, prompt_sample_rate=None, *, use_sampling=None, top_k=None,
-    top_p=None, temperature=None, cfg_coef=None)` returns a request id.  The sampling options are the request's own; None
+    `submit(description=None, duration=None, prompt=None, prompt_sample_rate=None, *, melody=None, melody_sample_rate=None,
+    use_sampling=None, top_k=None, top_p=None, temperature=None, cfg_coef=None)` returns a request id.  The sampling options are the request's own; None
     takes the value of `model.generation_params` when the generator was made.  Requests beyond `slots` wait in FIFO order.  A
     continuation prompt costs one decode step per prompt frame.  `cancel(request_id)` drops a waiting request or stops a
     decoding one, whose slot then takes the next waiting request; it returns False for a finished or unknown id, and a
@@ -395,7 +437,9 @@ class ContinuousGenerator:
     Without `chunk_duration`, `poll()` runs one scheduling round and returns `(request_id, wav)` (or `(request_id, wav,
     tokens)` with return_tokens) for the requests that finished in it.  `wav` is [1, C, T] and `tokens` [1, K, T_frames]:
     what `generate([description])` (or `generate_continuation` / `generate_unconditional`) returns for that request alone,
-    with its options, after the same `torch.manual_seed`.
+    with its options, after the same `torch.manual_seed`.  On a melody model a request with `melody` ([C, T] or [1, C, T] at
+    `melody_sample_rate`) returns what `generate_with_chroma([description], melody)` returns; without one its melody is
+    null, as in `generate`.  Each request's chroma and description prefix is prefilled into its slot at admission.
 
     With `chunk_duration`, a round runs at most `round(chunk_duration * frame_rate)` steps and `poll()` returns
     `(request_id, piece, final)` (or `(request_id, piece, tokens, final)`) events: `piece` [1, C, m] is the request's next
@@ -404,14 +448,16 @@ class ContinuousGenerator:
     requests admitted in one round share one stream decoder.  Refused before any device work: a codec without a stream
     decoder (NotImplementedError) and chunk_duration <= 0 (ValueError).
 
-    Refused (NotImplementedError, before any device work): durations beyond max_duration, melody models, two_step_cfg and
-    cfg_coef_beta."""
+    Refused before any device work: durations beyond max_duration, two_step_cfg and cfg_coef_beta (NotImplementedError), a
+    melody on a model without a melody conditioner (NotImplementedError), a melody together with a prompt, and a description
+    longer than max_text text positions (ValueError)."""
 
     def __init__(self, model, slots: int = 32, poll_steps: tp.Optional[int] = None, max_text: int = 64,
                  return_tokens: bool = False, chunk_duration: tp.Optional[float] = None):
         params = dict(model.generation_params)
-        if getattr(model, '_has_melody', False) or model.lm.has_prefix:
-            raise NotImplementedError("continuous batching of melody-conditioned models (a condition prefix) is not built")
+        if getattr(model, '_has_melody', False) != model.lm.has_prefix:
+            raise NotImplementedError("continuous batching takes a melody ('self_wav') conditioner only as a condition prefix "
+                                      "(prepend fuser), and a condition prefix only from one")
         if params.get('two_step_cfg'):
             raise NotImplementedError("continuous batching with two_step_cfg is not built")
         if params.get('cfg_coef_beta') is not None:
@@ -438,6 +484,7 @@ class ContinuousGenerator:
 
     def submit(self, description: tp.Optional[str] = None, duration: tp.Optional[float] = None,
                prompt: tp.Optional[torch.Tensor] = None, prompt_sample_rate: tp.Optional[int] = None, *,
+               melody: tp.Optional[torch.Tensor] = None, melody_sample_rate: tp.Optional[int] = None,
                use_sampling: tp.Optional[bool] = None, top_k: tp.Optional[int] = None, top_p: tp.Optional[float] = None,
                temperature: tp.Optional[float] = None, cfg_coef: tp.Optional[float] = None) -> int:
         from .audio_utils import convert_audio
@@ -456,6 +503,17 @@ class ContinuousGenerator:
                 prompt = prompt[None]
             if prompt.dim() != 3 or prompt.shape[0] != 1:
                 raise ValueError("prompt should be one item: [C, T] or [1, C, T]")
+        if melody is not None:
+            if not getattr(m, '_has_melody', False):
+                raise NotImplementedError("this model has no melody ('self_wav') conditioner; use a MusicGen-melody model")
+            if prompt is not None:
+                raise ValueError("a melody and a prompt together: generate_with_chroma takes no prompt")
+            if melody_sample_rate is None:
+                raise ValueError("melody_sample_rate is required with a melody")
+            if melody.dim() == 3 and melody.shape[0] == 1:
+                melody = melody[0]
+            if melody.dim() != 2:
+                raise ValueError("melody should be one item: [C, T] or [1, C, T]")
         given = dict(use_sampling=use_sampling, temp=temperature, top_k=top_k, top_p=top_p, cfg_coef=cfg_coef)
         options = {k: self.defaults[k] if v is None else v for k, v in given.items()}
         if options['cfg_coef'] is None:
@@ -463,15 +521,24 @@ class ContinuousGenerator:
         check_sampling(**options)
         if prompt is not None:
             prompt = convert_audio(prompt, prompt_sample_rate, m.sample_rate, m.audio_channels)
-        attributes, prompt_tokens = m._prepare_tokens_and_attributes([description], prompt)
+        if melody is not None:
+            attributes, prompt_tokens = m._prepare_melody([description], [melody], melody_sample_rate)
+        else:   # on a melody model every item carries a melody condition: a null one here
+            attributes, prompt_tokens = m._prepare_tokens_and_attributes([description], prompt)
         if prompt_tokens is not None and prompt_tokens.shape[-1] >= n:
             raise ValueError(f"the prompt ({prompt_tokens.shape[-1]} frames) must be shorter than the generation ({n})")
-        cross = m.lm._condition_tensors(attributes)[0] if m.lm.cross_attention else None
+        cross = prefix = None
+        if m.lm.cross_attention or m.lm.has_prefix:
+            cross, prefix = m.lm._condition_tensors(attributes)
+            cross = cross if m.lm.cross_attention else None
         if cross is not None and cross.shape[1] > self.session.max_text:
             raise ValueError(f"the description has {cross.shape[1]} text positions; the session holds {self.session.max_text}")
+        if prefix is not None and prefix.shape[1] > self.session.max_prefix:
+            raise ValueError(f"the condition prefix has {prefix.shape[1]} positions (chroma and description); the session holds "
+                             f"{self.session.max_prefix}: the description is longer than {self.session.max_text} text positions")
         seed = int(torch.randint(0, 2 ** 62, (1,)).item())   # drawn as LMModel.generate draws it
         rid = next(self._ids)
-        self.scheduler.submit(Request(n, cross, prompt_tokens, seed, rid, **options))
+        self.scheduler.submit(Request(n, cross, prompt_tokens, seed, rid, **options, prefix=prefix))
         return rid
 
     def cancel(self, request_id: int) -> bool:

@@ -29,8 +29,10 @@
 
 // Slot mode (acb_lm_begin_slots): per-slot device state, ACB_LM_SLOT_STRIDE ints per slot in buffers.slot_state.  The host
 // writes a slot only at admission (lm_slot_admit_kernel); the step's sampler advances POS and sets STATUS to FINISHED.
+// POS counts the sequence columns consumed; PREFIX is the slot's condition-prefix length, so column t runs at cache position
+// PREFIX + t.
 enum { ACB_SLOT_POS = 0, ACB_SLOT_STATUS = 1, ACB_SLOT_SEQ_LEN = 2, ACB_SLOT_TEXT_LEN = 3, ACB_SLOT_SEED_LO = 4,
-       ACB_SLOT_SEED_HI = 5, ACB_SLOT_DONE = 6 };
+       ACB_SLOT_SEED_HI = 5, ACB_SLOT_DONE = 6, ACB_SLOT_PREFIX = 7 };
 enum { SLOT_INACTIVE = 0, SLOT_ACTIVE = 1, SLOT_FINISHED = 2 };
 
 // ------------------------------------------------------------------------------------------------ helpers
@@ -87,14 +89,16 @@ __global__ void __launch_bounds__(256) lm_embed_kernel(const __half* __restrict_
 }
 
 // Slot mode (continuous batching): row r belongs to slot r % slots (cond rows [0, slots), null rows [slots, 2 slots)) and
-// reads that slot's sequence at the slot's own position.  An inactive slot embeds a finite, unused row.
+// reads that slot's sequence column at the slot's own position; the sin term is at cache position prefix + column, as
+// lm_embed_kernel's seq_off has it.  An inactive slot embeds a finite, unused row.
 __global__ void __launch_bounds__(256) lm_embed_slot_kernel(const __half* __restrict__ emb, const float* __restrict__ inv_freq,
                                                             const int64_t* __restrict__ seq, const int* __restrict__ slot_state,
                                                             float* __restrict__ x, int d, int n_q, int card, int max_seq,
                                                             int slots, float pos_scale, bool sin_pos) {
     const int r = blockIdx.x, b = r % slots;
-    embed_row(emb, inv_freq, seq, x, r, b, slot_state[b * ACB_LM_SLOT_STRIDE + ACB_SLOT_POS], d, n_q, card, max_seq, pos_scale,
-              sin_pos, 0);
+    const int* st = slot_state + b * ACB_LM_SLOT_STRIDE;
+    const int prefix = st[ACB_SLOT_PREFIX];
+    embed_row(emb, inv_freq, seq, x, r, b, prefix + st[ACB_SLOT_POS], d, n_q, card, max_seq, pos_scale, sin_pos, prefix);
 }
 
 // Condition-prefix prefill (the `prepend` fuser, conditioners.py:1703-1763): the grid's rows are (position, row) pairs
@@ -183,6 +187,7 @@ struct GemmParams {
     float* q32; __half* kc; __half* vc; int d, H, cache_len; const int* pos;  // QKV / CROSSKV
     int text_len, row0;                                                      // CROSSKV
     int rows_real;                                                           // QKV_PF: rows of the generation (GEMM row = tok * rows_real + row)
+    int row_stride;   // QKV_PF: row `row` of the generation is cache row row * row_stride of kc / vc (slots in an admission, else 1)
 };
 static_assert(sizeof(GemmParams) == 128, "GemmParams layout");
 
@@ -297,9 +302,9 @@ __global__ void __launch_bounds__(128) lm_gemm_kernel(GemmParams p) {
         } else if (EPI == EPI_GELU) {
             p.out_f16[(size_t)row * p.ld_out + n] = __float2half_rn(gelu_erf(half_round(v)));
         } else if (QKV) {   // q | k | v blocks of d features each (no integer division: cold code costs here)
-            // prefill: row = tk * rows_real + rr -> cache row rr, position cache_pos + tk
+            // prefill: row = tk * rows_real + rr -> cache row rr * row_stride, position cache_pos + tk
             const int which = n >= 2 * p.d ? 2 : (n >= p.d ? 1 : 0), nn = n - which * p.d;
-            const int tk = PF ? row / p.rows_real : 0, rr = row - tk * p.rows_real;
+            const int tk = PF ? row / p.rows_real : 0, rr = PF ? (row - tk * p.rows_real) * p.row_stride : row;
             if (ROPE && which < 2) {   // the pair partner is feature n ^ 1 of the same CTA (f0 % 16 == 0), same warp order
                 float other = 0.f;
 #pragma unroll
@@ -453,12 +458,13 @@ __global__ void __launch_bounds__(128, 1) lm_gemm_wide_kernel(const __grid_const
 // Slot mode's QKV epilogue as its own kernel: the QKV GEMM runs with the plain fp32 epilogue (EPI_F32, the same sums as
 // EPI_QKV / EPI_QKV_ROPE) into qkv [rows][3d], and this kernel does what those epilogues do at each row's own position: q to
 // q32 (fp32), k and v to the cache (fp16), q and k rotated first under rotary positions.  Only ACTIVE slots append to the cache.
+// The position is the cache position: the slot's prefix length + its column.
 __global__ void __launch_bounds__(256) lm_qkv_slot_kernel(const float* __restrict__ qkv, const int* __restrict__ slot_state,
                                                           float* __restrict__ q32, __half* __restrict__ kc, __half* __restrict__ vc,
                                                           int d, int H, int cache_len, int slots, const float* __restrict__ rope_freq,
                                                           float pos_scale, bool rope) {
     const int row = blockIdx.x, s = row % slots;
-    const int pos = slot_state[s * ACB_LM_SLOT_STRIDE + ACB_SLOT_POS];
+    const int pos = slot_state[s * ACB_LM_SLOT_STRIDE + ACB_SLOT_PREFIX] + slot_state[s * ACB_LM_SLOT_STRIDE + ACB_SLOT_POS];
     const bool live = slot_state[s * ACB_LM_SLOT_STRIDE + ACB_SLOT_STATUS] == SLOT_ACTIVE;
     const float* src = qkv + (size_t)row * 3 * d;
     for (int n = threadIdx.x; n < 3 * d; n += 256) {
@@ -480,6 +486,7 @@ struct AttnParams {
     const __half* kc; const __half* vc; __half* out;
     int H, d, cache_len; const int* pos; int fixed_len; float scale;
     int rows_real;                // prefill (PF kernels): rows of the generation
+    int row_stride;               // prefill (PF kernels): row r of the generation is cache row r * row_stride of kc / vc
 };
 
 constexpr int ATT_WARPS = 8;
@@ -501,7 +508,7 @@ __device__ __forceinline__ void osm_merge(OnlineSM& a, float m2, float l2, const
 // outstanding continuously, in shared memory instead of registers.
 // PF (prompt prefill): blockIdx.y is a (token, row) pair tok * rows_real + r; the query at position pos + tok attends to the
 // cache of row r up to and including its own position (the QKV GEMM of the same pass has already appended every token of the
-// pass: causal within the chunk).
+// pass: causal within the chunk); row r is cache row r * row_stride.
 constexpr int ATT2_DEPTH = 8;
 constexpr int ATT2_SMEM = ATT_WARPS * ATT2_DEPTH * 1024;   // the ring, 64 KB
 template <bool PF>
@@ -509,7 +516,7 @@ __global__ void __launch_bounds__(ATT_WARPS * 32) lm_attn2_kernel(AttnParams p) 
     extern __shared__ __align__(16) unsigned char att2sm[];   // [warp][depth][K | V][32 lanes][16 B]
     __shared__ float wm[ATT_WARPS], wl[ATT_WARPS], wacc[ATT_WARPS][64];
     const int h = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int qrow = blockIdx.y, row = PF ? qrow % p.rows_real : qrow, tok = PF ? qrow / p.rows_real : 0;
+    const int qrow = blockIdx.y, row = PF ? qrow % p.rows_real * p.row_stride : qrow, tok = PF ? qrow / p.rows_real : 0;
     const int sl = lane & 7, pg = lane >> 3;
     const int n = p.fixed_len > 0 ? p.fixed_len : p.pos[0] + tok + 1;
     const size_t base = ((size_t)row * p.H + h) * p.cache_len * 64 + sl * 8;
@@ -614,8 +621,8 @@ __global__ void __launch_bounds__(ATT_WARPS * 32) lm_attn2_kernel(AttnParams p) 
 
 
 // Slot mode: lm_attn2_kernel with each row at its own slot's position (a separate copy: the decode kernel stays as it is).
-// Row r of slot r % slots (p.rows_real = slots) attends to its slot's positions [0, pos]; the rows of a slot that is not ACTIVE
-// attend to no key and write zeros.
+// Row r of slot r % slots (p.rows_real = slots) attends to its slot's cache positions [0, prefix + pos]: the condition prefix
+// and the columns so far.  The rows of a slot that is not ACTIVE attend to no key and write zeros.
 __global__ void __launch_bounds__(ATT_WARPS * 32) lm_attn2_slot_kernel(AttnParams p, const int* __restrict__ slot_state) {
     extern __shared__ __align__(16) unsigned char att2sm[];   // [warp][depth][K | V][32 lanes][16 B]
     __shared__ float wm[ATT_WARPS], wl[ATT_WARPS], wacc[ATT_WARPS][64];
@@ -627,7 +634,7 @@ __global__ void __launch_bounds__(ATT_WARPS * 32) lm_attn2_slot_kernel(AttnParam
         if (tid < 64) p.out[(size_t)qrow * p.d + h * 64 + tid] = __float2half_rn(0.f);
         return;
     }
-    const int n = slot[ACB_SLOT_POS] + 1;
+    const int n = slot[ACB_SLOT_PREFIX] + slot[ACB_SLOT_POS] + 1;
     const size_t base = ((size_t)row * p.H + h) * p.cache_len * 64 + sl * 8;
     const __half* kb = p.kc + base;
     const __half* vb = p.vc + base;
@@ -789,7 +796,7 @@ __global__ void __launch_bounds__(256) lm_cross_attn_kernel(AttnParams p, int ro
     const int pair = blockIdx.x * 8 + (threadIdx.x >> 5);   // (row, head) index
     if (pair >= rows * p.H) return;                         // warp-uniform
     const int row = pair / p.H, h = pair % p.H;
-    cross_attn_body(p, row, h, PF ? row % p.rows_real : row, p.fixed_len);   // K / V of the generation row
+    cross_attn_body(p, row, h, PF ? row % p.rows_real * p.row_stride : row, p.fixed_len);   // K / V of the generation row
 }
 
 // Slot mode: row r attends to exactly its slot's own text length (p.rows_real = slots), not to a length shared by the batch,
@@ -1066,10 +1073,12 @@ __global__ void lm_slot_retire_kernel(int* slot_state, int slot) {
     slot_state[slot * ACB_LM_SLOT_STRIDE + ACB_SLOT_STATUS] = SLOT_INACTIVE;
 }
 
-// Admission: the slot starts at position 0 with its own sequence length, text length and seed.
-__global__ void lm_slot_admit_kernel(int* slot_state, int slot, int seq_len, int text_len, uint32_t seed_lo, uint32_t seed_hi) {
+// Admission: the slot starts at column 0 with its own sequence length, text length, condition-prefix length and seed.
+__global__ void lm_slot_admit_kernel(int* slot_state, int slot, int seq_len, int text_len, int prefix_len, uint32_t seed_lo,
+                                     uint32_t seed_hi) {
     int* st = slot_state + slot * ACB_LM_SLOT_STRIDE;
     st[ACB_SLOT_POS] = 0;
+    st[ACB_SLOT_PREFIX] = prefix_len;
     st[ACB_SLOT_STATUS] = SLOT_ACTIVE;
     st[ACB_SLOT_SEQ_LEN] = seq_len;
     st[ACB_SLOT_TEXT_LEN] = text_len;
@@ -1095,7 +1104,10 @@ struct acb_lm {
     int batch = 0, rows = 0, rows_pad = 0, text_len = 0, seq_len = 0, sms = 132;
     int slots = 0;                 // slot mode (acb_lm_begin_slots): batch = slots, rows = 2 * slots, per-slot device state
     int prefix_len = 0;            // condition-prefix positions in front of the tokens in the KV cache
-    const float* prefix = nullptr; // [rows][prefix_len][d] fp32, set only while acb_lm_begin_prefix enqueues the prefix passes
+    const float* prefix = nullptr; // [rows][prefix_len][d] fp32, set only while acb_lm_begin_prefix / _admit_prefix enqueue passes
+    // set only while acb_lm_admit_prefix enqueues a slot's prefix passes (-1 otherwise): the passes run on that slot's two
+    // rows (cache rows pf_slot and slots + pf_slot) with its own text length, as a generation of batch 1 with CFG would
+    int pf_slot = -1, pf_text_len = 0;
     int launches = 0;
     bool has_cross = false;
     // wide GEMM (max_rows > 64): one map per stacked weight matrix [L * N][K] (encoded by acb_lm_create) and per activation
@@ -1273,25 +1285,33 @@ static int acb_dbg(cudaStream_t s, bool capturing, const char* what, int layer) 
 // inside the pass because the QKV GEMM appends all of them to the cache before the attention kernel runs -- and stop after the
 // last layer (no logits: the next decode step consumes the last prompt position).
 // pf_prefix: the pass embeds condition-prefix vectors (lm->prefix) instead of tokens, otherwise it is a prefill pass like any other.
+// In an admission (lm->pf_slot >= 0) a pass serves the slot's two rows only: row j of the pass's generation is cache row
+// pf_slot + j * slots, and cross attention covers the slot's own text length.
+static int pass_rows(const acb_lm* lm) { return lm->pf_slot >= 0 ? 2 : lm->rows; }
+
 static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_launch, bool gemms_only = false,
                         bool capturing = false, int pf_tokens = 0, bool pf_prefix = false) {
     const acb_lm_config& c = lm->cfg;
     const acb_lm_buffers& B = lm->buf;
     const bool pf = pf_tokens > 0;
     ACB_REQUIRE(!pf_prefix || (pf && lm->prefix), "enqueue_step: a prefix pass needs the prefix of acb_lm_begin_prefix");
-    const int rows_real = lm->rows, rows = pf ? rows_real * pf_tokens : rows_real;
+    const bool slot_step = lm->slots && !pf;   // the session's decode step (its passes are an admission's prefix prefill)
+    const int rows_real = pf ? pass_rows(lm) : lm->rows, rows = pf ? rows_real * pf_tokens : rows_real;
+    const int row0 = pf && lm->pf_slot >= 0 ? lm->pf_slot : 0, row_stride = pf && lm->pf_slot >= 0 ? lm->slots : 1;
+    const int text_len = pf && lm->pf_slot >= 0 ? lm->pf_text_len : lm->text_len;
     const int d = c.dim, ffn = c.ffn_dim, L = c.num_layers, H = c.num_heads, nt = nt_for_rows(rows);
     // rows > 64 (then rows_real > 64 and a prefill pass holds one position per row): every GEMM but EPI_CROSSKV on the wide kernel
     const bool wide = rows > 64;
     const size_t part_stride = (size_t)(pf && !wide ? 8 * nt : lm->rows_pad) * d;
     const size_t kv_layer = (size_t)c.max_rows * H * c.max_seq * 64;
     const size_t ckv_layer = (size_t)c.max_rows * H * c.max_text * 64;
+    const size_t kv_row0 = (size_t)row0 * H * c.max_seq * 64, ckv_row0 = (size_t)row0 * H * c.max_text * 64;
     const float scale = 1.0f / sqrtf(64.f);
     int nl = 0, ks = 0;
 
     if (!gemms_only) {
         const bool sin_pos = c.positional_embedding != 1;
-        if (lm->slots) lm_embed_slot_kernel<<<rows, 256, 0, s>>>((const __half*)lm->w.emb, lm->w.inv_freq, B.seq, B.slot_state, B.x, d,
+        if (slot_step) lm_embed_slot_kernel<<<rows, 256, 0, s>>>((const __half*)lm->w.emb, lm->w.inv_freq, B.seq, B.slot_state, B.x, d,
                                                                 c.n_q, c.card, c.max_seq, lm->slots, c.pos_scale, sin_pos);
         else if (pf && pf_prefix) lm_embed_prefix_kernel<<<rows, 256, 0, s>>>(lm->prefix, lm->w.inv_freq, B.pos, B.x, d, lm->prefix_len,
                                                                        c.pos_scale, rows_real, sin_pos);
@@ -1331,12 +1351,12 @@ static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_la
         {
             const int ns = wide ? pick_split_wide(3 * d, d, lm->sms, false, &ks) : pick_split(3 * d, d, lm->sms, false, &ks);
             GemmParams p = base_gemm((const __half*)lm->w.w_qkv + (size_t)l * 3 * d * d, B.h16, 3 * d, d, rows, ks);
-            p.q32 = B.q32; p.kc = (__half*)B.k_cache + l * kv_layer; p.vc = (__half*)B.v_cache + l * kv_layer;
-            p.d = d; p.H = H; p.cache_len = c.max_seq; p.pos = B.pos; p.rows_real = rows_real;
+            p.q32 = B.q32; p.kc = (__half*)B.k_cache + l * kv_layer + kv_row0; p.vc = (__half*)B.v_cache + l * kv_layer + kv_row0;
+            p.d = d; p.H = H; p.cache_len = c.max_seq; p.pos = B.pos; p.rows_real = rows_real; p.row_stride = row_stride;
             p.rope_freq = lm->w.rope_freq; p.pos_scale = c.pos_scale;
             const bool rope = c.positional_embedding != 0;
             const int ft2 = pf ? 1 : pick_ft2(3 * d, d, 1, ks, nt, lm->sms);
-            if (lm->slots) {   // plain fp32 epilogue into part slot 0 (free between the LN and the out projection), then
+            if (slot_step) {   // plain fp32 epilogue into part slot 0 (free between the LN and the out projection), then
                                // the rotary + cache append at each row's own position
                 p.out_f32 = B.part; p.ld_out = 3 * d;
                 if (wide) ACB_TRY(launch_wide<EPI_F32>(lm->wmap[WM_QKV], lm->xmap_h16, l * 3 * d, p, ns, s));
@@ -1354,15 +1374,15 @@ static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_la
                                    : launch_wide<EPI_QKV>(lm->wmap[WM_QKV], lm->xmap_h16, l * 3 * d, p, ns, s));
             else if (pf) ACB_TRY(rope ? launch_gemm<EPI_QKV_PF_ROPE>(nt, p, 1, s, ft2) : launch_gemm<EPI_QKV_PF>(nt, p, 1, s, ft2));
             else ACB_TRY(rope ? launch_gemm<EPI_QKV_ROPE>(nt, p, 1, s, ft2) : launch_gemm<EPI_QKV>(nt, p, 1, s, ft2));
-            if (!lm->slots) {
+            if (!slot_step) {
                 ++nl;
                 DBG("gemm_EPI_QKV", l);
             }
         }
         if (!gemms_only) {
-            AttnParams a{B.q32, 1, 0, (__half*)B.k_cache + l * kv_layer, (__half*)B.v_cache + l * kv_layer, (__half*)B.a16,
-                         H, d, c.max_seq, B.pos, 0, scale, rows_real};
-            if (lm->slots) { a.rows_real = lm->slots; lm_attn2_slot_kernel<<<dim3(H, rows), ATT_WARPS * 32, ATT2_SMEM, s>>>(a, B.slot_state); }
+            AttnParams a{B.q32, 1, 0, (__half*)B.k_cache + l * kv_layer + kv_row0, (__half*)B.v_cache + l * kv_layer + kv_row0,
+                         (__half*)B.a16, H, d, c.max_seq, B.pos, 0, scale, rows_real, row_stride};
+            if (slot_step) { a.rows_real = lm->slots; lm_attn2_slot_kernel<<<dim3(H, rows), ATT_WARPS * 32, ATT2_SMEM, s>>>(a, B.slot_state); }
             else if (pf) lm_attn2_kernel<true><<<dim3(H, rows), ATT_WARPS * 32, ATT2_SMEM, s>>>(a);
             else lm_attn2_kernel<false><<<dim3(H, rows), ATT_WARPS * 32, ATT2_SMEM, s>>>(a);
             ACB_LAUNCH_CHECK();
@@ -1377,10 +1397,10 @@ static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_la
             const int nsq = pending;
             pending = 0;   // these partials are the cross-attention queries, not a residual update
             if (!gemms_only) {
-                AttnParams a{B.part, nsq, part_stride, (__half*)B.ck_cache + l * ckv_layer,
-                             (__half*)B.cv_cache + l * ckv_layer, (__half*)B.a16, H, d, c.max_text, B.pos, lm->text_len,
-                             scale, rows_real};
-                if (lm->slots) {
+                AttnParams a{B.part, nsq, part_stride, (__half*)B.ck_cache + l * ckv_layer + ckv_row0,
+                             (__half*)B.cv_cache + l * ckv_layer + ckv_row0, (__half*)B.a16, H, d, c.max_text, B.pos, text_len,
+                             scale, rows_real, row_stride};
+                if (slot_step) {
                     a.rows_real = lm->slots;
                     lm_cross_attn_slot_kernel<<<acb_ceil_div(rows * H, 8), 256, 0, s>>>(a, rows, B.slot_state);
                 } else if (pf) lm_cross_attn_kernel<true><<<acb_ceil_div(rows * H, 8), 256, 0, s>>>(a, rows);
@@ -1539,17 +1559,18 @@ __global__ void lm_set_pos_kernel(int* pos, int value) { pos[0] = value; }
 // Prefill passes over cache positions [pos0, pos0 + n) of every row, ACB_LM_PREFILL_ROWS / rows positions per pass (one above
 // 64 rows: the wide GEMM already shares each weight byte among all rows): token columns pos - prefix_len of buffers.seq, or
 // (prefix) the condition-prefix vectors.  Leaves pos = pos0 + n on the device and the padded decode rows [rows, rows_pad) of
-// the activation buffers zero.
+// the activation buffers zero.  In an admission (lm->pf_slot >= 0) the passes serve the slot's two rows, so a pass holds
+// ACB_LM_PREFILL_ROWS / 2 positions, as in a generation of batch 1 with CFG; the padding restored is the session's.
 static int prefill_passes(acb_lm* lm, cudaStream_t s, int pos0, int n, bool prefix) {
     const acb_lm_config& c = lm->cfg;
-    const int d = c.dim;
-    int per = lm->rows > ACB_LM_PREFILL_ROWS ? 1 : ACB_LM_PREFILL_ROWS / lm->rows;
+    const int d = c.dim, rows = pass_rows(lm);
+    int per = rows > ACB_LM_PREFILL_ROWS ? 1 : ACB_LM_PREFILL_ROWS / rows;
     // ACB_LM_PREFILL_PER=n: at most n positions per pass (n = 1: one position per pass, the reference order for tests)
     if (const char* e = getenv("ACB_LM_PREFILL_PER")) { const int cap = atoi(e); if (cap >= 1 && cap < per) per = cap; }
     int done = 0;
     while (done < n) {
         const int tc = n - done < per ? n - done : per;
-        const int vrows = lm->rows * tc, pad = 8 * nt_for_rows(vrows);
+        const int vrows = rows * tc, pad = 8 * nt_for_rows(vrows);
         lm_set_pos_kernel<<<1, 1, 0, s>>>(lm->buf.pos, pos0 + done);
         ACB_LAUNCH_CHECK();
         if (pad > vrows) {   // the GEMMs read their activation rows up to the tile height: rows >= vrows must be zero
@@ -1720,10 +1741,18 @@ extern "C" int acb_lm_begin_slots(acb_lm_t* lm, int slots, int max_text, int seq
 
 extern "C" int acb_lm_admit(acb_lm_t* lm, int slot, const float* cross, int text_len, int seq_len, uint64_t seed,
                             const acb_lm_sampling* sampling, void* stream) {
+    return acb_lm_admit_prefix(lm, slot, cross, text_len, nullptr, 0, seq_len, seed, sampling, stream);
+}
+
+extern "C" int acb_lm_admit_prefix(acb_lm_t* lm, int slot, const float* cross, int text_len, const float* prefix, int prefix_len,
+                                   int seq_len, uint64_t seed, const acb_lm_sampling* sampling, void* stream) {
     ACB_REQUIRE(lm && lm->slots > 0, "acb_lm_admit: call acb_lm_begin_slots first");
     const acb_lm_config& c = lm->cfg;
     ACB_REQUIRE(slot >= 0 && slot < lm->slots, "acb_lm_admit: slot %d not in [0, %d)", slot, lm->slots);
     ACB_REQUIRE(seq_len >= 2 && seq_len <= lm->seq_len, "acb_lm_admit: seq_len %d not in [2, %d]", seq_len, lm->seq_len);
+    ACB_REQUIRE(prefix_len >= 0 && (prefix_len == 0 || prefix), "acb_lm_admit: prefix_len %d without a prefix tensor", prefix_len);
+    ACB_REQUIRE(prefix_len + seq_len <= c.max_seq, "acb_lm_admit: prefix %d + seq_len %d > max_seq %d", prefix_len, seq_len,
+                c.max_seq);
     ACB_REQUIRE(!lm->has_cross || (cross && text_len >= 1 && text_len <= lm->text_len),
                 "acb_lm_admit: the model has cross attention: a condition of 1 .. %d text positions is required (got %d)",
                 lm->text_len, text_len);
@@ -1764,11 +1793,22 @@ extern "C" int acb_lm_admit(acb_lm_t* lm, int slot, const float* cross, int text
                 }
         }
     }
+    // the condition prefix fills cache positions [0, prefix_len) of the slot's two rows (after the cross K/V: the passes attend
+    // to them), in the passes acb_lm_begin_prefix runs for a generation of batch 1, so the K/V are the ones it writes.  The
+    // passes use the activation buffers and buffers.pos, which the session's step does not carry from one step to the next.
+    if (prefix_len > 0) {
+        lm->pf_slot = slot; lm->pf_text_len = lm->has_cross ? text_len : 0;
+        lm->prefix = prefix; lm->prefix_len = prefix_len;
+        const int rc = prefill_passes(lm, s, 0, prefix_len, true);
+        lm->pf_slot = -1; lm->pf_text_len = 0;
+        lm->prefix = nullptr; lm->prefix_len = 0;   // the session's step reads column = position (its sampler's seq_off is 0)
+        ACB_TRY(rc);
+    }
     lm_slot_sampling_kernel<<<1, 1, 0, s>>>(lm->buf.slot_sampling, slot, sp.use_sampling, sp.temp, sp.top_k, sp.top_p,
                                             sp.cfg_coef);
     ACB_LAUNCH_CHECK();
-    lm_slot_admit_kernel<<<1, 1, 0, s>>>(lm->buf.slot_state, slot, seq_len, lm->has_cross ? text_len : 0, (uint32_t)seed,
-                                         (uint32_t)(seed >> 32));
+    lm_slot_admit_kernel<<<1, 1, 0, s>>>(lm->buf.slot_state, slot, seq_len, lm->has_cross ? text_len : 0, prefix_len,
+                                         (uint32_t)seed, (uint32_t)(seed >> 32));
     ACB_LAUNCH_CHECK();
     return ACB_OK;
 }

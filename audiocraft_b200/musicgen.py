@@ -221,7 +221,9 @@ class BaseGenModel:
         generation parameters) and `cancel(request_id)` stops a request.  `poll()` / `run()` return `(request_id, wav[, tokens])`
         as requests finish, each equal to that request generated alone; with `chunk_duration` (seconds of decode steps per
         round) they return `(request_id, piece[, tokens], final)` audio pieces while the requests decode.  `max_text` bounds a
-        description's text positions."""
+        description's text positions.  On a melody model `submit(..., melody=, melody_sample_rate=)` conditions a request on
+        its melody as `generate_with_chroma` does (no melody: a null one); each request's chroma and description prefix is
+        prefilled into its slot when it is admitted."""
         from .batching import ContinuousGenerator
         return ContinuousGenerator(self, slots, poll_steps, max_text, return_tokens, chunk_duration)
 

@@ -220,7 +220,8 @@ typedef struct {
     /* slot mode only (acb_lm_begin_slots; NULL otherwise), with B = slots in seq above: */
     int32_t* slot_sampling; /* [slots][ACB_LM_SLOT_SAMPLING_STRIDE] 32-bit words per slot: use_sampling, temp (fp32 bits), top_k,
                                top_p (fp32 bits), cfg_coef (fp32 bits), 3 unused (written by the library at admission) */
-    int32_t* slot_state; /* [slots][ACB_LM_SLOT_STRIDE] per-slot position, status, lengths and seed (written by the library) */
+    int32_t* slot_state; /* [slots][ACB_LM_SLOT_STRIDE] per-slot position, status, lengths, seed and condition-prefix length
+                            (written by the library) */
     uint8_t* slot_mask;  /* [slots][n_q][max_seq] each slot's pattern validity mask (written by the caller before acb_lm_admit) */
 } acb_lm_buffers;
 
@@ -308,6 +309,18 @@ int acb_lm_begin_slots(acb_lm_t* lm, int slots, int max_text, int seq_len_max, c
  * temp == 0 takes the argmax. */
 int acb_lm_admit(acb_lm_t* lm, int slot, const float* cross, int text_len, int seq_len, uint64_t seed,
                  const acb_lm_sampling* sampling, void* stream);
+
+/* acb_lm_admit for a model whose fuser prepends conditions (`prepend`, MusicGen-melody): prefix is the request's fp32
+ * [2][prefix_len][d] ([cond; null] rows), which fills cache positions [0, prefix_len) of the slot's two rows, after the
+ * cross K/V, in the prefill passes acb_lm_begin_prefix runs for a generation of batch 1 with CFG (ACB_LM_PREFILL_ROWS / 2
+ * positions per pass), so the K/V are the ones that generation writes.  The slot then runs column t at cache position
+ * prefix_len + t; its position (acb_lm_slot_status) still counts columns.  Every slot has its own prefix length.  Writes only
+ * the slot's cache rows, sequence row, mask, sampling record and state; the passes use the activation buffers and
+ * buffers.pos, which the session's step does not carry between steps, and leave the session's padded activation rows zero.
+ * Needs prefix_len >= 0, a prefix when prefix_len > 0 and prefix_len + seq_len <= max_seq (else ACB_ERR_INVALID, before
+ * anything is enqueued).  prefix_len == 0 is acb_lm_admit. */
+int acb_lm_admit_prefix(acb_lm_t* lm, int slot, const float* cross, int text_len, const float* prefix, int prefix_len,
+                        int seq_len, uint64_t seed, const acb_lm_sampling* sampling, void* stream);
 
 /* Cancel the request in `slot` between steps: an ACTIVE or FINISHED slot becomes INACTIVE (status 0) and the next step skips
  * it, as it skips a slot never admitted; the slot is free for acb_lm_admit, which overwrites its K/V, mask and state.  One

@@ -20,6 +20,8 @@ ACB_LM_MAX_ROWS = 256
 ACB_LM_SLOT_STRIDE = 8
 ACB_LM_SLOT_SAMPLING_STRIDE = 8
 ACB_LM_MAX_SLOTS = 128
+ACB_LM_KV_PAGE = 64
+ACB_LM_MAX_PAGES_PER_ROW = 188
 
 
 class LMConfig(C.Structure):
@@ -98,6 +100,8 @@ def lib():
     L.acb_lm_admit.argtypes = [vp, ci, vp, ci, ci, C.c_uint64, C.POINTER(LMSampling), vp]
     L.acb_lm_admit_prefix.argtypes = [vp, ci, vp, ci, vp, ci, ci, C.c_uint64, C.POINTER(LMSampling), vp]
     L.acb_lm_retire.argtypes = [vp, ci, vp]
+    L.acb_lm_begin_slots_paged.argtypes = [vp, ci, ci, ci, ci, vp, vp, ci, vp, ci, vp, vp, C.POINTER(LMSampling), vp]
+    L.acb_lm_admit_paged.argtypes = [vp, ci, vp, ci, vp, ci, ci, C.c_uint64, C.POINTER(LMSampling), vp, ci, vp]
     L.acb_lm_slot_status.argtypes = [vp, vp, vp]
     L.acb_lm_prefill.argtypes = [vp, ci, ci, vp]
     L.acb_lm_step_logits.argtypes = [vp, vp, vp]
@@ -120,7 +124,7 @@ def lib():
                  'acb_conv1d_t6', 'acb_conv1d_t6_tile', 'acb_lm_prefill',
                  'acb_resblock', 'acb_resblock_supported', 'acb_lm_forward', 'acb_t5_encode', 'acb_groupnorm_stats',
                  'acb_groupnorm_apply', 'acb_overlap_add', 'acb_lm_begin_slots', 'acb_lm_admit', 'acb_lm_slot_status', 'acb_lm_retire',
-                 'acb_lm_admit_prefix'):
+                 'acb_lm_admit_prefix', 'acb_lm_begin_slots_paged', 'acb_lm_admit_paged'):
         getattr(L, name).restype = ci
     _lib = L
     return L
@@ -134,7 +138,7 @@ EXPORTS = ['acb_version', 'acb_last_error', 'acb_device_sm_count', 'acb_weight_n
            'acb_lm_prefill', 'acb_resblock', 'acb_resblock_supported', 'acb_lm_forward_workspace_bytes', 'acb_lm_forward',
            'acb_t5_workspace_bytes', 'acb_t5_encode', 'acb_groupnorm_workspace_bytes', 'acb_groupnorm_stats',
            'acb_groupnorm_apply', 'acb_overlap_add', 'acb_lstm_recurrent_carry', 'acb_lm_begin_slots', 'acb_lm_admit',
-           'acb_lm_slot_status', 'acb_lm_retire', 'acb_lm_admit_prefix']
+           'acb_lm_slot_status', 'acb_lm_retire', 'acb_lm_admit_prefix', 'acb_lm_begin_slots_paged', 'acb_lm_admit_paged']
 
 
 def check(rc: int, what: str = ''):

@@ -18,11 +18,18 @@ released layout, description positions, whose length P differs from request to r
 slot's own cache rows (acb_lm_admit_prefix), in the passes `generate` runs for that request alone, and the slot then runs
 column t at cache position P + t.  A session is sized for `max_prefix` prefix positions.
 
+With a KV budget (`SlotSession(kv_pages=N)`, `continuous(kv_cache_gb=...)`) the session's self-attention cache is a pool of
+pages of ACB_LM_KV_PAGE positions (acb_lm_begin_slots_paged) instead of `slots` rows of the longest length: a request holds
+2 * ceil((P + S) / ACB_LM_KV_PAGE) pages (its cond and null rows) from admission until it finishes or is cancelled, so
+the number of requests decoding at once follows their lengths.  A request computes exactly what it computes in a
+contiguous session; only the addresses of its keys and values differ.
+
 Each request has its own sampling options (use_sampling, temperature, top-k, top-p, CFG coefficient): admission writes them to
 the slot's record on the device, which the captured step reads, so requests with different options share one session.  A
 request can be cancelled between steps (acb_lm_retire), which frees its slot for the next admission.
 
-`ContinuousScheduler` is the host-side policy (FIFO admission, retirement, cancellation) over any object with the device
+`ContinuousScheduler` is the host-side policy (FIFO admission, head-of-line waiting for pages, retirement, cancellation)
+over any object with the device
 session's methods, so it is tested without a GPU.  `CohortStream` turns a session's progress into audio pieces while the
 requests decode; `ContinuousGenerator` (``BaseGenModel.continuous``) is the public entry point.
 """
@@ -89,6 +96,56 @@ def prefix_bound(lm, max_text: int) -> int:
     return chroma.chroma_len + (max_text if 'description' in lm.fuser.fuse2cond.get('prepend', []) else 0)
 
 
+def kv_page_bytes(lm) -> int:
+    """Bytes of one page of a paged session's pool: ACB_LM_KV_PAGE positions of fp16 K and V in every layer."""
+    return _lib.ACB_LM_KV_PAGE * 2 * lm.num_layers * lm.dim * 2
+
+
+def kv_pages_for_budget(lm, kv_cache_gb: float) -> int:
+    """The pages a budget of kv_cache_gb * 1e9 bytes holds: floor(kv_cache_gb * 1e9 / kv_page_bytes(lm))."""
+    if isinstance(kv_cache_gb, bool) or not isinstance(kv_cache_gb, (int, float)) or not (
+            math.isfinite(kv_cache_gb) and kv_cache_gb > 0):
+        raise ValueError(f"kv_cache_gb must be a finite number > 0, got {kv_cache_gb!r}")
+    return int(math.floor(kv_cache_gb * 1e9 / kv_page_bytes(lm)))
+
+
+class PagePool:
+    """Host bookkeeping of a paged session's KV pages: the free page ids and the pages each live slot holds.  A request of
+    `positions` = P + S cache positions takes `need(positions)` = 2 * ceil(positions / ACB_LM_KV_PAGE) pages, its cond row's
+    then its null row's."""
+
+    def __init__(self, n_pages: int):
+        self.n_pages = n_pages
+        self.free = list(range(n_pages - 1, -1, -1))   # pop() hands out the lowest ids first
+        self.held: tp.Dict[int, tp.List[int]] = {}
+        self.peak = 0
+
+    @staticmethod
+    def need(positions: int) -> int:
+        return 2 * -(-positions // _lib.ACB_LM_KV_PAGE)
+
+    def fits(self, positions: int) -> bool:
+        return self.need(positions) <= len(self.free)
+
+    @property
+    def in_use(self) -> int:
+        return self.n_pages - len(self.free)
+
+    def take(self, slot: int, positions: int) -> tp.List[int]:
+        if slot in self.held:
+            raise RuntimeError(f"slot {slot} still holds pages")
+        n = self.need(positions)
+        if n > len(self.free):
+            raise RuntimeError(f"{positions} positions need {n} pages; {len(self.free)} are free")
+        ids = [self.free.pop() for _ in range(n)]
+        self.held[slot] = ids
+        self.peak = max(self.peak, self.in_use)
+        return ids
+
+    def release(self, slot: int):
+        self.free.extend(reversed(self.held.pop(slot, [])))
+
+
 def pattern_sequence(lm, prompt: tp.Optional[torch.Tensor], max_gen_len: int, device='cpu'):
     """The delay-pattern sequence [1, K, S] and mask [K, S] `LMModel._generate_begin` builds for one item: the prompt written
     in, -1 where a token is still unknown, the special token where the pattern has no step.  Also returns the pattern."""
@@ -124,11 +181,18 @@ class SlotSession:
     (slot s owns rows s and slots + s).  Holds the model's decode handle until another generation call takes it.
 
     On a model with a condition prefix every request carries one of at most `max_prefix` positions (None: `prefix_bound`),
-    and the KV cache holds max_prefix + the longest sequence."""
+    and the KV cache holds max_prefix + the longest sequence.
+
+    `kv_pages`: a paged session.  Its self-attention cache is a pool of `kv_pages` pages (`kv_page_bytes` each) instead of
+    2 * slots rows of max_prefix + the longest sequence, and `pages` (a `PagePool`) tracks which slot holds which pages:
+    admission takes a request's pages, `collect` and `retire` return them.  Refused (ValueError, before any device work)
+    when the pool cannot hold one request of the longest sequence with max_prefix.  Besides the pool the session allocates
+    the cross-attention K/V for 2 * slots x max_text positions, a staging cache of 2 x max_prefix positions for admitting a
+    prefix, and the activation and split-K buffers of 2 * slots rows."""
 
     def __init__(self, lm, slots: int, max_gen_len: int, max_text: int = 64, use_sampling: bool = True, temp: float = 1.0,
                  top_k: int = 250, top_p: float = 0.0, cfg_coef: tp.Optional[float] = None,
-                 max_prefix: tp.Optional[int] = None):
+                 max_prefix: tp.Optional[int] = None, kv_pages: tp.Optional[int] = None):
         if not 1 <= slots <= _lib.ACB_LM_MAX_SLOTS:
             raise ValueError(f"slots must be in [1, {_lib.ACB_LM_MAX_SLOTS}], got {slots}")
         if max_gen_len < 1 or max_text < 1:
@@ -142,14 +206,42 @@ class SlotSession:
         self.max_prefix = max_prefix
         seq, _, pattern = pattern_sequence(lm, None, max_gen_len)
         self.seq_len_max, self.delays = seq.shape[-1], list(pattern.delays)
+        self._seq_lens = {max_gen_len: self.seq_len_max}
         coef = lm.cfg_coef if cfg_coef is None else cfg_coef
         self.sampling = dict(use_sampling=bool(use_sampling), temp=float(temp), top_k=int(top_k), top_p=float(top_p),
                              cfg_coef=float(coef))
+        self.pages = None
+        if kv_pages is not None:
+            if isinstance(kv_pages, bool) or not isinstance(kv_pages, int):
+                raise ValueError(f"kv_pages must be an integer, got {kv_pages!r}")
+            longest = max_prefix + self.seq_len_max
+            if kv_pages < PagePool.need(longest):
+                raise ValueError(f"a pool of {kv_pages} KV pages cannot hold one request of {longest} positions "
+                                 f"({PagePool.need(longest)} pages of {_lib.ACB_LM_KV_PAGE} positions, cond and null rows)")
+            self.pages = PagePool(kv_pages)
         with torch.cuda.device(lm.device):
-            lm._ensure(2 * slots, max_prefix + self.seq_len_max, max_text if lm.cross_attention else 0, slots)
+            sizes = (2 * slots, max_prefix + self.seq_len_max, max_text if lm.cross_attention else 0, slots)
+            if self.pages is None:
+                lm._ensure(*sizes)
+            else:
+                lm._ensure(*sizes, paged=True)
             samp = _lib.LMSampling(int(bool(use_sampling)), float(temp), int(top_k), float(top_p), float(coef), 0, 0, 0.0)
-            _lib.check(lm._lib.acb_lm_begin_slots(lm._handle, slots, max_text, self.seq_len_max, C.byref(samp),
-                                                  _lib.stream()), 'lm_begin_slots')
+            if self.pages is None:
+                _lib.check(lm._lib.acb_lm_begin_slots(lm._handle, slots, max_text, self.seq_len_max, C.byref(samp),
+                                                      _lib.stream()), 'lm_begin_slots')
+            else:
+                L, H, page, f16 = lm.num_layers, lm.num_heads, _lib.ACB_LM_KV_PAGE, torch.float16
+                per_row = PagePool.need(max_prefix + self.seq_len_max) // 2
+                # never read before written: a slot reads only the positions it has appended or had scattered in
+                self.k_pool = torch.empty((L, kv_pages, H, page, 64), device=lm.device, dtype=f16)
+                self.v_pool = torch.empty((L, kv_pages, H, page, 64), device=lm.device, dtype=f16)
+                self.page_table = torch.zeros((2 * slots, per_row), device=lm.device, dtype=torch.int32)
+                self._stage = [torch.empty((L, 2, H, max_prefix, 64), device=lm.device, dtype=f16) if max_prefix else None
+                               for _ in range(2)]
+                _lib.check(lm._lib.acb_lm_begin_slots_paged(
+                    lm._handle, slots, max_text, self.seq_len_max, max_prefix, _lib.ptr(self.k_pool), _lib.ptr(self.v_pool),
+                    kv_pages, _lib.ptr(self.page_table), per_row, _lib.ptr(self._stage[0]), _lib.ptr(self._stage[1]),
+                    C.byref(samp), _lib.stream()), 'lm_begin_slots_paged')
             lm.launches_per_step = lm._lib.acb_lm_launches_per_step(lm._handle)
             lm._session = self
             self._status = torch.zeros((slots, 2), device=lm.device, dtype=torch.int32)
@@ -161,6 +253,13 @@ class SlotSession:
     @property
     def max_delay(self) -> int:
         return max(self.delays)
+
+    def positions(self, req: Request) -> int:
+        """Cache positions the request occupies in each of its two rows: its prefix and its delay-pattern sequence."""
+        n = req.max_gen_len
+        if n not in self._seq_lens:
+            self._seq_lens[n] = pattern_sequence(self.lm, None, n)[0].shape[-1]
+        return (0 if req.prefix is None else req.prefix.shape[1]) + self._seq_lens[n]
 
     def admit(self, slot: int, req: Request):
         """Write the request's sequence and mask rows, then its sampling options, cross K/V, condition prefix and slot state
@@ -205,8 +304,18 @@ class SlotSession:
                 if not 1 <= T <= self.max_text:
                     raise ValueError(f"condition of {T} text positions: the session holds 1 .. {self.max_text}")
             prefix = req.prefix.to(lm.device, torch.float32).contiguous() if P else None
-            _lib.check(lm._lib.acb_lm_admit_prefix(lm._handle, slot, _lib.ptr(cross), T, _lib.ptr(prefix), P, S,
-                                                   C.c_uint64(req.seed), samp, _lib.stream()), 'lm_admit')
+            if self.pages is None:
+                _lib.check(lm._lib.acb_lm_admit_prefix(lm._handle, slot, _lib.ptr(cross), T, _lib.ptr(prefix), P, S,
+                                                       C.c_uint64(req.seed), samp, _lib.stream()), 'lm_admit')
+            else:
+                ids = self.pages.take(slot, P + S)
+                try:
+                    _lib.check(lm._lib.acb_lm_admit_paged(lm._handle, slot, _lib.ptr(cross), T, _lib.ptr(prefix), P, S,
+                                                          C.c_uint64(req.seed), samp, (C.c_int32 * len(ids))(*ids), len(ids),
+                                                          _lib.stream()), 'lm_admit_paged')
+                except Exception:
+                    self.pages.release(slot)
+                    raise
             # `keep`: the stream reads cross and the prefix after this call
             req.meta.update(S=S, mask=mask, pattern=pattern, keep=(cross, prefix))
 
@@ -215,6 +324,8 @@ class SlotSession:
         self._check_owner()
         with torch.cuda.device(self.lm.device):
             _lib.check(self.lm._lib.acb_lm_retire(self.lm._handle, slot, _lib.stream()), 'lm_retire')
+        if self.pages is not None:
+            self.pages.release(slot)
 
     def frames(self, slots: tp.List[int], t0: int, t1: int) -> torch.Tensor:
         """Codes [len(slots), K, t1 - t0] of frames [t0, t1) of the given slots, read from their delay-pattern sequences (frame t
@@ -248,10 +359,12 @@ class SlotSession:
             return [tuple(r) for r in self._status.cpu().tolist()]
 
     def collect(self, slot: int, req: Request) -> torch.Tensor:
-        """The finished request's codes [1, K, max_gen_len], prompt included."""
+        """The finished request's codes [1, K, max_gen_len], prompt included.  Returns its pages to a paged session's pool."""
         lm, m = self.lm, req.meta
         with torch.cuda.device(lm.device):
             seq = lm._bufs['seq'][slot:slot + 1, :, :m['S']].clone()
+            if self.pages is not None:
+                self.pages.release(slot)
             return revert_sequence(lm, seq, m['mask'], m['pattern'], req.max_gen_len)
 
 
@@ -260,7 +373,12 @@ class ContinuousScheduler:
     `collect(slot, req)`, and `retire(slot)` for cancellation).  Every active slot advances one column per step, so the host
     knows when each one finishes: a poll admits waiting requests into free slots, runs steps up to the next retirement (at
     most `poll_steps`), checks the device status once, and returns the finished requests with their codes.  `last_admitted`
-    holds the (slot, request) pairs the last poll admitted."""
+    holds the (slot, request) pairs the last poll admitted.
+
+    On a paged session (one whose `pages` is a `PagePool`; `positions(req)` gives a request's length) the head of the queue is
+    admitted only when a slot and its pages are free; while its pages are not, it waits and no later request overtakes it,
+    so a long request is never starved by shorter ones.  `page_wait_steps` counts the steps run while the head waited for
+    pages with a slot free, `page_steps` the pages in use summed over steps (mean: page_steps / steps_run)."""
 
     def __init__(self, session, slots: int, poll_steps: tp.Optional[int] = None):
         if poll_steps is not None and poll_steps < 1:
@@ -271,6 +389,8 @@ class ContinuousScheduler:
         self.pos: tp.Dict[int, int] = {}
         self.steps_run = 0
         self.busy_slot_steps = 0     # sum over steps of the active slots: occupancy = busy_slot_steps / (steps_run * slots)
+        self.page_wait_steps = 0
+        self.page_steps = 0
         self.last_admitted: tp.List[tp.Tuple[int, Request]] = []
 
     def submit(self, req: Request):
@@ -300,10 +420,15 @@ class ContinuousScheduler:
 
     def poll(self) -> tp.List[tp.Tuple[Request, torch.Tensor]]:
         self.last_admitted = []
+        pool = getattr(self.session, 'pages', None)
+        waits = False
         for slot in range(self.slots):
             if not self.waiting:
                 break
             if slot not in self.active:
+                if pool is not None and not pool.fits(self.session.positions(self.waiting[0])):
+                    waits = True
+                    break
                 req = self.waiting.popleft()
                 self.session.admit(slot, req)
                 self.active[slot] = req
@@ -317,6 +442,9 @@ class ContinuousScheduler:
         self.session.steps(n)
         self.steps_run += n
         self.busy_slot_steps += n * len(self.active)
+        if pool is not None:
+            self.page_steps += n * pool.in_use
+            self.page_wait_steps += n if waits else 0
         status = self.session.status()
         done = []
         for slot in sorted(self.active):
@@ -448,13 +576,20 @@ class ContinuousGenerator:
     requests admitted in one round share one stream decoder.  Refused before any device work: a codec without a stream
     decoder (NotImplementedError) and chunk_duration <= 0 (ValueError).
 
+    With `kv_cache_gb`, the session is paged (`SlotSession(kv_pages=...)`): its self-attention KV cache is a pool of
+    floor(kv_cache_gb * 1e9 / kv_page_bytes) pages, each request holds only the pages its own length needs, and a request
+    waits in FIFO order until a slot and its pages are free.  Refused before any device work: kv_cache_gb <= 0, and a budget
+    that cannot hold one request of max_duration (ValueError).  Results are those of the session without kv_cache_gb.
+
     Refused before any device work: durations beyond max_duration, two_step_cfg and cfg_coef_beta (NotImplementedError), a
     melody on a model without a melody conditioner (NotImplementedError), a melody together with a prompt, and a description
     longer than max_text text positions (ValueError)."""
 
     def __init__(self, model, slots: int = 32, poll_steps: tp.Optional[int] = None, max_text: int = 64,
-                 return_tokens: bool = False, chunk_duration: tp.Optional[float] = None):
+                 return_tokens: bool = False, chunk_duration: tp.Optional[float] = None,
+                 kv_cache_gb: tp.Optional[float] = None):
         params = dict(model.generation_params)
+        kv_pages = None if kv_cache_gb is None else kv_pages_for_budget(model.lm, kv_cache_gb)
         if getattr(model, '_has_melody', False) != model.lm.has_prefix:
             raise NotImplementedError("continuous batching takes a melody ('self_wav') conditioner only as a condition prefix "
                                       "(prepend fuser), and a condition prefix only from one")
@@ -474,7 +609,7 @@ class ContinuousGenerator:
         self.defaults = dict(use_sampling=params['use_sampling'], temp=params['temp'], top_k=params['top_k'],
                              top_p=params['top_p'], cfg_coef=params['cfg_coef'])
         max_gen_len = int(model.max_duration * model.frame_rate)
-        self.session = SlotSession(model.lm, slots, max_gen_len, max_text, **self.defaults)
+        self.session = SlotSession(model.lm, slots, max_gen_len, max_text, **self.defaults, kv_pages=kv_pages)
         self.scheduler = ContinuousScheduler(self.session, slots, poll_steps)
         self.stream = None
         if chunk_duration is not None:

@@ -24,6 +24,7 @@
 #include <cooperative_groups.h>
 #include <math.h>
 #include <new>
+#include <vector>
 #include <stdio.h>
 #include <stdlib.h>
 
@@ -459,13 +460,18 @@ __global__ void __launch_bounds__(128, 1) lm_gemm_wide_kernel(const __grid_const
 // EPI_QKV / EPI_QKV_ROPE) into qkv [rows][3d], and this kernel does what those epilogues do at each row's own position: q to
 // q32 (fp32), k and v to the cache (fp16), q and k rotated first under rotary positions.  Only ACTIVE slots append to the cache.
 // The position is the cache position: the slot's prefix length + its column.
-__global__ void __launch_bounds__(256) lm_qkv_slot_kernel(const float* __restrict__ qkv, const int* __restrict__ slot_state,
-                                                          float* __restrict__ q32, __half* __restrict__ kc, __half* __restrict__ vc,
-                                                          int d, int H, int cache_len, int slots, const float* __restrict__ rope_freq,
-                                                          float pos_scale, bool rope) {
+// PAGED (acb_lm_begin_slots_paged): kc / vc are the layer's page pool [n_pages][H][ACB_LM_KV_PAGE][64], and position pos of
+// row r is offset pos % ACB_LM_KV_PAGE of page table[r][pos / ACB_LM_KV_PAGE]; the values written are the same.
+template <bool PAGED>
+__device__ __forceinline__ void qkv_slot_body(const float* __restrict__ qkv, const int* __restrict__ slot_state,
+                                              float* __restrict__ q32, __half* __restrict__ kc, __half* __restrict__ vc, int d,
+                                              int H, int cache_len, int slots, const float* __restrict__ rope_freq, float pos_scale,
+                                              bool rope, const int* __restrict__ table, int pages_per_row) {
     const int row = blockIdx.x, s = row % slots;
     const int pos = slot_state[s * ACB_LM_SLOT_STRIDE + ACB_SLOT_PREFIX] + slot_state[s * ACB_LM_SLOT_STRIDE + ACB_SLOT_POS];
     const bool live = slot_state[s * ACB_LM_SLOT_STRIDE + ACB_SLOT_STATUS] == SLOT_ACTIVE;
+    int page = 0;
+    if constexpr (PAGED) page = live ? table[row * pages_per_row + pos / ACB_LM_KV_PAGE] : 0;   // a slot not decoding owns no page
     const float* src = qkv + (size_t)row * 3 * d;
     for (int n = threadIdx.x; n < 3 * d; n += 256) {
         const int which = n >= 2 * d ? 2 : (n >= d ? 1 : 0), nn = n - which * d;
@@ -475,9 +481,27 @@ __global__ void __launch_bounds__(256) lm_qkv_slot_kernel(const float* __restric
             q32[(size_t)row * d + nn] = v;
         } else if (live) {
             __half* cache = which == 2 ? vc : kc;
-            cache[(((size_t)row * H + (nn >> 6)) * cache_len + pos) * 64 + (nn & 63)] = __float2half_rn(v);
+            if constexpr (PAGED)
+                cache[(((size_t)page * H + (nn >> 6)) * ACB_LM_KV_PAGE + pos % ACB_LM_KV_PAGE) * 64 + (nn & 63)] = __float2half_rn(v);
+            else
+                cache[(((size_t)row * H + (nn >> 6)) * cache_len + pos) * 64 + (nn & 63)] = __float2half_rn(v);
         }
     }
+}
+
+__global__ void __launch_bounds__(256) lm_qkv_slot_kernel(const float* __restrict__ qkv, const int* __restrict__ slot_state,
+                                                          float* __restrict__ q32, __half* __restrict__ kc, __half* __restrict__ vc,
+                                                          int d, int H, int cache_len, int slots, const float* __restrict__ rope_freq,
+                                                          float pos_scale, bool rope) {
+    qkv_slot_body<false>(qkv, slot_state, q32, kc, vc, d, H, cache_len, slots, rope_freq, pos_scale, rope, nullptr, 0);
+}
+
+__global__ void __launch_bounds__(256) lm_qkv_slot_paged_kernel(const float* __restrict__ qkv, const int* __restrict__ slot_state,
+                                                                float* __restrict__ q32, __half* __restrict__ kc,
+                                                                __half* __restrict__ vc, int d, int H, int slots,
+                                                                const float* __restrict__ rope_freq, float pos_scale, bool rope,
+                                                                const int* __restrict__ table, int pages_per_row) {
+    qkv_slot_body<true>(qkv, slot_state, q32, kc, vc, d, H, 0, slots, rope_freq, pos_scale, rope, table, pages_per_row);
 }
 
 // ------------------------------------------------------------------------------------------------ attention (1 query)
@@ -648,6 +672,128 @@ __global__ void __launch_bounds__(ATT_WARPS * 32) lm_attn2_slot_kernel(AttnParam
                 const uint32_t d = ring + (uint32_t)((k % ATT2_DEPTH) * 1024);
                 asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d), "l"(kb + (size_t)pp * 64) : "memory");
                 asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d + 512u), "l"(vb + (size_t)pp * 64) : "memory");
+            }
+        }
+        asm volatile("cp.async.commit_group;" ::: "memory");
+    };
+#pragma unroll
+    for (int k = 0; k < ATT2_DEPTH - 1; ++k) issue(k);
+
+    float q[8];
+    {
+        const float4* qp = reinterpret_cast<const float4*>(p.q + (size_t)qrow * p.d + h * 64 + sl * 8);
+        const float4 qa = qp[0], qb = qp[1];
+        q[0] = half_round(qa.x) * p.scale; q[1] = half_round(qa.y) * p.scale; q[2] = half_round(qa.z) * p.scale;
+        q[3] = half_round(qa.w) * p.scale; q[4] = half_round(qb.x) * p.scale; q[5] = half_round(qb.y) * p.scale;
+        q[6] = half_round(qb.z) * p.scale; q[7] = half_round(qb.w) * p.scale;
+    }
+    OnlineSM st;
+    st.m = -INFINITY; st.l = 0.f;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) st.acc[e] = 0.f;
+
+    for (int k = 0; k < n_it; ++k) {                 // warp-uniform trip count (the shuffles need all 32 lanes)
+        issue(k + ATT2_DEPTH - 1);
+        asm volatile("cp.async.wait_group %0;" ::"n"(ATT2_DEPTH - 1) : "memory");   // iteration k's copies of this lane have landed
+        const int pp = (k * ATT_WARPS + warp) * 4 + pg;
+        const uint32_t sa = ring + (uint32_t)((k % ATT2_DEPTH) * 1024);
+        uint4 kv = make_uint4(0, 0, 0, 0), vv = make_uint4(0, 0, 0, 0);
+        if (pp < n) {
+            asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(kv.x), "=r"(kv.y), "=r"(kv.z), "=r"(kv.w) : "r"(sa));
+            asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(vv.x), "=r"(vv.y), "=r"(vv.z), "=r"(vv.w) : "r"(sa + 512u));
+        }
+        const __half2* k2 = reinterpret_cast<const __half2*>(&kv);
+        float s = 0.f;
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            const float2 f = __half22float2(k2[e]);
+            s = fmaf(q[2 * e], f.x, s);
+            s = fmaf(q[2 * e + 1], f.y, s);
+        }
+        s += __shfl_xor_sync(0xffffffffu, s, 1);
+        s += __shfl_xor_sync(0xffffffffu, s, 2);
+        s += __shfl_xor_sync(0xffffffffu, s, 4);
+        if (pp < n) {
+            const float mn = fmaxf(st.m, s);
+            const float corr = __expf(st.m - mn);   // exp(-inf) = 0 on the first position
+            const float pw = __expf(s - mn);
+            st.l = st.l * corr + pw;
+            const __half2* v2 = reinterpret_cast<const __half2*>(&vv);
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const float2 f = __half22float2(v2[e]);
+                st.acc[2 * e] = fmaf(pw, f.x, st.acc[2 * e] * corr);
+                st.acc[2 * e + 1] = fmaf(pw, f.y, st.acc[2 * e + 1] * corr);
+            }
+            st.m = mn;
+        }
+    }
+    asm volatile("cp.async.wait_group 0;" ::: "memory");
+    // merge the 4 position groups of the warp, then the warps
+#pragma unroll
+    for (int o = 8; o <= 16; o <<= 1) {
+        const float m2 = __shfl_xor_sync(0xffffffffu, st.m, o), l2 = __shfl_xor_sync(0xffffffffu, st.l, o);
+        float a2[8];
+#pragma unroll
+        for (int e = 0; e < 8; ++e) a2[e] = __shfl_xor_sync(0xffffffffu, st.acc[e], o);
+        osm_merge(st, m2, l2, a2);
+    }
+    if (pg == 0) {
+        if (sl == 0) { wm[warp] = st.m; wl[warp] = st.l; }
+#pragma unroll
+        for (int e = 0; e < 8; ++e) wacc[warp][sl * 8 + e] = st.acc[e];
+    }
+    __syncthreads();
+    if (tid < 64) {
+        float mx = wm[0];
+#pragma unroll
+        for (int w = 1; w < ATT_WARPS; ++w) mx = fmaxf(mx, wm[w]);
+        float l = 0.f, o = 0.f;
+#pragma unroll
+        for (int w = 0; w < ATT_WARPS; ++w) {
+            const float cw = wm[w] == -INFINITY ? 0.f : __expf(wm[w] - mx);
+            l = fmaf(wl[w], cw, l);
+            o = fmaf(wacc[w][tid], cw, o);
+        }
+        p.out[(size_t)qrow * p.d + h * 64 + tid] = __float2half_rn(o / l);
+    }
+}
+
+// Paged session (acb_lm_begin_slots_paged): lm_attn2_slot_kernel with p.kc / p.vc the layer's page pool; the row's page table (at most ACB_LM_MAX_PAGES_PER_ROW entries) is staged in
+// shared memory and position pp is read from offset pp % ACB_LM_KV_PAGE of page pt[pp / ACB_LM_KV_PAGE].  A page holds a
+// multiple of the 4-position groups, so one lane's 16-byte copy never crosses a page; the arithmetic and its order are the
+// contiguous kernel's.
+// (a separate copy: the contiguous kernel stays as it is)
+__global__ void __launch_bounds__(ATT_WARPS * 32) lm_attn2_slot_paged_kernel(AttnParams p, const int* __restrict__ slot_state,
+                                                                          const int* __restrict__ table, int pages_per_row) {
+    extern __shared__ __align__(16) unsigned char att2sm[];   // [warp][depth][K | V][32 lanes][16 B]
+    __shared__ float wm[ATT_WARPS], wl[ATT_WARPS], wacc[ATT_WARPS][64];
+    const int h = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int qrow = blockIdx.y, row = qrow;
+    const int sl = lane & 7, pg = lane >> 3;
+    const int* slot = slot_state + (row % p.rows_real) * ACB_LM_SLOT_STRIDE;
+    if (slot[ACB_SLOT_STATUS] != SLOT_ACTIVE) {   // block-uniform
+        if (tid < 64) p.out[(size_t)qrow * p.d + h * 64 + tid] = __float2half_rn(0.f);
+        return;
+    }
+    const int n = slot[ACB_SLOT_PREFIX] + slot[ACB_SLOT_POS] + 1;
+    __shared__ int pt[ACB_LM_MAX_PAGES_PER_ROW];
+    for (int i = tid; i < (n + ACB_LM_KV_PAGE - 1) / ACB_LM_KV_PAGE; i += ATT_WARPS * 32) pt[i] = table[row * pages_per_row + i];
+    __syncthreads();
+    const size_t base = (size_t)h * ACB_LM_KV_PAGE * 64 + sl * 8;   // position pp: + (pt[pp / page] * H * page + pp % page) * 64
+    const __half* kb = p.kc + base;
+    const __half* vb = p.vc + base;
+    const uint32_t ring = smem_u32(att2sm) + (uint32_t)(warp * ATT2_DEPTH * 1024 + lane * 16);
+    // iteration k of this warp covers positions (k * 8 + warp) * 4 + pg
+    const int n_it = (n + 31 - warp * 4) / 32 > 0 ? (n - warp * 4 + 31) / 32 : 0;   // iterations with at least one live position group
+    auto issue = [&](int k) {
+        if (k < n_it) {
+            const int pp = (k * ATT_WARPS + warp) * 4 + pg;
+            if (pp < n) {
+                const uint32_t d = ring + (uint32_t)((k % ATT2_DEPTH) * 1024);
+                const size_t o = ((size_t)pt[pp / ACB_LM_KV_PAGE] * p.H * ACB_LM_KV_PAGE + pp % ACB_LM_KV_PAGE) * 64;
+                asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d), "l"(kb + o) : "memory");
+                asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d + 512u), "l"(vb + o) : "memory");
             }
         }
         asm volatile("cp.async.commit_group;" ::: "memory");
@@ -1087,6 +1233,35 @@ __global__ void lm_slot_admit_kernel(int* slot_state, int slot, int seq_len, int
     st[ACB_SLOT_DONE] = 0;
 }
 
+// Paged session admission: the slot's two page-table rows (cond row r0, null row r1), n page ids each, passed by value.
+struct PageList { int ids[2 * ACB_LM_MAX_PAGES_PER_ROW]; };
+__global__ void lm_page_table_kernel(int* table, int pages_per_row, int r0, int r1, int n, PageList pl) {
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        table[r0 * pages_per_row + i] = pl.ids[i];
+        table[r1 * pages_per_row + i] = pl.ids[n + i];
+    }
+}
+
+// Paged session admission of a condition prefix: positions [0, P) of the staging cache [L][2][H][max_prefix][64] (its row 0 is
+// the slot's cond row r0, row 1 its null row r1) copied into the rows' pages, 16 bytes per thread.
+__global__ void lm_prefix_scatter_kernel(const __half* __restrict__ sk, const __half* __restrict__ sv, __half* __restrict__ pk,
+                                         __half* __restrict__ pv, const int* __restrict__ table, int pages_per_row, int r0,
+                                         int r1, int H, int max_prefix, int P, size_t pool_layer, size_t total) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= total) return;
+    const int c = (int)(i % 8);
+    size_t t = i / 8;
+    const int pos = (int)(t % P); t /= P;
+    const int h = (int)(t % H); t /= H;
+    const int j = (int)(t % 2);
+    const size_t l = t / 2;
+    const size_t src = (((l * 2 + j) * H + h) * max_prefix + pos) * 64 + c * 8;
+    const int page = table[(j ? r1 : r0) * pages_per_row + pos / ACB_LM_KV_PAGE];
+    const size_t dst = l * pool_layer + (((size_t)page * H + h) * ACB_LM_KV_PAGE + pos % ACB_LM_KV_PAGE) * 64 + c * 8;
+    *reinterpret_cast<uint4*>(pk + dst) = *reinterpret_cast<const uint4*>(sk + src);
+    *reinterpret_cast<uint4*>(pv + dst) = *reinterpret_cast<const uint4*>(sv + src);
+}
+
 __global__ void lm_f32_to_f16_kernel(const float* __restrict__ src, __half* __restrict__ dst, size_t n_valid, size_t n_total) {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n_total) dst[i] = __float2half_rn(i < n_valid ? src[i] : 0.f);
@@ -1110,6 +1285,14 @@ struct acb_lm {
     int pf_slot = -1, pf_text_len = 0;
     int launches = 0;
     bool has_cross = false;
+    // paged handle (created with buffers.k_cache == NULL): the session's self-attention cache is the page pool of
+    // acb_lm_begin_slots_paged, [L][n_pages][H][ACB_LM_KV_PAGE][64], and an admission's prefix passes run into the staging
+    // cache [L][2][H][max_prefix][64] of the slot's two rows
+    bool paged = false;
+    __half* pool_k = nullptr; __half* pool_v = nullptr;
+    int n_pages = 0, pages_per_row = 0, max_prefix = 0;
+    int* page_table = nullptr;
+    __half* stage_k = nullptr; __half* stage_v = nullptr;
     // wide GEMM (max_rows > 64): one map per stacked weight matrix [L * N][K] (encoded by acb_lm_create) and per activation
     // buffer [rows][K] of the current generation (encoded by acb_lm_begin_prefix)
     CUtensorMap wmap[7];
@@ -1303,9 +1486,16 @@ static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_la
     // rows > 64 (then rows_real > 64 and a prefill pass holds one position per row): every GEMM but EPI_CROSSKV on the wide kernel
     const bool wide = rows > 64;
     const size_t part_stride = (size_t)(pf && !wide ? 8 * nt : lm->rows_pad) * d;
-    const size_t kv_layer = (size_t)c.max_rows * H * c.max_seq * 64;
+    // self-attention cache: a paged session's step reads and appends through the page table (kv_layer: one layer of the
+    // pool), its admission's prefix passes run into the staging cache of the slot's two rows (rows 0 and 1)
+    const bool stage = pf && lm->paged;
+    const int kv_len = stage ? lm->max_prefix : c.max_seq, kv_stride = stage ? 1 : row_stride;
+    __half* const kv_k = stage ? lm->stage_k : (lm->paged ? lm->pool_k : (__half*)B.k_cache);
+    __half* const kv_v = stage ? lm->stage_v : (lm->paged ? lm->pool_v : (__half*)B.v_cache);
+    const size_t kv_layer = stage ? (size_t)2 * H * lm->max_prefix * 64
+                          : (lm->paged ? (size_t)lm->n_pages * H * ACB_LM_KV_PAGE * 64 : (size_t)c.max_rows * H * c.max_seq * 64);
     const size_t ckv_layer = (size_t)c.max_rows * H * c.max_text * 64;
-    const size_t kv_row0 = (size_t)row0 * H * c.max_seq * 64, ckv_row0 = (size_t)row0 * H * c.max_text * 64;
+    const size_t kv_row0 = lm->paged ? 0 : (size_t)row0 * H * c.max_seq * 64, ckv_row0 = (size_t)row0 * H * c.max_text * 64;
     const float scale = 1.0f / sqrtf(64.f);
     int nl = 0, ks = 0;
 
@@ -1351,8 +1541,8 @@ static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_la
         {
             const int ns = wide ? pick_split_wide(3 * d, d, lm->sms, false, &ks) : pick_split(3 * d, d, lm->sms, false, &ks);
             GemmParams p = base_gemm((const __half*)lm->w.w_qkv + (size_t)l * 3 * d * d, B.h16, 3 * d, d, rows, ks);
-            p.q32 = B.q32; p.kc = (__half*)B.k_cache + l * kv_layer + kv_row0; p.vc = (__half*)B.v_cache + l * kv_layer + kv_row0;
-            p.d = d; p.H = H; p.cache_len = c.max_seq; p.pos = B.pos; p.rows_real = rows_real; p.row_stride = row_stride;
+            p.q32 = B.q32; p.kc = kv_k + l * kv_layer + kv_row0; p.vc = kv_v + l * kv_layer + kv_row0;
+            p.d = d; p.H = H; p.cache_len = kv_len; p.pos = B.pos; p.rows_real = rows_real; p.row_stride = kv_stride;
             p.rope_freq = lm->w.rope_freq; p.pos_scale = c.pos_scale;
             const bool rope = c.positional_embedding != 0;
             const int ft2 = pf ? 1 : pick_ft2(3 * d, d, 1, ks, nt, lm->sms);
@@ -1363,7 +1553,14 @@ static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_la
                 else ACB_TRY(launch_gemm<EPI_F32>(nt, p, 1, s, ft2));
                 ++nl;
                 DBG("gemm_EPI_F32 (qkv)", l);
-                if (!gemms_only) {
+                if (!gemms_only && lm->paged) {
+                    lm_qkv_slot_paged_kernel<<<rows, 256, 0, s>>>(B.part, B.slot_state, B.q32, p.kc, p.vc, d, H, lm->slots,
+                                                                  lm->w.rope_freq, c.pos_scale, rope, lm->page_table,
+                                                                  lm->pages_per_row);
+                    ACB_LAUNCH_CHECK();
+                    ++nl;
+                    DBG("lm_qkv_slot_paged_kernel", l);
+                } else if (!gemms_only) {
                     lm_qkv_slot_kernel<<<rows, 256, 0, s>>>(B.part, B.slot_state, B.q32, p.kc, p.vc, d, H, c.max_seq, lm->slots,
                                                             lm->w.rope_freq, c.pos_scale, rope);
                     ACB_LAUNCH_CHECK();
@@ -1380,9 +1577,13 @@ static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_la
             }
         }
         if (!gemms_only) {
-            AttnParams a{B.q32, 1, 0, (__half*)B.k_cache + l * kv_layer + kv_row0, (__half*)B.v_cache + l * kv_layer + kv_row0,
-                         (__half*)B.a16, H, d, c.max_seq, B.pos, 0, scale, rows_real, row_stride};
-            if (slot_step) { a.rows_real = lm->slots; lm_attn2_slot_kernel<<<dim3(H, rows), ATT_WARPS * 32, ATT2_SMEM, s>>>(a, B.slot_state); }
+            AttnParams a{B.q32, 1, 0, kv_k + l * kv_layer + kv_row0, kv_v + l * kv_layer + kv_row0,
+                         (__half*)B.a16, H, d, kv_len, B.pos, 0, scale, rows_real, kv_stride};
+            if (slot_step && lm->paged) {
+                a.rows_real = lm->slots;
+                lm_attn2_slot_paged_kernel<<<dim3(H, rows), ATT_WARPS * 32, ATT2_SMEM, s>>>(a, B.slot_state, lm->page_table,
+                                                                                          lm->pages_per_row);
+            } else if (slot_step) { a.rows_real = lm->slots; lm_attn2_slot_kernel<<<dim3(H, rows), ATT_WARPS * 32, ATT2_SMEM, s>>>(a, B.slot_state); }
             else if (pf) lm_attn2_kernel<true><<<dim3(H, rows), ATT_WARPS * 32, ATT2_SMEM, s>>>(a);
             else lm_attn2_kernel<false><<<dim3(H, rows), ATT_WARPS * 32, ATT2_SMEM, s>>>(a);
             ACB_LAUNCH_CHECK();
@@ -1478,6 +1679,7 @@ extern "C" int acb_lm_create(const acb_lm_config* cfg, const acb_lm_weights* w, 
     acb_lm* lm = new (std::nothrow) acb_lm();
     ACB_REQUIRE(lm, "acb_lm_create: out of host memory");
     lm->cfg = *cfg; lm->w = *w; lm->buf = *buf;
+    lm->paged = !buf->k_cache && !buf->v_cache;
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&lm->sms, cudaDevAttrMultiProcessorCount, dev);
@@ -1503,6 +1705,9 @@ extern "C" int acb_lm_create(const acb_lm_config* cfg, const acb_lm_weights* w, 
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_cross_attn_slot_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_embed_slot_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_qkv_slot_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+    if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_attn2_slot_paged_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT2_SMEM);
+    if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_attn2_slot_paged_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+    if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_qkv_slot_paged_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_sample_slot_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_cross_attn_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_ln_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
@@ -1615,6 +1820,7 @@ extern "C" int acb_lm_begin(acb_lm_t* lm, const float* cross, int batch, int row
 extern "C" int acb_lm_begin_prefix(acb_lm_t* lm, const float* cross, const float* prefix, int prefix_len, int batch, int rows,
                                    int text_len, int seq_len, const acb_lm_sampling* sampling, void* stream) {
     ACB_REQUIRE(lm && sampling, "acb_lm_begin: null argument");
+    ACB_REQUIRE(!lm->paged, "acb_lm_begin: the handle has no contiguous KV cache (buffers.k_cache is NULL: a paged handle)");
     const acb_lm_config& c = lm->cfg;
     ACB_REQUIRE(batch >= 1 && (rows == batch || rows == 2 * batch || rows == 3 * batch), "acb_lm_begin: rows must be batch, 2*batch (CFG) or 3*batch (double CFG)");
     ACB_REQUIRE(rows <= c.max_rows, "acb_lm_begin: rows %d > max_rows %d", rows, c.max_rows);
@@ -1684,6 +1890,7 @@ extern "C" int acb_lm_begin_prefix(acb_lm_t* lm, const float* cross, const float
 // pos = prefix_len + pos0 + n_tokens on the device.
 extern "C" int acb_lm_prefill(acb_lm_t* lm, int pos0, int n_tokens, void* stream) {
     ACB_REQUIRE(lm && lm->rows > 0, "acb_lm_prefill: call acb_lm_begin first");
+    ACB_REQUIRE(!lm->paged, "acb_lm_prefill: the handle has no contiguous KV cache (a paged handle)");
     ACB_REQUIRE(!lm->slots, "acb_lm_prefill: a slot session consumes prompts one column per step");
     ACB_REQUIRE(pos0 >= 0 && n_tokens >= 0 && pos0 + n_tokens < lm->seq_len, "acb_lm_prefill: positions [%d, %d) exceed the sequence (%d)",
                 pos0, pos0 + n_tokens, lm->seq_len);
@@ -1691,9 +1898,8 @@ extern "C" int acb_lm_prefill(acb_lm_t* lm, int pos0, int n_tokens, void* stream
 }
 
 // ------------------------------------------------------------------------------------------------ slot mode
-extern "C" int acb_lm_begin_slots(acb_lm_t* lm, int slots, int max_text, int seq_len_max, const acb_lm_sampling* sampling,
-                                  void* stream) {
-    ACB_REQUIRE(lm && sampling, "acb_lm_begin_slots: null argument");
+// The session set-up shared by acb_lm_begin_slots and acb_lm_begin_slots_paged (which sets the pool fields first).
+static int begin_slots(acb_lm_t* lm, int slots, int max_text, int seq_len_max, const acb_lm_sampling* sampling, void* stream) {
     const acb_lm_config& c = lm->cfg;
     ACB_REQUIRE(lm->buf.slot_sampling && lm->buf.slot_state && lm->buf.slot_mask,
                 "acb_lm_begin_slots: buffers.slot_sampling, slot_state and slot_mask are required");
@@ -1739,14 +1945,44 @@ extern "C" int acb_lm_begin_slots(acb_lm_t* lm, int slots, int max_text, int seq
     return capture_step(lm);
 }
 
+extern "C" int acb_lm_begin_slots(acb_lm_t* lm, int slots, int max_text, int seq_len_max, const acb_lm_sampling* sampling,
+                                  void* stream) {
+    ACB_REQUIRE(lm && sampling, "acb_lm_begin_slots: null argument");
+    ACB_REQUIRE(!lm->paged, "acb_lm_begin_slots: the handle has no contiguous KV cache (a paged handle: acb_lm_begin_slots_paged)");
+    return begin_slots(lm, slots, max_text, seq_len_max, sampling, stream);
+}
+
+extern "C" int acb_lm_begin_slots_paged(acb_lm_t* lm, int slots, int max_text, int seq_len_max, int max_prefix, void* k_pool,
+                                        void* v_pool, int n_pages, int32_t* page_table, int pages_per_row, void* stage_k,
+                                        void* stage_v, const acb_lm_sampling* sampling, void* stream) {
+    ACB_REQUIRE(lm && sampling && k_pool && v_pool && page_table, "acb_lm_begin_slots_paged: null argument");
+    ACB_REQUIRE(lm->paged, "acb_lm_begin_slots_paged: the handle was created with a contiguous KV cache (buffers.k_cache)");
+    const acb_lm_config& c = lm->cfg;
+    ACB_REQUIRE(max_prefix >= 0 && seq_len_max >= 2 && max_prefix + seq_len_max <= c.max_seq,
+                "acb_lm_begin_slots_paged: max_prefix %d + seq_len_max %d not in [2, max_seq %d]", max_prefix, seq_len_max, c.max_seq);
+    ACB_REQUIRE(max_prefix == 0 || (stage_k && stage_v), "acb_lm_begin_slots_paged: max_prefix > 0 needs the staging buffers");
+    const int need = acb_ceil_div(max_prefix + seq_len_max, ACB_LM_KV_PAGE);
+    ACB_REQUIRE(pages_per_row >= need && pages_per_row <= ACB_LM_MAX_PAGES_PER_ROW,
+                "acb_lm_begin_slots_paged: pages_per_row %d not in [%d, %d]", pages_per_row, need, ACB_LM_MAX_PAGES_PER_ROW);
+    ACB_REQUIRE(n_pages >= 2 * need, "acb_lm_begin_slots_paged: %d pages cannot hold one request of %d positions (%d pages)",
+                n_pages, max_prefix + seq_len_max, 2 * need);
+    lm->pool_k = (__half*)k_pool; lm->pool_v = (__half*)v_pool; lm->n_pages = n_pages;
+    lm->page_table = page_table; lm->pages_per_row = pages_per_row;
+    lm->stage_k = (__half*)stage_k; lm->stage_v = (__half*)stage_v; lm->max_prefix = max_prefix;
+    return begin_slots(lm, slots, max_text, seq_len_max, sampling, stream);
+}
+
 extern "C" int acb_lm_admit(acb_lm_t* lm, int slot, const float* cross, int text_len, int seq_len, uint64_t seed,
                             const acb_lm_sampling* sampling, void* stream) {
     return acb_lm_admit_prefix(lm, slot, cross, text_len, nullptr, 0, seq_len, seed, sampling, stream);
 }
 
-extern "C" int acb_lm_admit_prefix(acb_lm_t* lm, int slot, const float* cross, int text_len, const float* prefix, int prefix_len,
-                                   int seq_len, uint64_t seed, const acb_lm_sampling* sampling, void* stream) {
+// acb_lm_admit_prefix and acb_lm_admit_paged: pages is NULL in a contiguous session, n_page_ids its length otherwise.
+static int admit(acb_lm_t* lm, int slot, const float* cross, int text_len, const float* prefix, int prefix_len, int seq_len,
+                 uint64_t seed, const acb_lm_sampling* sampling, const int32_t* pages, int n_page_ids, void* stream) {
     ACB_REQUIRE(lm && lm->slots > 0, "acb_lm_admit: call acb_lm_begin_slots first");
+    ACB_REQUIRE(lm->paged == (pages != nullptr), "%s", lm->paged ? "acb_lm_admit: a paged session admits with acb_lm_admit_paged"
+                                                                 : "acb_lm_admit_paged: the session is not paged");
     const acb_lm_config& c = lm->cfg;
     ACB_REQUIRE(slot >= 0 && slot < lm->slots, "acb_lm_admit: slot %d not in [0, %d)", slot, lm->slots);
     ACB_REQUIRE(seq_len >= 2 && seq_len <= lm->seq_len, "acb_lm_admit: seq_len %d not in [2, %d]", seq_len, lm->seq_len);
@@ -1767,8 +2003,28 @@ extern "C" int acb_lm_admit_prefix(acb_lm_t* lm, int slot, const float* cross, i
                     "acb_lm_admit: needs 0 <= temp < inf (got %g), top_k >= 0 (got %d), 0 <= top_p <= 1 (got %g) and a finite "
                     "cfg_coef (got %g)", sampling->temp, sampling->top_k, sampling->top_p, sampling->cfg_coef);
     }
+    PageList pl;
+    const int ppr = lm->paged ? acb_ceil_div(prefix_len + seq_len, ACB_LM_KV_PAGE) : 0;
+    if (lm->paged) {   // every check before anything is enqueued
+        ACB_REQUIRE(prefix_len <= lm->max_prefix, "acb_lm_admit_paged: prefix_len %d > the session's max_prefix %d", prefix_len,
+                    lm->max_prefix);
+        ACB_REQUIRE(n_page_ids == 2 * ppr && ppr <= lm->pages_per_row, "acb_lm_admit_paged: %d page ids for %d positions: needs "
+                    "2 x %d", n_page_ids, prefix_len + seq_len, ppr);
+        std::vector<uint8_t> seen((size_t)lm->n_pages, 0);
+        for (int i = 0; i < n_page_ids; ++i) {
+            const int id = pages[i];
+            ACB_REQUIRE(id >= 0 && id < lm->n_pages, "acb_lm_admit_paged: page id %d not in [0, %d)", id, lm->n_pages);
+            ACB_REQUIRE(!seen[id], "acb_lm_admit_paged: page %d given twice", id);
+            seen[id] = 1;
+            pl.ids[i] = id;
+        }
+    }
     const acb_lm_sampling& sp = sampling ? *sampling : lm->samp;
     cudaStream_t s = (cudaStream_t)stream;
+    if (lm->paged) {
+        lm_page_table_kernel<<<1, 256, 0, s>>>(lm->page_table, lm->pages_per_row, slot, lm->slots + slot, ppr, pl);
+        ACB_LAUNCH_CHECK();
+    }
     if (lm->has_cross) {
         // cross K/V of the slot's cond row (slot) and null row (slots + slot), each staged and projected on its own: the
         // EPI_CROSSKV epilogue writes cache row R / text_len = 0 of the destination pointer
@@ -1803,6 +2059,13 @@ extern "C" int acb_lm_admit_prefix(acb_lm_t* lm, int slot, const float* cross, i
         lm->pf_slot = -1; lm->pf_text_len = 0;
         lm->prefix = nullptr; lm->prefix_len = 0;   // the session's step reads column = position (its sampler's seq_off is 0)
         ACB_TRY(rc);
+        if (lm->paged) {   // the passes ran into the staging cache: copy it into the slot's pages
+            const size_t total = (size_t)c.num_layers * 2 * c.num_heads * prefix_len * 8;
+            lm_prefix_scatter_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(
+                lm->stage_k, lm->stage_v, lm->pool_k, lm->pool_v, lm->page_table, lm->pages_per_row, slot, lm->slots + slot,
+                c.num_heads, lm->max_prefix, prefix_len, (size_t)lm->n_pages * c.num_heads * ACB_LM_KV_PAGE * 64, total);
+            ACB_LAUNCH_CHECK();
+        }
     }
     lm_slot_sampling_kernel<<<1, 1, 0, s>>>(lm->buf.slot_sampling, slot, sp.use_sampling, sp.temp, sp.top_k, sp.top_p,
                                             sp.cfg_coef);
@@ -1811,6 +2074,18 @@ extern "C" int acb_lm_admit_prefix(acb_lm_t* lm, int slot, const float* cross, i
                                          (uint32_t)seed, (uint32_t)(seed >> 32));
     ACB_LAUNCH_CHECK();
     return ACB_OK;
+}
+
+extern "C" int acb_lm_admit_prefix(acb_lm_t* lm, int slot, const float* cross, int text_len, const float* prefix, int prefix_len,
+                                   int seq_len, uint64_t seed, const acb_lm_sampling* sampling, void* stream) {
+    return admit(lm, slot, cross, text_len, prefix, prefix_len, seq_len, seed, sampling, nullptr, 0, stream);
+}
+
+extern "C" int acb_lm_admit_paged(acb_lm_t* lm, int slot, const float* cross, int text_len, const float* prefix, int prefix_len,
+                                  int seq_len, uint64_t seed, const acb_lm_sampling* sampling, const int32_t* pages, int n,
+                                  void* stream) {
+    ACB_REQUIRE(pages, "acb_lm_admit_paged: null page list");
+    return admit(lm, slot, cross, text_len, prefix, prefix_len, seq_len, seed, sampling, pages, n, stream);
 }
 
 extern "C" int acb_lm_retire(acb_lm_t* lm, int slot, void* stream) {

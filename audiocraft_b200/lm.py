@@ -144,8 +144,13 @@ class LMModel:
                                                               'w_co', 'w_ff1', 'w_ff2', 'ln', 'out_norm', 'heads', 'rope_freq')])
 
     # ------------------------------------------------------------------ device state
-    def _ensure(self, rows: int, seq_len: int, text_len: int, batch: int):
+    def _ensure(self, rows: int, seq_len: int, text_len: int, batch: int, paged: bool = False):
+        """A decode handle with buffers for at least these sizes.  `paged`: a handle for a paged slot session
+        (acb_lm_begin_slots_paged), which has no contiguous [L][rows][H][max_seq][64] KV cache (the session owns its page
+        pool).  A call for the other layout rebuilds the handle at its own sizes."""
         shape = self._shape
+        if shape is not None and shape[4] != paged:
+            shape = None
         if shape is not None and rows <= shape[0] and seq_len <= shape[1] and text_len <= shape[2] and batch <= shape[3]:
             return
         self._destroy()
@@ -170,8 +175,8 @@ class LMModel:
         b['q32'] = torch.zeros((rp, d), device=dev, dtype=f32)
         b['part'] = torch.zeros((_lib.ACB_LM_PART_SLOTS, rp, max(3 * d, self.ffn_dim, self.n_q * self.card)), device=dev, dtype=f32)
         b['logits'] = torch.zeros((rp, self.n_q * self.card), device=dev, dtype=f32)
-        b['k_cache'] = torch.zeros((L, max_rows, H, max_seq, 64), device=dev, dtype=f16)
-        b['v_cache'] = torch.zeros((L, max_rows, H, max_seq, 64), device=dev, dtype=f16)
+        b['k_cache'] = None if paged else torch.zeros((L, max_rows, H, max_seq, 64), device=dev, dtype=f16)
+        b['v_cache'] = None if paged else torch.zeros((L, max_rows, H, max_seq, 64), device=dev, dtype=f16)
         if self.cross_attention:
             b['ck_cache'] = torch.zeros((L, max_rows, H, max_text, 64), device=dev, dtype=f16)
             b['cv_cache'] = torch.zeros((L, max_rows, H, max_text, 64), device=dev, dtype=f16)
@@ -197,7 +202,7 @@ class LMModel:
         handle = C.c_void_p()
         _lib.check(self._lib.acb_lm_create(C.byref(cfg), C.byref(wts), C.byref(bufs), C.byref(handle)), 'lm_create')
         self._handle = handle
-        self._shape = (max_rows, max_seq, max_text, max_batch)
+        self._shape = (max_rows, max_seq, max_text, max_batch, paged)
 
     def _destroy(self):
         if self._handle is not None:

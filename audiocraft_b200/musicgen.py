@@ -214,7 +214,8 @@ class BaseGenModel:
 
     # -- continuous batching
     def continuous(self, slots: int = 32, poll_steps: tp.Optional[int] = None, max_text: int = 64,
-                   return_tokens: bool = False, chunk_duration: tp.Optional[float] = None):
+                   return_tokens: bool = False, chunk_duration: tp.Optional[float] = None,
+                   kv_cache_gb: tp.Optional[float] = None):
         """A `batching.ContinuousGenerator` over this model: up to `slots` requests decode side by side, each admitted when a
         slot frees and retired when its last frame is sampled.  `submit(description, duration, prompt, prompt_sample_rate,
         use_sampling=, top_k=, top_p=, temperature=, cfg_coef=)` returns a request id (options left out take the current
@@ -223,9 +224,17 @@ class BaseGenModel:
         round) they return `(request_id, piece[, tokens], final)` audio pieces while the requests decode.  `max_text` bounds a
         description's text positions.  On a melody model `submit(..., melody=, melody_sample_rate=)` conditions a request on
         its melody as `generate_with_chroma` does (no melody: a null one); each request's chroma and description prefix is
-        prefilled into its slot when it is admitted."""
+        prefilled into its slot when it is admitted.
+
+        `kv_cache_gb` (None: every slot reserves the KV cache of the longest request) is a budget in GB (1e9 bytes) for the
+        self-attention KV cache: a pool of floor(kv_cache_gb * 1e9 / page_bytes) pages of 64 positions, page_bytes = 64 x
+        4 x num_layers x dim bytes, from which each request takes only the pages its own length needs; a request waits until
+        a slot and its pages are free.  The budget covers that pool only.  The session also allocates the cross-attention
+        K/V for 2 x slots x max_text positions, a staging cache of 2 x (chroma + description) positions for admitting a
+        melody prefix, and the split-K partial sums (`part`, 16 x the padded rows x max(3 dim, ffn, n_q x card) fp32).  A
+        request's result is the same with or without a budget."""
         from .batching import ContinuousGenerator
-        return ContinuousGenerator(self, slots, poll_steps, max_text, return_tokens, chunk_duration)
+        return ContinuousGenerator(self, slots, poll_steps, max_text, return_tokens, chunk_duration, kv_cache_gb)
 
 
 def _sampling_params(use_sampling, top_k, top_p, temperature, cfg_coef, two_step_cfg):

@@ -208,7 +208,7 @@ typedef struct {
     float* q32;        /* [rows_pad][d]            self-attention queries */
     float* part;       /* [ACB_LM_PART_SLOTS][rows_pad][max(3d, ffn, n_q*card)]  split-K partial sums */
     float* logits;     /* [rows_pad][n_q*card] */
-    void* k_cache;     /* [L][max_rows][H][max_seq][64] fp16 */
+    void* k_cache;     /* [L][max_rows][H][max_seq][64] fp16; NULL (with v_cache) for a paged handle (acb_lm_begin_slots_paged) */
     void* v_cache;     /* same */
     void* ck_cache;    /* [L][max_rows][H][max_text][64] fp16  cross-attention keys (computed once per generate) */
     void* cv_cache;    /* same, values */
@@ -233,6 +233,9 @@ typedef struct {
 #define ACB_LM_PREFILL_ROWS 64   /* (token, row) pairs one prefill pass handles = the tallest GEMM tile; above 64 rows a pass
                                     holds one position of every row */
 #define ACB_LM_MAX_ROWS 256      /* rows one handle decodes: the widest wgmma tile (N = 256) */
+#define ACB_LM_KV_PAGE 64        /* cache positions per page of a paged slot session (acb_lm_begin_slots_paged): a multiple of
+                                    the 4-position groups the attention kernel copies, so no 16-byte copy crosses a page */
+#define ACB_LM_MAX_PAGES_PER_ROW 188   /* ceil(12000 / ACB_LM_KV_PAGE): pages of one row at the largest max_seq */
 
 typedef struct {
     int use_sampling;  /* LMModel.generate(use_sampling, temp, top_k, top_p, cfg_coef), lm.py:421-436 */
@@ -321,6 +324,32 @@ int acb_lm_admit(acb_lm_t* lm, int slot, const float* cross, int text_len, int s
  * anything is enqueued).  prefix_len == 0 is acb_lm_admit. */
 int acb_lm_admit_prefix(acb_lm_t* lm, int slot, const float* cross, int text_len, const float* prefix, int prefix_len,
                         int seq_len, uint64_t seed, const acb_lm_sampling* sampling, void* stream);
+
+/* Paged slot session: acb_lm_begin_slots with the self-attention KV cache in a pool of pages instead of `slots` rows of
+ * max_seq positions, so a request holds only the pages its own length needs.  Only on a handle created with
+ * buffers.k_cache = buffers.v_cache = NULL (a paged handle; acb_lm_begin, acb_lm_begin_prefix, acb_lm_prefill and
+ * acb_lm_begin_slots return ACB_ERR_INVALID on it, and this call returns it on any other handle).
+ *   k_pool, v_pool  fp16 [L][n_pages][H][ACB_LM_KV_PAGE][64]: page j of a row holds its cache positions
+ *                   [ACB_LM_KV_PAGE * j, ACB_LM_KV_PAGE * (j + 1)).
+ *   page_table      int32 [2 * slots][pages_per_row] (device): row r's page ids, written by acb_lm_admit_paged for the
+ *                   slot's two rows; the captured step reads it at run time, so an admission recaptures nothing.
+ *                   ceil((max_prefix + seq_len_max) / ACB_LM_KV_PAGE) <= pages_per_row <= ACB_LM_MAX_PAGES_PER_ROW.
+ *   stage_k, stage_v  fp16 [L][2][H][max_prefix][64]: an admission runs a condition prefix's prefill passes into these
+ *                   (the passes acb_lm_admit_prefix runs) and copies them into the slot's pages; NULL when max_prefix == 0.
+ * Needs max_prefix + seq_len_max <= max_seq and n_pages >= 2 * ceil((max_prefix + seq_len_max) / ACB_LM_KV_PAGE) (one
+ * request of the longest length fits).  Everything else is acb_lm_begin_slots. */
+int acb_lm_begin_slots_paged(acb_lm_t* lm, int slots, int max_text, int seq_len_max, int max_prefix, void* k_pool, void* v_pool,
+                             int n_pages, int32_t* page_table, int pages_per_row, void* stage_k, void* stage_v,
+                             const acb_lm_sampling* sampling, void* stream);
+
+/* acb_lm_admit_prefix in a paged session: pages [2][n / 2] (host memory) are the page ids of the slot's cond row (slot) and
+ * null row (slots + slot), n = 2 * ceil((prefix_len + seq_len) / ACB_LM_KV_PAGE).  The caller gives pages no other live slot
+ * holds.  Returns ACB_ERR_INVALID before enqueuing anything when n is not that count, an id is outside [0, n_pages), an id
+ * appears twice, or prefix_len > max_prefix; else what acb_lm_admit_prefix checks.  The prefix K/V in the pages are, bit for
+ * bit, what acb_lm_admit_prefix writes into a contiguous session's rows.  acb_lm_admit and acb_lm_admit_prefix return
+ * ACB_ERR_INVALID in a paged session. */
+int acb_lm_admit_paged(acb_lm_t* lm, int slot, const float* cross, int text_len, const float* prefix, int prefix_len,
+                       int seq_len, uint64_t seed, const acb_lm_sampling* sampling, const int32_t* pages, int n, void* stream);
 
 /* Cancel the request in `slot` between steps: an ACTIVE or FINISHED slot becomes INACTIVE (status 0) and the next step skips
  * it, as it skips a slot never admitted; the slot is free for acb_lm_admit, which overwrites its K/V, mask and state.  One

@@ -11,7 +11,10 @@ A request in a session computes what `LMModel.generate` computes for it alone: t
 condition (no padding to other requests' text lengths), and Philox noise keyed by its own seed and column.  Its tokens are
 bit-identical to `generate` of that item alone when both run the same GEMM regime (up to 64 rows, i.e. <= 32 slots) and the
 prompt is not prefilled (``ACB_LM_PREFILL=0``): a session consumes a continuation prompt one column per step (teacher
-forcing), which costs one step per prompt column, where `generate` prefills it several positions per pass.
+forcing), which costs one step per prompt column, where `generate` prefills it several positions per pass.  A request with
+`prefill_cols` (`ContinuousGenerator(prefill_prompts=True)`) has its prompt prefilled at admission in `generate`'s passes
+(acb_lm_admit_prompt) and equals `generate`'s default path; such a session also runs requests longer than max_duration
+window by window (`WindowChain`), re-admitting each window into its slot as the previous one finishes.
 
 A melody model (the `prepend` fuser: MusicGen-melody) conditions a request on a prefix [2, P, d] of chroma and, in the
 released layout, description positions, whose length P differs from request to request.  Admission prefills it into the
@@ -43,6 +46,7 @@ from dataclasses import dataclass, field
 import torch
 
 from . import _lib
+from .musicgen import window_plan
 
 SLOT_INACTIVE, SLOT_ACTIVE, SLOT_FINISHED = 0, 1, 2
 
@@ -64,6 +68,10 @@ class Request:
     top_p: tp.Optional[float] = None
     cfg_coef: tp.Optional[float] = None
     prefix: tp.Optional[torch.Tensor] = None
+    # prompt columns prefilled at admission (acb_lm_admit_prompt); the slot starts decoding at this column
+    prefill_cols: int = 0
+    # a request longer than the session's max_duration: the windows after this one (None: this is the whole request)
+    chain: tp.Optional['WindowChain'] = None
 
 
 SAMPLING_OPTIONS = ('use_sampling', 'temp', 'top_k', 'top_p', 'cfg_coef')
@@ -160,6 +168,34 @@ def pattern_sequence(lm, prompt: tp.Optional[torch.Tensor], max_gen_len: int, de
     gen_codes[..., :prompt.shape[-1]] = prompt
     gen_sequence, _, mask = pattern.build_pattern_sequence(gen_codes, lm.special_token_id)
     return gen_sequence, mask, pattern
+
+
+def prefill_columns(lm, prompt_len: int, max_gen_len: int) -> int:
+    """The prompt columns `LMModel.generate` prefills for a prompt of `prompt_len` frames in a generation of max_gen_len
+    (`lm.prompt_prefill_columns`): 0 below the pass threshold or with ACB_LM_PREFILL=0."""
+    from .lm import prompt_prefill_columns
+    return prompt_prefill_columns(lm.pattern_provider.get_pattern(max_gen_len).get_first_step_with_timesteps(prompt_len))
+
+
+class WindowChain:
+    """The windows of one request longer than the session's max_duration, as `BaseGenModel._token_windows` runs them
+    (`musicgen.window_plan`).  `make(k, prompt)` builds window k's Request from its prompt; `advance(codes)` takes a finished
+    window's codes [1, K, length] and returns the next window's Request (prompted with codes[:, :, stride:]) or None after
+    the last.  `tokens()` is then the request's result: its prompt, then each window's new frames."""
+
+    def __init__(self, plan, make: tp.Callable[[int, tp.Optional[torch.Tensor]], Request],
+                 prompt: tp.Optional[torch.Tensor]):
+        self.plan, self.make, self.k = plan, make, 0
+        self.pieces: tp.List[torch.Tensor] = [] if prompt is None else [prompt]
+
+    def advance(self, codes: torch.Tensor) -> tp.Optional[Request]:
+        w = self.plan[self.k]
+        self.pieces.append(codes[:, :, w.prompt_len:])
+        self.k += 1
+        return self.make(self.k, codes[:, :, w.stride:]) if self.k < len(self.plan) else None
+
+    def tokens(self) -> torch.Tensor:
+        return torch.cat(self.pieces, dim=-1)
 
 
 def revert_sequence(lm, gen_sequence: torch.Tensor, mask: torch.Tensor, pattern, max_gen_len: int) -> torch.Tensor:
@@ -263,7 +299,7 @@ class SlotSession:
 
     def admit(self, slot: int, req: Request):
         """Write the request's sequence and mask rows, then its sampling options, cross K/V, condition prefix and slot state
-        (acb_lm_admit_prefix)."""
+        (acb_lm_admit_prefix), and with req.prefill_cols > 0 prefill that many prompt columns (acb_lm_admit_prompt)."""
         self._check_owner()
         lm = self.lm
         if req.max_gen_len > self.max_gen_len:
@@ -288,6 +324,8 @@ class SlotSession:
         with torch.cuda.device(lm.device):
             seq, mask, pattern = pattern_sequence(lm, req.prompt, req.max_gen_len, lm.device)
             S = seq.shape[-1]
+            if not 0 <= req.prefill_cols <= S - 2:
+                raise ValueError(f"prefill_cols {req.prefill_cols} not in [0, {S - 2}]")
             b = lm._bufs
             b['seq'][slot].fill_(-1)
             b['seq'][slot, :, :S] = seq[0]
@@ -304,15 +342,25 @@ class SlotSession:
                 if not 1 <= T <= self.max_text:
                     raise ValueError(f"condition of {T} text positions: the session holds 1 .. {self.max_text}")
             prefix = req.prefix.to(lm.device, torch.float32).contiguous() if P else None
-            if self.pages is None:
+            F = req.prefill_cols
+            if self.pages is None and F:
+                _lib.check(lm._lib.acb_lm_admit_prompt(lm._handle, slot, _lib.ptr(cross), T, _lib.ptr(prefix), P, S, F,
+                                                       C.c_uint64(req.seed), samp, None, 0, _lib.stream()), 'lm_admit_prompt')
+            elif self.pages is None:
                 _lib.check(lm._lib.acb_lm_admit_prefix(lm._handle, slot, _lib.ptr(cross), T, _lib.ptr(prefix), P, S,
                                                        C.c_uint64(req.seed), samp, _lib.stream()), 'lm_admit')
             else:
                 ids = self.pages.take(slot, P + S)
                 try:
-                    _lib.check(lm._lib.acb_lm_admit_paged(lm._handle, slot, _lib.ptr(cross), T, _lib.ptr(prefix), P, S,
-                                                          C.c_uint64(req.seed), samp, (C.c_int32 * len(ids))(*ids), len(ids),
-                                                          _lib.stream()), 'lm_admit_paged')
+                    pages = (C.c_int32 * len(ids))(*ids)
+                    if F:
+                        _lib.check(lm._lib.acb_lm_admit_prompt(lm._handle, slot, _lib.ptr(cross), T, _lib.ptr(prefix), P, S, F,
+                                                               C.c_uint64(req.seed), samp, pages, len(ids), _lib.stream()),
+                                   'lm_admit_prompt')
+                    else:
+                        _lib.check(lm._lib.acb_lm_admit_paged(lm._handle, slot, _lib.ptr(cross), T, _lib.ptr(prefix), P, S,
+                                                              C.c_uint64(req.seed), samp, pages, len(ids), _lib.stream()),
+                                   'lm_admit_paged')
                 except Exception:
                     self.pages.release(slot)
                     raise
@@ -378,7 +426,13 @@ class ContinuousScheduler:
     On a paged session (one whose `pages` is a `PagePool`; `positions(req)` gives a request's length) the head of the queue is
     admitted only when a slot and its pages are free; while its pages are not, it waits and no later request overtakes it,
     so a long request is never starved by shorter ones.  `page_wait_steps` counts the steps run while the head waited for
-    pages with a slot free, `page_steps` the pages in use summed over steps (mean: page_steps / steps_run)."""
+    pages with a slot free, `page_steps` the pages in use summed over steps (mean: page_steps / steps_run).
+
+    A request with prefilled prompt columns (`prefill_cols`) starts at that column.  A request longer than the session's
+    window (`chain`, a `WindowChain`) is admitted as its first window; when a window finishes, the next one is admitted in the
+    same poll into the same slot, ahead of every waiting request, and in a paged session it takes pages from those the
+    finished window released (it never needs more).  The request is returned once, after its last window, with all its
+    tokens.  `readmitted` counts those re-admissions."""
 
     def __init__(self, session, slots: int, poll_steps: tp.Optional[int] = None):
         if poll_steps is not None and poll_steps < 1:
@@ -392,6 +446,7 @@ class ContinuousScheduler:
         self.page_wait_steps = 0
         self.page_steps = 0
         self.last_admitted: tp.List[tp.Tuple[int, Request]] = []
+        self.readmitted = 0
 
     def submit(self, req: Request):
         self.waiting.append(req)
@@ -432,7 +487,7 @@ class ContinuousScheduler:
                 req = self.waiting.popleft()
                 self.session.admit(slot, req)
                 self.active[slot] = req
-                self.pos[slot] = 0
+                self.pos[slot] = req.prefill_cols
                 self.last_admitted.append((slot, req))
         if not self.active:
             return []
@@ -456,7 +511,18 @@ class ContinuousScheduler:
                 raise RuntimeError(f"slot {slot}: device at position {pos} status {st}, expected {self.pos[slot]} "
                                    f"{'finished' if finished else 'decoding'}")
             if finished:
-                done.append((req, self.session.collect(slot, req)))
+                codes = self.session.collect(slot, req)
+                nxt = req.chain.advance(codes) if req.chain is not None else None
+                if nxt is not None:   # the request's next window, before any waiting request
+                    assert self.session.positions(nxt) <= self.session.positions(req), \
+                        "a later window needs more cache positions than the first"
+                    assert pool is None or pool.fits(self.session.positions(nxt))
+                    self.session.admit(slot, nxt)
+                    self.active[slot] = nxt
+                    self.pos[slot] = nxt.prefill_cols
+                    self.readmitted += 1
+                    continue
+                done.append((req, codes if req.chain is None else req.chain.tokens()))
                 del self.active[slot]
                 del self.pos[slot]
         return done
@@ -467,11 +533,12 @@ class ContinuousScheduler:
 
 
 class _Cohort:
-    """Requests admitted in the same poll: they advance in lock-step and share one stream decoder."""
+    """Requests admitted in the same poll at the same start column: they advance in lock-step and share one stream decoder."""
 
-    def __init__(self, members: tp.List[tp.Tuple[int, Request]], decoder, start: int):
+    def __init__(self, members: tp.List[tp.Tuple[int, Request]], decoder, start: int, col0: int = 0):
         self.members, self.decoder = members, decoder
         self.start = start           # the scheduler's steps_run when the cohort was admitted
+        self.col0 = col0             # the members' start column (their prefilled prompt columns)
         self.frames = 0              # frames handed to the decoder
 
 
@@ -479,8 +546,9 @@ class CohortStream:
     """Audio pieces of a session's requests while they decode, one codec call per cohort and poll.
 
     `stream_decoder(n)` makes a decoder over n items (`push(codes [n, K, m]) -> [n, C, m']`, `flush()`, `select(items)`).
-    After a poll in which a request has run s steps, its frames below s - max_delay are final (as in
-    `LMModel.generate_blocks`); the scheduler knows every position on the host, so nothing is read back to find them.  Each
+    After a poll in which a request is at column c (its start column plus the steps it has run), its frames below
+    c - max_delay are final (as in `LMModel.generate_blocks`), so a prefilled prompt's frames are final at admission and the
+    requests admitted in one poll form one cohort per start column; the scheduler knows every position on the host, so nothing is read back to find them.  Each
     cohort's new frames go to its decoder in one push.  Members that finish are split out with `select` and flushed together
     (members of one cohort that finish in the same poll have the same length), the rest keep decoding in the remaining
     decoder.  A cancelled member is dropped from its cohort the same way.  `poll()` returns `(request_id, piece, tokens, final)`
@@ -511,8 +579,11 @@ class CohortStream:
         sch = self.scheduler
         start = sch.steps_run
         done = sch.poll()
-        if sch.last_admitted:
-            self.cohorts.append(_Cohort(list(sch.last_admitted), self.stream_decoder(len(sch.last_admitted)), start))
+        by_col: tp.Dict[int, tp.List[tp.Tuple[int, Request]]] = {}
+        for slot, req in sch.last_admitted:
+            by_col.setdefault(req.prefill_cols, []).append((slot, req))
+        for col0, members in by_col.items():
+            self.cohorts.append(_Cohort(members, self.stream_decoder(len(members)), start, col0))
         finished = {req.id for req, _ in done}
         events = []
         for co in list(self.cohorts):
@@ -522,7 +593,7 @@ class CohortStream:
     def _advance(self, co: _Cohort, finished: tp.Set[int]) -> list:
         members = co.members
         fin = [i for i, (_, r) in enumerate(members) if r.id in finished]
-        ready = max(0, self.scheduler.steps_run - co.start - self.max_delay)
+        ready = max(0, co.col0 + self.scheduler.steps_run - co.start - self.max_delay)
         if ready == co.frames:   # no new frame, so no member finished either (its last step makes its last frame final)
             assert not fin
             return []
@@ -581,13 +652,27 @@ class ContinuousGenerator:
     waits in FIFO order until a slot and its pages are free.  Refused before any device work: kv_cache_gb <= 0, and a budget
     that cannot hold one request of max_duration (ValueError).  Results are those of the session without kv_cache_gb.
 
-    Refused before any device work: durations beyond max_duration, two_step_cfg and cfg_coef_beta (NotImplementedError), a
-    melody on a model without a melody conditioner (NotImplementedError), a melody together with a prompt, and a description
-    longer than max_text text positions (ValueError)."""
+    With `prefill_prompts`, a request's results are those of `generate`'s default path instead of ``ACB_LM_PREFILL=0``: its
+    prompt columns [0, first) (first as `LMModel.generate` computes it, `prefill_columns`) are prefilled into its slot at
+    admission (acb_lm_admit_prompt), in the passes `generate` runs for it alone, and the slot decodes from column `first`.
+    A continuation then occupies its slot `first` fewer steps, but its passes (32 positions each) run between two steps, so
+    every other slot waits for them: prefill lowers a prompted request's latency and can cost the session's throughput when
+    many slots are busy.  It also serves durations beyond max_duration, window by window as `generate` does
+    (`musicgen.window_plan`, `extend_stride` of the model's generation parameters): each window after the first is admitted
+    into the same slot as soon as the previous one finishes, with the previous window's tail prefilled as its prompt, and on a
+    melody model with the melody re-sliced from the window's offset.  `submit` draws one seed per window, in `generate`'s
+    order.  A long request is returned once, with all its frames; it is refused with `chunk_duration` (NotImplementedError),
+    as a stream decoder is not carried from one window to the next.
+
+    Refused before any device work: durations beyond max_duration without prefill_prompts, two_step_cfg and cfg_coef_beta
+    (NotImplementedError), a melody on a model without a melody conditioner (NotImplementedError), a melody together with a
+    prompt, and a description longer than max_text text positions (ValueError)."""
+
+    prefill_prompts = False
 
     def __init__(self, model, slots: int = 32, poll_steps: tp.Optional[int] = None, max_text: int = 64,
                  return_tokens: bool = False, chunk_duration: tp.Optional[float] = None,
-                 kv_cache_gb: tp.Optional[float] = None):
+                 kv_cache_gb: tp.Optional[float] = None, prefill_prompts: bool = False):
         params = dict(model.generation_params)
         kv_pages = None if kv_cache_gb is None else kv_pages_for_budget(model.lm, kv_cache_gb)
         if getattr(model, '_has_melody', False) != model.lm.has_prefix:
@@ -605,7 +690,7 @@ class ContinuousGenerator:
             model.compression_model.stream_decoder(1)   # GroupNorm and transformers' chunked codecs refuse here
             block = max(1, int(round(chunk_duration * model.frame_rate)))
             poll_steps = block if poll_steps is None else min(poll_steps, block)
-        self.model, self.return_tokens = model, return_tokens
+        self.model, self.return_tokens, self.prefill_prompts = model, return_tokens, bool(prefill_prompts)
         self.defaults = dict(use_sampling=params['use_sampling'], temp=params['temp'], top_k=params['top_k'],
                              top_p=params['top_p'], cfg_coef=params['cfg_coef'])
         max_gen_len = int(model.max_duration * model.frame_rate)
@@ -625,9 +710,13 @@ class ContinuousGenerator:
         from .audio_utils import convert_audio
         m = self.model
         duration = m.duration if duration is None else float(duration)
-        if duration > m.max_duration:
-            raise NotImplementedError(f"duration {duration} > max_duration {m.max_duration}: window extension is not built "
-                                      "for continuous batching")
+        long = duration > m.max_duration
+        if long and not self.prefill_prompts:
+            raise NotImplementedError(f"duration {duration} > max_duration {m.max_duration}: window extension needs a session "
+                                      "with prefill_prompts=True")
+        if long and self.stream is not None:
+            raise NotImplementedError(f"duration {duration} > max_duration {m.max_duration} with chunk_duration: streaming a "
+                                      "request across windows is not built")
         n = int(duration * m.frame_rate)
         if n < 1:
             raise ValueError(f"duration {duration} s is less than one frame")
@@ -660,8 +749,34 @@ class ContinuousGenerator:
             attributes, prompt_tokens = m._prepare_melody([description], [melody], melody_sample_rate)
         else:   # on a melody model every item carries a melody condition: a null one here
             attributes, prompt_tokens = m._prepare_tokens_and_attributes([description], prompt)
-        if prompt_tokens is not None and prompt_tokens.shape[-1] >= n:
-            raise ValueError(f"the prompt ({prompt_tokens.shape[-1]} frames) must be shorter than the generation ({n})")
+        T0 = 0 if prompt_tokens is None else prompt_tokens.shape[-1]
+        plan = window_plan(duration, m.max_duration, m.extend_stride, m.frame_rate, T0) if long else None
+        first_len = plan[0].length if long else n
+        if prompt_tokens is not None and T0 >= first_len:
+            raise ValueError(f"the prompt ({T0} frames) must be shorter than the generation ({first_len})")
+        # a long request's windows in generate's order: window k's conditions (a melody re-sliced from its offset), then
+        # its seed, drawn as LMModel.generate draws it
+        windows = []
+        for k in range(len(plan) if long else 1):
+            if k == 0 or getattr(m, '_has_melody', False):   # a text condition is the same in every window
+                attrs = m._window_attributes(attributes, plan[k].time_offset) if long else attributes
+                cross, prefix = self._conditions(attrs)
+            windows.append((cross, prefix, int(torch.randint(0, 2 ** 62, (1,)).item())))
+        rid = next(self._ids)
+
+        def make(k: int, prompt: tp.Optional[torch.Tensor]) -> Request:
+            length = plan[k].length if long else n
+            cols = prefill_columns(m.lm, prompt.shape[-1], length) if self.prefill_prompts and prompt is not None else 0
+            cross, prefix, seed = windows[k]
+            return Request(length, cross, prompt, seed, rid, **options, prefix=prefix, prefill_cols=cols, chain=chain)
+
+        chain = WindowChain(plan, make, prompt_tokens) if long else None
+        self.scheduler.submit(make(0, prompt_tokens))
+        return rid
+
+    def _conditions(self, attributes):
+        """A request's cross [2, T, d] and prefix [2, P, d] (None where the model has none), checked against the session."""
+        m = self.model
         cross = prefix = None
         if m.lm.cross_attention or m.lm.has_prefix:
             cross, prefix = m.lm._condition_tensors(attributes)
@@ -671,10 +786,7 @@ class ContinuousGenerator:
         if prefix is not None and prefix.shape[1] > self.session.max_prefix:
             raise ValueError(f"the condition prefix has {prefix.shape[1]} positions (chroma and description); the session holds "
                              f"{self.session.max_prefix}: the description is longer than {self.session.max_text} text positions")
-        seed = int(torch.randint(0, 2 ** 62, (1,)).item())   # drawn as LMModel.generate draws it
-        rid = next(self._ids)
-        self.scheduler.submit(Request(n, cross, prompt_tokens, seed, rid, **options, prefix=prefix))
-        return rid
+        return cross, prefix
 
     def cancel(self, request_id: int) -> bool:
         """Drop a waiting request or stop a decoding one (acb_lm_retire); False for a finished or unknown id."""

@@ -504,6 +504,32 @@ __global__ void __launch_bounds__(256) lm_qkv_slot_paged_kernel(const float* __r
     qkv_slot_body<true>(qkv, slot_state, q32, kc, vc, d, H, 0, slots, rope_freq, pos_scale, rope, table, pages_per_row);
 }
 
+// Paged admission pass (acb_lm_admit_prompt in a paged session): what the EPI_QKV_PF / EPI_QKV_PF_ROPE epilogue does, after
+// the QKV GEMM's plain fp32 epilogue (qkv [rows][3d]).  GEMM row r is position P[0] + r / rows_real of generation row
+// j = r % rows_real, whose page table row is r0 + j * row_stride; k and v go to offset pos % ACB_LM_KV_PAGE of its page.  The
+// rotary input is the same fp32 sum the epilogue rotates, so q, k and v are bit-identical to a contiguous pass.
+__global__ void __launch_bounds__(256) lm_qkv_pf_paged_kernel(const float* __restrict__ qkv, const int* __restrict__ P,
+                                                              float* __restrict__ q32, __half* __restrict__ kc,
+                                                              __half* __restrict__ vc, int d, int H, int rows_real,
+                                                              const float* __restrict__ rope_freq, float pos_scale, bool rope,
+                                                              const int* __restrict__ table, int pages_per_row, int r0,
+                                                              int row_stride) {
+    const int row = blockIdx.x, tk = row / rows_real, j = row - tk * rows_real, pos = P[0] + tk;
+    const int page = table[(r0 + j * row_stride) * pages_per_row + pos / ACB_LM_KV_PAGE];
+    const float* src = qkv + (size_t)row * 3 * d;
+    for (int n = threadIdx.x; n < 3 * d; n += 256) {
+        const int which = n >= 2 * d ? 2 : (n >= d ? 1 : 0), nn = n - which * d;
+        float v = src[n];
+        if (rope && which < 2) v = rope_rotate(rope_freq, pos_scale, half_round(v), half_round(src[n ^ 1]), nn & 63, pos);
+        if (which == 0) {
+            q32[(size_t)row * d + nn] = v;
+        } else {
+            __half* cache = which == 2 ? vc : kc;
+            cache[(((size_t)page * H + (nn >> 6)) * ACB_LM_KV_PAGE + pos % ACB_LM_KV_PAGE) * 64 + (nn & 63)] = __float2half_rn(v);
+        }
+    }
+}
+
 // ------------------------------------------------------------------------------------------------ attention (1 query)
 struct AttnParams {
     const float* q; int q_nsplit; size_t q_split_stride;  // q[s][row][d] fp32 partial sums
@@ -779,6 +805,123 @@ __global__ void __launch_bounds__(ATT_WARPS * 32) lm_attn2_slot_paged_kernel(Att
     const int n = slot[ACB_SLOT_PREFIX] + slot[ACB_SLOT_POS] + 1;
     __shared__ int pt[ACB_LM_MAX_PAGES_PER_ROW];
     for (int i = tid; i < (n + ACB_LM_KV_PAGE - 1) / ACB_LM_KV_PAGE; i += ATT_WARPS * 32) pt[i] = table[row * pages_per_row + i];
+    __syncthreads();
+    const size_t base = (size_t)h * ACB_LM_KV_PAGE * 64 + sl * 8;   // position pp: + (pt[pp / page] * H * page + pp % page) * 64
+    const __half* kb = p.kc + base;
+    const __half* vb = p.vc + base;
+    const uint32_t ring = smem_u32(att2sm) + (uint32_t)(warp * ATT2_DEPTH * 1024 + lane * 16);
+    // iteration k of this warp covers positions (k * 8 + warp) * 4 + pg
+    const int n_it = (n + 31 - warp * 4) / 32 > 0 ? (n - warp * 4 + 31) / 32 : 0;   // iterations with at least one live position group
+    auto issue = [&](int k) {
+        if (k < n_it) {
+            const int pp = (k * ATT_WARPS + warp) * 4 + pg;
+            if (pp < n) {
+                const uint32_t d = ring + (uint32_t)((k % ATT2_DEPTH) * 1024);
+                const size_t o = ((size_t)pt[pp / ACB_LM_KV_PAGE] * p.H * ACB_LM_KV_PAGE + pp % ACB_LM_KV_PAGE) * 64;
+                asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d), "l"(kb + o) : "memory");
+                asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d + 512u), "l"(vb + o) : "memory");
+            }
+        }
+        asm volatile("cp.async.commit_group;" ::: "memory");
+    };
+#pragma unroll
+    for (int k = 0; k < ATT2_DEPTH - 1; ++k) issue(k);
+
+    float q[8];
+    {
+        const float4* qp = reinterpret_cast<const float4*>(p.q + (size_t)qrow * p.d + h * 64 + sl * 8);
+        const float4 qa = qp[0], qb = qp[1];
+        q[0] = half_round(qa.x) * p.scale; q[1] = half_round(qa.y) * p.scale; q[2] = half_round(qa.z) * p.scale;
+        q[3] = half_round(qa.w) * p.scale; q[4] = half_round(qb.x) * p.scale; q[5] = half_round(qb.y) * p.scale;
+        q[6] = half_round(qb.z) * p.scale; q[7] = half_round(qb.w) * p.scale;
+    }
+    OnlineSM st;
+    st.m = -INFINITY; st.l = 0.f;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) st.acc[e] = 0.f;
+
+    for (int k = 0; k < n_it; ++k) {                 // warp-uniform trip count (the shuffles need all 32 lanes)
+        issue(k + ATT2_DEPTH - 1);
+        asm volatile("cp.async.wait_group %0;" ::"n"(ATT2_DEPTH - 1) : "memory");   // iteration k's copies of this lane have landed
+        const int pp = (k * ATT_WARPS + warp) * 4 + pg;
+        const uint32_t sa = ring + (uint32_t)((k % ATT2_DEPTH) * 1024);
+        uint4 kv = make_uint4(0, 0, 0, 0), vv = make_uint4(0, 0, 0, 0);
+        if (pp < n) {
+            asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(kv.x), "=r"(kv.y), "=r"(kv.z), "=r"(kv.w) : "r"(sa));
+            asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(vv.x), "=r"(vv.y), "=r"(vv.z), "=r"(vv.w) : "r"(sa + 512u));
+        }
+        const __half2* k2 = reinterpret_cast<const __half2*>(&kv);
+        float s = 0.f;
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            const float2 f = __half22float2(k2[e]);
+            s = fmaf(q[2 * e], f.x, s);
+            s = fmaf(q[2 * e + 1], f.y, s);
+        }
+        s += __shfl_xor_sync(0xffffffffu, s, 1);
+        s += __shfl_xor_sync(0xffffffffu, s, 2);
+        s += __shfl_xor_sync(0xffffffffu, s, 4);
+        if (pp < n) {
+            const float mn = fmaxf(st.m, s);
+            const float corr = __expf(st.m - mn);   // exp(-inf) = 0 on the first position
+            const float pw = __expf(s - mn);
+            st.l = st.l * corr + pw;
+            const __half2* v2 = reinterpret_cast<const __half2*>(&vv);
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const float2 f = __half22float2(v2[e]);
+                st.acc[2 * e] = fmaf(pw, f.x, st.acc[2 * e] * corr);
+                st.acc[2 * e + 1] = fmaf(pw, f.y, st.acc[2 * e + 1] * corr);
+            }
+            st.m = mn;
+        }
+    }
+    asm volatile("cp.async.wait_group 0;" ::: "memory");
+    // merge the 4 position groups of the warp, then the warps
+#pragma unroll
+    for (int o = 8; o <= 16; o <<= 1) {
+        const float m2 = __shfl_xor_sync(0xffffffffu, st.m, o), l2 = __shfl_xor_sync(0xffffffffu, st.l, o);
+        float a2[8];
+#pragma unroll
+        for (int e = 0; e < 8; ++e) a2[e] = __shfl_xor_sync(0xffffffffu, st.acc[e], o);
+        osm_merge(st, m2, l2, a2);
+    }
+    if (pg == 0) {
+        if (sl == 0) { wm[warp] = st.m; wl[warp] = st.l; }
+#pragma unroll
+        for (int e = 0; e < 8; ++e) wacc[warp][sl * 8 + e] = st.acc[e];
+    }
+    __syncthreads();
+    if (tid < 64) {
+        float mx = wm[0];
+#pragma unroll
+        for (int w = 1; w < ATT_WARPS; ++w) mx = fmaxf(mx, wm[w]);
+        float l = 0.f, o = 0.f;
+#pragma unroll
+        for (int w = 0; w < ATT_WARPS; ++w) {
+            const float cw = wm[w] == -INFINITY ? 0.f : __expf(wm[w] - mx);
+            l = fmaf(wl[w], cw, l);
+            o = fmaf(wacc[w][tid], cw, o);
+        }
+        p.out[(size_t)qrow * p.d + h * 64 + tid] = __float2half_rn(o / l);
+    }
+}
+
+// Paged admission pass (acb_lm_admit_prompt in a paged session): lm_attn2_kernel<true> reading K and V through the page table.
+// blockIdx.y is a (token, row) pair tok * rows_real + j; the query at position pos[0] + tok attends to positions
+// [0, pos[0] + tok] of page table row r0 + j * row_stride (the pass's own positions are already appended:
+// lm_qkv_pf_paged_kernel ran before).  The row's table is staged in shared memory as in lm_attn2_slot_paged_kernel, and the
+// arithmetic and its order are lm_attn2_kernel's.  (A separate copy: the other kernels stay as they are.)
+__global__ void __launch_bounds__(ATT_WARPS * 32) lm_attn2_pf_paged_kernel(AttnParams p, const int* __restrict__ table,
+                                                                        int pages_per_row, int r0) {
+    extern __shared__ __align__(16) unsigned char att2sm[];   // [warp][depth][K | V][32 lanes][16 B]
+    __shared__ float wm[ATT_WARPS], wl[ATT_WARPS], wacc[ATT_WARPS][64];
+    __shared__ int pt[ACB_LM_MAX_PAGES_PER_ROW];
+    const int h = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int qrow = blockIdx.y, tok = qrow / p.rows_real, trow = r0 + (qrow - tok * p.rows_real) * p.row_stride;
+    const int sl = lane & 7, pg = lane >> 3;
+    const int n = p.pos[0] + tok + 1;
+    for (int i = tid; i < (n + ACB_LM_KV_PAGE - 1) / ACB_LM_KV_PAGE; i += ATT_WARPS * 32) pt[i] = table[trow * pages_per_row + i];
     __syncthreads();
     const size_t base = (size_t)h * ACB_LM_KV_PAGE * 64 + sl * 8;   // position pp: + (pt[pp / page] * H * page + pp % page) * 64
     const __half* kb = p.kc + base;
@@ -1487,8 +1630,9 @@ static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_la
     const bool wide = rows > 64;
     const size_t part_stride = (size_t)(pf && !wide ? 8 * nt : lm->rows_pad) * d;
     // self-attention cache: a paged session's step reads and appends through the page table (kv_layer: one layer of the
-    // pool), its admission's prefix passes run into the staging cache of the slot's two rows (rows 0 and 1)
-    const bool stage = pf && lm->paged;
+    // pool), its admission's prefix passes run into the staging cache of the slot's two rows (rows 0 and 1), and its prompt
+    // passes (paged_pass) write and read the slot's pages through the table
+    const bool stage = pf && pf_prefix && lm->paged, paged_pass = pf && !pf_prefix && lm->paged;
     const int kv_len = stage ? lm->max_prefix : c.max_seq, kv_stride = stage ? 1 : row_stride;
     __half* const kv_k = stage ? lm->stage_k : (lm->paged ? lm->pool_k : (__half*)B.k_cache);
     __half* const kv_v = stage ? lm->stage_v : (lm->paged ? lm->pool_v : (__half*)B.v_cache);
@@ -1505,6 +1649,11 @@ static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_la
                                                                 c.n_q, c.card, c.max_seq, lm->slots, c.pos_scale, sin_pos);
         else if (pf && pf_prefix) lm_embed_prefix_kernel<<<rows, 256, 0, s>>>(lm->prefix, lm->w.inv_freq, B.pos, B.x, d, lm->prefix_len,
                                                                        c.pos_scale, rows_real, sin_pos);
+        else if (pf && lm->pf_slot >= 0)   // an admission's prompt pass: both rows read the slot's sequence row, as item 0 of a
+                                           // generation of batch 1 reads its own
+            lm_embed_kernel<true><<<rows, 256, 0, s>>>((const __half*)lm->w.emb, lm->w.inv_freq,
+                                                       B.seq + (size_t)lm->pf_slot * c.n_q * c.max_seq, B.pos, B.x, d, c.n_q,
+                                                       c.card, c.max_seq, 1, c.pos_scale, rows_real, sin_pos, lm->prefix_len);
         else if (pf) lm_embed_kernel<true><<<rows, 256, 0, s>>>((const __half*)lm->w.emb, lm->w.inv_freq, B.seq, B.pos, B.x, d, c.n_q,
                                                               c.card, c.max_seq, lm->batch, c.pos_scale, rows_real, sin_pos,
                                                               lm->prefix_len);
@@ -1567,11 +1716,21 @@ static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_la
                     ++nl;
                     DBG("lm_qkv_slot_kernel", l);
                 }
+            } else if (paged_pass) {   // the pass's plain fp32 epilogue, then the append through the page table
+                p.out_f32 = B.part; p.ld_out = 3 * d;
+                ACB_TRY(launch_gemm<EPI_F32>(nt, p, 1, s, ft2));
+                ++nl;
+                DBG("gemm_EPI_F32 (qkv pass)", l);
+                lm_qkv_pf_paged_kernel<<<rows, 256, 0, s>>>(B.part, B.pos, B.q32, p.kc, p.vc, d, H, rows_real, lm->w.rope_freq,
+                                                            c.pos_scale, rope, lm->page_table, lm->pages_per_row, row0, row_stride);
+                ACB_LAUNCH_CHECK();
+                ++nl;
+                DBG("lm_qkv_pf_paged_kernel", l);
             } else if (wide) ACB_TRY(rope ? launch_wide<EPI_QKV_ROPE>(lm->wmap[WM_QKV], lm->xmap_h16, l * 3 * d, p, ns, s)
                                    : launch_wide<EPI_QKV>(lm->wmap[WM_QKV], lm->xmap_h16, l * 3 * d, p, ns, s));
             else if (pf) ACB_TRY(rope ? launch_gemm<EPI_QKV_PF_ROPE>(nt, p, 1, s, ft2) : launch_gemm<EPI_QKV_PF>(nt, p, 1, s, ft2));
             else ACB_TRY(rope ? launch_gemm<EPI_QKV_ROPE>(nt, p, 1, s, ft2) : launch_gemm<EPI_QKV>(nt, p, 1, s, ft2));
-            if (!slot_step) {
+            if (!slot_step && !paged_pass) {
                 ++nl;
                 DBG("gemm_EPI_QKV", l);
             }
@@ -1584,6 +1743,8 @@ static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_la
                 lm_attn2_slot_paged_kernel<<<dim3(H, rows), ATT_WARPS * 32, ATT2_SMEM, s>>>(a, B.slot_state, lm->page_table,
                                                                                           lm->pages_per_row);
             } else if (slot_step) { a.rows_real = lm->slots; lm_attn2_slot_kernel<<<dim3(H, rows), ATT_WARPS * 32, ATT2_SMEM, s>>>(a, B.slot_state); }
+            else if (paged_pass) lm_attn2_pf_paged_kernel<<<dim3(H, rows), ATT_WARPS * 32, ATT2_SMEM, s>>>(a, lm->page_table,
+                                                                                                      lm->pages_per_row, row0);
             else if (pf) lm_attn2_kernel<true><<<dim3(H, rows), ATT_WARPS * 32, ATT2_SMEM, s>>>(a);
             else lm_attn2_kernel<false><<<dim3(H, rows), ATT_WARPS * 32, ATT2_SMEM, s>>>(a);
             ACB_LAUNCH_CHECK();
@@ -1708,6 +1869,8 @@ extern "C" int acb_lm_create(const acb_lm_config* cfg, const acb_lm_weights* w, 
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_attn2_slot_paged_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT2_SMEM);
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_attn2_slot_paged_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_qkv_slot_paged_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+    if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_attn2_pf_paged_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT2_SMEM);
+    if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_attn2_pf_paged_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_sample_slot_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_cross_attn_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_ln_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
@@ -1977,9 +2140,11 @@ extern "C" int acb_lm_admit(acb_lm_t* lm, int slot, const float* cross, int text
     return acb_lm_admit_prefix(lm, slot, cross, text_len, nullptr, 0, seq_len, seed, sampling, stream);
 }
 
-// acb_lm_admit_prefix and acb_lm_admit_paged: pages is NULL in a contiguous session, n_page_ids its length otherwise.
+// acb_lm_admit_prefix, acb_lm_admit_paged and acb_lm_admit_prompt: pages is NULL in a contiguous session, n_page_ids its
+// length otherwise; prefill_cols sequence columns are prefilled after the prefix and the slot starts at that column.
 static int admit(acb_lm_t* lm, int slot, const float* cross, int text_len, const float* prefix, int prefix_len, int seq_len,
-                 uint64_t seed, const acb_lm_sampling* sampling, const int32_t* pages, int n_page_ids, void* stream) {
+                 int prefill_cols, uint64_t seed, const acb_lm_sampling* sampling, const int32_t* pages, int n_page_ids,
+                 void* stream) {
     ACB_REQUIRE(lm && lm->slots > 0, "acb_lm_admit: call acb_lm_begin_slots first");
     ACB_REQUIRE(lm->paged == (pages != nullptr), "%s", lm->paged ? "acb_lm_admit: a paged session admits with acb_lm_admit_paged"
                                                                  : "acb_lm_admit_paged: the session is not paged");
@@ -1989,6 +2154,8 @@ static int admit(acb_lm_t* lm, int slot, const float* cross, int text_len, const
     ACB_REQUIRE(prefix_len >= 0 && (prefix_len == 0 || prefix), "acb_lm_admit: prefix_len %d without a prefix tensor", prefix_len);
     ACB_REQUIRE(prefix_len + seq_len <= c.max_seq, "acb_lm_admit: prefix %d + seq_len %d > max_seq %d", prefix_len, seq_len,
                 c.max_seq);
+    ACB_REQUIRE(prefill_cols >= 0 && prefill_cols <= seq_len - 2, "acb_lm_admit_prompt: prefill_cols %d not in [0, seq_len - 2 = %d]",
+                prefill_cols, seq_len - 2);
     ACB_REQUIRE(!lm->has_cross || (cross && text_len >= 1 && text_len <= lm->text_len),
                 "acb_lm_admit: the model has cross attention: a condition of 1 .. %d text positions is required (got %d)",
                 lm->text_len, text_len);
@@ -2067,25 +2234,46 @@ static int admit(acb_lm_t* lm, int slot, const float* cross, int text_len, const
             ACB_LAUNCH_CHECK();
         }
     }
+    // the prompt's columns [0, prefill_cols) at cache positions prefix_len + column, after the prefix (they attend to it), in
+    // the passes acb_lm_prefill runs for a generation of batch 1 with CFG.  Both rows embed the slot's sequence row; a paged
+    // session's passes append to and attend through the slot's pages (lm_qkv_pf_paged_kernel, lm_attn2_pf_paged_kernel).
+    if (prefill_cols > 0) {
+        lm->pf_slot = slot; lm->pf_text_len = lm->has_cross ? text_len : 0;
+        lm->prefix = nullptr; lm->prefix_len = prefix_len;
+        const int rc = prefill_passes(lm, s, prefix_len, prefill_cols, false);
+        lm->pf_slot = -1; lm->pf_text_len = 0;
+        lm->prefix_len = 0;
+        ACB_TRY(rc);
+    }
     lm_slot_sampling_kernel<<<1, 1, 0, s>>>(lm->buf.slot_sampling, slot, sp.use_sampling, sp.temp, sp.top_k, sp.top_p,
                                             sp.cfg_coef);
     ACB_LAUNCH_CHECK();
     lm_slot_admit_kernel<<<1, 1, 0, s>>>(lm->buf.slot_state, slot, seq_len, lm->has_cross ? text_len : 0, prefix_len,
                                          (uint32_t)seed, (uint32_t)(seed >> 32));
     ACB_LAUNCH_CHECK();
+    if (prefill_cols > 0) {   // the slot starts at column prefill_cols (the admission kernel starts it at 0)
+        lm_set_pos_kernel<<<1, 1, 0, s>>>(lm->buf.slot_state + (size_t)slot * ACB_LM_SLOT_STRIDE + ACB_SLOT_POS, prefill_cols);
+        ACB_LAUNCH_CHECK();
+    }
     return ACB_OK;
 }
 
 extern "C" int acb_lm_admit_prefix(acb_lm_t* lm, int slot, const float* cross, int text_len, const float* prefix, int prefix_len,
                                    int seq_len, uint64_t seed, const acb_lm_sampling* sampling, void* stream) {
-    return admit(lm, slot, cross, text_len, prefix, prefix_len, seq_len, seed, sampling, nullptr, 0, stream);
+    return admit(lm, slot, cross, text_len, prefix, prefix_len, seq_len, 0, seed, sampling, nullptr, 0, stream);
 }
 
 extern "C" int acb_lm_admit_paged(acb_lm_t* lm, int slot, const float* cross, int text_len, const float* prefix, int prefix_len,
                                   int seq_len, uint64_t seed, const acb_lm_sampling* sampling, const int32_t* pages, int n,
                                   void* stream) {
     ACB_REQUIRE(pages, "acb_lm_admit_paged: null page list");
-    return admit(lm, slot, cross, text_len, prefix, prefix_len, seq_len, seed, sampling, pages, n, stream);
+    return admit(lm, slot, cross, text_len, prefix, prefix_len, seq_len, 0, seed, sampling, pages, n, stream);
+}
+
+extern "C" int acb_lm_admit_prompt(acb_lm_t* lm, int slot, const float* cross, int text_len, const float* prefix, int prefix_len,
+                                   int seq_len, int prefill_cols, uint64_t seed, const acb_lm_sampling* sampling,
+                                   const int32_t* pages, int n_page_ids, void* stream) {
+    return admit(lm, slot, cross, text_len, prefix, prefix_len, seq_len, prefill_cols, seed, sampling, pages, n_page_ids, stream);
 }
 
 extern "C" int acb_lm_retire(acb_lm_t* lm, int slot, void* stream) {

@@ -21,6 +21,16 @@ from .patterns import DelayedPatternProvider
 import ctypes as C
 
 
+def prompt_prefill_columns(start_offset_sequence: int) -> int:
+    """Sequence columns [0, first) a prompted generation prefills instead of decoding one step each: first =
+    start_offset_sequence - 1 (the pattern's first step with the first unknown timestep, minus one), 0 when that is below 2
+    or when ``ACB_LM_PREFILL=0``.  `LMModel.generate` and a continuous-batching session with prefill_prompts share it."""
+    import os
+    if start_offset_sequence - 1 >= 2 and os.environ.get('ACB_LM_PREFILL', '1') != '0':
+        return start_offset_sequence - 1
+    return 0
+
+
 @dataclass
 class LMOutput:
     """audiocraft/models/lm.py:95-101: logits [B,K,T,card] (NaN where the pattern gives no prediction) and mask [B,K,T]."""
@@ -415,10 +425,8 @@ class LMModel:
             # Prompt prefill (the reference's multi-token first call, lm.py:513-534, transformer.py:240-247): positions
             # [0, start - 1) only feed the KV cache -- their tokens are known and the first sampled position is `start` -- so
             # they go through acb_lm_prefill, several positions per pass, instead of one decode step each.
-            first = 0
-            import os as _os
-            if start_offset_sequence - 1 >= 2 and _os.environ.get('ACB_LM_PREFILL', '1') != '0':
-                first = start_offset_sequence - 1
+            first = prompt_prefill_columns(start_offset_sequence)
+            if first:
                 _lib.check(self._lib.acb_lm_prefill(self._handle, 0, first, _lib.stream()), 'lm_prefill')
             return dict(B=B, K=K, bufs=bufs, first=first, n_steps=n_steps, S=S, pattern=pattern, mask=mask,
                         start_offset=start_offset, start_offset_sequence=start_offset_sequence, max_gen_len=max_gen_len)

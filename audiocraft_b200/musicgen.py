@@ -16,6 +16,7 @@ Melody conditioning (`generate_with_chroma`, musicgen.py:155-249) runs its chrom
 hands the LM a condition prefix; style conditioning is not built and raises.
 """
 import typing as tp
+from dataclasses import dataclass
 
 import torch
 
@@ -26,6 +27,39 @@ from .lm import LMModel
 
 Waveform = torch.Tensor
 Tokens = torch.Tensor
+
+
+@dataclass(frozen=True)
+class Window:
+    """One LM window of a generation: it generates `length` frames, its first `prompt_len` given (already part of the output),
+    starts `start` frames (`time_offset` seconds) into the generation, and its frames from `stride` on are the next window's
+    prompt."""
+    length: int
+    prompt_len: int
+    start: int
+    time_offset: float
+    stride: int
+
+
+def window_plan(duration: float, max_duration: float, extend_stride: tp.Optional[float], frame_rate: float,
+                prompt_len: int = 0) -> tp.List[Window]:
+    """The windows of a generation of `duration` seconds from a prompt of `prompt_len` frames, as `_token_windows` runs
+    them: one window of int(duration * frame_rate) frames up to max_duration; past it, windows of at most max_duration
+    seconds, each starting int(frame_rate * extend_stride) frames after the previous one and prompted with the previous
+    window's frames from that stride on, until int(duration * frame_rate) frames are produced."""
+    n_total = int(duration * frame_rate)
+    if duration <= max_duration:
+        return [Window(n_total, prompt_len, 0, 0.0, 0)]
+    assert extend_stride is not None, "Stride should be defined to generate beyond max_duration"
+    assert extend_stride < max_duration, "Cannot stride by more than max generation duration."
+    stride = int(frame_rate * extend_stride)
+    plan, done, have = [], 0, prompt_len
+    while done + have < n_total:
+        length = int(min(duration - done / frame_rate, max_duration) * frame_rate)
+        plan.append(Window(length, have, done, done / frame_rate, stride))
+        have = max(0, length - stride)
+        done += stride
+    return plan
 
 
 class BaseGenModel:
@@ -111,7 +145,6 @@ class BaseGenModel:
         `window(prompt, attributes, n_tokens, callback)` runs the LM on one window and yields that window's tokens (its prompt
         included) in one or more pieces; past max_duration each window's new frames are yielded as they arrive."""
         fr = self.frame_rate
-        n_total = int(self.duration * fr)
         done_before_window = 0
 
         def report(done_in_window: int, total_in_window: int):
@@ -125,33 +158,29 @@ class BaseGenModel:
         if prompt_tokens is not None:
             assert int(min(self.duration, self.max_duration) * fr) >= prompt_tokens.shape[-1], \
                 "Prompt is longer than audio to generate"
+        plan = window_plan(self.duration, self.max_duration, self.extend_stride, fr,
+                           0 if prompt_tokens is None else prompt_tokens.shape[-1])
         if self.duration <= self.max_duration:
-            yield from window(prompt_tokens, attributes, n_total, callback)
+            yield from window(prompt_tokens, attributes, plan[0].length, callback)
             return
 
         # longer than the model's window: slide by `extend_stride`, each window prompted with the tail of the previous
-        assert self.extend_stride is not None, "Stride should be defined to generate beyond max_duration"
-        assert self.extend_stride < self.max_duration, "Cannot stride by more than max generation duration."
-        stride = int(fr * self.extend_stride)
         if prompt_tokens is not None:
             yield prompt_tokens
-        have = 0 if prompt_tokens is None else prompt_tokens.shape[-1]
         ref_attributes = attributes
-        while done_before_window + have < n_total:
-            window_s = min(self.duration - done_before_window / fr, self.max_duration)
-            attributes = self._window_attributes(ref_attributes, done_before_window / fr)
-            skip = 0 if prompt_tokens is None else prompt_tokens.shape[-1]   # the window's prompt was yielded already
+        for w in plan:
+            done_before_window = w.start
+            attributes = self._window_attributes(ref_attributes, w.time_offset)
+            skip = w.prompt_len   # the window's prompt was yielded already
             got: tp.List[Tokens] = []
             seen = 0
-            for piece in window(prompt_tokens, attributes, int(window_s * fr), callback):
+            for piece in window(prompt_tokens, attributes, w.length, callback):
                 got.append(piece)
                 new = piece[:, :, max(0, skip - seen):]
                 seen += piece.shape[-1]
                 if new.shape[-1]:
                     yield new
-            prompt_tokens = torch.cat(got, dim=-1)[:, :, stride:]
-            have = prompt_tokens.shape[-1]
-            done_before_window += stride
+            prompt_tokens = torch.cat(got, dim=-1)[:, :, w.stride:]
 
     def _window_attributes(self, attributes, time_offset: float):
         """The conditions of the window starting `time_offset` seconds into a generation longer than max_duration."""
@@ -215,7 +244,7 @@ class BaseGenModel:
     # -- continuous batching
     def continuous(self, slots: int = 32, poll_steps: tp.Optional[int] = None, max_text: int = 64,
                    return_tokens: bool = False, chunk_duration: tp.Optional[float] = None,
-                   kv_cache_gb: tp.Optional[float] = None):
+                   kv_cache_gb: tp.Optional[float] = None, prefill_prompts: bool = False):
         """A `batching.ContinuousGenerator` over this model: up to `slots` requests decode side by side, each admitted when a
         slot frees and retired when its last frame is sampled.  `submit(description, duration, prompt, prompt_sample_rate,
         use_sampling=, top_k=, top_p=, temperature=, cfg_coef=)` returns a request id (options left out take the current
@@ -232,9 +261,16 @@ class BaseGenModel:
         a slot and its pages are free.  The budget covers that pool only.  The session also allocates the cross-attention
         K/V for 2 x slots x max_text positions, a staging cache of 2 x (chroma + description) positions for admitting a
         melody prefix, and the split-K partial sums (`part`, 16 x the padded rows x max(3 dim, ffn, n_q x card) fp32).  A
-        request's result is the same with or without a budget."""
+        request's result is the same with or without a budget.
+
+        `prefill_prompts` (default False: a continuation prompt is consumed one decode step per frame, and results equal
+        `generate` with ACB_LM_PREFILL=0) prefills each request's prompt into its slot at admission, as `generate` prefills
+        it, so results equal `generate`'s default path; it also serves durations beyond max_duration window by window, as
+        `generate` does (not with chunk_duration).  The passes stall every slot while they run: it lowers a prompted
+        request's latency and can cost throughput in a busy session (see `batching.ContinuousGenerator`)."""
         from .batching import ContinuousGenerator
-        return ContinuousGenerator(self, slots, poll_steps, max_text, return_tokens, chunk_duration, kv_cache_gb)
+        return ContinuousGenerator(self, slots, poll_steps, max_text, return_tokens, chunk_duration, kv_cache_gb,
+                                   prefill_prompts)
 
 
 def _sampling_params(use_sampling, top_k, top_p, temperature, cfg_coef, two_step_cfg):

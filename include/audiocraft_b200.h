@@ -351,6 +351,18 @@ int acb_lm_begin_slots_paged(acb_lm_t* lm, int slots, int max_text, int seq_len_
 int acb_lm_admit_paged(acb_lm_t* lm, int slot, const float* cross, int text_len, const float* prefix, int prefix_len,
                        int seq_len, uint64_t seed, const acb_lm_sampling* sampling, const int32_t* pages, int n, void* stream);
 
+/* acb_lm_admit_prefix (pages == NULL, contiguous session) or acb_lm_admit_paged (pages, n_page_ids) that also prefills the
+ * request's prompt: after the prefix, sequence columns [0, prefill_cols) of buffers.seq[slot] (their tokens written by the
+ * caller) fill cache positions prefix_len + column of the slot's two rows, in the passes acb_lm_prefill runs for a generation
+ * of batch 1 with CFG (ACB_LM_PREFILL_ROWS / 2 positions per pass, ACB_LM_PREFILL_PER honoured), so the K/V are bit for bit
+ * the ones that generation writes.  The slot then starts at column prefill_cols (acb_lm_slot_status reports it) and finishes
+ * after seq_len - 1 - prefill_cols steps.  In a paged session the passes write and read the slot's pages through the page
+ * table; nothing is staged for the prompt.  Needs 0 <= prefill_cols <= seq_len - 2 (else ACB_ERR_INVALID, before anything is
+ * enqueued) and whatever the call without a prompt needs.  prefill_cols == 0 is acb_lm_admit_prefix / acb_lm_admit_paged. */
+int acb_lm_admit_prompt(acb_lm_t* lm, int slot, const float* cross, int text_len, const float* prefix, int prefix_len,
+                        int seq_len, int prefill_cols, uint64_t seed, const acb_lm_sampling* sampling, const int32_t* pages,
+                        int n_page_ids, void* stream);
+
 /* Cancel the request in `slot` between steps: an ACTIVE or FINISHED slot becomes INACTIVE (status 0) and the next step skips
  * it, as it skips a slot never admitted; the slot is free for acb_lm_admit, which overwrites its K/V, mask and state.  One
  * single-thread kernel on the stream; retiring an INACTIVE slot changes nothing. */

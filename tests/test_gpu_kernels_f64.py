@@ -126,12 +126,19 @@ def _flip(v64, bnd):
     return r, torch.maximum((lo - r).abs(), (hi - r).abs())
 
 
-def check_rope(got, v64, bnd, pos0: int, cfg: dict, f16_out: bool, what: str):
-    """q / k [R, H, T, 64] with rotary positions pos0 .. pos0 + T - 1: the kernel rotates fp16(its fp32 sum) in fp32.  The
-    reference is the oracle's fp32 rotation of fp16(v64); the tolerance adds the input flips (|cos|, |sin| <= 1 with
-    positional_scale in [0, 1]), both sides' fp32 rotation error and, for an fp16 output, half an ulp."""
+def check_rope(got, v64, bnd, pos0, cfg: dict, f16_out: bool, what: str):
+    """q / k [R, H, T, 64] with rotary positions pos0 .. pos0 + T - 1 (pos0 an int, or a tensor [R]: each row from its own
+    position): the kernel rotates fp16(its fp32 sum) in fp32.  The reference is the oracle's fp32 rotation of fp16(v64); the
+    tolerance adds the input flips (|cos|, |sin| <= 1 with positional_scale in [0, 1]), both sides' fp32 rotation error and,
+    for an fp16 output, half an ulp."""
     r, dev = _flip(v64, bnd)
-    ref = LO.rope_rotate(r.float().cpu(), pos0, cfg['max_period'], cfg['positional_scale']).to(v64.device).double()
+    rot = (lambda t, p: LO.rope_rotate(t, p, cfg['max_period'], cfg['positional_scale']))
+    r32 = r.float().cpu()
+    if isinstance(pos0, int):
+        ref = rot(r32, pos0)
+    else:
+        ref = torch.cat([rot(r32[i:i + 1], int(p)) for i, p in enumerate(pos0.tolist())])
+    ref = ref.to(v64.device).double()
     pair = dev.unflatten(-1, (32, 2)).sum(-1, keepdim=True).expand(*dev.shape[:-1], 32, 2).flatten(-2)
     mag = r.abs().unflatten(-1, (32, 2)).sum(-1, keepdim=True).expand(*dev.shape[:-1], 32, 2).flatten(-2)
     tol = pair + 8 * U * mag

@@ -101,6 +101,7 @@ def lib():
     L.acb_lm_admit_prefix.argtypes = [vp, ci, vp, ci, vp, ci, ci, C.c_uint64, C.POINTER(LMSampling), vp]
     L.acb_lm_retire.argtypes = [vp, ci, vp]
     L.acb_lm_begin_slots_paged.argtypes = [vp, ci, ci, ci, ci, vp, vp, ci, vp, ci, vp, vp, C.POINTER(LMSampling), vp]
+    L.acb_lm_begin_slots_paged_fp8.argtypes = [vp, ci, ci, ci, ci, vp, vp, vp, vp, ci, vp, ci, vp, vp, C.POINTER(LMSampling), vp]
     L.acb_lm_admit_paged.argtypes = [vp, ci, vp, ci, vp, ci, ci, C.c_uint64, C.POINTER(LMSampling), vp, ci, vp]
     L.acb_lm_admit_prompt.argtypes = [vp, ci, vp, ci, vp, ci, ci, ci, C.c_uint64, C.POINTER(LMSampling), vp, ci, vp]
     L.acb_lm_slot_status.argtypes = [vp, vp, vp]
@@ -125,7 +126,8 @@ def lib():
                  'acb_conv1d_t6', 'acb_conv1d_t6_tile', 'acb_lm_prefill',
                  'acb_resblock', 'acb_resblock_supported', 'acb_lm_forward', 'acb_t5_encode', 'acb_groupnorm_stats',
                  'acb_groupnorm_apply', 'acb_overlap_add', 'acb_lm_begin_slots', 'acb_lm_admit', 'acb_lm_slot_status', 'acb_lm_retire',
-                 'acb_lm_admit_prefix', 'acb_lm_begin_slots_paged', 'acb_lm_admit_paged', 'acb_lm_admit_prompt'):
+                 'acb_lm_admit_prefix', 'acb_lm_begin_slots_paged', 'acb_lm_admit_paged', 'acb_lm_admit_prompt',
+                 'acb_lm_begin_slots_paged_fp8'):
         getattr(L, name).restype = ci
     _lib = L
     return L
@@ -140,7 +142,7 @@ EXPORTS = ['acb_version', 'acb_last_error', 'acb_device_sm_count', 'acb_weight_n
            'acb_t5_workspace_bytes', 'acb_t5_encode', 'acb_groupnorm_workspace_bytes', 'acb_groupnorm_stats',
            'acb_groupnorm_apply', 'acb_overlap_add', 'acb_lstm_recurrent_carry', 'acb_lm_begin_slots', 'acb_lm_admit',
            'acb_lm_slot_status', 'acb_lm_retire', 'acb_lm_admit_prefix', 'acb_lm_begin_slots_paged', 'acb_lm_admit_paged',
-           'acb_lm_admit_prompt']
+           'acb_lm_admit_prompt', 'acb_lm_begin_slots_paged_fp8']
 
 
 def check(rc: int, what: str = ''):

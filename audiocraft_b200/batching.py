@@ -104,17 +104,30 @@ def prefix_bound(lm, max_text: int) -> int:
     return chroma.chroma_len + (max_text if 'description' in lm.fuser.fuse2cond.get('prepend', []) else 0)
 
 
-def kv_page_bytes(lm) -> int:
-    """Bytes of one page of a paged session's pool: ACB_LM_KV_PAGE positions of fp16 K and V in every layer."""
-    return _lib.ACB_LM_KV_PAGE * 2 * lm.num_layers * lm.dim * 2
+KV_DTYPES = ('fp16', 'fp8')
 
 
-def kv_pages_for_budget(lm, kv_cache_gb: float) -> int:
-    """The pages a budget of kv_cache_gb * 1e9 bytes holds: floor(kv_cache_gb * 1e9 / kv_page_bytes(lm))."""
+def check_kv_dtype(kv_dtype) -> str:
+    if kv_dtype not in KV_DTYPES:
+        raise ValueError(f"the KV cache dtype must be one of {KV_DTYPES}, got {kv_dtype!r}")
+    return kv_dtype
+
+
+def kv_page_bytes(lm, kv_dtype: str = 'fp16') -> int:
+    """Bytes of one page of a paged session's pool: ACB_LM_KV_PAGE positions of K and V in every layer, fp16
+    (64 L 4 d) or 'fp8': e4m3 codes and one fp32 scale per position and head (64 L (2 d + 8 H))."""
+    page, L, d = _lib.ACB_LM_KV_PAGE, lm.num_layers, lm.dim
+    if check_kv_dtype(kv_dtype) == 'fp8':
+        return page * L * (2 * d + 8 * lm.num_heads)
+    return page * 2 * L * d * 2
+
+
+def kv_pages_for_budget(lm, kv_cache_gb: float, kv_dtype: str = 'fp16') -> int:
+    """The pages a budget of kv_cache_gb * 1e9 bytes holds: floor(kv_cache_gb * 1e9 / kv_page_bytes(lm, kv_dtype))."""
     if isinstance(kv_cache_gb, bool) or not isinstance(kv_cache_gb, (int, float)) or not (
             math.isfinite(kv_cache_gb) and kv_cache_gb > 0):
         raise ValueError(f"kv_cache_gb must be a finite number > 0, got {kv_cache_gb!r}")
-    return int(math.floor(kv_cache_gb * 1e9 / kv_page_bytes(lm)))
+    return int(math.floor(kv_cache_gb * 1e9 / kv_page_bytes(lm, kv_dtype)))
 
 
 class PagePool:
@@ -224,13 +237,21 @@ class SlotSession:
     admission takes a request's pages, `collect` and `retire` return them.  Refused (ValueError, before any device work)
     when the pool cannot hold one request of the longest sequence with max_prefix.  Besides the pool the session allocates
     the cross-attention K/V for 2 * slots x max_text positions, a staging cache of 2 x max_prefix positions for admitting a
-    prefix, and the activation and split-K buffers of 2 * slots rows."""
+    prefix, and the activation and split-K buffers of 2 * slots rows.
+
+    `kv_dtype='fp8'` (paged sessions only; ValueError otherwise, before any device work): the pool holds each K or V vector
+    of 64 values as e4m3 codes (`k_pool` / `v_pool`, torch.float8_e4m3fn) and one fp32 scale (`k_scale` / `v_scale`
+    [L, kv_pages, H, ACB_LM_KV_PAGE]), acb_lm_begin_slots_paged_fp8.  Quantization is local to one row and position, so a
+    request's result is that of the same request alone in an fp8 session, but no longer that of an fp16 session."""
 
     def __init__(self, lm, slots: int, max_gen_len: int, max_text: int = 64, use_sampling: bool = True, temp: float = 1.0,
                  top_k: int = 250, top_p: float = 0.0, cfg_coef: tp.Optional[float] = None,
-                 max_prefix: tp.Optional[int] = None, kv_pages: tp.Optional[int] = None):
+                 max_prefix: tp.Optional[int] = None, kv_pages: tp.Optional[int] = None, kv_dtype: str = 'fp16'):
         if not 1 <= slots <= _lib.ACB_LM_MAX_SLOTS:
             raise ValueError(f"slots must be in [1, {_lib.ACB_LM_MAX_SLOTS}], got {slots}")
+        self.kv_dtype = check_kv_dtype(kv_dtype)
+        if kv_dtype == 'fp8' and kv_pages is None:
+            raise ValueError("kv_dtype='fp8' is built for paged sessions only: pass kv_pages")
         if max_gen_len < 1 or max_text < 1:
             raise ValueError("max_gen_len and max_text must be >= 1")
         if not lm.has_prefix and max_prefix:
@@ -269,15 +290,25 @@ class SlotSession:
                 L, H, page, f16 = lm.num_layers, lm.num_heads, _lib.ACB_LM_KV_PAGE, torch.float16
                 per_row = PagePool.need(max_prefix + self.seq_len_max) // 2
                 # never read before written: a slot reads only the positions it has appended or had scattered in
-                self.k_pool = torch.empty((L, kv_pages, H, page, 64), device=lm.device, dtype=f16)
-                self.v_pool = torch.empty((L, kv_pages, H, page, 64), device=lm.device, dtype=f16)
+                code = torch.float8_e4m3fn if kv_dtype == 'fp8' else f16
+                self.k_pool = torch.empty((L, kv_pages, H, page, 64), device=lm.device, dtype=code)
+                self.v_pool = torch.empty((L, kv_pages, H, page, 64), device=lm.device, dtype=code)
                 self.page_table = torch.zeros((2 * slots, per_row), device=lm.device, dtype=torch.int32)
                 self._stage = [torch.empty((L, 2, H, max_prefix, 64), device=lm.device, dtype=f16) if max_prefix else None
                                for _ in range(2)]
-                _lib.check(lm._lib.acb_lm_begin_slots_paged(
-                    lm._handle, slots, max_text, self.seq_len_max, max_prefix, _lib.ptr(self.k_pool), _lib.ptr(self.v_pool),
-                    kv_pages, _lib.ptr(self.page_table), per_row, _lib.ptr(self._stage[0]), _lib.ptr(self._stage[1]),
-                    C.byref(samp), _lib.stream()), 'lm_begin_slots_paged')
+                if kv_dtype == 'fp8':
+                    self.k_scale = torch.empty((L, kv_pages, H, page), device=lm.device, dtype=torch.float32)
+                    self.v_scale = torch.empty((L, kv_pages, H, page), device=lm.device, dtype=torch.float32)
+                    _lib.check(lm._lib.acb_lm_begin_slots_paged_fp8(
+                        lm._handle, slots, max_text, self.seq_len_max, max_prefix, _lib.ptr(self.k_pool),
+                        _lib.ptr(self.v_pool), _lib.ptr(self.k_scale), _lib.ptr(self.v_scale), kv_pages,
+                        _lib.ptr(self.page_table), per_row, _lib.ptr(self._stage[0]), _lib.ptr(self._stage[1]),
+                        C.byref(samp), _lib.stream()), 'lm_begin_slots_paged_fp8')
+                else:
+                    _lib.check(lm._lib.acb_lm_begin_slots_paged(
+                        lm._handle, slots, max_text, self.seq_len_max, max_prefix, _lib.ptr(self.k_pool),
+                        _lib.ptr(self.v_pool), kv_pages, _lib.ptr(self.page_table), per_row, _lib.ptr(self._stage[0]),
+                        _lib.ptr(self._stage[1]), C.byref(samp), _lib.stream()), 'lm_begin_slots_paged')
             lm.launches_per_step = lm._lib.acb_lm_launches_per_step(lm._handle)
             lm._session = self
             self._status = torch.zeros((slots, 2), device=lm.device, dtype=torch.int32)
@@ -652,6 +683,11 @@ class ContinuousGenerator:
     waits in FIFO order until a slot and its pages are free.  Refused before any device work: kv_cache_gb <= 0, and a budget
     that cannot hold one request of max_duration (ValueError).  Results are those of the session without kv_cache_gb.
 
+    With `kv_cache_dtype='fp8'` (default 'fp16'; needs kv_cache_gb) the pool holds e4m3 codes and one fp32 scale per
+    position and head (`SlotSession(kv_dtype='fp8')`), so the same budget holds about 1.88x the pages.  Results then equal
+    the same request alone in an fp8 session, not `generate` or the fp16 session.  Refused before any device work: another
+    kv_cache_dtype, and 'fp8' without kv_cache_gb (ValueError).
+
     With `prefill_prompts`, a request's results are those of `generate`'s default path instead of ``ACB_LM_PREFILL=0``: its
     prompt columns [0, first) (first as `LMModel.generate` computes it, `prefill_columns`) are prefilled into its slot at
     admission (acb_lm_admit_prompt), in the passes `generate` runs for it alone, and the slot decodes from column `first`.
@@ -669,12 +705,16 @@ class ContinuousGenerator:
     prompt, and a description longer than max_text text positions (ValueError)."""
 
     prefill_prompts = False
+    DECODE_GROUP = 32   # requests per codec call in poll()
 
     def __init__(self, model, slots: int = 32, poll_steps: tp.Optional[int] = None, max_text: int = 64,
                  return_tokens: bool = False, chunk_duration: tp.Optional[float] = None,
-                 kv_cache_gb: tp.Optional[float] = None, prefill_prompts: bool = False):
+                 kv_cache_gb: tp.Optional[float] = None, prefill_prompts: bool = False, kv_cache_dtype: str = 'fp16'):
         params = dict(model.generation_params)
-        kv_pages = None if kv_cache_gb is None else kv_pages_for_budget(model.lm, kv_cache_gb)
+        check_kv_dtype(kv_cache_dtype)
+        if kv_cache_dtype == 'fp8' and kv_cache_gb is None:
+            raise ValueError("kv_cache_dtype='fp8' is built for the paged KV cache only: pass kv_cache_gb")
+        kv_pages = None if kv_cache_gb is None else kv_pages_for_budget(model.lm, kv_cache_gb, kv_cache_dtype)
         if getattr(model, '_has_melody', False) != model.lm.has_prefix:
             raise NotImplementedError("continuous batching takes a melody ('self_wav') conditioner only as a condition prefix "
                                       "(prepend fuser), and a condition prefix only from one")
@@ -694,7 +734,8 @@ class ContinuousGenerator:
         self.defaults = dict(use_sampling=params['use_sampling'], temp=params['temp'], top_k=params['top_k'],
                              top_p=params['top_p'], cfg_coef=params['cfg_coef'])
         max_gen_len = int(model.max_duration * model.frame_rate)
-        self.session = SlotSession(model.lm, slots, max_gen_len, max_text, **self.defaults, kv_pages=kv_pages)
+        self.session = SlotSession(model.lm, slots, max_gen_len, max_text, **self.defaults, kv_pages=kv_pages,
+                                   kv_dtype=kv_cache_dtype)
         self.scheduler = ContinuousScheduler(self.session, slots, poll_steps)
         self.stream = None
         if chunk_duration is not None:
@@ -815,11 +856,15 @@ class ContinuousGenerator:
         by_len: tp.Dict[int, tp.List[tp.Tuple[Request, torch.Tensor]]] = collections.defaultdict(list)
         for req, tokens in done:
             by_len[tokens.shape[-1]].append((req, tokens))
-        for group in by_len.values():   # the items that finished together and have one length: one codec call
-            tokens = torch.cat([t for _, t in group], dim=0)
-            wav = self.model.generate_audio(tokens)
-            for i, (req, tok) in enumerate(group):
-                out[req.id] = (req.id, wav[i:i + 1], tok) if self.return_tokens else (req.id, wav[i:i + 1])
+        for same_len in by_len.values():   # the items that finished together and have one length: one codec call per
+            # DECODE_GROUP of them, so a wide session whose requests finish together (128 slots of 30 s) does not hold the
+            # codec's activations for all of them at once
+            for g0 in range(0, len(same_len), self.DECODE_GROUP):
+                group = same_len[g0:g0 + self.DECODE_GROUP]
+                tokens = torch.cat([t for _, t in group], dim=0)
+                wav = self.model.generate_audio(tokens)
+                for i, (req, tok) in enumerate(group):
+                    out[req.id] = (req.id, wav[i:i + 1], tok) if self.return_tokens else (req.id, wav[i:i + 1])
         return [out[req.id] for req, _ in done]
 
     def run(self) -> tp.Iterator[tuple]:

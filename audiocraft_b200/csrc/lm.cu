@@ -22,6 +22,7 @@
 #include "tma.cuh"
 #include "wgmma.cuh"
 #include <cooperative_groups.h>
+#include <cuda_fp8.h>
 #include <math.h>
 #include <new>
 #include <vector>
@@ -530,6 +531,80 @@ __global__ void __launch_bounds__(256) lm_qkv_pf_paged_kernel(const float* __res
     }
 }
 
+// ------------------------------------------------------------------------------------------------ FP8 KV pool
+// An FP8 paged session (acb_lm_begin_slots_paged_fp8) keeps each 64-value K or V vector (one position of one head of one
+// layer in one row) as 64 e4m3 codes in the pool [L][n_pages][H][ACB_LM_KV_PAGE][64] (uint8) and one fp32 scale in
+// [L][n_pages][H][ACB_LM_KV_PAGE]; the vector reads back as code * scale.
+struct Fp8Pool { uint8_t* k; uint8_t* v; float* ks; float* vs; };
+
+// Quantize one vector, held by a warp as lane's values x0, x1 at dims 2 lane, 2 lane + 1: amax = max |x|,
+// code = cvt.rn.satfinite.e4m3(x * (448 / amax)), scale = amax / 448 (both divisions correctly rounded, independent of
+// compiler flags); amax == 0 gives zero codes and a zero scale.  codes points at the vector's 64 bytes.
+__device__ __forceinline__ void quant_e4m3_warp(float x0, float x1, uint8_t* __restrict__ codes, float* __restrict__ scale,
+                                                int lane) {
+    const float amax = warp_max(fmaxf(fabsf(x0), fabsf(x1)));
+    __nv_fp8x2_storage_t c = 0;
+    float sc = 0.f;
+    if (amax > 0.f) {
+        const float inv = __fdiv_rn(448.f, amax);
+        c = __nv_cvt_float2_to_fp8x2(make_float2(x0 * inv, x1 * inv), __NV_SATFINITE, __NV_E4M3);
+        sc = __fdiv_rn(amax, 448.f);
+    }
+    reinterpret_cast<__nv_fp8x2_storage_t*>(codes)[lane] = c;
+    if (lane == 0) *scale = sc;
+}
+
+// What qkv_slot_body<true> / lm_qkv_pf_paged_kernel do for one row at cache position pos, into an FP8 pool: q (rotated under
+// rotary positions) to q32 in fp32, and, when `live`, each head's k (rotated) and v quantized into offset pos % page of `page`.
+// The values quantized are the fp32 values the fp16 kernels round with __float2half_rn.  Warp w quantizes vectors
+// w, w + 8, ... of the row's 2 H (K heads, then V heads).
+__device__ __forceinline__ void qkv_fp8_row(const float* __restrict__ src, float* __restrict__ q32, Fp8Pool pool, int d, int H,
+                                            const float* __restrict__ rope_freq, float pos_scale, bool rope, int row, int pos,
+                                            int page, bool live) {
+    for (int n = threadIdx.x; n < d; n += 256) {
+        float v = src[n];
+        if (rope) v = rope_rotate(rope_freq, pos_scale, half_round(v), half_round(src[n ^ 1]), n & 63, pos);
+        q32[(size_t)row * d + n] = v;
+    }
+    if (!live) return;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int vec = warp; vec < 2 * H; vec += 8) {   // warp-uniform
+        const int which = vec >= H, h = vec - which * H, i = 2 * lane;
+        const float* s = src + (size_t)(1 + which) * d + h * 64;
+        float x0 = s[i], x1 = s[i + 1];
+        if (rope && !which) {
+            const float a = half_round(x0), b = half_round(x1);
+            x0 = rope_rotate(rope_freq, pos_scale, a, b, i, pos);
+            x1 = rope_rotate(rope_freq, pos_scale, b, a, i + 1, pos);
+        }
+        const size_t at = ((size_t)page * H + h) * ACB_LM_KV_PAGE + pos % ACB_LM_KV_PAGE;
+        quant_e4m3_warp(x0, x1, (which ? pool.v : pool.k) + at * 64, (which ? pool.vs : pool.ks) + at, lane);
+    }
+}
+
+// lm_qkv_slot_paged_kernel into an FP8 pool (one layer's codes and scales in `pool`).
+__global__ void __launch_bounds__(256) lm_qkv_slot_paged_fp8_kernel(const float* __restrict__ qkv, const int* __restrict__ slot_state,
+                                                                    float* __restrict__ q32, Fp8Pool pool, int d, int H, int slots,
+                                                                    const float* __restrict__ rope_freq, float pos_scale, bool rope,
+                                                                    const int* __restrict__ table, int pages_per_row) {
+    const int row = blockIdx.x, s = row % slots;
+    const int pos = slot_state[s * ACB_LM_SLOT_STRIDE + ACB_SLOT_PREFIX] + slot_state[s * ACB_LM_SLOT_STRIDE + ACB_SLOT_POS];
+    const bool live = slot_state[s * ACB_LM_SLOT_STRIDE + ACB_SLOT_STATUS] == SLOT_ACTIVE;
+    const int page = live ? table[row * pages_per_row + pos / ACB_LM_KV_PAGE] : 0;
+    qkv_fp8_row(qkv + (size_t)row * 3 * d, q32, pool, d, H, rope_freq, pos_scale, rope, row, pos, page, live);
+}
+
+// lm_qkv_pf_paged_kernel into an FP8 pool.
+__global__ void __launch_bounds__(256) lm_qkv_pf_paged_fp8_kernel(const float* __restrict__ qkv, const int* __restrict__ P,
+                                                                  float* __restrict__ q32, Fp8Pool pool, int d, int H, int rows_real,
+                                                                  const float* __restrict__ rope_freq, float pos_scale, bool rope,
+                                                                  const int* __restrict__ table, int pages_per_row, int r0,
+                                                                  int row_stride) {
+    const int row = blockIdx.x, tk = row / rows_real, j = row - tk * rows_real, pos = P[0] + tk;
+    const int page = table[(r0 + j * row_stride) * pages_per_row + pos / ACB_LM_KV_PAGE];
+    qkv_fp8_row(qkv + (size_t)row * 3 * d, q32, pool, d, H, rope_freq, pos_scale, rope, row, pos, page, true);
+}
+
 // ------------------------------------------------------------------------------------------------ attention (1 query)
 struct AttnParams {
     const float* q; int q_nsplit; size_t q_split_stride;  // q[s][row][d] fp32 partial sums
@@ -1024,6 +1099,158 @@ __global__ void __launch_bounds__(ATT_WARPS * 32) lm_attn2_pf_paged_kernel(AttnP
     }
 }
 
+// Self attention over an FP8 pool: lm_attn2_slot_paged_kernel's CTA (query row, head), online softmax and cp.async ring, with
+// a lane's 16-byte copy holding 16 e4m3 codes: 4 lanes share a position (16 dims each), a warp instruction covers 8
+// consecutive positions (a page holds whole groups of 8, so no copy crosses a page), and iteration k of a warp covers
+// positions (k * 8 + warp) * 8 + pg.  Lanes 0 and 1 of a position also copy its K and V scale into the stage.  Each lane
+// dots its 16 codes (exact in fp16) with q in an fp32 FMA chain, the 4 lanes add in a 2-level shuffle tree, and the sum is
+// multiplied by the K scale; the V scale multiplies the softmax weight before it scales the codes.  Queries attend to
+// positions [0, n) of page-table row trow.
+constexpr int ATT2F8_STAGE = 1024 + 64;   // per warp and stage: K codes, V codes [32 lanes][16 B], scales [8 positions][K, V]
+constexpr int ATT2F8_SMEM = ATT_WARPS * ATT2_DEPTH * ATT2F8_STAGE;
+__device__ __forceinline__ void attn2_paged_fp8_body(const AttnParams& p, const Fp8Pool& pool, const int* __restrict__ table,
+                                                     int pages_per_row, int qrow, int trow, int n) {
+    extern __shared__ __align__(16) unsigned char att2sm[];   // [warp][depth][K | V | scales]
+    __shared__ float wm[ATT_WARPS], wl[ATT_WARPS], wacc[ATT_WARPS][64];
+    __shared__ int pt[ACB_LM_MAX_PAGES_PER_ROW];
+    const int h = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int sl = lane & 3, pg = lane >> 2;
+    for (int i = tid; i < (n + ACB_LM_KV_PAGE - 1) / ACB_LM_KV_PAGE; i += ATT_WARPS * 32) pt[i] = table[trow * pages_per_row + i];
+    __syncthreads();
+    // position pp: codes at (pt[pp / page] * H * page + pp % page) * 64 + base, scales at the same index / 64 + h * page
+    const uint8_t* kb = pool.k + (size_t)h * ACB_LM_KV_PAGE * 64 + sl * 16;
+    const uint8_t* vb = pool.v + (size_t)h * ACB_LM_KV_PAGE * 64 + sl * 16;
+    const float* sb = (sl ? pool.vs : pool.ks) + (size_t)h * ACB_LM_KV_PAGE;
+    const uint32_t ring = smem_u32(att2sm) + (uint32_t)(warp * ATT2_DEPTH * ATT2F8_STAGE);
+    const int n_it = n > warp * 8 ? (n - warp * 8 + 63) / 64 : 0;   // iterations with at least one live position group
+    auto issue = [&](int k) {
+        if (k < n_it) {
+            const int pp = (k * ATT_WARPS + warp) * 8 + pg;
+            if (pp < n) {
+                const uint32_t st = ring + (uint32_t)((k % ATT2_DEPTH) * ATT2F8_STAGE);
+                const size_t o = (size_t)pt[pp / ACB_LM_KV_PAGE] * p.H * ACB_LM_KV_PAGE + pp % ACB_LM_KV_PAGE;
+                asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(st + lane * 16), "l"(kb + o * 64) : "memory");
+                asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(st + 512u + lane * 16), "l"(vb + o * 64) : "memory");
+                if (sl < 2)
+                    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(st + 1024u + pg * 8 + sl * 4), "l"(sb + o)
+                                 : "memory");
+            }
+        }
+        asm volatile("cp.async.commit_group;" ::: "memory");
+    };
+#pragma unroll
+    for (int k = 0; k < ATT2_DEPTH - 1; ++k) issue(k);
+
+    float q[16];
+    {
+        const float4* qp = reinterpret_cast<const float4*>(p.q + (size_t)qrow * p.d + h * 64 + sl * 16);
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+            const float4 a = qp[c];
+            q[4 * c] = half_round(a.x) * p.scale; q[4 * c + 1] = half_round(a.y) * p.scale;
+            q[4 * c + 2] = half_round(a.z) * p.scale; q[4 * c + 3] = half_round(a.w) * p.scale;
+        }
+    }
+    float m = -INFINITY, l = 0.f, acc[16];
+#pragma unroll
+    for (int e = 0; e < 16; ++e) acc[e] = 0.f;
+
+    for (int k = 0; k < n_it; ++k) {                 // warp-uniform trip count (the shuffles need all 32 lanes)
+        __syncwarp();                                // every lane has read stage k - 1 before issue() refills it
+        issue(k + ATT2_DEPTH - 1);
+        asm volatile("cp.async.wait_group %0;" ::"n"(ATT2_DEPTH - 1) : "memory");   // iteration k's copies of this lane have landed
+        __syncwarp();                                // and the scales lanes 0 / 1 of each position copied are visible
+        const int pp = (k * ATT_WARPS + warp) * 8 + pg;
+        const uint32_t sa = ring + (uint32_t)((k % ATT2_DEPTH) * ATT2F8_STAGE);
+        uint4 kv = make_uint4(0, 0, 0, 0), vv = make_uint4(0, 0, 0, 0);
+        float ksc = 0.f, vsc = 0.f;
+        if (pp < n) {
+            asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(kv.x), "=r"(kv.y), "=r"(kv.z), "=r"(kv.w) : "r"(sa + lane * 16));
+            asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(vv.x), "=r"(vv.y), "=r"(vv.z), "=r"(vv.w)
+                         : "r"(sa + 512u + lane * 16));
+            asm volatile("ld.shared.v2.f32 {%0,%1}, [%2];" : "=f"(ksc), "=f"(vsc) : "r"(sa + 1024u + pg * 8));
+        }
+        const __nv_fp8x2_storage_t* k2 = reinterpret_cast<const __nv_fp8x2_storage_t*>(&kv);
+        float s = 0.f;
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+            const float2 f = __half22float2(__half2(__nv_cvt_fp8x2_to_halfraw2(k2[e], __NV_E4M3)));
+            s = fmaf(q[2 * e], f.x, s);
+            s = fmaf(q[2 * e + 1], f.y, s);
+        }
+        s += __shfl_xor_sync(0xffffffffu, s, 1);
+        s += __shfl_xor_sync(0xffffffffu, s, 2);
+        s *= ksc;
+        if (pp < n) {
+            const float mn = fmaxf(m, s);
+            const float corr = __expf(m - mn);      // exp(-inf) = 0 on the first position
+            const float pw = __expf(s - mn);
+            l = l * corr + pw;
+            const float pv = pw * vsc;
+            const __nv_fp8x2_storage_t* v2 = reinterpret_cast<const __nv_fp8x2_storage_t*>(&vv);
+#pragma unroll
+            for (int e = 0; e < 8; ++e) {
+                const float2 f = __half22float2(__half2(__nv_cvt_fp8x2_to_halfraw2(v2[e], __NV_E4M3)));
+                acc[2 * e] = fmaf(pv, f.x, acc[2 * e] * corr);
+                acc[2 * e + 1] = fmaf(pv, f.y, acc[2 * e + 1] * corr);
+            }
+            m = mn;
+        }
+    }
+    asm volatile("cp.async.wait_group 0;" ::: "memory");
+    // merge the 8 position groups of the warp (xor 4, 8, 16), then the warps
+#pragma unroll
+    for (int o = 4; o <= 16; o <<= 1) {
+        const float m2 = __shfl_xor_sync(0xffffffffu, m, o), l2 = __shfl_xor_sync(0xffffffffu, l, o);
+        const float mn = fmaxf(m, m2);
+        const float ca = m == -INFINITY ? 0.f : __expf(m - mn), cb = m2 == -INFINITY ? 0.f : __expf(m2 - mn);
+        l = l * ca + l2 * cb;
+#pragma unroll
+        for (int e = 0; e < 16; ++e) acc[e] = acc[e] * ca + __shfl_xor_sync(0xffffffffu, acc[e], o) * cb;
+        m = mn;
+    }
+    if (pg == 0) {
+        if (sl == 0) { wm[warp] = m; wl[warp] = l; }
+#pragma unroll
+        for (int e = 0; e < 16; ++e) wacc[warp][sl * 16 + e] = acc[e];
+    }
+    __syncthreads();
+    if (tid < 64) {
+        float mx = wm[0];
+#pragma unroll
+        for (int w = 1; w < ATT_WARPS; ++w) mx = fmaxf(mx, wm[w]);
+        float lt = 0.f, o = 0.f;
+#pragma unroll
+        for (int w = 0; w < ATT_WARPS; ++w) {
+            const float cw = wm[w] == -INFINITY ? 0.f : __expf(wm[w] - mx);
+            lt = fmaf(wl[w], cw, lt);
+            o = fmaf(wacc[w][tid], cw, o);
+        }
+        p.out[(size_t)qrow * p.d + h * 64 + tid] = __float2half_rn(o / lt);
+    }
+}
+
+// lm_attn2_slot_paged_kernel over an FP8 pool (one layer's codes and scales in `pool`).
+__global__ void __launch_bounds__(ATT_WARPS * 32) lm_attn2_slot_paged_fp8_kernel(AttnParams p, Fp8Pool pool,
+                                                                              const int* __restrict__ slot_state,
+                                                                              const int* __restrict__ table, int pages_per_row) {
+    const int qrow = blockIdx.y;
+    const int* slot = slot_state + (qrow % p.rows_real) * ACB_LM_SLOT_STRIDE;
+    if (slot[ACB_SLOT_STATUS] != SLOT_ACTIVE) {   // block-uniform
+        if (threadIdx.x < 64) p.out[(size_t)qrow * p.d + blockIdx.x * 64 + threadIdx.x] = __float2half_rn(0.f);
+        return;
+    }
+    attn2_paged_fp8_body(p, pool, table, pages_per_row, qrow, qrow, slot[ACB_SLOT_PREFIX] + slot[ACB_SLOT_POS] + 1);
+}
+
+// lm_attn2_pf_paged_kernel over an FP8 pool.
+__global__ void __launch_bounds__(ATT_WARPS * 32) lm_attn2_pf_paged_fp8_kernel(AttnParams p, Fp8Pool pool,
+                                                                            const int* __restrict__ table, int pages_per_row,
+                                                                            int r0) {
+    const int qrow = blockIdx.y, tok = qrow / p.rows_real;
+    attn2_paged_fp8_body(p, pool, table, pages_per_row, qrow, r0 + (qrow - tok * p.rows_real) * p.row_stride, p.pos[0] + tok + 1);
+}
+
 // Cross attention over the (short) text condition: one WARP per (row, head), lane = text position for the scores,
 // lane = 2 output dims for the weighted sum.  K/V were computed once per generate() (acb_lm_begin).
 // The warp's query row `row`, head h attends to the first n >= 1 text positions of cache row `crow`.
@@ -1405,6 +1632,28 @@ __global__ void lm_prefix_scatter_kernel(const __half* __restrict__ sk, const __
     *reinterpret_cast<uint4*>(pv + dst) = *reinterpret_cast<const uint4*>(sv + src);
 }
 
+// lm_prefix_scatter_kernel into an FP8 pool (pool: layer 0's codes and scales; pool_layer: elements of one layer's scales):
+// one warp per staged fp16 vector (K or V of one position of one head of one layer in one row), quantized as the step
+// quantizes its own.
+__global__ void lm_prefix_scatter_fp8_kernel(const __half* __restrict__ sk, const __half* __restrict__ sv, Fp8Pool pool,
+                                             const int* __restrict__ table, int pages_per_row, int r0, int r1, int H,
+                                             int max_prefix, int P, size_t pool_layer, size_t n_vec) {
+    const size_t i = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (i >= n_vec) return;   // warp-uniform
+    size_t t = i;
+    const int which = (int)(t % 2); t /= 2;
+    const int pos = (int)(t % P); t /= P;
+    const int h = (int)(t % H); t /= H;
+    const int j = (int)(t % 2);
+    const size_t l = t / 2;
+    const size_t src = (((l * 2 + j) * H + h) * max_prefix + pos) * 64 + 2 * lane;
+    const float2 x = __half22float2(*reinterpret_cast<const __half2*>((which ? sv : sk) + src));
+    const int page = table[(j ? r1 : r0) * pages_per_row + pos / ACB_LM_KV_PAGE];
+    const size_t at = l * pool_layer + ((size_t)page * H + h) * ACB_LM_KV_PAGE + pos % ACB_LM_KV_PAGE;
+    quant_e4m3_warp(x.x, x.y, (which ? pool.v : pool.k) + at * 64, (which ? pool.vs : pool.ks) + at, lane);
+}
+
 __global__ void lm_f32_to_f16_kernel(const float* __restrict__ src, __half* __restrict__ dst, size_t n_valid, size_t n_total) {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n_total) dst[i] = __float2half_rn(i < n_valid ? src[i] : 0.f);
@@ -1436,6 +1685,10 @@ struct acb_lm {
     int n_pages = 0, pages_per_row = 0, max_prefix = 0;
     int* page_table = nullptr;
     __half* stage_k = nullptr; __half* stage_v = nullptr;
+    // FP8 paged session (acb_lm_begin_slots_paged_fp8): pool_k / pool_v hold e4m3 codes and pool_ks / pool_vs the scales
+    // [L][n_pages][H][ACB_LM_KV_PAGE]
+    bool fp8 = false;
+    float* pool_ks = nullptr; float* pool_vs = nullptr;
     // wide GEMM (max_rows > 64): one map per stacked weight matrix [L * N][K] (encoded by acb_lm_create) and per activation
     // buffer [rows][K] of the current generation (encoded by acb_lm_begin_prefix)
     CUtensorMap wmap[7];
@@ -1641,6 +1894,11 @@ static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_la
     const size_t ckv_layer = (size_t)c.max_rows * H * c.max_text * 64;
     const size_t kv_row0 = lm->paged ? 0 : (size_t)row0 * H * c.max_seq * 64, ckv_row0 = (size_t)row0 * H * c.max_text * 64;
     const float scale = 1.0f / sqrtf(64.f);
+    // an FP8 pool's layer l: kv_layer codes (bytes) and kv_layer / 64 scales per layer
+    auto fp8_layer = [&](int l) {
+        return Fp8Pool{(uint8_t*)lm->pool_k + l * kv_layer, (uint8_t*)lm->pool_v + l * kv_layer,
+                       lm->pool_ks + l * (kv_layer / 64), lm->pool_vs + l * (kv_layer / 64)};
+    };
     int nl = 0, ks = 0;
 
     if (!gemms_only) {
@@ -1702,7 +1960,14 @@ static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_la
                 else ACB_TRY(launch_gemm<EPI_F32>(nt, p, 1, s, ft2));
                 ++nl;
                 DBG("gemm_EPI_F32 (qkv)", l);
-                if (!gemms_only && lm->paged) {
+                if (!gemms_only && lm->fp8) {
+                    lm_qkv_slot_paged_fp8_kernel<<<rows, 256, 0, s>>>(B.part, B.slot_state, B.q32, fp8_layer(l), d, H, lm->slots,
+                                                                      lm->w.rope_freq, c.pos_scale, rope, lm->page_table,
+                                                                      lm->pages_per_row);
+                    ACB_LAUNCH_CHECK();
+                    ++nl;
+                    DBG("lm_qkv_slot_paged_fp8_kernel", l);
+                } else if (!gemms_only && lm->paged) {
                     lm_qkv_slot_paged_kernel<<<rows, 256, 0, s>>>(B.part, B.slot_state, B.q32, p.kc, p.vc, d, H, lm->slots,
                                                                   lm->w.rope_freq, c.pos_scale, rope, lm->page_table,
                                                                   lm->pages_per_row);
@@ -1721,8 +1986,14 @@ static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_la
                 ACB_TRY(launch_gemm<EPI_F32>(nt, p, 1, s, ft2));
                 ++nl;
                 DBG("gemm_EPI_F32 (qkv pass)", l);
-                lm_qkv_pf_paged_kernel<<<rows, 256, 0, s>>>(B.part, B.pos, B.q32, p.kc, p.vc, d, H, rows_real, lm->w.rope_freq,
-                                                            c.pos_scale, rope, lm->page_table, lm->pages_per_row, row0, row_stride);
+                if (lm->fp8)
+                    lm_qkv_pf_paged_fp8_kernel<<<rows, 256, 0, s>>>(B.part, B.pos, B.q32, fp8_layer(l), d, H, rows_real,
+                                                                    lm->w.rope_freq, c.pos_scale, rope, lm->page_table,
+                                                                    lm->pages_per_row, row0, row_stride);
+                else
+                    lm_qkv_pf_paged_kernel<<<rows, 256, 0, s>>>(B.part, B.pos, B.q32, p.kc, p.vc, d, H, rows_real, lm->w.rope_freq,
+                                                                c.pos_scale, rope, lm->page_table, lm->pages_per_row, row0,
+                                                                row_stride);
                 ACB_LAUNCH_CHECK();
                 ++nl;
                 DBG("lm_qkv_pf_paged_kernel", l);
@@ -1738,11 +2009,17 @@ static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_la
         if (!gemms_only) {
             AttnParams a{B.q32, 1, 0, kv_k + l * kv_layer + kv_row0, kv_v + l * kv_layer + kv_row0,
                          (__half*)B.a16, H, d, kv_len, B.pos, 0, scale, rows_real, kv_stride};
-            if (slot_step && lm->paged) {
+            if (slot_step && lm->fp8) {
+                a.rows_real = lm->slots;
+                lm_attn2_slot_paged_fp8_kernel<<<dim3(H, rows), ATT_WARPS * 32, ATT2F8_SMEM, s>>>(a, fp8_layer(l), B.slot_state,
+                                                                                                lm->page_table, lm->pages_per_row);
+            } else if (slot_step && lm->paged) {
                 a.rows_real = lm->slots;
                 lm_attn2_slot_paged_kernel<<<dim3(H, rows), ATT_WARPS * 32, ATT2_SMEM, s>>>(a, B.slot_state, lm->page_table,
                                                                                           lm->pages_per_row);
             } else if (slot_step) { a.rows_real = lm->slots; lm_attn2_slot_kernel<<<dim3(H, rows), ATT_WARPS * 32, ATT2_SMEM, s>>>(a, B.slot_state); }
+            else if (paged_pass && lm->fp8) lm_attn2_pf_paged_fp8_kernel<<<dim3(H, rows), ATT_WARPS * 32, ATT2F8_SMEM, s>>>(
+                    a, fp8_layer(l), lm->page_table, lm->pages_per_row, row0);
             else if (paged_pass) lm_attn2_pf_paged_kernel<<<dim3(H, rows), ATT_WARPS * 32, ATT2_SMEM, s>>>(a, lm->page_table,
                                                                                                       lm->pages_per_row, row0);
             else if (pf) lm_attn2_kernel<true><<<dim3(H, rows), ATT_WARPS * 32, ATT2_SMEM, s>>>(a);
@@ -1871,6 +2148,11 @@ extern "C" int acb_lm_create(const acb_lm_config* cfg, const acb_lm_weights* w, 
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_qkv_slot_paged_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_attn2_pf_paged_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT2_SMEM);
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_attn2_pf_paged_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+    if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_attn2_slot_paged_fp8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT2F8_SMEM);
+    if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_attn2_slot_paged_fp8_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+    if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_qkv_slot_paged_fp8_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+    if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_attn2_pf_paged_fp8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT2F8_SMEM);
+    if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_attn2_pf_paged_fp8_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_sample_slot_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_cross_attn_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_ln_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
@@ -2115,9 +2397,10 @@ extern "C" int acb_lm_begin_slots(acb_lm_t* lm, int slots, int max_text, int seq
     return begin_slots(lm, slots, max_text, seq_len_max, sampling, stream);
 }
 
-extern "C" int acb_lm_begin_slots_paged(acb_lm_t* lm, int slots, int max_text, int seq_len_max, int max_prefix, void* k_pool,
-                                        void* v_pool, int n_pages, int32_t* page_table, int pages_per_row, void* stage_k,
-                                        void* stage_v, const acb_lm_sampling* sampling, void* stream) {
+// acb_lm_begin_slots_paged (k_scale = v_scale = NULL: an fp16 pool) and acb_lm_begin_slots_paged_fp8.
+static int begin_slots_paged(acb_lm_t* lm, int slots, int max_text, int seq_len_max, int max_prefix, void* k_pool, void* v_pool,
+                             float* k_scale, float* v_scale, int n_pages, int32_t* page_table, int pages_per_row, void* stage_k,
+                             void* stage_v, const acb_lm_sampling* sampling, void* stream) {
     ACB_REQUIRE(lm && sampling && k_pool && v_pool && page_table, "acb_lm_begin_slots_paged: null argument");
     ACB_REQUIRE(lm->paged, "acb_lm_begin_slots_paged: the handle was created with a contiguous KV cache (buffers.k_cache)");
     const acb_lm_config& c = lm->cfg;
@@ -2132,7 +2415,24 @@ extern "C" int acb_lm_begin_slots_paged(acb_lm_t* lm, int slots, int max_text, i
     lm->pool_k = (__half*)k_pool; lm->pool_v = (__half*)v_pool; lm->n_pages = n_pages;
     lm->page_table = page_table; lm->pages_per_row = pages_per_row;
     lm->stage_k = (__half*)stage_k; lm->stage_v = (__half*)stage_v; lm->max_prefix = max_prefix;
+    lm->fp8 = k_scale != nullptr; lm->pool_ks = k_scale; lm->pool_vs = v_scale;
     return begin_slots(lm, slots, max_text, seq_len_max, sampling, stream);
+}
+
+extern "C" int acb_lm_begin_slots_paged(acb_lm_t* lm, int slots, int max_text, int seq_len_max, int max_prefix, void* k_pool,
+                                        void* v_pool, int n_pages, int32_t* page_table, int pages_per_row, void* stage_k,
+                                        void* stage_v, const acb_lm_sampling* sampling, void* stream) {
+    return begin_slots_paged(lm, slots, max_text, seq_len_max, max_prefix, k_pool, v_pool, nullptr, nullptr, n_pages, page_table,
+                             pages_per_row, stage_k, stage_v, sampling, stream);
+}
+
+extern "C" int acb_lm_begin_slots_paged_fp8(acb_lm_t* lm, int slots, int max_text, int seq_len_max, int max_prefix,
+                                            void* k_pool, void* v_pool, float* k_scale, float* v_scale, int n_pages,
+                                            int32_t* page_table, int pages_per_row, void* stage_k, void* stage_v,
+                                            const acb_lm_sampling* sampling, void* stream) {
+    ACB_REQUIRE(k_scale && v_scale, "acb_lm_begin_slots_paged_fp8: null scale pool");
+    return begin_slots_paged(lm, slots, max_text, seq_len_max, max_prefix, k_pool, v_pool, k_scale, v_scale, n_pages, page_table,
+                             pages_per_row, stage_k, stage_v, sampling, stream);
 }
 
 extern "C" int acb_lm_admit(acb_lm_t* lm, int slot, const float* cross, int text_len, int seq_len, uint64_t seed,
@@ -2226,7 +2526,14 @@ static int admit(acb_lm_t* lm, int slot, const float* cross, int text_len, const
         lm->pf_slot = -1; lm->pf_text_len = 0;
         lm->prefix = nullptr; lm->prefix_len = 0;   // the session's step reads column = position (its sampler's seq_off is 0)
         ACB_TRY(rc);
-        if (lm->paged) {   // the passes ran into the staging cache: copy it into the slot's pages
+        if (lm->fp8) {   // the passes ran into the fp16 staging cache: quantize it into the slot's pages
+            const size_t n_vec = (size_t)c.num_layers * 2 * c.num_heads * prefix_len * 2;
+            lm_prefix_scatter_fp8_kernel<<<(unsigned)((n_vec * 32 + 255) / 256), 256, 0, s>>>(
+                lm->stage_k, lm->stage_v, Fp8Pool{(uint8_t*)lm->pool_k, (uint8_t*)lm->pool_v, lm->pool_ks, lm->pool_vs},
+                lm->page_table, lm->pages_per_row, slot, lm->slots + slot, c.num_heads, lm->max_prefix, prefix_len,
+                (size_t)lm->n_pages * c.num_heads * ACB_LM_KV_PAGE, n_vec);
+            ACB_LAUNCH_CHECK();
+        } else if (lm->paged) {   // the passes ran into the staging cache: copy it into the slot's pages
             const size_t total = (size_t)c.num_layers * 2 * c.num_heads * prefix_len * 8;
             lm_prefix_scatter_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(
                 lm->stage_k, lm->stage_v, lm->pool_k, lm->pool_v, lm->page_table, lm->pages_per_row, slot, lm->slots + slot,

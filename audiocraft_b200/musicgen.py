@@ -244,7 +244,7 @@ class BaseGenModel:
     # -- continuous batching
     def continuous(self, slots: int = 32, poll_steps: tp.Optional[int] = None, max_text: int = 64,
                    return_tokens: bool = False, chunk_duration: tp.Optional[float] = None,
-                   kv_cache_gb: tp.Optional[float] = None, prefill_prompts: bool = False):
+                   kv_cache_gb: tp.Optional[float] = None, prefill_prompts: bool = False, kv_cache_dtype: str = 'fp16'):
         """A `batching.ContinuousGenerator` over this model: up to `slots` requests decode side by side, each admitted when a
         slot frees and retired when its last frame is sampled.  `submit(description, duration, prompt, prompt_sample_rate,
         use_sampling=, top_k=, top_p=, temperature=, cfg_coef=)` returns a request id (options left out take the current
@@ -267,10 +267,22 @@ class BaseGenModel:
         `generate` with ACB_LM_PREFILL=0) prefills each request's prompt into its slot at admission, as `generate` prefills
         it, so results equal `generate`'s default path; it also serves durations beyond max_duration window by window, as
         `generate` does (not with chunk_duration).  The passes stall every slot while they run: it lowers a prompted
-        request's latency and can cost throughput in a busy session (see `batching.ContinuousGenerator`)."""
+        request's latency and can cost throughput in a busy session (see `batching.ContinuousGenerator`).
+
+        `kv_cache_dtype='fp8'` (with kv_cache_gb only) stores the paged self-attention cache in FP8: each K or V vector of
+        64 values (one position of one head of one layer in one row) is 64 e4m3 codes plus one fp32 scale, page_bytes =
+        64 x num_layers x (2 dim + 8 num_heads), about 1.88x the pages of an fp16 pool in the same budget.  A vector x, the
+        fp32 value the fp16 cache rounds to fp16 (after rotary positions for K), is stored as amax = max |x_j|, code_j =
+        e4m3(x_j * (448 / amax)) rounded to nearest even and saturated at +-448, scale = amax / 448 (both divisions
+        correctly rounded; amax = 0 stores zeros), and every read of the cache sees code x scale.  Decode steps and prompt
+        prefill quantize their own K/V; a melody prefix is prefilled into an fp16 staging cache, then quantized into the
+        request's pages.  Cross-attention K/V, queries, activations and weights stay as they are.  Results then differ from
+        `generate` and from the fp16 session; since quantization is local to one row and position, each request's result
+        still equals that request alone in an fp8 session.  Refused before any device work (ValueError): any other
+        kv_cache_dtype, and 'fp8' without kv_cache_gb."""
         from .batching import ContinuousGenerator
         return ContinuousGenerator(self, slots, poll_steps, max_text, return_tokens, chunk_duration, kv_cache_gb,
-                                   prefill_prompts)
+                                   prefill_prompts, kv_cache_dtype)
 
 
 def _sampling_params(use_sampling, top_k, top_p, temperature, cfg_coef, two_step_cfg):

@@ -342,6 +342,21 @@ int acb_lm_begin_slots_paged(acb_lm_t* lm, int slots, int max_text, int seq_len_
                              int n_pages, int32_t* page_table, int pages_per_row, void* stage_k, void* stage_v,
                              const acb_lm_sampling* sampling, void* stream);
 
+/* acb_lm_begin_slots_paged with an FP8 pool: each K or V vector (64 values of one position, head, layer and row) is 64 e4m3
+ * codes (finite variant, max 448) and one fp32 scale, and reads back as code * scale.
+ *   k_pool, v_pool    uint8 [L][n_pages][H][ACB_LM_KV_PAGE][64] e4m3 codes
+ *   k_scale, v_scale  fp32 [L][n_pages][H][ACB_LM_KV_PAGE]
+ * A vector x (the fp32 value the fp16 pool rounds to fp16: after rotary positions for K) is stored as amax = max |x_j|,
+ * code_j = cvt.rn.satfinite.e4m3(x_j * (448 / amax)), scale = amax / 448, both divisions correctly rounded; amax == 0
+ * stores zero codes and a zero scale.  Decode steps and prompt passes quantize their own K / V; a condition prefix still runs
+ * its passes on the fp16 staging cache, whose values admission quantizes into the pages.  Every read of the pool, the
+ * position a step has just appended included, sees code * scale.  The cross-attention K/V and the staging cache stay fp16.
+ * acb_lm_admit_paged, acb_lm_admit_prompt, acb_lm_steps, acb_lm_step_logits and acb_lm_retire serve the session as they
+ * serve an fp16 one.  Everything else is acb_lm_begin_slots_paged. */
+int acb_lm_begin_slots_paged_fp8(acb_lm_t* lm, int slots, int max_text, int seq_len_max, int max_prefix, void* k_pool,
+                                 void* v_pool, float* k_scale, float* v_scale, int n_pages, int32_t* page_table,
+                                 int pages_per_row, void* stage_k, void* stage_v, const acb_lm_sampling* sampling, void* stream);
+
 /* acb_lm_admit_prefix in a paged session: pages [2][n / 2] (host memory) are the page ids of the slot's cond row (slot) and
  * null row (slots + slot), n = 2 * ceil((prefix_len + seq_len) / ACB_LM_KV_PAGE).  The caller gives pages no other live slot
  * holds.  Returns ACB_ERR_INVALID before enqueuing anything when n is not that count, an id is outside [0, n_pages), an id

@@ -457,23 +457,40 @@ __global__ void __launch_bounds__(128, 1) lm_gemm_wide_kernel(const __grid_const
     if (cs > 1) cg::this_cluster().sync();   // the other CTAs read this CTA's tile until here
 }
 
-// Slot mode's QKV epilogue as its own kernel: the QKV GEMM runs with the plain fp32 epilogue (EPI_F32, the same sums as
-// EPI_QKV / EPI_QKV_ROPE) into qkv [rows][3d], and this kernel does what those epilogues do at each row's own position: q to
-// q32 (fp32), k and v to the cache (fp16), q and k rotated first under rotary positions.  Only ACTIVE slots append to the cache.
-// The position is the cache position: the slot's prefix length + its column.
-// PAGED (acb_lm_begin_slots_paged): kc / vc are the layer's page pool [n_pages][H][ACB_LM_KV_PAGE][64], and position pos of
-// row r is offset pos % ACB_LM_KV_PAGE of page table[r][pos / ACB_LM_KV_PAGE]; the values written are the same.
-template <bool PAGED>
-__device__ __forceinline__ void qkv_slot_body(const float* __restrict__ qkv, const int* __restrict__ slot_state,
-                                              float* __restrict__ q32, __half* __restrict__ kc, __half* __restrict__ vc, int d,
-                                              int H, int cache_len, int slots, const float* __restrict__ rope_freq, float pos_scale,
-                                              bool rope, const int* __restrict__ table, int pages_per_row) {
-    const int row = blockIdx.x, s = row % slots;
-    const int pos = slot_state[s * ACB_LM_SLOT_STRIDE + ACB_SLOT_PREFIX] + slot_state[s * ACB_LM_SLOT_STRIDE + ACB_SLOT_POS];
-    const bool live = slot_state[s * ACB_LM_SLOT_STRIDE + ACB_SLOT_STATUS] == SLOT_ACTIVE;
-    int page = 0;
-    if constexpr (PAGED) page = live ? table[row * pages_per_row + pos / ACB_LM_KV_PAGE] : 0;   // a slot not decoding owns no page
-    const float* src = qkv + (size_t)row * 3 * d;
+// Which cache position a row of a decode step or of a prompt pass appends at (and attends up to), shared by the fp16 and FP8
+// QKV and attention kernels.
+// Decode step (slot mode): row `row` belongs to slot row % slots and is at its cache position prefix + column.  Only the rows
+// of an ACTIVE slot append or attend, and only they look their page up in `table` (a paged cache; null for a contiguous
+// one or where the caller stages the whole table row): a slot not decoding owns no page.
+struct SlotRow { int pos, page; bool live; };
+__device__ __forceinline__ SlotRow slot_row(const int* __restrict__ slot_state, int slots, int row, const int* __restrict__ table,
+                                            int pages_per_row) {
+    const int* slot = slot_state + (row % slots) * ACB_LM_SLOT_STRIDE;
+    SlotRow r;
+    r.pos = slot[ACB_SLOT_PREFIX] + slot[ACB_SLOT_POS];
+    r.live = slot[ACB_SLOT_STATUS] == SLOT_ACTIVE;
+    r.page = r.live && table ? table[row * pages_per_row + r.pos / ACB_LM_KV_PAGE] : 0;
+    return r;
+}
+
+// Prompt pass in a paged session (acb_lm_admit_prompt): GEMM row `row` is position P[0] + row / rows_real of generation row
+// j = row % rows_real, whose page-table row is r0 + j * row_stride.
+struct PassRow { int pos, trow; };
+__device__ __forceinline__ PassRow pass_row(const int* __restrict__ P, int row, int rows_real, int r0, int row_stride) {
+    const int tk = row / rows_real;
+    return {P[0] + tk, r0 + (row - tk * rows_real) * row_stride};
+}
+
+// Slot mode's QKV epilogue and the paged prompt pass's, as kernels of their own: the QKV GEMM runs with the plain fp32
+// epilogue (EPI_F32, the same sums as EPI_QKV / EPI_QKV_ROPE / EPI_QKV_PF*) into qkv [rows][3d], and these kernels do what
+// those epilogues do at each row's own cache position pos: q to q32 (fp32), k and v to the cache (fp16), q and k rotated
+// first under rotary positions, so q, k and v are bit-identical to the epilogues'.
+// One row: k and v go to the cache only when `live`, each head's vector at ((x * H + head) * len + at) * 64, with x = row,
+// len = cache_len, at = pos in a contiguous cache [rows][H][cache_len][64], and x = the page holding pos, len =
+// ACB_LM_KV_PAGE, at = pos % ACB_LM_KV_PAGE in a page pool [n_pages][H][ACB_LM_KV_PAGE][64].
+__device__ __forceinline__ void qkv_f16_row(const float* __restrict__ src, float* __restrict__ q32, __half* __restrict__ kc,
+                                            __half* __restrict__ vc, int d, int H, const float* __restrict__ rope_freq,
+                                            float pos_scale, bool rope, int row, int pos, int x, int len, int at, bool live) {
     for (int n = threadIdx.x; n < 3 * d; n += 256) {
         const int which = n >= 2 * d ? 2 : (n >= d ? 1 : 0), nn = n - which * d;
         float v = src[n];
@@ -482,10 +499,7 @@ __device__ __forceinline__ void qkv_slot_body(const float* __restrict__ qkv, con
             q32[(size_t)row * d + nn] = v;
         } else if (live) {
             __half* cache = which == 2 ? vc : kc;
-            if constexpr (PAGED)
-                cache[(((size_t)page * H + (nn >> 6)) * ACB_LM_KV_PAGE + pos % ACB_LM_KV_PAGE) * 64 + (nn & 63)] = __float2half_rn(v);
-            else
-                cache[(((size_t)row * H + (nn >> 6)) * cache_len + pos) * 64 + (nn & 63)] = __float2half_rn(v);
+            cache[(((size_t)x * H + (nn >> 6)) * len + at) * 64 + (nn & 63)] = __float2half_rn(v);
         }
     }
 }
@@ -494,41 +508,37 @@ __global__ void __launch_bounds__(256) lm_qkv_slot_kernel(const float* __restric
                                                           float* __restrict__ q32, __half* __restrict__ kc, __half* __restrict__ vc,
                                                           int d, int H, int cache_len, int slots, const float* __restrict__ rope_freq,
                                                           float pos_scale, bool rope) {
-    qkv_slot_body<false>(qkv, slot_state, q32, kc, vc, d, H, cache_len, slots, rope_freq, pos_scale, rope, nullptr, 0);
+    const int row = blockIdx.x;
+    const SlotRow r = slot_row(slot_state, slots, row, nullptr, 0);
+    qkv_f16_row(qkv + (size_t)row * 3 * d, q32, kc, vc, d, H, rope_freq, pos_scale, rope, row, r.pos, row, cache_len, r.pos,
+                r.live);
 }
 
+// Paged session (acb_lm_begin_slots_paged): kc / vc are the layer's page pool.
 __global__ void __launch_bounds__(256) lm_qkv_slot_paged_kernel(const float* __restrict__ qkv, const int* __restrict__ slot_state,
                                                                 float* __restrict__ q32, __half* __restrict__ kc,
                                                                 __half* __restrict__ vc, int d, int H, int slots,
                                                                 const float* __restrict__ rope_freq, float pos_scale, bool rope,
                                                                 const int* __restrict__ table, int pages_per_row) {
-    qkv_slot_body<true>(qkv, slot_state, q32, kc, vc, d, H, 0, slots, rope_freq, pos_scale, rope, table, pages_per_row);
+    const int row = blockIdx.x;
+    const SlotRow r = slot_row(slot_state, slots, row, table, pages_per_row);
+    qkv_f16_row(qkv + (size_t)row * 3 * d, q32, kc, vc, d, H, rope_freq, pos_scale, rope, row, r.pos, r.page, ACB_LM_KV_PAGE,
+                r.pos % ACB_LM_KV_PAGE, r.live);
 }
 
-// Paged admission pass (acb_lm_admit_prompt in a paged session): what the EPI_QKV_PF / EPI_QKV_PF_ROPE epilogue does, after
-// the QKV GEMM's plain fp32 epilogue (qkv [rows][3d]).  GEMM row r is position P[0] + r / rows_real of generation row
-// j = r % rows_real, whose page table row is r0 + j * row_stride; k and v go to offset pos % ACB_LM_KV_PAGE of its page.  The
-// rotary input is the same fp32 sum the epilogue rotates, so q, k and v are bit-identical to a contiguous pass.
+// Paged admission pass (acb_lm_admit_prompt in a paged session): what the EPI_QKV_PF / EPI_QKV_PF_ROPE epilogue does, through
+// the page table.
 __global__ void __launch_bounds__(256) lm_qkv_pf_paged_kernel(const float* __restrict__ qkv, const int* __restrict__ P,
                                                               float* __restrict__ q32, __half* __restrict__ kc,
                                                               __half* __restrict__ vc, int d, int H, int rows_real,
                                                               const float* __restrict__ rope_freq, float pos_scale, bool rope,
                                                               const int* __restrict__ table, int pages_per_row, int r0,
                                                               int row_stride) {
-    const int row = blockIdx.x, tk = row / rows_real, j = row - tk * rows_real, pos = P[0] + tk;
-    const int page = table[(r0 + j * row_stride) * pages_per_row + pos / ACB_LM_KV_PAGE];
-    const float* src = qkv + (size_t)row * 3 * d;
-    for (int n = threadIdx.x; n < 3 * d; n += 256) {
-        const int which = n >= 2 * d ? 2 : (n >= d ? 1 : 0), nn = n - which * d;
-        float v = src[n];
-        if (rope && which < 2) v = rope_rotate(rope_freq, pos_scale, half_round(v), half_round(src[n ^ 1]), nn & 63, pos);
-        if (which == 0) {
-            q32[(size_t)row * d + nn] = v;
-        } else {
-            __half* cache = which == 2 ? vc : kc;
-            cache[(((size_t)page * H + (nn >> 6)) * ACB_LM_KV_PAGE + pos % ACB_LM_KV_PAGE) * 64 + (nn & 63)] = __float2half_rn(v);
-        }
-    }
+    const int row = blockIdx.x;
+    const PassRow r = pass_row(P, row, rows_real, r0, row_stride);
+    const int page = table[r.trow * pages_per_row + r.pos / ACB_LM_KV_PAGE];
+    qkv_f16_row(qkv + (size_t)row * 3 * d, q32, kc, vc, d, H, rope_freq, pos_scale, rope, row, r.pos, page, ACB_LM_KV_PAGE,
+                r.pos % ACB_LM_KV_PAGE, true);
 }
 
 // ------------------------------------------------------------------------------------------------ FP8 KV pool
@@ -554,10 +564,10 @@ __device__ __forceinline__ void quant_e4m3_warp(float x0, float x1, uint8_t* __r
     if (lane == 0) *scale = sc;
 }
 
-// What qkv_slot_body<true> / lm_qkv_pf_paged_kernel do for one row at cache position pos, into an FP8 pool: q (rotated under
-// rotary positions) to q32 in fp32, and, when `live`, each head's k (rotated) and v quantized into offset pos % page of `page`.
-// The values quantized are the fp32 values the fp16 kernels round with __float2half_rn.  Warp w quantizes vectors
-// w, w + 8, ... of the row's 2 H (K heads, then V heads).
+// qkv_f16_row into an FP8 pool, for one row at cache position pos: q (rotated under rotary positions) to q32 in fp32, and,
+// when `live`, each head's k (rotated) and v quantized into offset pos % page of `page`.  The values quantized are the fp32
+// values the fp16 kernels round with __float2half_rn.  Warp w quantizes vectors w, w + 8, ... of the row's 2 H (K heads,
+// then V heads).
 __device__ __forceinline__ void qkv_fp8_row(const float* __restrict__ src, float* __restrict__ q32, Fp8Pool pool, int d, int H,
                                             const float* __restrict__ rope_freq, float pos_scale, bool rope, int row, int pos,
                                             int page, bool live) {
@@ -587,11 +597,9 @@ __global__ void __launch_bounds__(256) lm_qkv_slot_paged_fp8_kernel(const float*
                                                                     float* __restrict__ q32, Fp8Pool pool, int d, int H, int slots,
                                                                     const float* __restrict__ rope_freq, float pos_scale, bool rope,
                                                                     const int* __restrict__ table, int pages_per_row) {
-    const int row = blockIdx.x, s = row % slots;
-    const int pos = slot_state[s * ACB_LM_SLOT_STRIDE + ACB_SLOT_PREFIX] + slot_state[s * ACB_LM_SLOT_STRIDE + ACB_SLOT_POS];
-    const bool live = slot_state[s * ACB_LM_SLOT_STRIDE + ACB_SLOT_STATUS] == SLOT_ACTIVE;
-    const int page = live ? table[row * pages_per_row + pos / ACB_LM_KV_PAGE] : 0;
-    qkv_fp8_row(qkv + (size_t)row * 3 * d, q32, pool, d, H, rope_freq, pos_scale, rope, row, pos, page, live);
+    const int row = blockIdx.x;
+    const SlotRow r = slot_row(slot_state, slots, row, table, pages_per_row);
+    qkv_fp8_row(qkv + (size_t)row * 3 * d, q32, pool, d, H, rope_freq, pos_scale, rope, row, r.pos, r.page, r.live);
 }
 
 // lm_qkv_pf_paged_kernel into an FP8 pool.
@@ -600,9 +608,10 @@ __global__ void __launch_bounds__(256) lm_qkv_pf_paged_fp8_kernel(const float* _
                                                                   const float* __restrict__ rope_freq, float pos_scale, bool rope,
                                                                   const int* __restrict__ table, int pages_per_row, int r0,
                                                                   int row_stride) {
-    const int row = blockIdx.x, tk = row / rows_real, j = row - tk * rows_real, pos = P[0] + tk;
-    const int page = table[(r0 + j * row_stride) * pages_per_row + pos / ACB_LM_KV_PAGE];
-    qkv_fp8_row(qkv + (size_t)row * 3 * d, q32, pool, d, H, rope_freq, pos_scale, rope, row, pos, page, true);
+    const int row = blockIdx.x;
+    const PassRow r = pass_row(P, row, rows_real, r0, row_stride);
+    const int page = table[r.trow * pages_per_row + r.pos / ACB_LM_KV_PAGE];
+    qkv_fp8_row(qkv + (size_t)row * 3 * d, q32, pool, d, H, rope_freq, pos_scale, rope, row, r.pos, page, true);
 }
 
 // ------------------------------------------------------------------------------------------------ attention (1 query)
@@ -626,498 +635,212 @@ __device__ __forceinline__ void osm_merge(OnlineSM& a, float m2, float l2, const
     a.m = mn;
 }
 
-// Self attention for one query token: CTA = (query row, head), 8 warps, ONE pass over K and V with an online softmax.  A warp
-// instruction covers 4 consecutive cache positions (4 x 128 B = 512 contiguous bytes), 8 lanes share a position (8 dims each).
-// Every lane copies its 16-byte slices of K and V with cp.async into a private slot of a per-warp shared-memory ring,
-// ATT2_DEPTH iterations deep, and reads them back (its own 32 bytes) one iteration at a time: up to 8 x 32 bytes per lane stay
-// outstanding continuously, in shared memory instead of registers.
+// Where position pp of a row's K/V lies, in 64-value vectors from the head's position 0: a contiguous cache row holds its
+// positions in order; a paged row holds position pp at offset pp % ACB_LM_KV_PAGE of page pt[pp / ACB_LM_KV_PAGE], a page
+// being [H][ACB_LM_KV_PAGE] vectors.  A page holds whole groups of the positions one warp instruction covers (4 in fp16,
+// 8 in FP8), so no lane's 16-byte copy crosses a page.
+struct RowAt {
+    __device__ __forceinline__ size_t operator()(int pp) const { return (size_t)pp; }
+};
+struct PagedAt {
+    const int* pt; int H;
+    __device__ __forceinline__ size_t operator()(int pp) const {
+        return (size_t)pt[pp / ACB_LM_KV_PAGE] * H * ACB_LM_KV_PAGE + pp % ACB_LM_KV_PAGE;
+    }
+};
+
+// A paged attention CTA stages the first ceil(n / ACB_LM_KV_PAGE) entries (at most ACB_LM_MAX_PAGES_PER_ROW) of its page-table
+// row trow in shared memory, behind one barrier.
+__device__ __forceinline__ PagedAt stage_pages(const int* __restrict__ table, int pages_per_row, int trow, int n, int H) {
+    __shared__ int pt[ACB_LM_MAX_PAGES_PER_ROW];
+    for (int i = threadIdx.x; i < (n + ACB_LM_KV_PAGE - 1) / ACB_LM_KV_PAGE; i += ATT_WARPS * 32) pt[i] = table[trow * pages_per_row + i];
+    __syncthreads();
+    return {pt, H};
+}
+
+// The rows of a slot that is not ACTIVE attend to no key: the CTA (query row qrow, head blockIdx.x) writes zeros.
+__device__ __forceinline__ void attn2_zero(const AttnParams& p, int qrow) {
+    if (threadIdx.x < 64) p.out[(size_t)qrow * p.d + blockIdx.x * 64 + threadIdx.x] = __float2half_rn(0.f);
+}
+
+// The end of every self-attention CTA: each warp's merged online-softmax state (running max m, sum l, and E output dims per
+// lane at sl * E, held by the lanes with `writer` set) goes to shared memory, and thread t < 64 merges the 8 warps for output
+// dim t of the head, stored at out[t].
+template <int E>
+__device__ __forceinline__ void attn2_merge_store(float m, float l, const float (&acc)[E], bool writer, int sl,
+                                                  __half* __restrict__ out) {
+    __shared__ float wm[ATT_WARPS], wl[ATT_WARPS], wacc[ATT_WARPS][64];
+    const int tid = threadIdx.x, warp = tid >> 5;
+    if (writer) {
+        if (sl == 0) { wm[warp] = m; wl[warp] = l; }
+#pragma unroll
+        for (int e = 0; e < E; ++e) wacc[warp][sl * E + e] = acc[e];
+    }
+    __syncthreads();
+    if (tid < 64) {
+        float mx = wm[0];
+#pragma unroll
+        for (int w = 1; w < ATT_WARPS; ++w) mx = fmaxf(mx, wm[w]);
+        float lt = 0.f, o = 0.f;
+#pragma unroll
+        for (int w = 0; w < ATT_WARPS; ++w) {
+            const float cw = wm[w] == -INFINITY ? 0.f : __expf(wm[w] - mx);
+            lt = fmaf(wl[w], cw, lt);
+            o = fmaf(wacc[w][tid], cw, o);
+        }
+        out[tid] = __float2half_rn(o / lt);
+    }
+}
+
+// Self attention for one query token over an fp16 cache: CTA = (query row, head), 8 warps, ONE pass over K and V with an
+// online softmax.  A warp instruction covers 4 consecutive cache positions (4 x 128 B = 512 contiguous bytes), 8 lanes share
+// a position (8 dims each).  Every lane copies its 16-byte slices of K and V with cp.async into a private slot of a per-warp
+// shared-memory ring, ATT2_DEPTH iterations deep, and reads them back (its own 32 bytes) one iteration at a time: up to
+// 8 x 32 bytes per lane stay outstanding continuously, in shared memory instead of registers.
+// Every instance runs this one body: query row qrow (of p.q and p.out) attends to positions [0, n) of the K/V whose head
+// starts `head` vectors into p.kc / p.vc, position pp at(pp) vectors further (RowAt or PagedAt).  So the sums, and their
+// order, are the same whatever the layout, and a paged session's results are bit-identical to a contiguous one's.
+constexpr int ATT2_DEPTH = 8;
+constexpr int ATT2_SMEM = ATT_WARPS * ATT2_DEPTH * 1024;   // the ring, 64 KB
+template <class At>
+__device__ __forceinline__ void attn2_body(const AttnParams& p, int qrow, int n, size_t head, At at) {
+    extern __shared__ __align__(16) unsigned char att2sm[];   // [warp][depth][K | V][32 lanes][16 B]
+    const int h = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int sl = lane & 7, pg = lane >> 3;
+    const __half* kb = p.kc + (head * 64 + sl * 8);
+    const __half* vb = p.vc + (head * 64 + sl * 8);
+    const uint32_t ring = smem_u32(att2sm) + (uint32_t)(warp * ATT2_DEPTH * 1024 + lane * 16);
+    // iteration k of this warp covers positions (k * 8 + warp) * 4 + pg
+    const int n_it = (n + 31 - warp * 4) / 32 > 0 ? (n - warp * 4 + 31) / 32 : 0;   // iterations with at least one live position group
+    auto issue = [&](int k) {
+        if (k < n_it) {
+            const int pp = (k * ATT_WARPS + warp) * 4 + pg;
+            if (pp < n) {
+                const uint32_t d = ring + (uint32_t)((k % ATT2_DEPTH) * 1024);
+                const size_t o = at(pp) * 64;
+                asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d), "l"(kb + o) : "memory");
+                asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d + 512u), "l"(vb + o) : "memory");
+            }
+        }
+        asm volatile("cp.async.commit_group;" ::: "memory");
+    };
+#pragma unroll
+    for (int k = 0; k < ATT2_DEPTH - 1; ++k) issue(k);
+
+    float q[8];
+    {
+        const float4* qp = reinterpret_cast<const float4*>(p.q + (size_t)qrow * p.d + h * 64 + sl * 8);
+        const float4 qa = qp[0], qb = qp[1];
+        q[0] = half_round(qa.x) * p.scale; q[1] = half_round(qa.y) * p.scale; q[2] = half_round(qa.z) * p.scale;
+        q[3] = half_round(qa.w) * p.scale; q[4] = half_round(qb.x) * p.scale; q[5] = half_round(qb.y) * p.scale;
+        q[6] = half_round(qb.z) * p.scale; q[7] = half_round(qb.w) * p.scale;
+    }
+    OnlineSM st;
+    st.m = -INFINITY; st.l = 0.f;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) st.acc[e] = 0.f;
+
+    for (int k = 0; k < n_it; ++k) {                 // warp-uniform trip count (the shuffles need all 32 lanes)
+        issue(k + ATT2_DEPTH - 1);
+        asm volatile("cp.async.wait_group %0;" ::"n"(ATT2_DEPTH - 1) : "memory");   // iteration k's copies of this lane have landed
+        const int pp = (k * ATT_WARPS + warp) * 4 + pg;
+        const uint32_t sa = ring + (uint32_t)((k % ATT2_DEPTH) * 1024);
+        uint4 kv = make_uint4(0, 0, 0, 0), vv = make_uint4(0, 0, 0, 0);
+        if (pp < n) {
+            asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(kv.x), "=r"(kv.y), "=r"(kv.z), "=r"(kv.w) : "r"(sa));
+            asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(vv.x), "=r"(vv.y), "=r"(vv.z), "=r"(vv.w) : "r"(sa + 512u));
+        }
+        const __half2* k2 = reinterpret_cast<const __half2*>(&kv);
+        float s = 0.f;
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            const float2 f = __half22float2(k2[e]);
+            s = fmaf(q[2 * e], f.x, s);
+            s = fmaf(q[2 * e + 1], f.y, s);
+        }
+        s += __shfl_xor_sync(0xffffffffu, s, 1);
+        s += __shfl_xor_sync(0xffffffffu, s, 2);
+        s += __shfl_xor_sync(0xffffffffu, s, 4);
+        if (pp < n) {
+            const float mn = fmaxf(st.m, s);
+            const float corr = __expf(st.m - mn);   // exp(-inf) = 0 on the first position
+            const float pw = __expf(s - mn);
+            st.l = st.l * corr + pw;
+            const __half2* v2 = reinterpret_cast<const __half2*>(&vv);
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const float2 f = __half22float2(v2[e]);
+                st.acc[2 * e] = fmaf(pw, f.x, st.acc[2 * e] * corr);
+                st.acc[2 * e + 1] = fmaf(pw, f.y, st.acc[2 * e + 1] * corr);
+            }
+            st.m = mn;
+        }
+    }
+    asm volatile("cp.async.wait_group 0;" ::: "memory");
+    // merge the 4 position groups of the warp, then the warps
+#pragma unroll
+    for (int o = 8; o <= 16; o <<= 1) {
+        const float m2 = __shfl_xor_sync(0xffffffffu, st.m, o), l2 = __shfl_xor_sync(0xffffffffu, st.l, o);
+        float a2[8];
+#pragma unroll
+        for (int e = 0; e < 8; ++e) a2[e] = __shfl_xor_sync(0xffffffffu, st.acc[e], o);
+        osm_merge(st, m2, l2, a2);
+    }
+    attn2_merge_store(st.m, st.l, st.acc, pg == 0, sl, p.out + (size_t)qrow * p.d + h * 64);
+}
+
+// The decode step of generate (n = p.fixed_len, or p.pos[0] + 1) and prompt prefill.
 // PF (prompt prefill): blockIdx.y is a (token, row) pair tok * rows_real + r; the query at position pos + tok attends to the
 // cache of row r up to and including its own position (the QKV GEMM of the same pass has already appended every token of the
 // pass: causal within the chunk); row r is cache row r * row_stride.
-constexpr int ATT2_DEPTH = 8;
-constexpr int ATT2_SMEM = ATT_WARPS * ATT2_DEPTH * 1024;   // the ring, 64 KB
 template <bool PF>
 __global__ void __launch_bounds__(ATT_WARPS * 32) lm_attn2_kernel(AttnParams p) {
-    extern __shared__ __align__(16) unsigned char att2sm[];   // [warp][depth][K | V][32 lanes][16 B]
-    __shared__ float wm[ATT_WARPS], wl[ATT_WARPS], wacc[ATT_WARPS][64];
-    const int h = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int qrow = blockIdx.y, row = PF ? qrow % p.rows_real * p.row_stride : qrow, tok = PF ? qrow / p.rows_real : 0;
-    const int sl = lane & 7, pg = lane >> 3;
     const int n = p.fixed_len > 0 ? p.fixed_len : p.pos[0] + tok + 1;
-    const size_t base = ((size_t)row * p.H + h) * p.cache_len * 64 + sl * 8;
-    const __half* kb = p.kc + base;
-    const __half* vb = p.vc + base;
-    const uint32_t ring = smem_u32(att2sm) + (uint32_t)(warp * ATT2_DEPTH * 1024 + lane * 16);
-    // iteration k of this warp covers positions (k * 8 + warp) * 4 + pg
-    const int n_it = (n + 31 - warp * 4) / 32 > 0 ? (n - warp * 4 + 31) / 32 : 0;   // iterations with at least one live position group
-    auto issue = [&](int k) {
-        if (k < n_it) {
-            const int pp = (k * ATT_WARPS + warp) * 4 + pg;
-            if (pp < n) {
-                const uint32_t d = ring + (uint32_t)((k % ATT2_DEPTH) * 1024);
-                asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d), "l"(kb + (size_t)pp * 64) : "memory");
-                asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d + 512u), "l"(vb + (size_t)pp * 64) : "memory");
-            }
-        }
-        asm volatile("cp.async.commit_group;" ::: "memory");
-    };
-#pragma unroll
-    for (int k = 0; k < ATT2_DEPTH - 1; ++k) issue(k);
-
-    float q[8];
-    {
-        const float4* qp = reinterpret_cast<const float4*>(p.q + (size_t)qrow * p.d + h * 64 + sl * 8);
-        const float4 qa = qp[0], qb = qp[1];
-        q[0] = half_round(qa.x) * p.scale; q[1] = half_round(qa.y) * p.scale; q[2] = half_round(qa.z) * p.scale;
-        q[3] = half_round(qa.w) * p.scale; q[4] = half_round(qb.x) * p.scale; q[5] = half_round(qb.y) * p.scale;
-        q[6] = half_round(qb.z) * p.scale; q[7] = half_round(qb.w) * p.scale;
-    }
-    OnlineSM st;
-    st.m = -INFINITY; st.l = 0.f;
-#pragma unroll
-    for (int e = 0; e < 8; ++e) st.acc[e] = 0.f;
-
-    for (int k = 0; k < n_it; ++k) {                 // warp-uniform trip count (the shuffles need all 32 lanes)
-        issue(k + ATT2_DEPTH - 1);
-        asm volatile("cp.async.wait_group %0;" ::"n"(ATT2_DEPTH - 1) : "memory");   // iteration k's copies of this lane have landed
-        const int pp = (k * ATT_WARPS + warp) * 4 + pg;
-        const uint32_t sa = ring + (uint32_t)((k % ATT2_DEPTH) * 1024);
-        uint4 kv = make_uint4(0, 0, 0, 0), vv = make_uint4(0, 0, 0, 0);
-        if (pp < n) {
-            asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(kv.x), "=r"(kv.y), "=r"(kv.z), "=r"(kv.w) : "r"(sa));
-            asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(vv.x), "=r"(vv.y), "=r"(vv.z), "=r"(vv.w) : "r"(sa + 512u));
-        }
-        const __half2* k2 = reinterpret_cast<const __half2*>(&kv);
-        float s = 0.f;
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-            const float2 f = __half22float2(k2[e]);
-            s = fmaf(q[2 * e], f.x, s);
-            s = fmaf(q[2 * e + 1], f.y, s);
-        }
-        s += __shfl_xor_sync(0xffffffffu, s, 1);
-        s += __shfl_xor_sync(0xffffffffu, s, 2);
-        s += __shfl_xor_sync(0xffffffffu, s, 4);
-        if (pp < n) {
-            const float mn = fmaxf(st.m, s);
-            const float corr = __expf(st.m - mn);   // exp(-inf) = 0 on the first position
-            const float pw = __expf(s - mn);
-            st.l = st.l * corr + pw;
-            const __half2* v2 = reinterpret_cast<const __half2*>(&vv);
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                const float2 f = __half22float2(v2[e]);
-                st.acc[2 * e] = fmaf(pw, f.x, st.acc[2 * e] * corr);
-                st.acc[2 * e + 1] = fmaf(pw, f.y, st.acc[2 * e + 1] * corr);
-            }
-            st.m = mn;
-        }
-    }
-    asm volatile("cp.async.wait_group 0;" ::: "memory");
-    // merge the 4 position groups of the warp, then the warps
-#pragma unroll
-    for (int o = 8; o <= 16; o <<= 1) {
-        const float m2 = __shfl_xor_sync(0xffffffffu, st.m, o), l2 = __shfl_xor_sync(0xffffffffu, st.l, o);
-        float a2[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) a2[e] = __shfl_xor_sync(0xffffffffu, st.acc[e], o);
-        osm_merge(st, m2, l2, a2);
-    }
-    if (pg == 0) {
-        if (sl == 0) { wm[warp] = st.m; wl[warp] = st.l; }
-#pragma unroll
-        for (int e = 0; e < 8; ++e) wacc[warp][sl * 8 + e] = st.acc[e];
-    }
-    __syncthreads();
-    if (tid < 64) {
-        float mx = wm[0];
-#pragma unroll
-        for (int w = 1; w < ATT_WARPS; ++w) mx = fmaxf(mx, wm[w]);
-        float l = 0.f, o = 0.f;
-#pragma unroll
-        for (int w = 0; w < ATT_WARPS; ++w) {
-            const float cw = wm[w] == -INFINITY ? 0.f : __expf(wm[w] - mx);
-            l = fmaf(wl[w], cw, l);
-            o = fmaf(wacc[w][tid], cw, o);
-        }
-        p.out[(size_t)qrow * p.d + h * 64 + tid] = __float2half_rn(o / l);
-    }
+    attn2_body(p, qrow, n, ((size_t)row * p.H + blockIdx.x) * p.cache_len, RowAt{});
 }
 
-
-// Slot mode: lm_attn2_kernel with each row at its own slot's position (a separate copy: the decode kernel stays as it is).
-// Row r of slot r % slots (p.rows_real = slots) attends to its slot's cache positions [0, prefix + pos]: the condition prefix
-// and the columns so far.  The rows of a slot that is not ACTIVE attend to no key and write zeros.
+// Slot mode: each row at its own slot's position.  Row r of slot r % slots (p.rows_real = slots) attends to its slot's cache
+// positions [0, prefix + pos]: the condition prefix and the columns so far.
 __global__ void __launch_bounds__(ATT_WARPS * 32) lm_attn2_slot_kernel(AttnParams p, const int* __restrict__ slot_state) {
-    extern __shared__ __align__(16) unsigned char att2sm[];   // [warp][depth][K | V][32 lanes][16 B]
-    __shared__ float wm[ATT_WARPS], wl[ATT_WARPS], wacc[ATT_WARPS][64];
-    const int h = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int qrow = blockIdx.y, row = qrow;
-    const int sl = lane & 7, pg = lane >> 3;
-    const int* slot = slot_state + (row % p.rows_real) * ACB_LM_SLOT_STRIDE;
-    if (slot[ACB_SLOT_STATUS] != SLOT_ACTIVE) {   // block-uniform
-        if (tid < 64) p.out[(size_t)qrow * p.d + h * 64 + tid] = __float2half_rn(0.f);
-        return;
-    }
-    const int n = slot[ACB_SLOT_PREFIX] + slot[ACB_SLOT_POS] + 1;
-    const size_t base = ((size_t)row * p.H + h) * p.cache_len * 64 + sl * 8;
-    const __half* kb = p.kc + base;
-    const __half* vb = p.vc + base;
-    const uint32_t ring = smem_u32(att2sm) + (uint32_t)(warp * ATT2_DEPTH * 1024 + lane * 16);
-    // iteration k of this warp covers positions (k * 8 + warp) * 4 + pg
-    const int n_it = (n + 31 - warp * 4) / 32 > 0 ? (n - warp * 4 + 31) / 32 : 0;   // iterations with at least one live position group
-    auto issue = [&](int k) {
-        if (k < n_it) {
-            const int pp = (k * ATT_WARPS + warp) * 4 + pg;
-            if (pp < n) {
-                const uint32_t d = ring + (uint32_t)((k % ATT2_DEPTH) * 1024);
-                asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d), "l"(kb + (size_t)pp * 64) : "memory");
-                asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d + 512u), "l"(vb + (size_t)pp * 64) : "memory");
-            }
-        }
-        asm volatile("cp.async.commit_group;" ::: "memory");
-    };
-#pragma unroll
-    for (int k = 0; k < ATT2_DEPTH - 1; ++k) issue(k);
-
-    float q[8];
-    {
-        const float4* qp = reinterpret_cast<const float4*>(p.q + (size_t)qrow * p.d + h * 64 + sl * 8);
-        const float4 qa = qp[0], qb = qp[1];
-        q[0] = half_round(qa.x) * p.scale; q[1] = half_round(qa.y) * p.scale; q[2] = half_round(qa.z) * p.scale;
-        q[3] = half_round(qa.w) * p.scale; q[4] = half_round(qb.x) * p.scale; q[5] = half_round(qb.y) * p.scale;
-        q[6] = half_round(qb.z) * p.scale; q[7] = half_round(qb.w) * p.scale;
-    }
-    OnlineSM st;
-    st.m = -INFINITY; st.l = 0.f;
-#pragma unroll
-    for (int e = 0; e < 8; ++e) st.acc[e] = 0.f;
-
-    for (int k = 0; k < n_it; ++k) {                 // warp-uniform trip count (the shuffles need all 32 lanes)
-        issue(k + ATT2_DEPTH - 1);
-        asm volatile("cp.async.wait_group %0;" ::"n"(ATT2_DEPTH - 1) : "memory");   // iteration k's copies of this lane have landed
-        const int pp = (k * ATT_WARPS + warp) * 4 + pg;
-        const uint32_t sa = ring + (uint32_t)((k % ATT2_DEPTH) * 1024);
-        uint4 kv = make_uint4(0, 0, 0, 0), vv = make_uint4(0, 0, 0, 0);
-        if (pp < n) {
-            asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(kv.x), "=r"(kv.y), "=r"(kv.z), "=r"(kv.w) : "r"(sa));
-            asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(vv.x), "=r"(vv.y), "=r"(vv.z), "=r"(vv.w) : "r"(sa + 512u));
-        }
-        const __half2* k2 = reinterpret_cast<const __half2*>(&kv);
-        float s = 0.f;
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-            const float2 f = __half22float2(k2[e]);
-            s = fmaf(q[2 * e], f.x, s);
-            s = fmaf(q[2 * e + 1], f.y, s);
-        }
-        s += __shfl_xor_sync(0xffffffffu, s, 1);
-        s += __shfl_xor_sync(0xffffffffu, s, 2);
-        s += __shfl_xor_sync(0xffffffffu, s, 4);
-        if (pp < n) {
-            const float mn = fmaxf(st.m, s);
-            const float corr = __expf(st.m - mn);   // exp(-inf) = 0 on the first position
-            const float pw = __expf(s - mn);
-            st.l = st.l * corr + pw;
-            const __half2* v2 = reinterpret_cast<const __half2*>(&vv);
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                const float2 f = __half22float2(v2[e]);
-                st.acc[2 * e] = fmaf(pw, f.x, st.acc[2 * e] * corr);
-                st.acc[2 * e + 1] = fmaf(pw, f.y, st.acc[2 * e + 1] * corr);
-            }
-            st.m = mn;
-        }
-    }
-    asm volatile("cp.async.wait_group 0;" ::: "memory");
-    // merge the 4 position groups of the warp, then the warps
-#pragma unroll
-    for (int o = 8; o <= 16; o <<= 1) {
-        const float m2 = __shfl_xor_sync(0xffffffffu, st.m, o), l2 = __shfl_xor_sync(0xffffffffu, st.l, o);
-        float a2[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) a2[e] = __shfl_xor_sync(0xffffffffu, st.acc[e], o);
-        osm_merge(st, m2, l2, a2);
-    }
-    if (pg == 0) {
-        if (sl == 0) { wm[warp] = st.m; wl[warp] = st.l; }
-#pragma unroll
-        for (int e = 0; e < 8; ++e) wacc[warp][sl * 8 + e] = st.acc[e];
-    }
-    __syncthreads();
-    if (tid < 64) {
-        float mx = wm[0];
-#pragma unroll
-        for (int w = 1; w < ATT_WARPS; ++w) mx = fmaxf(mx, wm[w]);
-        float l = 0.f, o = 0.f;
-#pragma unroll
-        for (int w = 0; w < ATT_WARPS; ++w) {
-            const float cw = wm[w] == -INFINITY ? 0.f : __expf(wm[w] - mx);
-            l = fmaf(wl[w], cw, l);
-            o = fmaf(wacc[w][tid], cw, o);
-        }
-        p.out[(size_t)qrow * p.d + h * 64 + tid] = __float2half_rn(o / l);
-    }
+    const int qrow = blockIdx.y;
+    const SlotRow r = slot_row(slot_state, p.rows_real, qrow, nullptr, 0);
+    if (!r.live) { attn2_zero(p, qrow); return; }   // block-uniform
+    attn2_body(p, qrow, r.pos + 1, ((size_t)qrow * p.H + blockIdx.x) * p.cache_len, RowAt{});
 }
 
-// Paged session (acb_lm_begin_slots_paged): lm_attn2_slot_kernel with p.kc / p.vc the layer's page pool; the row's page table (at most ACB_LM_MAX_PAGES_PER_ROW entries) is staged in
-// shared memory and position pp is read from offset pp % ACB_LM_KV_PAGE of page pt[pp / ACB_LM_KV_PAGE].  A page holds a
-// multiple of the 4-position groups, so one lane's 16-byte copy never crosses a page; the arithmetic and its order are the
-// contiguous kernel's.
-// (a separate copy: the contiguous kernel stays as it is)
+// Paged session (acb_lm_begin_slots_paged): lm_attn2_slot_kernel with p.kc / p.vc the layer's page pool.
 __global__ void __launch_bounds__(ATT_WARPS * 32) lm_attn2_slot_paged_kernel(AttnParams p, const int* __restrict__ slot_state,
                                                                           const int* __restrict__ table, int pages_per_row) {
-    extern __shared__ __align__(16) unsigned char att2sm[];   // [warp][depth][K | V][32 lanes][16 B]
-    __shared__ float wm[ATT_WARPS], wl[ATT_WARPS], wacc[ATT_WARPS][64];
-    const int h = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int qrow = blockIdx.y, row = qrow;
-    const int sl = lane & 7, pg = lane >> 3;
-    const int* slot = slot_state + (row % p.rows_real) * ACB_LM_SLOT_STRIDE;
-    if (slot[ACB_SLOT_STATUS] != SLOT_ACTIVE) {   // block-uniform
-        if (tid < 64) p.out[(size_t)qrow * p.d + h * 64 + tid] = __float2half_rn(0.f);
-        return;
-    }
-    const int n = slot[ACB_SLOT_PREFIX] + slot[ACB_SLOT_POS] + 1;
-    __shared__ int pt[ACB_LM_MAX_PAGES_PER_ROW];
-    for (int i = tid; i < (n + ACB_LM_KV_PAGE - 1) / ACB_LM_KV_PAGE; i += ATT_WARPS * 32) pt[i] = table[row * pages_per_row + i];
-    __syncthreads();
-    const size_t base = (size_t)h * ACB_LM_KV_PAGE * 64 + sl * 8;   // position pp: + (pt[pp / page] * H * page + pp % page) * 64
-    const __half* kb = p.kc + base;
-    const __half* vb = p.vc + base;
-    const uint32_t ring = smem_u32(att2sm) + (uint32_t)(warp * ATT2_DEPTH * 1024 + lane * 16);
-    // iteration k of this warp covers positions (k * 8 + warp) * 4 + pg
-    const int n_it = (n + 31 - warp * 4) / 32 > 0 ? (n - warp * 4 + 31) / 32 : 0;   // iterations with at least one live position group
-    auto issue = [&](int k) {
-        if (k < n_it) {
-            const int pp = (k * ATT_WARPS + warp) * 4 + pg;
-            if (pp < n) {
-                const uint32_t d = ring + (uint32_t)((k % ATT2_DEPTH) * 1024);
-                const size_t o = ((size_t)pt[pp / ACB_LM_KV_PAGE] * p.H * ACB_LM_KV_PAGE + pp % ACB_LM_KV_PAGE) * 64;
-                asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d), "l"(kb + o) : "memory");
-                asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d + 512u), "l"(vb + o) : "memory");
-            }
-        }
-        asm volatile("cp.async.commit_group;" ::: "memory");
-    };
-#pragma unroll
-    for (int k = 0; k < ATT2_DEPTH - 1; ++k) issue(k);
-
-    float q[8];
-    {
-        const float4* qp = reinterpret_cast<const float4*>(p.q + (size_t)qrow * p.d + h * 64 + sl * 8);
-        const float4 qa = qp[0], qb = qp[1];
-        q[0] = half_round(qa.x) * p.scale; q[1] = half_round(qa.y) * p.scale; q[2] = half_round(qa.z) * p.scale;
-        q[3] = half_round(qa.w) * p.scale; q[4] = half_round(qb.x) * p.scale; q[5] = half_round(qb.y) * p.scale;
-        q[6] = half_round(qb.z) * p.scale; q[7] = half_round(qb.w) * p.scale;
-    }
-    OnlineSM st;
-    st.m = -INFINITY; st.l = 0.f;
-#pragma unroll
-    for (int e = 0; e < 8; ++e) st.acc[e] = 0.f;
-
-    for (int k = 0; k < n_it; ++k) {                 // warp-uniform trip count (the shuffles need all 32 lanes)
-        issue(k + ATT2_DEPTH - 1);
-        asm volatile("cp.async.wait_group %0;" ::"n"(ATT2_DEPTH - 1) : "memory");   // iteration k's copies of this lane have landed
-        const int pp = (k * ATT_WARPS + warp) * 4 + pg;
-        const uint32_t sa = ring + (uint32_t)((k % ATT2_DEPTH) * 1024);
-        uint4 kv = make_uint4(0, 0, 0, 0), vv = make_uint4(0, 0, 0, 0);
-        if (pp < n) {
-            asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(kv.x), "=r"(kv.y), "=r"(kv.z), "=r"(kv.w) : "r"(sa));
-            asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(vv.x), "=r"(vv.y), "=r"(vv.z), "=r"(vv.w) : "r"(sa + 512u));
-        }
-        const __half2* k2 = reinterpret_cast<const __half2*>(&kv);
-        float s = 0.f;
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-            const float2 f = __half22float2(k2[e]);
-            s = fmaf(q[2 * e], f.x, s);
-            s = fmaf(q[2 * e + 1], f.y, s);
-        }
-        s += __shfl_xor_sync(0xffffffffu, s, 1);
-        s += __shfl_xor_sync(0xffffffffu, s, 2);
-        s += __shfl_xor_sync(0xffffffffu, s, 4);
-        if (pp < n) {
-            const float mn = fmaxf(st.m, s);
-            const float corr = __expf(st.m - mn);   // exp(-inf) = 0 on the first position
-            const float pw = __expf(s - mn);
-            st.l = st.l * corr + pw;
-            const __half2* v2 = reinterpret_cast<const __half2*>(&vv);
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                const float2 f = __half22float2(v2[e]);
-                st.acc[2 * e] = fmaf(pw, f.x, st.acc[2 * e] * corr);
-                st.acc[2 * e + 1] = fmaf(pw, f.y, st.acc[2 * e + 1] * corr);
-            }
-            st.m = mn;
-        }
-    }
-    asm volatile("cp.async.wait_group 0;" ::: "memory");
-    // merge the 4 position groups of the warp, then the warps
-#pragma unroll
-    for (int o = 8; o <= 16; o <<= 1) {
-        const float m2 = __shfl_xor_sync(0xffffffffu, st.m, o), l2 = __shfl_xor_sync(0xffffffffu, st.l, o);
-        float a2[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) a2[e] = __shfl_xor_sync(0xffffffffu, st.acc[e], o);
-        osm_merge(st, m2, l2, a2);
-    }
-    if (pg == 0) {
-        if (sl == 0) { wm[warp] = st.m; wl[warp] = st.l; }
-#pragma unroll
-        for (int e = 0; e < 8; ++e) wacc[warp][sl * 8 + e] = st.acc[e];
-    }
-    __syncthreads();
-    if (tid < 64) {
-        float mx = wm[0];
-#pragma unroll
-        for (int w = 1; w < ATT_WARPS; ++w) mx = fmaxf(mx, wm[w]);
-        float l = 0.f, o = 0.f;
-#pragma unroll
-        for (int w = 0; w < ATT_WARPS; ++w) {
-            const float cw = wm[w] == -INFINITY ? 0.f : __expf(wm[w] - mx);
-            l = fmaf(wl[w], cw, l);
-            o = fmaf(wacc[w][tid], cw, o);
-        }
-        p.out[(size_t)qrow * p.d + h * 64 + tid] = __float2half_rn(o / l);
-    }
+    const int qrow = blockIdx.y;
+    const SlotRow r = slot_row(slot_state, p.rows_real, qrow, nullptr, 0);
+    if (!r.live) { attn2_zero(p, qrow); return; }   // block-uniform
+    attn2_body(p, qrow, r.pos + 1, (size_t)blockIdx.x * ACB_LM_KV_PAGE, stage_pages(table, pages_per_row, qrow, r.pos + 1, p.H));
 }
 
 // Paged admission pass (acb_lm_admit_prompt in a paged session): lm_attn2_kernel<true> reading K and V through the page table.
-// blockIdx.y is a (token, row) pair tok * rows_real + j; the query at position pos[0] + tok attends to positions
-// [0, pos[0] + tok] of page table row r0 + j * row_stride (the pass's own positions are already appended:
-// lm_qkv_pf_paged_kernel ran before).  The row's table is staged in shared memory as in lm_attn2_slot_paged_kernel, and the
-// arithmetic and its order are lm_attn2_kernel's.  (A separate copy: the other kernels stay as they are.)
+// The query of pass row qrow attends to positions [0, its own] of its page-table row (the pass's own positions are already
+// appended: lm_qkv_pf_paged_kernel ran before).
 __global__ void __launch_bounds__(ATT_WARPS * 32) lm_attn2_pf_paged_kernel(AttnParams p, const int* __restrict__ table,
                                                                         int pages_per_row, int r0) {
-    extern __shared__ __align__(16) unsigned char att2sm[];   // [warp][depth][K | V][32 lanes][16 B]
-    __shared__ float wm[ATT_WARPS], wl[ATT_WARPS], wacc[ATT_WARPS][64];
-    __shared__ int pt[ACB_LM_MAX_PAGES_PER_ROW];
-    const int h = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int qrow = blockIdx.y, tok = qrow / p.rows_real, trow = r0 + (qrow - tok * p.rows_real) * p.row_stride;
-    const int sl = lane & 7, pg = lane >> 3;
-    const int n = p.pos[0] + tok + 1;
-    for (int i = tid; i < (n + ACB_LM_KV_PAGE - 1) / ACB_LM_KV_PAGE; i += ATT_WARPS * 32) pt[i] = table[trow * pages_per_row + i];
-    __syncthreads();
-    const size_t base = (size_t)h * ACB_LM_KV_PAGE * 64 + sl * 8;   // position pp: + (pt[pp / page] * H * page + pp % page) * 64
-    const __half* kb = p.kc + base;
-    const __half* vb = p.vc + base;
-    const uint32_t ring = smem_u32(att2sm) + (uint32_t)(warp * ATT2_DEPTH * 1024 + lane * 16);
-    // iteration k of this warp covers positions (k * 8 + warp) * 4 + pg
-    const int n_it = (n + 31 - warp * 4) / 32 > 0 ? (n - warp * 4 + 31) / 32 : 0;   // iterations with at least one live position group
-    auto issue = [&](int k) {
-        if (k < n_it) {
-            const int pp = (k * ATT_WARPS + warp) * 4 + pg;
-            if (pp < n) {
-                const uint32_t d = ring + (uint32_t)((k % ATT2_DEPTH) * 1024);
-                const size_t o = ((size_t)pt[pp / ACB_LM_KV_PAGE] * p.H * ACB_LM_KV_PAGE + pp % ACB_LM_KV_PAGE) * 64;
-                asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d), "l"(kb + o) : "memory");
-                asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d + 512u), "l"(vb + o) : "memory");
-            }
-        }
-        asm volatile("cp.async.commit_group;" ::: "memory");
-    };
-#pragma unroll
-    for (int k = 0; k < ATT2_DEPTH - 1; ++k) issue(k);
-
-    float q[8];
-    {
-        const float4* qp = reinterpret_cast<const float4*>(p.q + (size_t)qrow * p.d + h * 64 + sl * 8);
-        const float4 qa = qp[0], qb = qp[1];
-        q[0] = half_round(qa.x) * p.scale; q[1] = half_round(qa.y) * p.scale; q[2] = half_round(qa.z) * p.scale;
-        q[3] = half_round(qa.w) * p.scale; q[4] = half_round(qb.x) * p.scale; q[5] = half_round(qb.y) * p.scale;
-        q[6] = half_round(qb.z) * p.scale; q[7] = half_round(qb.w) * p.scale;
-    }
-    OnlineSM st;
-    st.m = -INFINITY; st.l = 0.f;
-#pragma unroll
-    for (int e = 0; e < 8; ++e) st.acc[e] = 0.f;
-
-    for (int k = 0; k < n_it; ++k) {                 // warp-uniform trip count (the shuffles need all 32 lanes)
-        issue(k + ATT2_DEPTH - 1);
-        asm volatile("cp.async.wait_group %0;" ::"n"(ATT2_DEPTH - 1) : "memory");   // iteration k's copies of this lane have landed
-        const int pp = (k * ATT_WARPS + warp) * 4 + pg;
-        const uint32_t sa = ring + (uint32_t)((k % ATT2_DEPTH) * 1024);
-        uint4 kv = make_uint4(0, 0, 0, 0), vv = make_uint4(0, 0, 0, 0);
-        if (pp < n) {
-            asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(kv.x), "=r"(kv.y), "=r"(kv.z), "=r"(kv.w) : "r"(sa));
-            asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(vv.x), "=r"(vv.y), "=r"(vv.z), "=r"(vv.w) : "r"(sa + 512u));
-        }
-        const __half2* k2 = reinterpret_cast<const __half2*>(&kv);
-        float s = 0.f;
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-            const float2 f = __half22float2(k2[e]);
-            s = fmaf(q[2 * e], f.x, s);
-            s = fmaf(q[2 * e + 1], f.y, s);
-        }
-        s += __shfl_xor_sync(0xffffffffu, s, 1);
-        s += __shfl_xor_sync(0xffffffffu, s, 2);
-        s += __shfl_xor_sync(0xffffffffu, s, 4);
-        if (pp < n) {
-            const float mn = fmaxf(st.m, s);
-            const float corr = __expf(st.m - mn);   // exp(-inf) = 0 on the first position
-            const float pw = __expf(s - mn);
-            st.l = st.l * corr + pw;
-            const __half2* v2 = reinterpret_cast<const __half2*>(&vv);
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                const float2 f = __half22float2(v2[e]);
-                st.acc[2 * e] = fmaf(pw, f.x, st.acc[2 * e] * corr);
-                st.acc[2 * e + 1] = fmaf(pw, f.y, st.acc[2 * e + 1] * corr);
-            }
-            st.m = mn;
-        }
-    }
-    asm volatile("cp.async.wait_group 0;" ::: "memory");
-    // merge the 4 position groups of the warp, then the warps
-#pragma unroll
-    for (int o = 8; o <= 16; o <<= 1) {
-        const float m2 = __shfl_xor_sync(0xffffffffu, st.m, o), l2 = __shfl_xor_sync(0xffffffffu, st.l, o);
-        float a2[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) a2[e] = __shfl_xor_sync(0xffffffffu, st.acc[e], o);
-        osm_merge(st, m2, l2, a2);
-    }
-    if (pg == 0) {
-        if (sl == 0) { wm[warp] = st.m; wl[warp] = st.l; }
-#pragma unroll
-        for (int e = 0; e < 8; ++e) wacc[warp][sl * 8 + e] = st.acc[e];
-    }
-    __syncthreads();
-    if (tid < 64) {
-        float mx = wm[0];
-#pragma unroll
-        for (int w = 1; w < ATT_WARPS; ++w) mx = fmaxf(mx, wm[w]);
-        float l = 0.f, o = 0.f;
-#pragma unroll
-        for (int w = 0; w < ATT_WARPS; ++w) {
-            const float cw = wm[w] == -INFINITY ? 0.f : __expf(wm[w] - mx);
-            l = fmaf(wl[w], cw, l);
-            o = fmaf(wacc[w][tid], cw, o);
-        }
-        p.out[(size_t)qrow * p.d + h * 64 + tid] = __float2half_rn(o / l);
-    }
+    const int qrow = blockIdx.y;
+    const PassRow r = pass_row(p.pos, qrow, p.rows_real, r0, p.row_stride);
+    attn2_body(p, qrow, r.pos + 1, (size_t)blockIdx.x * ACB_LM_KV_PAGE, stage_pages(table, pages_per_row, r.trow, r.pos + 1, p.H));
 }
 
-// Self attention over an FP8 pool: lm_attn2_slot_paged_kernel's CTA (query row, head), online softmax and cp.async ring, with
-// a lane's 16-byte copy holding 16 e4m3 codes: 4 lanes share a position (16 dims each), a warp instruction covers 8
-// consecutive positions (a page holds whole groups of 8, so no copy crosses a page), and iteration k of a warp covers
-// positions (k * 8 + warp) * 8 + pg.  Lanes 0 and 1 of a position also copy its K and V scale into the stage.  Each lane
-// dots its 16 codes (exact in fp16) with q in an fp32 FMA chain, the 4 lanes add in a 2-level shuffle tree, and the sum is
-// multiplied by the K scale; the V scale multiplies the softmax weight before it scales the codes.  Queries attend to
-// positions [0, n) of page-table row trow.
+// Self attention over an FP8 pool: attn2_body's CTA (query row, head), online softmax and cp.async ring, with a lane's
+// 16-byte copy holding 16 e4m3 codes: 4 lanes share a position (16 dims each), a warp instruction covers 8 consecutive
+// positions, and iteration k of a warp covers positions (k * 8 + warp) * 8 + pg.  Lanes 0 and 1 of a position also copy its
+// K and V scale into the stage.  Each lane dots its 16 codes (exact in fp16) with q in an fp32 FMA chain, the 4 lanes add in
+// a 2-level shuffle tree, and the sum is multiplied by the K scale; the V scale multiplies the softmax weight before it
+// scales the codes.  Query row qrow attends to positions [0, n) of the page-table row staged in `at`.
 constexpr int ATT2F8_STAGE = 1024 + 64;   // per warp and stage: K codes, V codes [32 lanes][16 B], scales [8 positions][K, V]
 constexpr int ATT2F8_SMEM = ATT_WARPS * ATT2_DEPTH * ATT2F8_STAGE;
-__device__ __forceinline__ void attn2_paged_fp8_body(const AttnParams& p, const Fp8Pool& pool, const int* __restrict__ table,
-                                                     int pages_per_row, int qrow, int trow, int n) {
+__device__ __forceinline__ void attn2_paged_fp8_body(const AttnParams& p, const Fp8Pool& pool, int qrow, int n, PagedAt at) {
     extern __shared__ __align__(16) unsigned char att2sm[];   // [warp][depth][K | V | scales]
-    __shared__ float wm[ATT_WARPS], wl[ATT_WARPS], wacc[ATT_WARPS][64];
-    __shared__ int pt[ACB_LM_MAX_PAGES_PER_ROW];
     const int h = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int sl = lane & 3, pg = lane >> 2;
-    for (int i = tid; i < (n + ACB_LM_KV_PAGE - 1) / ACB_LM_KV_PAGE; i += ATT_WARPS * 32) pt[i] = table[trow * pages_per_row + i];
-    __syncthreads();
-    // position pp: codes at (pt[pp / page] * H * page + pp % page) * 64 + base, scales at the same index / 64 + h * page
+    // position pp: codes at at(pp) * 64 + base, scales at at(pp) + h * page
     const uint8_t* kb = pool.k + (size_t)h * ACB_LM_KV_PAGE * 64 + sl * 16;
     const uint8_t* vb = pool.v + (size_t)h * ACB_LM_KV_PAGE * 64 + sl * 16;
     const float* sb = (sl ? pool.vs : pool.ks) + (size_t)h * ACB_LM_KV_PAGE;
@@ -1128,7 +851,7 @@ __device__ __forceinline__ void attn2_paged_fp8_body(const AttnParams& p, const 
             const int pp = (k * ATT_WARPS + warp) * 8 + pg;
             if (pp < n) {
                 const uint32_t st = ring + (uint32_t)((k % ATT2_DEPTH) * ATT2F8_STAGE);
-                const size_t o = (size_t)pt[pp / ACB_LM_KV_PAGE] * p.H * ACB_LM_KV_PAGE + pp % ACB_LM_KV_PAGE;
+                const size_t o = at(pp);
                 asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(st + lane * 16), "l"(kb + o * 64) : "memory");
                 asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(st + 512u + lane * 16), "l"(vb + o * 64) : "memory");
                 if (sl < 2)
@@ -1209,25 +932,7 @@ __device__ __forceinline__ void attn2_paged_fp8_body(const AttnParams& p, const 
         for (int e = 0; e < 16; ++e) acc[e] = acc[e] * ca + __shfl_xor_sync(0xffffffffu, acc[e], o) * cb;
         m = mn;
     }
-    if (pg == 0) {
-        if (sl == 0) { wm[warp] = m; wl[warp] = l; }
-#pragma unroll
-        for (int e = 0; e < 16; ++e) wacc[warp][sl * 16 + e] = acc[e];
-    }
-    __syncthreads();
-    if (tid < 64) {
-        float mx = wm[0];
-#pragma unroll
-        for (int w = 1; w < ATT_WARPS; ++w) mx = fmaxf(mx, wm[w]);
-        float lt = 0.f, o = 0.f;
-#pragma unroll
-        for (int w = 0; w < ATT_WARPS; ++w) {
-            const float cw = wm[w] == -INFINITY ? 0.f : __expf(wm[w] - mx);
-            lt = fmaf(wl[w], cw, lt);
-            o = fmaf(wacc[w][tid], cw, o);
-        }
-        p.out[(size_t)qrow * p.d + h * 64 + tid] = __float2half_rn(o / lt);
-    }
+    attn2_merge_store(m, l, acc, pg == 0, sl, p.out + (size_t)qrow * p.d + h * 64);
 }
 
 // lm_attn2_slot_paged_kernel over an FP8 pool (one layer's codes and scales in `pool`).
@@ -1235,20 +940,18 @@ __global__ void __launch_bounds__(ATT_WARPS * 32) lm_attn2_slot_paged_fp8_kernel
                                                                               const int* __restrict__ slot_state,
                                                                               const int* __restrict__ table, int pages_per_row) {
     const int qrow = blockIdx.y;
-    const int* slot = slot_state + (qrow % p.rows_real) * ACB_LM_SLOT_STRIDE;
-    if (slot[ACB_SLOT_STATUS] != SLOT_ACTIVE) {   // block-uniform
-        if (threadIdx.x < 64) p.out[(size_t)qrow * p.d + blockIdx.x * 64 + threadIdx.x] = __float2half_rn(0.f);
-        return;
-    }
-    attn2_paged_fp8_body(p, pool, table, pages_per_row, qrow, qrow, slot[ACB_SLOT_PREFIX] + slot[ACB_SLOT_POS] + 1);
+    const SlotRow r = slot_row(slot_state, p.rows_real, qrow, nullptr, 0);
+    if (!r.live) { attn2_zero(p, qrow); return; }   // block-uniform
+    attn2_paged_fp8_body(p, pool, qrow, r.pos + 1, stage_pages(table, pages_per_row, qrow, r.pos + 1, p.H));
 }
 
 // lm_attn2_pf_paged_kernel over an FP8 pool.
 __global__ void __launch_bounds__(ATT_WARPS * 32) lm_attn2_pf_paged_fp8_kernel(AttnParams p, Fp8Pool pool,
                                                                             const int* __restrict__ table, int pages_per_row,
                                                                             int r0) {
-    const int qrow = blockIdx.y, tok = qrow / p.rows_real;
-    attn2_paged_fp8_body(p, pool, table, pages_per_row, qrow, r0 + (qrow - tok * p.rows_real) * p.row_stride, p.pos[0] + tok + 1);
+    const int qrow = blockIdx.y;
+    const PassRow r = pass_row(p.pos, qrow, p.rows_real, r0, p.row_stride);
+    attn2_paged_fp8_body(p, pool, qrow, r.pos + 1, stage_pages(table, pages_per_row, r.trow, r.pos + 1, p.H));
 }
 
 // Cross attention over the (short) text condition: one WARP per (row, head), lane = text position for the scores,

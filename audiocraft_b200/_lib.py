@@ -25,14 +25,31 @@ ACB_LM_MAX_PAGES_PER_ROW = 188
 
 
 class LMConfig(C.Structure):
+    """acb_lm_config.  `_fields_` lists the fields up to positional_embedding, and callers build the structure from that
+    list; every instance also carries the trailing `int weight_dtype` (0, fp16, unless given), so whatever builds it, the
+    library never reads past its end."""
     _fields_ = [('dim', C.c_int), ('num_heads', C.c_int), ('num_layers', C.c_int), ('ffn_dim', C.c_int),
                 ('n_q', C.c_int), ('card', C.c_int), ('cross_attention', C.c_int), ('max_rows', C.c_int),
                 ('max_seq', C.c_int), ('max_text', C.c_int), ('pos_scale', C.c_float), ('positional_embedding', C.c_int)]
 
+    def __init__(self, *args, weight_dtype: int = 0, **kw):
+        super().__init__(*args, **kw)
+        C.resize(self, C.sizeof(LMConfig) + C.sizeof(C.c_int))   # the added bytes are zero
+        self.weight_dtype = weight_dtype
+
+    @property
+    def weight_dtype(self) -> int:
+        return C.c_int.from_address(C.addressof(self) + C.sizeof(LMConfig)).value
+
+    @weight_dtype.setter
+    def weight_dtype(self, v: int):
+        C.c_int.from_address(C.addressof(self) + C.sizeof(LMConfig)).value = int(v)
+
 
 class LMWeights(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ('emb', 'inv_freq', 'w_qkv', 'w_o', 'w_cq', 'w_ckv', 'w_co', 'w_ff1',
-                                           'w_ff2', 'ln', 'out_norm', 'heads', 'rope_freq')]
+                                           'w_ff2', 'ln', 'out_norm', 'heads', 'rope_freq', 's_qkv', 's_o', 's_cq', 's_ckv',
+                                           's_co', 's_ff1', 's_ff2')]
 
 
 class LMBuffers(C.Structure):

@@ -206,6 +206,24 @@ __device__ __noinline__ float rope_rotate(const float* rope_freq, float pos_scal
     return even ? re * rr - im * ri : re * ri + im * rr;
 }
 
+// FP8 weights (acb_lm_config.weight_dtype = 1): two e4m3 codes -> two fp16 values, exactly (every e4m3 value is an fp16
+// value); the upper byte becomes the upper half.
+__device__ __forceinline__ uint32_t e4m3x2_to_f16x2(uint32_t two_codes) {
+    uint32_t r;
+    asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(r) : "h"((uint16_t)two_codes));
+    return r;
+}
+// 8 codes (k .. k + 7, k at the lowest byte) -> the 8 fp16 values an fp16 slab holds in one uint4
+__device__ __forceinline__ uint4 e4m3x8_to_f16x8(uint2 c) {
+    return make_uint4(e4m3x2_to_f16x2(c.x), e4m3x2_to_f16x2(c.x >> 16), e4m3x2_to_f16x2(c.y), e4m3x2_to_f16x2(c.y >> 16));
+}
+
+// Bytes per staged weight row: fp16 as lm_gemm_kernel computes it (+64 for conflict-free LDS.128), e4m3 for lm_gemm_fp8_kernel.
+// e4m3: rows 32 bytes apart modulo 128, so the 4 rows one half-warp's LDS.64 touch lie in 4 different 8-bank groups.
+__host__ __device__ __forceinline__ int gemm_pitch(int kslice, bool w8) {
+    return w8 ? (kslice + 127) / 128 * 128 + 32 : kslice * 2 + 64;
+}
+
 // CTA = 4 warps, tile = 16 output features x kslice of K.  The CTA's 16 x kslice weight slab is fetched by ONE thread
 // with 16 TMA bulk copies (one per W row, padded pitch => conflict-free fragment reads), issued before the first activation
 // read so that the weight bytes are in flight while the activations load.
@@ -328,6 +346,131 @@ __global__ void __launch_bounds__(128) lm_gemm_kernel(GemmParams p) {
     }
 }
 
+// lm_gemm_kernel on FP8 weights (acb_lm_config.weight_dtype = 1), a kernel of its own so that the fp16 instances keep their
+// code and their parameter layout: the same tiles, split, FT2 and epilogues.  The slab is e4m3 codes (p.W points at bytes);
+// each lane reads 8 codes where the fp16 slab gives it 8 halves, so the k order against the activations is the fp16 one, and
+// unpacks them exactly to fp16 for the same MMAs.  wscale[n] (the row's fp32 scale) multiplies output n's fixed-order sum
+// once, before the epilogue does anything else with it (an EPI_PARTIAL slice is scaled before it is stored).
+// (128, 4): without the occupancy target ptxas spilled 8 bytes in <2, EPI_QKV, 2>; with it no instance spills.
+template <int NT, int EPI, int FT2 = 1>
+__global__ void __launch_bounds__(128, 4) lm_gemm_fp8_kernel(GemmParams p, const float* __restrict__ wscale) {
+    constexpr int U = NT <= 2 ? 4 : (NT <= 4 ? 2 : 1);   // k-blocks per batch of activation loads
+    constexpr int RP = 8 * NT + 1;
+    constexpr int FB = 16 * FT2;                     // output features per CTA
+    constexpr bool ROPE = EPI == EPI_QKV_ROPE || EPI == EPI_QKV_PF_ROPE, PF = EPI == EPI_QKV_PF || EPI == EPI_QKV_PF_ROPE;
+    constexpr bool QKV = EPI == EPI_QKV || PF || ROPE;
+    extern __shared__ __align__(128) unsigned char gsm[];
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, c4 = lane & 3;
+    const int f0 = blockIdx.x * FB;
+    const int k0 = blockIdx.y * p.kslice;
+    const int ks = min(p.kslice, p.K - k0);          // elements of K this CTA reduces over
+    const int pitch = gemm_pitch(p.kslice, true);    // bytes per staged W row
+    uint64_t* bar = reinterpret_cast<uint64_t*>(gsm + FB * pitch);
+    float* red = reinterpret_cast<float*>(gsm + FB * pitch + 16);   // [4][FB][RP]
+
+    if (tid == 0) mbar_init(bar, 1);
+    __syncthreads();
+    if (tid == 0) {
+        const uint8_t* wc = reinterpret_cast<const uint8_t*>(p.W);   // codes: one byte per weight
+        mbar_expect_tx(bar, (uint32_t)FB * (uint32_t)ks);
+#pragma unroll 1
+        for (int r = 0; r < FB; ++r) bulk_g2s(gsm + r * pitch, wc + (size_t)(f0 + r) * p.K + k0, (uint32_t)ks, bar);
+    }
+    int cache_pos = 0;
+    if (QKV) cache_pos = p.pos[0];   // requested now, consumed in the epilogue: off the critical path
+
+    float c[FT2][NT][4];
+#pragma unroll
+    for (int ft = 0; ft < FT2; ++ft)
+#pragma unroll
+        for (int j = 0; j < NT; ++j) c[ft][j][0] = c[ft][j][1] = c[ft][j][2] = c[ft][j][3] = 0.f;
+
+    const int nkb = ks >> 5;
+    const int kbw = (nkb + 3) >> 2;
+    const int kb0 = min(nkb, warp * kbw), kb1 = min(nkb, kb0 + kbw);
+    const __half* xr = p.X + (size_t)g * p.K + k0 + 8 * c4;
+    const unsigned char* wr0 = gsm + g * pitch + 8 * c4;
+    const unsigned char* wr1 = wr0 + 8 * pitch;
+
+    bool w_ready = false;
+    for (int kb = kb0; kb < kb1; kb += U) {
+        uint4 xv[U][NT];
+#pragma unroll
+        for (int u = 0; u < U; ++u)
+#pragma unroll
+            for (int j = 0; j < NT; ++j)
+                xv[u][j] = (kb + u < kb1) ? *reinterpret_cast<const uint4*>(xr + (size_t)(8 * j) * p.K + (size_t)(kb + u) * 32)
+                                          : make_uint4(0, 0, 0, 0);
+        if (!w_ready) { mbar_wait(bar, 0); w_ready = true; }
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+            if (kb + u < kb1) {
+#pragma unroll
+                for (int ft = 0; ft < FT2; ++ft) {
+                    const uint4 wa = e4m3x8_to_f16x8(*reinterpret_cast<const uint2*>(wr0 + ft * 16 * pitch + (kb + u) * 32));
+                    const uint4 wb = e4m3x8_to_f16x8(*reinterpret_cast<const uint2*>(wr1 + ft * 16 * pitch + (kb + u) * 32));
+#pragma unroll
+                    for (int j = 0; j < NT; ++j) {
+                        mma16816(c[ft][j], wa.x, wb.x, wa.y, wb.y, xv[u][j].x, xv[u][j].y);
+                        mma16816(c[ft][j], wa.z, wb.z, wa.w, wb.w, xv[u][j].z, xv[u][j].w);
+                    }
+                }
+            }
+        }
+    }
+    if (!w_ready) mbar_wait(bar, 0);   // never leave with a bulk copy in flight
+    // cross-warp (split-K inside the CTA) reduction in a fixed order
+#pragma unroll
+    for (int ft = 0; ft < FT2; ++ft)
+#pragma unroll
+        for (int j = 0; j < NT; ++j) {
+            float* r0 = red + (warp * FB + ft * 16 + g) * RP + 8 * j + 2 * c4;
+            r0[0] = c[ft][j][0];
+            r0[1] = c[ft][j][1];
+            r0[8 * RP] = c[ft][j][2];
+            r0[8 * RP + 1] = c[ft][j][3];
+        }
+    __syncthreads();
+    for (int idx = tid; idx < FB * 8 * NT; idx += 128) {
+        const int row = idx / FB, feat = idx % FB;
+        if (row >= p.rows) continue;
+        float v = 0.f;
+#pragma unroll
+        for (int w = 0; w < 4; ++w) v += red[(w * FB + feat) * RP + row];
+        const int n = f0 + feat;
+        v *= wscale[n];   // the row scale, once, on the fixed-order sum
+        if (EPI == EPI_PARTIAL) {
+            p.out_f32[blockIdx.y * p.split_stride + (size_t)row * p.ld_out + n] = v;
+        } else if (EPI == EPI_F32) {
+            p.out_f32[(size_t)row * p.ld_out + n] = v;
+        } else if (EPI == EPI_GELU) {
+            p.out_f16[(size_t)row * p.ld_out + n] = __float2half_rn(gelu_erf(half_round(v)));
+        } else if (QKV) {   // q | k | v blocks of d features each (no integer division: cold code costs here)
+            // prefill: row = tk * rows_real + rr -> cache row rr * row_stride, position cache_pos + tk
+            const int which = n >= 2 * p.d ? 2 : (n >= p.d ? 1 : 0), nn = n - which * p.d;
+            const int tk = PF ? row / p.rows_real : 0, rr = PF ? (row - tk * p.rows_real) * p.row_stride : row;
+            if (ROPE && which < 2) {   // the pair partner is feature n ^ 1 of the same CTA (f0 % 16 == 0), same warp order
+                float other = 0.f;
+#pragma unroll
+                for (int w = 0; w < 4; ++w) other += red[(w * FB + (feat ^ 1)) * RP + row];
+                other *= wscale[n ^ 1];
+                v = rope_rotate(p.rope_freq, p.pos_scale, half_round(v), half_round(other), nn & 63, cache_pos + tk);
+            }
+            if (which == 0) {
+                p.q32[(size_t)row * p.d + nn] = v;
+            } else {
+                __half* cache = which == 2 ? p.vc : p.kc;
+                cache[(((size_t)rr * p.H + (nn >> 6)) * p.cache_len + cache_pos + tk) * 64 + (nn & 63)] = __float2half_rn(v);
+            }
+        } else {  // EPI_CROSSKV: GEMM rows are (row, text position) pairs
+            const int R = p.row0 + row, r = R / p.text_len, tc = R % p.text_len;
+            const int which = n / p.d, nn = n % p.d, h = nn >> 6, dd = nn & 63;
+            __half* cache = which ? p.vc : p.kc;
+            cache[(((size_t)r * p.H + h) * p.cache_len + tc) * 64 + dd] = __float2half_rn(v);
+        }
+    }
+}
+
 // ------------------------------------------------------------------------------------------------ wide GEMM (65-256 rows)
 // The decode GEMM for rows > 64, where lm_gemm_kernel's mma.sync tile (8 * NT <= 64 rows in registers) cannot grow.  Swap-AB
 // on wgmma: the output tile is 64 features x all NPAD rows, D = W[64 x k] . X[NPAD x k]^T with the weight slab as the A
@@ -342,9 +485,9 @@ __global__ void __launch_bounds__(128) lm_gemm_kernel(GemmParams p) {
 // batch of this range.
 constexpr int WIDE_KC = 64;   // K elements per chunk: one 128-byte swizzle row
 static_assert(WIDE_KC == TMA_BOX_K, "the tensor maps (encode_map) deliver one chunk per box");
-template <int NPAD>
+template <int NPAD, int W_ELEM_BYTES = 2>
 struct WideCfg {
-    static constexpr int W_BYTES = 64 * WIDE_KC * 2;
+    static constexpr int W_BYTES = 64 * WIDE_KC * W_ELEM_BYTES;
     static constexpr int STAGE = W_BYTES + NPAD * WIDE_KC * 2;
     static constexpr int STAGES = NPAD <= 128 ? 6 : 5;
     static constexpr int LDS = 68;   // pitch (floats) of the [NPAD][64] fp32 staging tile: conflict-free fragment stores
@@ -354,10 +497,14 @@ struct WideCfg {
 
 // EPI is EPI_PARTIAL, EPI_QKV, EPI_QKV_ROPE, EPI_GELU or EPI_F32.  Prefill passes above 64 rows carry one position per row,
 // so their QKV epilogue is the decode one (token 0 of the pass at position pos).
-template <int NPAD, int EPI>
-__global__ void __launch_bounds__(128, 1) lm_gemm_wide_kernel(const __grid_constant__ CUtensorMap wmap,
-                                                              const __grid_constant__ CUtensorMap xmap, GemmParams p, int w_row0) {
-    using Cfg = WideCfg<NPAD>;
+// W8 (FP8 weights): the weight chunk is 64 rows x 64 e4m3 codes, staged by a uint8 map with the 64-byte swizzle (16-byte
+// unit c of row r at unit c ^ ((r >> 1) & 3)), so the 8 rows of one LDS.U16 fall in 8 different 4-bank groups.  Each warp
+// unpacks its 16 rows into the A fragment in registers (exact fp16), the MMAs take A from registers and the activations from
+// the same swizzled stage as in fp16, and wscale[n] multiplies output n's sum after the cluster's fixed-order reduction.
+template <int NPAD, int EPI, bool W8>
+__device__ __forceinline__ void wide_body(const CUtensorMap& wmap, const CUtensorMap& xmap, const GemmParams& p, int w_row0,
+                                          const float* __restrict__ wscale) {
+    using Cfg = WideCfg<NPAD, W8 ? 1 : 2>;
     constexpr bool ROPE = EPI == EPI_QKV_ROPE, QKV = EPI == EPI_QKV || ROPE;
     extern __shared__ unsigned char wsm_raw[];
     unsigned char* wsm = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(wsm_raw) + 1023) & ~(uintptr_t)1023);
@@ -390,10 +537,28 @@ __global__ void __launch_bounds__(128, 1) lm_gemm_wide_kernel(const __grid_const
         const int s = c % Cfg::STAGES;
         mbar_wait(&full[s], (uint32_t)(c / Cfg::STAGES) & 1u);
         const uint32_t a = smem_u32(wsm + s * Cfg::STAGE), b = a + Cfg::W_BYTES;
-        wgmma_fence();
+        if constexpr (W8) {
+            // lane (g, c4) of warp w: codes k = 16 kk + 2 c4 (+1) and + 8 of rows 16 w + g and 16 w + g + 8
+            const int g = lane >> 2, c4 = lane & 3, r0 = 16 * warp + g, r1 = r0 + 8;
+            const unsigned char* st = wsm + s * Cfg::STAGE;
+            uint32_t af[WIDE_KC / 16][4];
 #pragma unroll
-        for (int kk = 0; kk < WIDE_KC / 16; ++kk)   // a 16-element K step advances the start address by 32 bytes
-            wgmma_f16<NPAD>(acc, wgmma_desc_sw128(a + 32 * kk), wgmma_desc_sw128(b + 32 * kk), 1u);
+            for (int kk = 0; kk < WIDE_KC / 16; ++kk) {
+                const int o0 = r0 * 64 + 16 * (kk ^ ((r0 >> 1) & 3)) + 2 * c4, o1 = r1 * 64 + 16 * (kk ^ ((r1 >> 1) & 3)) + 2 * c4;
+                af[kk][0] = e4m3x2_to_f16x2(*reinterpret_cast<const uint16_t*>(st + o0));
+                af[kk][1] = e4m3x2_to_f16x2(*reinterpret_cast<const uint16_t*>(st + o1));
+                af[kk][2] = e4m3x2_to_f16x2(*reinterpret_cast<const uint16_t*>(st + o0 + 8));
+                af[kk][3] = e4m3x2_to_f16x2(*reinterpret_cast<const uint16_t*>(st + o1 + 8));
+            }
+            wgmma_fence();
+#pragma unroll
+            for (int kk = 0; kk < WIDE_KC / 16; ++kk) wgmma_f16_ra<NPAD>(acc, af[kk], wgmma_desc_sw128(b + 32 * kk), 1u);
+        } else {
+            wgmma_fence();
+#pragma unroll
+            for (int kk = 0; kk < WIDE_KC / 16; ++kk)   // a 16-element K step advances the start address by 32 bytes
+                wgmma_f16<NPAD>(acc, wgmma_desc_sw128(a + 32 * kk), wgmma_desc_sw128(b + 32 * kk), 1u);
+        }
         wgmma_commit();
         wgmma_wait<0>();
         wgmma_fence_regs(acc);
@@ -431,6 +596,7 @@ __global__ void __launch_bounds__(128, 1) lm_gemm_wide_kernel(const __grid_const
 #pragma unroll
         for (int r = 0; r < 4; ++r)   // fixed order: slice 0 first
             if (r < cs) v += src[r][row * Cfg::LDS + feat];
+        if constexpr (W8) v *= wscale[n];
         if (EPI == EPI_PARTIAL) {
             p.out_f32[blockIdx.y * p.split_stride + (size_t)row * p.ld_out + n] = v;
         } else if (EPI == EPI_F32) {
@@ -444,6 +610,7 @@ __global__ void __launch_bounds__(128, 1) lm_gemm_wide_kernel(const __grid_const
 #pragma unroll
                 for (int r = 0; r < 4; ++r)
                     if (r < cs) other += src[r][row * Cfg::LDS + (feat ^ 1)];
+                if constexpr (W8) other *= wscale[n ^ 1];
                 v = rope_rotate(p.rope_freq, p.pos_scale, half_round(v), half_round(other), nn & 63, cache_pos);
             }
             if (which == 0) {
@@ -455,6 +622,19 @@ __global__ void __launch_bounds__(128, 1) lm_gemm_wide_kernel(const __grid_const
         }
     }
     if (cs > 1) cg::this_cluster().sync();   // the other CTAs read this CTA's tile until here
+}
+
+template <int NPAD, int EPI>
+__global__ void __launch_bounds__(128, 1) lm_gemm_wide_kernel(const __grid_constant__ CUtensorMap wmap,
+                                                              const __grid_constant__ CUtensorMap xmap, GemmParams p, int w_row0) {
+    wide_body<NPAD, EPI, false>(wmap, xmap, p, w_row0, nullptr);
+}
+
+template <int NPAD, int EPI>
+__global__ void __launch_bounds__(128, 1) lm_gemm_wide_fp8_kernel(const __grid_constant__ CUtensorMap wmap,
+                                                                  const __grid_constant__ CUtensorMap xmap, GemmParams p,
+                                                                  int w_row0, const float* __restrict__ wscale) {
+    wide_body<NPAD, EPI, true>(wmap, xmap, p, w_row0, wscale);
 }
 
 // Which cache position a row of a decode step or of a prompt pass appends at (and attends up to), shared by the fp16 and FP8
@@ -1396,57 +1576,69 @@ struct acb_lm {
     // buffer [rows][K] of the current generation (encoded by acb_lm_begin_prefix)
     CUtensorMap wmap[7];
     CUtensorMap xmap_h16, xmap_a16, xmap_f16;
+    bool w8 = false;   // weight_dtype 1: e4m3 per-layer matrices with row scales (lm_gemm_fp8_kernel, lm_gemm_wide_fp8_kernel)
 };
 enum { WM_QKV = 0, WM_O, WM_CQ, WM_CO, WM_FF1, WM_FF2, WM_HEADS };
 
 static int nt_for_rows(int rows) { return rows <= 8 ? 1 : (rows <= 16 ? 2 : (rows <= 32 ? 4 : 8)); }
 
-static size_t gemm_smem_bytes(int nt, int kslice, int ft2 = 1) {
-    return (size_t)16 * ft2 * (kslice * 2 + 64) + 16 + (size_t)4 * 16 * ft2 * (8 * nt + 1) * sizeof(float);
+static size_t gemm_smem_bytes(int nt, int kslice, int ft2 = 1, bool w8 = false) {
+    return (size_t)16 * ft2 * gemm_pitch(kslice, w8) + 16 + (size_t)4 * 16 * ft2 * (8 * nt + 1) * sizeof(float);
 }
 constexpr int GEMM_MAX_SMEM = 120 * 1024;
 
+// wscale: the row scales of an FP8 matrix (p.W holds its codes), NULL for fp16
 template <int EPI, int FT2>
-static int launch_gemm_ft(int nt, const GemmParams& p, int nsplit, cudaStream_t s) {
+static int launch_gemm_ft(int nt, const GemmParams& p, int nsplit, cudaStream_t s, const float* wscale) {
     dim3 grid(p.N / (16 * FT2), nsplit);
-    const size_t smem = gemm_smem_bytes(nt, p.kslice, FT2);
+    const size_t smem = gemm_smem_bytes(nt, p.kslice, FT2, wscale != nullptr);
     ACB_REQUIRE(smem <= (size_t)GEMM_MAX_SMEM && p.N % (16 * FT2) == 0, "lm_gemm: tile does not fit (N=%d kslice=%d ft2=%d)", p.N, p.kslice, FT2);
-    switch (nt) {
-        case 1: lm_gemm_kernel<1, EPI, FT2><<<grid, 128, smem, s>>>(p); break;
-        case 2: lm_gemm_kernel<2, EPI, FT2><<<grid, 128, smem, s>>>(p); break;
-        case 4: lm_gemm_kernel<4, EPI, FT2><<<grid, 128, smem, s>>>(p); break;
-        default: lm_gemm_kernel<8, EPI, FT2><<<grid, 128, smem, s>>>(p); break;
+    if (wscale) {
+        switch (nt) {
+            case 1: lm_gemm_fp8_kernel<1, EPI, FT2><<<grid, 128, smem, s>>>(p, wscale); break;
+            case 2: lm_gemm_fp8_kernel<2, EPI, FT2><<<grid, 128, smem, s>>>(p, wscale); break;
+            case 4: lm_gemm_fp8_kernel<4, EPI, FT2><<<grid, 128, smem, s>>>(p, wscale); break;
+            default: lm_gemm_fp8_kernel<8, EPI, FT2><<<grid, 128, smem, s>>>(p, wscale); break;
+        }
+    } else {
+        switch (nt) {
+            case 1: lm_gemm_kernel<1, EPI, FT2><<<grid, 128, smem, s>>>(p); break;
+            case 2: lm_gemm_kernel<2, EPI, FT2><<<grid, 128, smem, s>>>(p); break;
+            case 4: lm_gemm_kernel<4, EPI, FT2><<<grid, 128, smem, s>>>(p); break;
+            default: lm_gemm_kernel<8, EPI, FT2><<<grid, 128, smem, s>>>(p); break;
+        }
     }
     ACB_LAUNCH_CHECK();
     return ACB_OK;
 }
 template <int EPI>
-static int launch_gemm(int nt, const GemmParams& p, int nsplit, cudaStream_t s, int ft2 = 1) {
+static int launch_gemm(int nt, const GemmParams& p, int nsplit, cudaStream_t s, int ft2 = 1, const float* wscale = nullptr) {
     if (ft2 == 2) {
         if constexpr (EPI == EPI_CROSSKV || EPI == EPI_QKV_PF || EPI == EPI_QKV_PF_ROPE) { acb_set_error("lm_gemm: this epilogue uses 16-feature tiles"); return ACB_ERR_INVALID; }
-        else return launch_gemm_ft<EPI, 2>(nt, p, nsplit, s);
+        else return launch_gemm_ft<EPI, 2>(nt, p, nsplit, s, wscale);
     }
-    return launch_gemm_ft<EPI, 1>(nt, p, nsplit, s);
+    return launch_gemm_ft<EPI, 1>(nt, p, nsplit, s, wscale);
 }
 
 template <int NT, int EPI, int FT2>
-static cudaError_t gemm_attr_one() {
-    cudaError_t e = cudaFuncSetAttribute(lm_gemm_kernel<NT, EPI, FT2>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_MAX_SMEM);
+static cudaError_t gemm_attr_one(bool w8) {
+    const void* f = w8 ? (const void*)lm_gemm_fp8_kernel<NT, EPI, FT2> : (const void*)lm_gemm_kernel<NT, EPI, FT2>;
+    cudaError_t e = cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_MAX_SMEM);
     if (e != cudaSuccess) return e;
-    return cudaFuncSetAttribute(lm_gemm_kernel<NT, EPI, FT2>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+    return cudaFuncSetAttribute(f, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
 }
 template <int EPI>
-static cudaError_t gemm_attr_all() {
+static cudaError_t gemm_attr_all(bool w8 = false) {
     cudaError_t e;
-    if ((e = gemm_attr_one<1, EPI, 1>()) != cudaSuccess) return e;
-    if ((e = gemm_attr_one<2, EPI, 1>()) != cudaSuccess) return e;
-    if ((e = gemm_attr_one<4, EPI, 1>()) != cudaSuccess) return e;
-    if ((e = gemm_attr_one<8, EPI, 1>()) != cudaSuccess) return e;
+    if ((e = gemm_attr_one<1, EPI, 1>(w8)) != cudaSuccess) return e;
+    if ((e = gemm_attr_one<2, EPI, 1>(w8)) != cudaSuccess) return e;
+    if ((e = gemm_attr_one<4, EPI, 1>(w8)) != cudaSuccess) return e;
+    if ((e = gemm_attr_one<8, EPI, 1>(w8)) != cudaSuccess) return e;
     if constexpr (EPI != EPI_CROSSKV && EPI != EPI_QKV_PF && EPI != EPI_QKV_PF_ROPE) {
-        if ((e = gemm_attr_one<1, EPI, 2>()) != cudaSuccess) return e;
-        if ((e = gemm_attr_one<2, EPI, 2>()) != cudaSuccess) return e;
-        if ((e = gemm_attr_one<4, EPI, 2>()) != cudaSuccess) return e;
-        if ((e = gemm_attr_one<8, EPI, 2>()) != cudaSuccess) return e;
+        if ((e = gemm_attr_one<1, EPI, 2>(w8)) != cudaSuccess) return e;
+        if ((e = gemm_attr_one<2, EPI, 2>(w8)) != cudaSuccess) return e;
+        if ((e = gemm_attr_one<4, EPI, 2>(w8)) != cudaSuccess) return e;
+        if ((e = gemm_attr_one<8, EPI, 2>(w8)) != cudaSuccess) return e;
     }
     return cudaSuccess;
 }
@@ -1500,7 +1692,8 @@ static int pick_split_wide(int N, int K, int sms, bool allow_split, int* kslice)
 
 // grid (N / 64, ny); the non-PARTIAL epilogues run ny as one cluster that reduces the K slices
 template <int EPI>
-static int launch_wide(const CUtensorMap& wm, const CUtensorMap& xm, int w_row0, const GemmParams& p, int ny, cudaStream_t s) {
+static int launch_wide(const CUtensorMap& wm, const CUtensorMap& xm, int w_row0, const GemmParams& p, int ny, cudaStream_t s,
+                       const float* wscale = nullptr) {
     ACB_REQUIRE(p.N % 64 == 0 && p.rows <= 256, "lm_gemm_wide: N=%d rows=%d", p.N, p.rows);
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(p.N / 64, ny);
@@ -1514,7 +1707,13 @@ static int launch_wide(const CUtensorMap& wm, const CUtensorMap& xm, int w_row0,
     cfg.attrs = at;
     cfg.numAttrs = 1;
     cudaError_t e;
-    if (wide_npad(p.rows) == 128) {
+    if (wscale && wide_npad(p.rows) == 128) {
+        cfg.dynamicSmemBytes = WideCfg<128, 1>::SMEM;
+        e = cudaLaunchKernelEx(&cfg, lm_gemm_wide_fp8_kernel<128, EPI>, wm, xm, p, w_row0, wscale);
+    } else if (wscale) {
+        cfg.dynamicSmemBytes = WideCfg<256, 1>::SMEM;
+        e = cudaLaunchKernelEx(&cfg, lm_gemm_wide_fp8_kernel<256, EPI>, wm, xm, p, w_row0, wscale);
+    } else if (wide_npad(p.rows) == 128) {
         cfg.dynamicSmemBytes = WideCfg<128>::SMEM;
         e = cudaLaunchKernelEx(&cfg, lm_gemm_wide_kernel<128, EPI>, wm, xm, p, w_row0);
     } else {
@@ -1536,6 +1735,24 @@ static cudaError_t wide_attr_all() {
     cudaError_t e = wide_attr_one<128, EPI>();
     return e != cudaSuccess ? e : wide_attr_one<256, EPI>();
 }
+template <int NPAD, int EPI>
+static cudaError_t wide_fp8_attr_one() {
+    cudaError_t e = cudaFuncSetAttribute(lm_gemm_wide_fp8_kernel<NPAD, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         WideCfg<NPAD, 1>::SMEM);
+    if (e != cudaSuccess) return e;
+    return cudaFuncSetAttribute(lm_gemm_wide_fp8_kernel<NPAD, EPI>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+}
+template <int EPI>
+static cudaError_t wide_fp8_attr_all() {
+    cudaError_t e = wide_fp8_attr_one<128, EPI>();
+    return e != cudaSuccess ? e : wide_fp8_attr_one<256, EPI>();
+}
+
+// Layer l's [N][K] block of a stacked per-layer matrix (fp16 or e4m3 codes) and its row scales (NULL for fp16).
+static const void* layer_w(const acb_lm* lm, const void* w, int l, int N, int K) {
+    return static_cast<const unsigned char*>(w) + (size_t)l * N * K * (lm->w8 ? 1 : 2);
+}
+static const float* layer_s(const acb_lm* lm, const float* s, int l, int N) { return lm->w8 ? s + (size_t)l * N : nullptr; }
 
 static GemmParams base_gemm(const void* W, const void* X, int N, int K, int rows, int kslice) {
     GemmParams p{};
@@ -1633,12 +1850,14 @@ static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_la
         DBG("lm_ln_kernel", layer);
         return ACB_OK;
     };
-    auto partial_gemm = [&](const __half* W, const void* X, int N, int K, int layer, int wm, const CUtensorMap& xm) -> int {
+    auto partial_gemm = [&](const void* W, const float* S, const void* X, int N, int K, int layer, int wm,
+                            const CUtensorMap& xm) -> int {
         const int ns = wide ? pick_split_wide(N, K, lm->sms, true, &ks) : pick_split(N, K, lm->sms, true, &ks);
-        GemmParams p = base_gemm(W, X, N, K, rows, ks);
+        GemmParams p = base_gemm(layer_w(lm, W, layer, N, K), X, N, K, rows, ks);
         p.out_f32 = B.part; p.ld_out = N; p.split_stride = part_stride;
-        if (wide) ACB_TRY(launch_wide<EPI_PARTIAL>(lm->wmap[wm], xm, layer * N, p, ns, s));
-        else ACB_TRY(launch_gemm<EPI_PARTIAL>(nt, p, ns, s, pick_ft2(N, K, ns, ks, nt, lm->sms)));
+        const float* ws = layer_s(lm, S, layer, N);
+        if (wide) ACB_TRY(launch_wide<EPI_PARTIAL>(lm->wmap[wm], xm, layer * N, p, ns, s, ws));
+        else ACB_TRY(launch_gemm<EPI_PARTIAL>(nt, p, ns, s, pick_ft2(N, K, ns, ks, nt, lm->sms), ws));
         ++nl;
         DBG("gemm_EPI_PARTIAL", layer);
         pending = ns;
@@ -1650,7 +1869,8 @@ static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_la
         ACB_TRY(ln_launch(ln, ln + d, l));
         {
             const int ns = wide ? pick_split_wide(3 * d, d, lm->sms, false, &ks) : pick_split(3 * d, d, lm->sms, false, &ks);
-            GemmParams p = base_gemm((const __half*)lm->w.w_qkv + (size_t)l * 3 * d * d, B.h16, 3 * d, d, rows, ks);
+            GemmParams p = base_gemm(layer_w(lm, lm->w.w_qkv, l, 3 * d, d), B.h16, 3 * d, d, rows, ks);
+            const float* ws = layer_s(lm, lm->w.s_qkv, l, 3 * d);
             p.q32 = B.q32; p.kc = kv_k + l * kv_layer + kv_row0; p.vc = kv_v + l * kv_layer + kv_row0;
             p.d = d; p.H = H; p.cache_len = kv_len; p.pos = B.pos; p.rows_real = rows_real; p.row_stride = kv_stride;
             p.rope_freq = lm->w.rope_freq; p.pos_scale = c.pos_scale;
@@ -1659,8 +1879,8 @@ static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_la
             if (slot_step) {   // plain fp32 epilogue into part slot 0 (free between the LN and the out projection), then
                                // the rotary + cache append at each row's own position
                 p.out_f32 = B.part; p.ld_out = 3 * d;
-                if (wide) ACB_TRY(launch_wide<EPI_F32>(lm->wmap[WM_QKV], lm->xmap_h16, l * 3 * d, p, ns, s));
-                else ACB_TRY(launch_gemm<EPI_F32>(nt, p, 1, s, ft2));
+                if (wide) ACB_TRY(launch_wide<EPI_F32>(lm->wmap[WM_QKV], lm->xmap_h16, l * 3 * d, p, ns, s, ws));
+                else ACB_TRY(launch_gemm<EPI_F32>(nt, p, 1, s, ft2, ws));
                 ++nl;
                 DBG("gemm_EPI_F32 (qkv)", l);
                 if (!gemms_only && lm->fp8) {
@@ -1686,7 +1906,7 @@ static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_la
                 }
             } else if (paged_pass) {   // the pass's plain fp32 epilogue, then the append through the page table
                 p.out_f32 = B.part; p.ld_out = 3 * d;
-                ACB_TRY(launch_gemm<EPI_F32>(nt, p, 1, s, ft2));
+                ACB_TRY(launch_gemm<EPI_F32>(nt, p, 1, s, ft2, ws));
                 ++nl;
                 DBG("gemm_EPI_F32 (qkv pass)", l);
                 if (lm->fp8)
@@ -1700,10 +1920,10 @@ static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_la
                 ACB_LAUNCH_CHECK();
                 ++nl;
                 DBG("lm_qkv_pf_paged_kernel", l);
-            } else if (wide) ACB_TRY(rope ? launch_wide<EPI_QKV_ROPE>(lm->wmap[WM_QKV], lm->xmap_h16, l * 3 * d, p, ns, s)
-                                   : launch_wide<EPI_QKV>(lm->wmap[WM_QKV], lm->xmap_h16, l * 3 * d, p, ns, s));
-            else if (pf) ACB_TRY(rope ? launch_gemm<EPI_QKV_PF_ROPE>(nt, p, 1, s, ft2) : launch_gemm<EPI_QKV_PF>(nt, p, 1, s, ft2));
-            else ACB_TRY(rope ? launch_gemm<EPI_QKV_ROPE>(nt, p, 1, s, ft2) : launch_gemm<EPI_QKV>(nt, p, 1, s, ft2));
+            } else if (wide) ACB_TRY(rope ? launch_wide<EPI_QKV_ROPE>(lm->wmap[WM_QKV], lm->xmap_h16, l * 3 * d, p, ns, s, ws)
+                                   : launch_wide<EPI_QKV>(lm->wmap[WM_QKV], lm->xmap_h16, l * 3 * d, p, ns, s, ws));
+            else if (pf) ACB_TRY(rope ? launch_gemm<EPI_QKV_PF_ROPE>(nt, p, 1, s, ft2, ws) : launch_gemm<EPI_QKV_PF>(nt, p, 1, s, ft2, ws));
+            else ACB_TRY(rope ? launch_gemm<EPI_QKV_ROPE>(nt, p, 1, s, ft2, ws) : launch_gemm<EPI_QKV>(nt, p, 1, s, ft2, ws));
             if (!slot_step && !paged_pass) {
                 ++nl;
                 DBG("gemm_EPI_QKV", l);
@@ -1731,11 +1951,11 @@ static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_la
             ++nl;
             DBG("lm_attn2_kernel", l);
         }
-        ACB_TRY(partial_gemm((const __half*)lm->w.w_o + (size_t)l * d * d, B.a16, d, d, l, WM_O, lm->xmap_a16));
+        ACB_TRY(partial_gemm(lm->w.w_o, lm->w.s_o, B.a16, d, d, l, WM_O, lm->xmap_a16));
         // --- cross attention
         if (lm->has_cross) {
             ACB_TRY(ln_launch(ln + 2 * d, ln + 3 * d, l));
-            ACB_TRY(partial_gemm((const __half*)lm->w.w_cq + (size_t)l * d * d, B.h16, d, d, l, WM_CQ, lm->xmap_h16));
+            ACB_TRY(partial_gemm(lm->w.w_cq, lm->w.s_cq, B.h16, d, d, l, WM_CQ, lm->xmap_h16));
             const int nsq = pending;
             pending = 0;   // these partials are the cross-attention queries, not a residual update
             if (!gemms_only) {
@@ -1751,20 +1971,21 @@ static int enqueue_step(acb_lm* lm, cudaStream_t s, float* logits_out, int* n_la
                 ++nl;
                 DBG("lm_cross_attn_kernel", l);
             }
-            ACB_TRY(partial_gemm((const __half*)lm->w.w_co + (size_t)l * d * d, B.a16, d, d, l, WM_CO, lm->xmap_a16));
+            ACB_TRY(partial_gemm(lm->w.w_co, lm->w.s_co, B.a16, d, d, l, WM_CO, lm->xmap_a16));
         }
         // --- feed forward
         ACB_TRY(ln_launch(ln + 4 * d, ln + 5 * d, l));
         {
             const int ns = wide ? pick_split_wide(ffn, d, lm->sms, false, &ks) : pick_split(ffn, d, lm->sms, false, &ks);
-            GemmParams p = base_gemm((const __half*)lm->w.w_ff1 + (size_t)l * ffn * d, B.h16, ffn, d, rows, ks);
+            GemmParams p = base_gemm(layer_w(lm, lm->w.w_ff1, l, ffn, d), B.h16, ffn, d, rows, ks);
             p.out_f16 = (__half*)B.f16; p.ld_out = ffn;
-            if (wide) ACB_TRY(launch_wide<EPI_GELU>(lm->wmap[WM_FF1], lm->xmap_h16, l * ffn, p, ns, s));
-            else ACB_TRY(launch_gemm<EPI_GELU>(nt, p, 1, s, pick_ft2(ffn, d, 1, ks, nt, lm->sms)));
+            const float* ws = layer_s(lm, lm->w.s_ff1, l, ffn);
+            if (wide) ACB_TRY(launch_wide<EPI_GELU>(lm->wmap[WM_FF1], lm->xmap_h16, l * ffn, p, ns, s, ws));
+            else ACB_TRY(launch_gemm<EPI_GELU>(nt, p, 1, s, pick_ft2(ffn, d, 1, ks, nt, lm->sms), ws));
             ++nl;
             DBG("gemm_EPI_GELU", l);
         }
-        ACB_TRY(partial_gemm((const __half*)lm->w.w_ff2 + (size_t)l * d * ffn, B.f16, d, ffn, l, WM_FF2, lm->xmap_f16));
+        ACB_TRY(partial_gemm(lm->w.w_ff2, lm->w.s_ff2, B.f16, d, ffn, l, WM_FF2, lm->xmap_f16));
     }
     if (pf) {   // no output norm / heads / sampler: the pass only fills the KV cache
         if (n_launch) *n_launch = nl;
@@ -1817,10 +2038,16 @@ extern "C" int acb_lm_create(const acb_lm_config* cfg, const acb_lm_weights* w, 
     ACB_REQUIRE(cfg->positional_embedding >= 0 && cfg->positional_embedding <= 2, "acb_lm_create: positional_embedding %d not in [0,2]",
                 cfg->positional_embedding);
     ACB_REQUIRE(cfg->positional_embedding == 0 || w->rope_freq, "acb_lm_create: rotary positions need weights.rope_freq");
+    ACB_REQUIRE(cfg->weight_dtype == 0 || cfg->weight_dtype == 1, "acb_lm_create: weight_dtype %d not 0 (fp16) or 1 (e4m3)",
+                cfg->weight_dtype);
+    ACB_REQUIRE(cfg->weight_dtype == 0 || (w->s_qkv && w->s_o && w->s_ff1 && w->s_ff2 &&
+                                           (!cfg->cross_attention || (w->s_cq && w->s_ckv && w->s_co))),
+                "acb_lm_create: weight_dtype 1 (e4m3) needs the row scales of every per-layer matrix the model has");
     acb_lm* lm = new (std::nothrow) acb_lm();
     ACB_REQUIRE(lm, "acb_lm_create: out of host memory");
     lm->cfg = *cfg; lm->w = *w; lm->buf = *buf;
     lm->paged = !buf->k_cache && !buf->v_cache;
+    lm->w8 = cfg->weight_dtype == 1;
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&lm->sms, cudaDevAttrMultiProcessorCount, dev);
@@ -1837,6 +2064,16 @@ extern "C" int acb_lm_create(const acb_lm_config* cfg, const acb_lm_weights* w, 
     if (ea == cudaSuccess) ea = gemm_attr_all<EPI_QKV_PF>();
     if (ea == cudaSuccess) ea = gemm_attr_all<EPI_QKV_ROPE>();
     if (ea == cudaSuccess) ea = gemm_attr_all<EPI_QKV_PF_ROPE>();
+    if (lm->w8) {
+        if (ea == cudaSuccess) ea = gemm_attr_all<EPI_PARTIAL>(true);
+        if (ea == cudaSuccess) ea = gemm_attr_all<EPI_QKV>(true);
+        if (ea == cudaSuccess) ea = gemm_attr_all<EPI_GELU>(true);
+        if (ea == cudaSuccess) ea = gemm_attr_all<EPI_F32>(true);
+        if (ea == cudaSuccess) ea = gemm_attr_all<EPI_CROSSKV>(true);
+        if (ea == cudaSuccess) ea = gemm_attr_all<EPI_QKV_PF>(true);
+        if (ea == cudaSuccess) ea = gemm_attr_all<EPI_QKV_ROPE>(true);
+        if (ea == cudaSuccess) ea = gemm_attr_all<EPI_QKV_PF_ROPE>(true);
+    }
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_attn2_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT2_SMEM);
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_attn2_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     if (ea == cudaSuccess) ea = cudaFuncSetAttribute(lm_attn2_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT2_SMEM);
@@ -1868,6 +2105,13 @@ extern "C" int acb_lm_create(const acb_lm_config* cfg, const acb_lm_weights* w, 
         if (ea == cudaSuccess) ea = wide_attr_all<EPI_QKV_ROPE>();
         if (ea == cudaSuccess) ea = wide_attr_all<EPI_GELU>();
         if (ea == cudaSuccess) ea = wide_attr_all<EPI_F32>();
+        if (lm->w8) {
+            if (ea == cudaSuccess) ea = wide_fp8_attr_all<EPI_PARTIAL>();
+            if (ea == cudaSuccess) ea = wide_fp8_attr_all<EPI_QKV>();
+            if (ea == cudaSuccess) ea = wide_fp8_attr_all<EPI_QKV_ROPE>();
+            if (ea == cudaSuccess) ea = wide_fp8_attr_all<EPI_GELU>();
+            if (ea == cudaSuccess) ea = wide_fp8_attr_all<EPI_F32>();
+        }
     }
     if (ea != cudaSuccess) {
         acb_set_error("acb_lm_create: cudaFuncSetAttribute: %s", cudaGetErrorString(ea));
@@ -1877,12 +2121,13 @@ extern "C" int acb_lm_create(const acb_lm_config* cfg, const acb_lm_weights* w, 
     }
     if (cfg->max_rows > 64) {   // the wide GEMM's weight maps: each stacked matrix as [L * N][K], 64-row boxes
         const int d = cfg->dim, ffn = cfg->ffn_dim, L = cfg->num_layers;
-        int rc = encode_map(&lm->wmap[WM_QKV], w->w_qkv, d, L * 3 * d, 64);
-        if (rc == ACB_OK) rc = encode_map(&lm->wmap[WM_O], w->w_o, d, L * d, 64);
-        if (rc == ACB_OK && cfg->cross_attention) rc = encode_map(&lm->wmap[WM_CQ], w->w_cq, d, L * d, 64);
-        if (rc == ACB_OK && cfg->cross_attention) rc = encode_map(&lm->wmap[WM_CO], w->w_co, d, L * d, 64);
-        if (rc == ACB_OK) rc = encode_map(&lm->wmap[WM_FF1], w->w_ff1, d, L * ffn, 64);
-        if (rc == ACB_OK) rc = encode_map(&lm->wmap[WM_FF2], w->w_ff2, ffn, L * d, 64);
+        auto wmap = lm->w8 ? encode_map_u8 : encode_map;
+        int rc = wmap(&lm->wmap[WM_QKV], w->w_qkv, d, L * 3 * d, 64);
+        if (rc == ACB_OK) rc = wmap(&lm->wmap[WM_O], w->w_o, d, L * d, 64);
+        if (rc == ACB_OK && cfg->cross_attention) rc = wmap(&lm->wmap[WM_CQ], w->w_cq, d, L * d, 64);
+        if (rc == ACB_OK && cfg->cross_attention) rc = wmap(&lm->wmap[WM_CO], w->w_co, d, L * d, 64);
+        if (rc == ACB_OK) rc = wmap(&lm->wmap[WM_FF1], w->w_ff1, d, L * ffn, 64);
+        if (rc == ACB_OK) rc = wmap(&lm->wmap[WM_FF2], w->w_ff2, ffn, L * d, 64);
         if (rc == ACB_OK) rc = encode_map(&lm->wmap[WM_HEADS], w->heads, d, cfg->n_q * cfg->card, 64);
         if (rc != ACB_OK) {
             cudaStreamDestroy(lm->capture_stream);
@@ -2011,11 +2256,11 @@ extern "C" int acb_lm_begin_prefix(acb_lm_t* lm, const float* cross, const float
             for (size_t r0 = 0; r0 < M; r0 += 64) {
                 int ks = 0;
                 pick_split(2 * d, d, lm->sms, false, &ks);
-                GemmParams p = base_gemm((const __half*)lm->w.w_ckv + (size_t)l * 2 * d * d,
+                GemmParams p = base_gemm(layer_w(lm, lm->w.w_ckv, l, 2 * d, d),
                                          (const __half*)lm->buf.cross16 + r0 * d, 2 * d, d, (int)min((size_t)64, M - r0), ks);
                 p.kc = (__half*)lm->buf.ck_cache + l * ckv_layer; p.vc = (__half*)lm->buf.cv_cache + l * ckv_layer;
                 p.d = d; p.H = H; p.cache_len = c.max_text; p.text_len = text_len; p.row0 = (int)r0;
-                ACB_TRY(launch_gemm<EPI_CROSSKV>(8, p, 1, s));
+                ACB_TRY(launch_gemm<EPI_CROSSKV>(8, p, 1, s, 1, layer_s(lm, lm->w.s_ckv, l, 2 * d)));
             }
     }
     // the condition prefix fills cache positions [0, prefix_len) once per generate (after the cross K/V: the passes attend to
@@ -2210,12 +2455,12 @@ static int admit(acb_lm_t* lm, int slot, const float* cross, int text_len, const
                 for (size_t r0 = 0; r0 < M; r0 += 64) {
                     int ks = 0;
                     pick_split(2 * d, d, lm->sms, false, &ks);
-                    GemmParams p = base_gemm((const __half*)lm->w.w_ckv + (size_t)l * 2 * d * d,
+                    GemmParams p = base_gemm(layer_w(lm, lm->w.w_ckv, l, 2 * d, d),
                                              (const __half*)lm->buf.cross16 + r0 * d, 2 * d, d, (int)min((size_t)64, M - r0), ks);
                     p.kc = (__half*)lm->buf.ck_cache + l * ckv_layer + dst * row_elems;
                     p.vc = (__half*)lm->buf.cv_cache + l * ckv_layer + dst * row_elems;
                     p.d = d; p.H = H; p.cache_len = c.max_text; p.text_len = text_len; p.row0 = (int)r0;
-                    ACB_TRY(launch_gemm<EPI_CROSSKV>(8, p, 1, s));
+                    ACB_TRY(launch_gemm<EPI_CROSSKV>(8, p, 1, s, 1, layer_s(lm, lm->w.s_ckv, l, 2 * d)));
                 }
         }
     }

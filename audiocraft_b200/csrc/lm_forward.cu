@@ -18,6 +18,7 @@
 #include "fwd_attn.cuh"
 #include "fwd_gemm.cuh"
 #include "lm_math.cuh"
+#include <cuda_fp8.h>
 #include <math.h>
 
 // ------------------------------------------------------------------------------------------------ embedding
@@ -84,10 +85,35 @@ __global__ void lm_fwd_f32_to_f16_kernel(const float* __restrict__ src, __half* 
     if (i < n) dst[i] = __float2half_rn(src[i]);
 }
 
+// ------------------------------------------------------------------------------------------------ FP8 weights
+// weight_dtype 1: before a layer's GEMMs, its seven e4m3 matrices become fp16(code * scale[row]) (the product in fp32) in the
+// workspace, where that layer's tensor maps point.  One launch per layer, grid.y = matrix.
+struct DequantJob { const uint8_t* codes; const float* scale; __half* dst; size_t n; int K; };
+struct DequantJobs { DequantJob j[7]; };
+__global__ void __launch_bounds__(256) lm_fwd_dequant_kernel(DequantJobs jobs) {
+    const DequantJob J = jobs.j[blockIdx.y];
+    for (size_t i = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) * 8; i < J.n; i += (size_t)gridDim.x * blockDim.x * 8) {
+        const uint2 c = *reinterpret_cast<const uint2*>(J.codes + i);   // K % 8 == 0: the 8 codes share row i / K
+        const float sc = J.scale[i / J.K];
+        const uint32_t w[2] = {c.x, c.y};
+        uint32_t o[4];
+#pragma unroll
+        for (int h = 0; h < 4; ++h) {
+            const __half2 v = __half2(__nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(w[h >> 1] >> (16 * (h & 1))), __NV_E4M3));
+            const float2 f = __half22float2(v);
+            const __half2 r = __floats2half2_rn(f.x * sc, f.y * sc);
+            o[h] = *reinterpret_cast<const uint32_t*>(&r);
+        }
+        *reinterpret_cast<uint4*>(J.dst + i) = make_uint4(o[0], o[1], o[2], o[3]);
+    }
+}
+
 // ------------------------------------------------------------------------------------------------ host side
 namespace {
 struct FwdLayout {
-    size_t x, h16, q, k, v, a16, f16, c16, ck, cv, total;
+    size_t x, h16, q, k, v, a16, f16, c16, ck, cv;
+    size_t wq, wo, wcq, wckv, wco, wff1, wff2;   // weight_dtype 1: one layer's matrices in fp16
+    size_t total;
 };
 
 size_t fwd_take(size_t* off, size_t bytes) {
@@ -107,6 +133,8 @@ int fwd_layout(const acb_lm_config* c, int batch, int prefix_len, int seq_len, i
                 "acb_lm_forward: n_q %d must be in [1, 16] and card %d even", c->n_q, c->card);
     ACB_REQUIRE(c->positional_embedding >= 0 && c->positional_embedding <= 2, "acb_lm_forward: positional_embedding %d not in [0,2]",
                 c->positional_embedding);
+    ACB_REQUIRE(c->weight_dtype == 0 || c->weight_dtype == 1, "acb_lm_forward: weight_dtype %d not 0 (fp16) or 1 (e4m3)",
+                c->weight_dtype);
     ACB_REQUIRE(batch >= 1 && seq_len >= 1 && prefix_len >= 0 && text_len >= 0,
                 "acb_lm_forward: batch %d, seq_len %d, prefix_len %d, text_len %d", batch, seq_len, prefix_len, text_len);
     ACB_REQUIRE(!c->cross_attention || text_len >= 1, "acb_lm_forward: the model has cross attention, text_len must be >= 1");
@@ -128,6 +156,14 @@ int fwd_layout(const acb_lm_config* c, int batch, int prefix_len, int seq_len, i
     L->c16 = fwd_take(&off, Mt * d * h);
     L->ck = fwd_take(&off, Mt * d * h);
     L->cv = fwd_take(&off, Mt * d * h);
+    const size_t dq = c->weight_dtype == 1 ? d * h : 0, ffn = c->ffn_dim, xd = c->cross_attention ? d : 0;
+    L->wq = fwd_take(&off, 3 * d * dq);
+    L->wo = fwd_take(&off, d * dq);
+    L->wcq = fwd_take(&off, xd * dq);
+    L->wckv = fwd_take(&off, 2 * xd * dq);
+    L->wco = fwd_take(&off, xd * dq);
+    L->wff1 = fwd_take(&off, ffn * dq);
+    L->wff2 = fwd_take(&off, ffn * dq);
     L->total = off;
     return ACB_OK;
 }
@@ -158,6 +194,9 @@ extern "C" int acb_lm_forward(const acb_lm_config* cfg, const acb_lm_weights* w,
     ACB_REQUIRE(w->emb && w->w_qkv && w->w_o && w->w_ff1 && w->w_ff2 && w->ln && w->out_norm && w->heads &&
                 (!sin_pos || w->inv_freq) && (!rope || w->rope_freq) && (!has_cross || (w->w_cq && w->w_ckv && w->w_co)),
                 "acb_lm_forward: a weight the config needs is NULL");
+    const bool w8 = c.weight_dtype == 1;
+    ACB_REQUIRE(!w8 || (w->s_qkv && w->s_o && w->s_ff1 && w->s_ff2 && (!has_cross || (w->s_cq && w->s_ckv && w->s_co))),
+                "acb_lm_forward: weight_dtype 1 (e4m3) needs the row scales of every per-layer matrix the model has");
     ACB_REQUIRE((prefix_len > 0) == (prefix != nullptr), "acb_lm_forward: prefix must be given exactly when prefix_len > 0 (%d)",
                 prefix_len);
     ACB_REQUIRE(has_cross == (cross != nullptr), "acb_lm_forward: the condition tensor must be given exactly when the model has "
@@ -175,21 +214,29 @@ extern "C" int acb_lm_forward(const acb_lm_config* cfg, const acb_lm_weights* w,
     const int d = c.dim, ffn = c.ffn_dim, H = c.num_heads, NL = c.num_layers, T = prefix_len + seq_len, M = batch * T;
     const int Mt = has_cross ? batch * text_len : 0, NV = c.n_q * c.card;
 
-    // tensor maps: activations [rows][K] and stacked weights [L * N][K], 128-row boxes
+    // tensor maps: activations [rows][K] and stacked weights [L * N][K], 128-row boxes.  FP8 weights: the maps cover the
+    // workspace's fp16 copy of one layer (LW = 1), which lm_fwd_dequant_kernel rewrites before each layer's GEMMs.
+    const int LW = w8 ? 1 : NL;
+    const void *wq = w->w_qkv, *wo = w->w_o, *wcq = w->w_cq, *wckv = w->w_ckv, *wco = w->w_co, *wff1 = w->w_ff1, *wff2 = w->w_ff2;
+    if (w8) {
+        wq = ws + L.wq; wo = ws + L.wo; wcq = ws + L.wcq; wckv = ws + L.wckv; wco = ws + L.wco; wff1 = ws + L.wff1;
+        wff2 = ws + L.wff2;
+    }
+    auto row0 = [&](int l, int N) { return w8 ? 0 : l * N; };   // layer l's first row in its map
     CUtensorMap m_h16, m_a16, m_f16, m_c16, m_qkv, m_o, m_cq, m_ckv, m_co, m_ff1, m_ff2, m_heads;
     ACB_TRY(encode_map(&m_h16, h16, d, M, FG_BM));
     ACB_TRY(encode_map(&m_a16, a16, d, M, FG_BM));
     ACB_TRY(encode_map(&m_f16, f16, ffn, M, FG_BM));
-    ACB_TRY(encode_map(&m_qkv, w->w_qkv, d, NL * 3 * d, FG_BN));
-    ACB_TRY(encode_map(&m_o, w->w_o, d, NL * d, FG_BN));
-    ACB_TRY(encode_map(&m_ff1, w->w_ff1, d, NL * ffn, FG_BN));
-    ACB_TRY(encode_map(&m_ff2, w->w_ff2, ffn, NL * d, FG_BN));
+    ACB_TRY(encode_map(&m_qkv, wq, d, LW * 3 * d, FG_BN));
+    ACB_TRY(encode_map(&m_o, wo, d, LW * d, FG_BN));
+    ACB_TRY(encode_map(&m_ff1, wff1, d, LW * ffn, FG_BN));
+    ACB_TRY(encode_map(&m_ff2, wff2, ffn, LW * d, FG_BN));
     ACB_TRY(encode_map(&m_heads, w->heads, d, NV, FG_BN));
     if (has_cross) {
         ACB_TRY(encode_map(&m_c16, c16, d, Mt, FG_BM));
-        ACB_TRY(encode_map(&m_cq, w->w_cq, d, NL * d, FG_BN));
-        ACB_TRY(encode_map(&m_ckv, w->w_ckv, d, NL * 2 * d, FG_BN));
-        ACB_TRY(encode_map(&m_co, w->w_co, d, NL * d, FG_BN));
+        ACB_TRY(encode_map(&m_cq, wcq, d, LW * d, FG_BN));
+        ACB_TRY(encode_map(&m_ckv, wckv, d, LW * 2 * d, FG_BN));
+        ACB_TRY(encode_map(&m_co, wco, d, LW * d, FG_BN));
     }
 
     lm_fwd_embed_kernel<<<M, 256, 0, s>>>((const __half*)w->emb, w->inv_freq, seq, prefix, x, d, c.n_q, c.card, T, prefix_len,
@@ -212,36 +259,55 @@ extern "C" int acb_lm_forward(const acb_lm_config* cfg, const acb_lm_weights* w,
     };
     for (int l = 0; l < NL; ++l) {
         const float* lnw = w->ln + (size_t)l * 6 * d;
+        if (w8) {
+            DequantJobs jobs{};
+            int nj = 0;
+            auto job = [&](const void* codes, const float* scale, const void* dst, int N, int K) {
+                jobs.j[nj++] = DequantJob{static_cast<const uint8_t*>(codes) + (size_t)l * N * K, scale + (size_t)l * N,
+                                          (__half*)dst, (size_t)N * K, K};
+            };
+            job(w->w_qkv, w->s_qkv, wq, 3 * d, d);
+            job(w->w_o, w->s_o, wo, d, d);
+            job(w->w_ff1, w->s_ff1, wff1, ffn, d);
+            job(w->w_ff2, w->s_ff2, wff2, d, ffn);
+            if (has_cross) {
+                job(w->w_cq, w->s_cq, wcq, d, d);
+                job(w->w_ckv, w->s_ckv, wckv, 2 * d, d);
+                job(w->w_co, w->s_co, wco, d, d);
+            }
+            lm_fwd_dequant_kernel<<<dim3(264, nj), 256, 0, s>>>(jobs);
+            ACB_LAUNCH_CHECK();
+        }
         // self attention
         ACB_TRY(ln(lnw, lnw + d));
         FwdGemmParams p = base;
-        p.N = 3 * d; p.w_row0 = l * 3 * d;
+        p.N = 3 * d; p.w_row0 = row0(l, 3 * d);
         ACB_TRY(rope ? fwd_gemm<FE_QKV_ROPE>(m_h16, m_qkv, p, s) : fwd_gemm<FE_QKV>(m_h16, m_qkv, p, s));
         ACB_TRY(fwd_attn(true, FwdAttnParams{q, k, v, a16, H, T, T, d, scale}, batch, s));
         p = base;
-        p.N = d; p.w_row0 = l * d;
+        p.N = d; p.w_row0 = row0(l, d);
         ACB_TRY(fwd_gemm<FE_RESID>(m_a16, m_o, p, s));
         // cross attention: queries of the tokens, K / V of the condition (this layer's)
         if (has_cross) {
             ACB_TRY(ln(lnw + 2 * d, lnw + 3 * d));
             p = base;
-            p.N = d; p.w_row0 = l * d;   // q alone: every column is in the q block
+            p.N = d; p.w_row0 = row0(l, d);   // q alone: every column is in the q block
             ACB_TRY(fwd_gemm<FE_QKV>(m_h16, m_cq, p, s));
             p = base;
-            p.M = Mt; p.N = 2 * d; p.w_row0 = l * 2 * d; p.T = text_len; p.k = ck; p.v = cv;
+            p.M = Mt; p.N = 2 * d; p.w_row0 = row0(l, 2 * d); p.T = text_len; p.k = ck; p.v = cv;
             ACB_TRY(fwd_gemm<FE_CKV>(m_c16, m_ckv, p, s));
             ACB_TRY(fwd_attn(false, FwdAttnParams{q, ck, cv, a16, H, T, text_len, d, scale}, batch, s));
             p = base;
-            p.N = d; p.w_row0 = l * d;
+            p.N = d; p.w_row0 = row0(l, d);
             ACB_TRY(fwd_gemm<FE_RESID>(m_a16, m_co, p, s));
         }
         // feed forward
         ACB_TRY(ln(lnw + 4 * d, lnw + 5 * d));
         p = base;
-        p.N = ffn; p.w_row0 = l * ffn;
+        p.N = ffn; p.w_row0 = row0(l, ffn);
         ACB_TRY(fwd_gemm<FE_GELU>(m_h16, m_ff1, p, s));
         p = base;
-        p.N = d; p.K = ffn; p.w_row0 = l * d;
+        p.N = d; p.K = ffn; p.w_row0 = row0(l, d);
         ACB_TRY(fwd_gemm<FE_RESID>(m_f16, m_ff2, p, s));
     }
     ACB_TRY(ln(w->out_norm, w->out_norm + d));

@@ -41,16 +41,17 @@ static PFN_cuTensorMapEncodeTiled_v12000 tensor_map_encoder() {
     return fn;
 }
 
-// Tensor map of a row-major [outer][inner] matrix of `elem_bytes`-byte elements read in boxes of box_outer rows x one 128-byte
-// swizzle row (box_inner elements), 128-byte swizzled; boxes past either edge are zero-filled.
+// Tensor map of a row-major [outer][inner] matrix of `elem_bytes`-byte elements read in boxes of box_outer rows x one
+// swizzle row (box_inner elements), 128-byte swizzled unless `swizzle` says otherwise; boxes past either edge are zero-filled.
 static int encode_map_typed(CUtensorMap* m, const void* base, int inner, int outer, int box_outer, CUtensorMapDataType dt,
-                            int elem_bytes, int box_inner, const char* what) {
+                            int elem_bytes, int box_inner, const char* what,
+                            CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B) {
     PFN_cuTensorMapEncodeTiled_v12000 fn = tensor_map_encoder();
     ACB_REQUIRE(fn, "lm: cuTensorMapEncodeTiled is not available from the CUDA driver");
     cuuint64_t dims[2] = {(cuuint64_t)inner, (cuuint64_t)outer}, strides[1] = {(cuuint64_t)inner * elem_bytes};
     cuuint32_t box[2] = {(cuuint32_t)box_inner, (cuuint32_t)box_outer}, es[2] = {1, 1};
     const CUresult r = fn(m, dt, 2, const_cast<void*>(base), dims, strides, box, es,
-                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                          CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                           CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     ACB_REQUIRE(r == CUDA_SUCCESS, "lm: cuTensorMapEncodeTiled failed (%d) for a [%d][%d] %s matrix", (int)r, outer, inner, what);
     return ACB_OK;
@@ -65,4 +66,9 @@ static int encode_map(CUtensorMap* m, const void* base, int inner, int outer, in
 constexpr int TMA_BOX_K_F32 = 32;
 static int encode_map_f32(CUtensorMap* m, const void* base, int inner, int outer, int box_outer) {
     return encode_map_typed(m, base, inner, outer, box_outer, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, TMA_BOX_K_F32, "fp32");
+}
+// e4m3 matrix (FP8 weights of the wide decode GEMM), boxes of 64 bytes in the 64-byte swizzle (lm_gemm_wide_fp8_kernel)
+static int encode_map_u8(CUtensorMap* m, const void* base, int inner, int outer, int box_outer) {
+    return encode_map_typed(m, base, inner, outer, box_outer, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, 64, "e4m3",
+                            CU_TENSOR_MAP_SWIZZLE_64B);
 }

@@ -7,7 +7,9 @@ step with sampling, CFG mixing, masking and the sequence write-back on the devic
 
 Weights: reference-layout LM ``state_dict`` (SURVEY.md section 8b), cast to fp16 like the reference does on CUDA
 (audiocraft/models/loaders.py:115-118); LayerNorm parameters stay fp32.  Accumulation, residual stream, LayerNorm and
-softmax are fp32.  No CPU path exists.
+softmax are fp32.  No CPU path exists.  ``weight_dtype='fp8'`` stores the seven per-layer matrices as e4m3 codes with one
+fp32 scale per output row (``quantize_rows_e4m3``), halving the bytes each decode step streams; results then differ from
+fp16 on purpose.
 """
 import typing as tp
 from dataclasses import dataclass
@@ -19,6 +21,32 @@ from .conditioners import (ConditionFuser, ConditioningAttributes, ConditioningP
 from .patterns import DelayedPatternProvider
 
 import ctypes as C
+
+
+E4M3_MAX = 448.0
+WEIGHT_DTYPES = {'fp16': 0, 'fp8': 1}   # acb_lm_config.weight_dtype
+
+
+def check_weight_dtype(weight_dtype) -> str:
+    """The LM weight format: 'fp16', or 'fp8' (e4m3 per-layer matrices with fp32 row scales); ValueError otherwise."""
+    if not isinstance(weight_dtype, str) or weight_dtype not in WEIGHT_DTYPES:
+        raise ValueError(f"weight_dtype must be one of {sorted(WEIGHT_DTYPES)}, got {weight_dtype!r}")
+    return weight_dtype
+
+
+def quantize_rows_e4m3(w: torch.Tensor) -> tp.Tuple[torch.Tensor, torch.Tensor]:
+    """w [..., K] -> (codes [..., K] torch.float8_e4m3fn, scales [...] fp32), one scale per row of K values:
+    amax = max |w| (in fp32), code = e4m3(w * (448 / amax)) rounded to nearest even and saturated at +-448, scale =
+    amax / 448, each operation one fp32 rounding; a row with amax == 0 has zero codes and a zero scale.  The row reads back
+    as code * scale.  The self-attention FP8 KV pool quantizes each 64-value vector by the same formula."""
+    x = w.float()
+    amax = x.abs().amax(-1)
+    live = amax > 0
+    e4m3_max = torch.tensor(E4M3_MAX, device=x.device)   # tensor / tensor: a python scalar numerator is a reciprocal and a product
+    inv = torch.where(live, e4m3_max / torch.where(live, amax, torch.ones_like(amax)), torch.zeros_like(amax))
+    codes = (x * inv.unsqueeze(-1)).to(torch.float8_e4m3fn).view(torch.uint8)
+    codes = torch.where(live.unsqueeze(-1), codes, torch.zeros_like(codes))
+    return codes.view(torch.float8_e4m3fn), torch.where(live, amax / e4m3_max, torch.zeros_like(amax))
 
 
 def prompt_prefill_columns(start_offset_sequence: int) -> int:
@@ -41,7 +69,8 @@ class LMOutput:
 class LMModel:
     def __init__(self, state_dict: tp.Dict[str, torch.Tensor], cfg: dict,
                  condition_provider: tp.Optional[ConditioningProvider] = None,
-                 fuser: tp.Optional[ConditionFuser] = None, device='cuda'):
+                 fuser: tp.Optional[ConditionFuser] = None, device='cuda', weight_dtype: str = 'fp16'):
+        self.weight_dtype = check_weight_dtype(weight_dtype)
         self.device = _lib.require_cuda(device)
         self._lib = _lib.lib()
         self.cfg_dict = dict(cfg)
@@ -74,18 +103,27 @@ class LMModel:
     # ------------------------------------------------------------------ weights
     def _load_weights(self, sd, cfg):
         dev, L, d = self.device, self.num_layers, self.dim
+        fp8 = self.weight_dtype == 'fp8'
 
         def h(t):
             return t.to(dev, torch.float16).contiguous()
 
         def stack(fmt, rows=None):
+            """[L, N, K] fp16, or (fp8) ([L, N, K] e4m3 codes, [L, N] fp32 row scales) of the fp16 weights, layer by layer."""
             first = sd[fmt.format(0)]
             shape = first.shape if rows is None else (rows[1] - rows[0],) + tuple(first.shape[1:])
-            out = torch.empty((L,) + tuple(shape), device=dev, dtype=torch.float16)
+            out = torch.empty((L,) + tuple(shape), device=dev, dtype=torch.float8_e4m3fn if fp8 else torch.float16)
+            scales = torch.empty((L, shape[0]), device=dev, dtype=torch.float32) if fp8 else None
             for li in range(L):
                 t = sd[fmt.format(li)]
-                out[li].copy_(t if rows is None else t[rows[0]:rows[1]])
-            return out
+                t = t if rows is None else t[rows[0]:rows[1]]
+                if fp8:
+                    codes, sc = quantize_rows_e4m3(h(t))
+                    out[li].copy_(codes)
+                    scales[li].copy_(sc)
+                else:
+                    out[li].copy_(t)
+            return out, scales
 
         w = {}
         w['emb'] = torch.stack([h(sd[f'emb.{k}.weight']) for k in range(self.n_q)]).contiguous()
@@ -94,16 +132,16 @@ class LMModel:
         # divisor table of create_sin_embedding (transformer.py:84-88), computed by the same torch ops
         w['inv_freq'] = (torch.tensor(float(cfg['max_period'])) ** (adim / (half - 1))).to(dev).contiguous()
         p = 'transformer.layers.{}.'
-        w['w_qkv'] = stack(p + 'self_attn.in_proj_weight')
-        w['w_o'] = stack(p + 'self_attn.out_proj.weight')
+        w['w_qkv'], w['s_qkv'] = stack(p + 'self_attn.in_proj_weight')
+        w['w_o'], w['s_o'] = stack(p + 'self_attn.out_proj.weight')
         if self.cross_attention:
-            w['w_cq'] = stack(p + 'cross_attention.in_proj_weight', rows=(0, d))
-            w['w_ckv'] = stack(p + 'cross_attention.in_proj_weight', rows=(d, 3 * d))
-            w['w_co'] = stack(p + 'cross_attention.out_proj.weight')
+            w['w_cq'], w['s_cq'] = stack(p + 'cross_attention.in_proj_weight', rows=(0, d))
+            w['w_ckv'], w['s_ckv'] = stack(p + 'cross_attention.in_proj_weight', rows=(d, 3 * d))
+            w['w_co'], w['s_co'] = stack(p + 'cross_attention.out_proj.weight')
         else:
-            w['w_cq'] = w['w_ckv'] = w['w_co'] = None
-        w['w_ff1'] = stack(p + 'linear1.weight')
-        w['w_ff2'] = stack(p + 'linear2.weight')
+            w['w_cq'] = w['w_ckv'] = w['w_co'] = w['s_cq'] = w['s_ckv'] = w['s_co'] = None
+        w['w_ff1'], w['s_ff1'] = stack(p + 'linear1.weight')
+        w['w_ff2'], w['s_ff2'] = stack(p + 'linear2.weight')
         ln = torch.zeros((L, 6, d), device=dev, dtype=torch.float32)
         for li in range(L):
             names = ['norm1', 'norm_cross', 'norm2'] if self.cross_attention else ['norm1', None, 'norm2']
@@ -126,7 +164,7 @@ class LMModel:
         self._w = w
         self.weight_bytes_per_step = sum(
             t.numel() * t.element_size() for k, t in w.items()
-            if t is not None and k not in ('emb', 'inv_freq', 'w_ckv', 'rope_freq'))
+            if t is not None and k not in ('emb', 'inv_freq', 'w_ckv', 's_ckv', 'rope_freq'))
 
     # ------------------------------------------------------------------ reference attributes
     @property
@@ -147,11 +185,13 @@ class LMModel:
         return _lib.LMConfig(self.dim, self.num_heads, self.num_layers, self.ffn_dim, self.n_q, self.card,
                              int(self.cross_attention), max_rows, max_seq, max_text,
                              float(self.cfg_dict.get('positional_scale', 1.0)),
-                             {'sin': 0, 'rope': 1, 'sin_rope': 2}[self.positional_embedding])
+                             {'sin': 0, 'rope': 1, 'sin_rope': 2}[self.positional_embedding],
+                             weight_dtype=WEIGHT_DTYPES[self.weight_dtype])
 
     def _weights(self) -> _lib.LMWeights:
         return _lib.LMWeights(*[_lib.ptr(self._w[n]) for n in ('emb', 'inv_freq', 'w_qkv', 'w_o', 'w_cq', 'w_ckv',
-                                                              'w_co', 'w_ff1', 'w_ff2', 'ln', 'out_norm', 'heads', 'rope_freq')])
+                                                              'w_co', 'w_ff1', 'w_ff2', 'ln', 'out_norm', 'heads', 'rope_freq',
+                                                              's_qkv', 's_o', 's_cq', 's_ckv', 's_co', 's_ff1', 's_ff2')])
 
     # ------------------------------------------------------------------ device state
     def _ensure(self, rows: int, seq_len: int, text_len: int, batch: int, paged: bool = False):

@@ -15,7 +15,7 @@ from . import synth
 from .conditioners import (ChromaStemConditioner, ConditionFuser, ConditioningProvider, PrecomputedTextConditioner,
                            T5Conditioner, identity_stem_separator)
 from .encodec import EncodecModel
-from .lm import LMModel
+from .lm import LMModel, check_weight_dtype
 
 _SCALES = {'small': 'musicgen_small', 'medium': 'musicgen_medium', 'large': 'musicgen_large', 'melody': 'musicgen_melody',
            'stereo-small': 'musicgen_stereo_small', 'stereo-medium': 'musicgen_stereo_medium',
@@ -200,9 +200,12 @@ def hash_str(s: str) -> int:
     return h
 
 
-def load_lm_model(name: str, device='cuda', seed: int = 0, text_encoder=None, stem_separator=None) -> LMModel:
+def load_lm_model(name: str, device='cuda', seed: int = 0, text_encoder=None, stem_separator=None,
+                  weight_dtype: str = 'fp16') -> LMModel:
     """`stem_separator`: callable (wav [B,C,T], sample_rate) -> melody stems [B,1,T] standing in for Demucs in a melody
-    checkpoint; `synthetic/melody` uses `identity_stem_separator` (the mono mix is the melody) when none is given."""
+    checkpoint; `synthetic/melody` uses `identity_stem_separator` (the mono mix is the melody) when none is given.
+    `weight_dtype`: 'fp16', or 'fp8' to quantize the per-layer matrices at load (LMModel)."""
+    check_weight_dtype(weight_dtype)
     if name.startswith('synthetic/'):
         arch = name.split('/', 1)[1]
         cfg = synth.lm_config(_SCALES.get(arch, arch))
@@ -213,9 +216,9 @@ def load_lm_model(name: str, device='cuda', seed: int = 0, text_encoder=None, st
                        chroma=dict(n_chroma=cfg['n_chroma'], radix2_exp=cfg['radix2_exp'], argmax=True, match_len_on_eval=False,
                                    sample_rate=cfg['sample_rate'], duration=cfg['duration']))
             provider, fuser = _melody_parts(cfg, enc, stem_separator or identity_stem_separator, device)
-            return LMModel(sd, cfg, provider, fuser, device)
+            return LMModel(sd, cfg, provider, fuser, device, weight_dtype)
         provider = ConditioningProvider({'description': _text_conditioner(cfg, enc, device)})
-        return LMModel(sd, cfg, provider, ConditionFuser({'cross': ['description']}), device)
+        return LMModel(sd, cfg, provider, ConditionFuser({'cross': ['description']}), device, weight_dtype)
     if os.path.isfile(name):
         pkg = _load_pkg(name)
         xp = _cfg_from_yaml(pkg['xp.cfg']) if isinstance(pkg['xp.cfg'], str) else pkg['xp.cfg']
@@ -230,14 +233,14 @@ def load_lm_model(name: str, device='cuda', seed: int = 0, text_encoder=None, st
                 raise RuntimeError("this checkpoint is text-conditioned: pass text_encoder=<local T5 directory> or <callable "
                                    f"returning the frozen T5 hidden states [B,T,{cfg['cond_dim']}] and attention mask>")
             provider, fuser = _melody_parts(cfg, text_encoder, stem_separator, device)
-            return LMModel(pkg['best_state'], cfg, provider, fuser, device)
+            return LMModel(pkg['best_state'], cfg, provider, fuser, device, weight_dtype)
         if cfg['cross_attention']:
             if text_encoder is None:
                 raise RuntimeError("this checkpoint is text-conditioned: pass text_encoder=<local T5 directory in Hugging Face "
                                    "layout> or <callable returning the frozen T5 hidden states "
                                    f"[B,T,{cfg['cond_dim']}] and attention mask>")
             provider = ConditioningProvider({'description': _text_conditioner(cfg, text_encoder, device)})
-        return LMModel(pkg['best_state'], cfg, provider, ConditionFuser({'cross': ['description']}), device)
+        return LMModel(pkg['best_state'], cfg, provider, ConditionFuser({'cross': ['description']}), device, weight_dtype)
     raise FileNotFoundError(f"LM '{name}': not a local checkpoint and not 'synthetic/<scale>'")
 
 
@@ -250,15 +253,16 @@ def _wrap_from_xp(cm, lm_ckpt: str):
     return get_wrapped_compression_model(cm, xp.get('interleave_stereo_codebooks'), xp.get('compression_model_n_q'))
 
 
-def load_musicgen(name: str, device=None, seed: int = 0, text_encoder=None, stem_separator=None):
+def load_musicgen(name: str, device=None, seed: int = 0, text_encoder=None, stem_separator=None, weight_dtype: str = 'fp16'):
     """`text_encoder`: a local T5 directory in Hugging Face layout (config.json, model.safetensors or pytorch_model.bin,
     spiece.model), run on the device by T5Conditioner, or a callable list[str] -> (hidden [B,T,cond_dim], mask [B,T]) giving
     the frozen T5's output (the reference instantiates T5 from the HF hub, conditioners.py:422-515).
-    `stem_separator`: the Demucs stand-in a melody checkpoint needs (see load_lm_model)."""
+    `stem_separator`: the Demucs stand-in a melody checkpoint needs (see load_lm_model); `weight_dtype` as for load_lm_model."""
     from .musicgen import MusicGen
+    check_weight_dtype(weight_dtype)
     device = 'cuda' if device is None else device
     if name.startswith('synthetic/'):
-        lm = load_lm_model(name, device, seed, text_encoder, stem_separator)
+        lm = load_lm_model(name, device, seed, text_encoder, stem_separator, weight_dtype)
         cm = load_compression_model('synthetic/encodec_32k', device, seed + 1)
         if name.split('/', 1)[1].startswith('stereo-'):
             from .encodec import get_wrapped_compression_model
@@ -266,26 +270,27 @@ def load_musicgen(name: str, device=None, seed: int = 0, text_encoder=None, stem
         return MusicGen(name, cm, lm, max_duration=30)
     if os.path.isdir(name):
         lm_path = os.path.join(name, 'state_dict.bin')
-        lm = load_lm_model(lm_path, device, text_encoder=text_encoder, stem_separator=stem_separator)
+        lm = load_lm_model(lm_path, device, text_encoder=text_encoder, stem_separator=stem_separator, weight_dtype=weight_dtype)
         cm = _wrap_from_xp(load_compression_model(os.path.join(name, 'compression_state_dict.bin'), device), lm_path)
         return MusicGen(name, cm, lm, max_duration=30)
     raise FileNotFoundError(f"MusicGen '{name}': pass a local checkpoint directory or 'synthetic/<scale>' "
                             f"({', '.join(_SCALES)})")
 
 
-def load_audiogen(name: str, device=None, seed: int = 0, text_encoder=None):
+def load_audiogen(name: str, device=None, seed: int = 0, text_encoder=None, weight_dtype: str = 'fp16'):
     """`synthetic/audiogen-medium` (seeded random weights of the released architecture) or a local checkpoint directory;
-    `text_encoder` as for load_musicgen."""
+    `text_encoder` and `weight_dtype` as for load_musicgen."""
     from .musicgen import AudioGen
+    check_weight_dtype(weight_dtype)
     device = 'cuda' if device is None else device
     if name.startswith('synthetic/'):
         scale = name.split('/', 1)[1].replace('audiogen-', '')
-        lm = load_lm_model(f'synthetic/{scale}', device, seed, text_encoder)
+        lm = load_lm_model(f'synthetic/{scale}', device, seed, text_encoder, weight_dtype=weight_dtype)
         cm = load_compression_model('synthetic/encodec_16k', device, seed + 1)
         return AudioGen(name, cm, lm, max_duration=10)
     if os.path.isdir(name):
         lm_path = os.path.join(name, 'state_dict.bin')
-        lm = load_lm_model(lm_path, device, text_encoder=text_encoder)
+        lm = load_lm_model(lm_path, device, text_encoder=text_encoder, weight_dtype=weight_dtype)
         cm = _wrap_from_xp(load_compression_model(os.path.join(name, 'compression_state_dict.bin'), device), lm_path)
         return AudioGen(name, cm, lm, max_duration=10)
     raise FileNotFoundError(f"AudioGen '{name}': pass a local checkpoint directory or 'synthetic/audiogen-medium'")

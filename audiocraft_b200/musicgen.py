@@ -307,14 +307,17 @@ class MusicGen(BaseGenModel):
         return cp is not None and 'self_wav' in cp.conditioners
 
     @staticmethod
-    def get_pretrained(name: str = 'facebook/musicgen-medium', device=None, text_encoder=None, stem_separator=None):
+    def get_pretrained(name: str = 'facebook/musicgen-medium', device=None, text_encoder=None, stem_separator=None,
+                       weight_dtype: str = 'fp16'):
         """The reference pulls checkpoints from the HF hub (musicgen.py:56-94); offline this accepts a directory holding
         the reference's exported `state_dict.bin` + `compression_state_dict.bin` (then `text_encoder` is required: a local T5
         directory in Hugging Face layout, run on the device, or a callable returning the frozen T5's hidden states and mask), or
         `synthetic/<small|medium|large|melody>` and `synthetic/stereo-<small|medium|large|melody|melody-large>` for seeded random
-        weights of the released architectures (the stereo ones on the interleaved stereo codec, 8 codebooks)."""
+        weights of the released architectures (the stereo ones on the interleaved stereo codec, 8 codebooks).
+        `weight_dtype='fp8'` quantizes the LM's per-layer matrices to e4m3 with fp32 row scales at load (LMModel)."""
         from .loaders import load_musicgen
-        return load_musicgen(name, device=device, text_encoder=text_encoder, stem_separator=stem_separator)
+        return load_musicgen(name, device=device, text_encoder=text_encoder, stem_separator=stem_separator,
+                             weight_dtype=weight_dtype)
 
     def set_generation_params(self, use_sampling: bool = True, top_k: int = 250, top_p: float = 0.0,
                               temperature: float = 1.0, duration: float = 30.0, cfg_coef: float = 3.0,
@@ -414,9 +417,9 @@ class AudioGen(BaseGenModel):
         self.set_generation_params(duration=5)
 
     @staticmethod
-    def get_pretrained(name: str = 'facebook/audiogen-medium', device=None, text_encoder=None):
+    def get_pretrained(name: str = 'facebook/audiogen-medium', device=None, text_encoder=None, weight_dtype: str = 'fp16'):
         from .loaders import load_audiogen
-        return load_audiogen(name, device=device, text_encoder=text_encoder)
+        return load_audiogen(name, device=device, text_encoder=text_encoder, weight_dtype=weight_dtype)
 
     def set_generation_params(self, use_sampling: bool = True, top_k: int = 250, top_p: float = 0.0,
                               temperature: float = 1.0, duration: float = 10.0, cfg_coef: float = 3.0,

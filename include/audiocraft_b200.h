@@ -180,9 +180,17 @@ typedef struct {
     float pos_scale;  /* positional_scale */
     int positional_embedding; /* 0 'sin' (released MusicGen), 1 'rope', 2 'sin_rope'  (modules/transformer.py:632-637, 701-705).
                                  rope and sin_rope need weights.rope_freq */
+    int weight_dtype; /* the seven per-layer matrices w_qkv .. w_ff2: 0 fp16; 1 e4m3 codes (one byte each, same [L][N][K]
+                         layout) with one fp32 scale per output row in s_qkv .. s_ff2, W[n][k] = code[n][k] * scale[n] with
+                         scale = amax_k |W[n][k]| / 448 (see audiocraft_b200.lm.quantize_rows_e4m3).  The decode GEMMs unpack
+                         the codes exactly to fp16, accumulate code x activation in fp32 and multiply each output's sum by its
+                         row scale once; acb_lm_forward dequantizes one layer at a time into its workspace.  emb, heads and
+                         the norms stay as they are.  acb_lm_create / acb_lm_forward return ACB_ERR_INVALID when a scale the
+                         model needs is NULL or the value is neither 0 nor 1. */
 } acb_lm_config;
 
-/* fp16 matrices in the reference's own [out_features][in_features] layout, stacked over layers. */
+/* fp16 matrices in the reference's own [out_features][in_features] layout, stacked over layers (the seven per-layer
+ * matrices as e4m3 codes in the same layout when acb_lm_config.weight_dtype is 1). */
 typedef struct {
     const void* emb;      /* [n_q][card+1][d] fp16       LMModel.emb, lm.py:160-163 */
     const float* inv_freq;/* [d/2] fp32: max_period^(i/(d/2-1)), create_sin_embedding transformer.py:70-89 */
@@ -197,6 +205,15 @@ typedef struct {
     const float* out_norm;/* [2][d] fp32 */
     const void* heads;    /* [n_q*card][d] fp16  LMModel.linears, lm.py:172 */
     const float* rope_freq; /* [32] fp32: 1 / max_period^(2i/64), RotaryEmbedding.frequencies rope.py:68-69 (NULL without rope) */
+    /* weight_dtype 1 only (NULL otherwise): fp32 row scales of w_qkv .. w_ff2, [L][N] with N their output features
+       (3d, d, d, 2d, d, ffn, d); s_cq, s_ckv and s_co are needed only with cross attention */
+    const float* s_qkv;
+    const float* s_o;
+    const float* s_cq;
+    const float* s_ckv;
+    const float* s_co;
+    const float* s_ff1;
+    const float* s_ff2;
 } acb_lm_weights;
 
 /* Caller-owned state; sizes in elements.  rows_pad = acb_lm_rows_pad(max_rows) (a multiple of 16). */
@@ -420,7 +437,9 @@ int acb_lm_launches_per_step(const acb_lm_t* lm);
  *   workspace: at least acb_lm_forward_workspace_bytes(...) bytes of device memory, 256-byte aligned.
  * cfg->max_rows, max_seq and max_text are ignored.  Needs dim = 64 * num_heads <= 2048, ffn_dim % 8 == 0, even card,
  * n_q <= 16.  Every output element is summed in one fixed order (no split-K): an item's logits are bit-identical whatever
- * batch it is in.  Tensor maps are encoded per call; all work is on `stream`. */
+ * batch it is in.  Tensor maps are encoded per call; all work is on `stream`.  With cfg->weight_dtype 1 a kernel writes each
+ * layer's seven matrices as fp16(code * scale) into the workspace before that layer's GEMMs, which read them from there: the
+ * workspace is larger by one layer's matrices (fp16). */
 int64_t acb_lm_forward_workspace_bytes(const acb_lm_config* cfg, int batch, int prefix_len, int seq_len, int text_len);
 int acb_lm_forward(const acb_lm_config* cfg, const acb_lm_weights* w, const int64_t* seq, const float* cross,
                    const float* prefix, int batch, int prefix_len, int seq_len, int text_len, float* logits,
